@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """bench.py -- genome-pairs/sec of the `skani triangle` hot path on synthetic 5 Mbp bacterial genomes.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config north|c2|dense|c5] [--shuffle-order] ...
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config north|c2|dense|c5] [--shuffle-order]
+                  [--dump-outputs DIR] ...
   (N > 1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...)
 
 A "step" is one full pass of the hot path (FracMinHash seeding -> marker screen -> chaining/ANI) over the whole
@@ -14,6 +15,8 @@ checksum of (ref, query, ani, af_ref, af_query) are all-reduced over the ranks (
 sample of kept pairs is re-chained by the CPU oracle (1e-4).  With N > 1 (or --shuffle-order) the whole measurement is
 repeated on a seeded random permutation of the genome order (input order unrelated to relatedness: the worst case of the
 multi-GPU exchange) and reported under "shuffled".
+`--dump-outputs DIR` writes the kept results of the last timed step of the headline (`value`) leg as DIR/<field>.npy, one
+array per result field, rows sorted by (ref_id, query_id); the inputs are seeded, so two builds can be compared row by row.
 `--impl reference` times the reference's CPU algorithm (the C++ restatement in oracle/: the Rust crate cannot be built
 in this image) on all host cores on the SAME configuration (full genome set).
 """
@@ -28,18 +31,21 @@ import time
 
 import numpy as np
 
+sys.dont_write_bytecode = True   # the tree may be read-only: nothing is written into it
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 UNIT = "genome-pairs/s"
 CONFIGS = {   # BASELINE.json configs that are a triangle on one box (c3 = search, see tools/bench_search.py)
-    "north": dict(genomes=10000, genome_len=5_000_000, cluster=20, c=125, marker_c=1000, rescue_small=True,
-                  metric="genome-pairs/sec, skani triangle 10k x 5 Mbp synthetic"),
+    # sized for one 80 GB H100: the value leg holds 25 GB of bases next to the sketches, and the end-to-end legs hold the
+    # grow-only arenas of both contexts of the pipelined triangle (8k genomes run out of memory there)
+    "north": dict(genomes=5000, genome_len=5_000_000, cluster=20, c=125, marker_c=1000, rescue_small=True,
+                  metric="genome-pairs/sec, skani triangle 5k x 5 Mbp synthetic"),
     "c2": dict(genomes=1000, genome_len=5_000_000, cluster=20, c=125, marker_c=1000, rescue_small=True,
                metric="genome-pairs/sec, skani triangle 1k x 5 Mbp synthetic (BASELINE.json configs[1])"),
     "c4": dict(genomes=50000, genome_len=5_000_000, cluster=20, c=125, marker_c=1000, rescue_small=True,
-               metric="genome-pairs/sec, skani triangle 50k x 5 Mbp synthetic (BASELINE.json configs[3]; needs --gpus 8: 31 GB of bases and 14 GB of sketches per GPU; not measured this round)"),
+               metric="genome-pairs/sec, skani triangle 50k x 5 Mbp synthetic (BASELINE.json configs[3]; needs --gpus 8: 31 GB of bases and 14 GB of sketches per GPU; not measured)"),
     "dense": dict(genomes=2000, genome_len=5_000_000, cluster=2000, c=125, marker_c=1000, rescue_small=True,
                   metric="genome-pairs/sec, skani triangle 2000 x 5 Mbp synthetic, ONE cluster (every pair is chained)"),
     "c5": dict(genomes=200000, genome_len=30_000, cluster=10, c=30, marker_c=200, rescue_small=False,
@@ -64,6 +70,8 @@ def parse():
     ap.add_argument("--no-shuffle", action="store_true", help="skip the permuted-order measurement (A/B sessions)")
     ap.add_argument("--perm-seed", type=int, default=12345)
     ap.add_argument("--spot-check", type=int, default=200, help="kept pairs re-chained by the CPU oracle after the timed legs")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the kept results of the last timed step of the value leg as DIR/<field>.npy")
     a = ap.parse_args()
     cfg = dict(CONFIGS[a.config])
     for k in ("genomes", "genome_len", "cluster"):
@@ -124,10 +132,9 @@ class ClockSampler:
 # CPU baseline (oracle = C++ restatement of the reference algorithm; "port")
 # ------------------------------------------------------------------------------------------------------------
 def host_threads():
-    """Threads for the CPU arm: all host CPUs this process may actually use.  The GPU boxes expose 128 logical CPUs but the
-    container's cgroup grants a CPU-time quota (cpu.max, 16 CPUs on the round-1 boxes); running 128 threads under that quota
-    is SLOWER than 32 (measured: seeding speed-up 15.9x at 16 threads, 18.7x at 32, 9.2x at 128), so use 2 threads per
-    granted CPU, capped by the visible CPUs."""
+    """Threads for the CPU arm: all host CPUs this process may actually use.  A container's cgroup may grant a CPU-time
+    quota (cpu.max) well below the logical CPUs it exposes, and far more threads than the quota run slower, so use 2
+    threads per granted CPU, capped by the visible CPUs."""
     n = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     quota = None
     try:
@@ -146,7 +153,8 @@ def oracle_setup(native):
     import oracle_py as O
     how = "-march=x86-64-v3 (portable build)"
     if native:
-        path = O.build_native()
+        import tempfile
+        path = O.build_native(tempfile.mkdtemp(prefix="skani_oracle_native_"))
         if path and os.path.exists(path):
             O.use_library(path)
             how = "-march=native (built on this box)"
@@ -242,8 +250,6 @@ def run_reference(args):
     i = 0
     while i < warm + steps:
         d = cpu_triangle(O, cfg, N, threads)
-        if i == 0 and d["t_total"] > 30:   # one step already takes longer than the 30 s budget: no warm-up, at most 2 steps
-            warm, steps = 0, min(steps, 2)
         if i >= warm:
             runs.append(d)
         i += 1
@@ -437,6 +443,8 @@ def main():
             step(False)
         ms_val, _, launches = timed(False, args.steps)
         ck_val = allreduce_count_checksum(len(last["res"]), result_checksum(last["res"]), world)
+        if args.dump_outputs and order == "contiguous":
+            dump_outputs(args.dump_outputs, last["res"], world, rank)
         roof = roof_chain = None
         if rank == 0 and order == "contiguous":
             roof = measure_hashpass(ctx, dev_bases, off, goc, nloc, sp, L)
@@ -543,16 +551,32 @@ def _peak():
     try:
         return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
     except Exception:
-        return 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3"
 
 
-def _ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per unit of work from THIS round's ncu --set full capture
-    (profiles/r02_traffic.json, written by tools/profile_step.py + tools/summarize_ncu.py); None if absent."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))[kernel]
-    except Exception:
-        return None
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(out_dir, res, world, rank):
+    """Kept results of the last timed step as out_dir/<field>.npy: float fields as float32, integer fields as float64
+    (exact), rows sorted by (ref_id, query_id); above DUMP_LIMIT bytes a fixed seeded sample of the sorted rows."""
+    if world > 1:
+        import torch
+        parts = [None] * world
+        torch.distributed.all_gather_object(parts, np.asarray(res))
+        res = np.concatenate(parts)
+    if rank != 0:
+        return
+    res = np.asarray(res)
+    res = res[np.lexsort((res["query_id"], res["ref_id"]))]
+    names = res.dtype.names
+    row_bytes = sum(4 if res.dtype[n].kind == "f" else 8 for n in names)
+    if len(res) * row_bytes > DUMP_LIMIT:
+        keep = DUMP_LIMIT // row_bytes
+        res = res[np.sort(np.random.default_rng(0).choice(len(res), keep, replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    for n in names:
+        np.save(os.path.join(out_dir, n + ".npy"), res[n].astype(np.float32 if res.dtype[n].kind == "f" else np.float64))
 
 
 def measure_hashpass(ctx, dev_bases, off, goc, nloc, sp, L):
@@ -578,24 +602,12 @@ def measure_hashpass(ctx, dev_bases, off, goc, nloc, sp, L):
     peak, peak_src = _peak()
     ach = genomes_per_launch * bytes_per_genome / sec_per_launch / 1e9
     stage_ms = sum(v[0] for v in t.values())
-    tr = _ncu_traffic("hashpass_kernel")      # {"dram_bytes_per_base": ..., "issue_active_pct": ..., "inst_per_window": ..., "source": ...}
-    traffic = tr["dram_bytes_per_base"] * L * genomes_per_launch if tr else None
-    alu = None
-    if tr and tr.get("inst_per_window"):
-        # issue roofline: one warp instruction per cycle per SM sub-partition (4 per SM); windows/s at that rate
-        sm, mhz = 148, 1965.0
-        peak_windows = sm * 4 * 32 * mhz * 1e6 / tr["inst_per_window"]
-        alu = {"inst_per_window": tr["inst_per_window"], "issue_active_pct": tr.get("issue_active_pct"),
-               "busiest_pipe_pct": tr.get("sm_throughput_pct"),     # ncu sm__throughput: the integer ALU pipe (half-rate LOP3/SHF/IADD3)
-               "windows_per_s": genomes_per_launch * L / sec_per_launch, "issue_peak_windows_per_s": peak_windows,
-               "frac_of_issue_peak": genomes_per_launch * L / sec_per_launch / peak_windows}
-    return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
-            "traffic_source": tr["source"] if tr else None, "alu": alu,
+    return {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
             "kernel": "hashpass_kernel", "launch_ms": sec_per_launch * 1e3, "genomes_per_launch": genomes_per_launch,
             "algorithmic_bytes_per_genome": bytes_per_genome,
             "gbases_per_s": genomes_per_launch * L / sec_per_launch / 1e9,
             "kernel_ms": {k: round(v[0] / reps, 3) for k, v in t.items()}, "timed_kernels_ms_per_rep": round(stage_ms / reps, 3),
-            "note": "nominal bound = HBM (north_star); the kernel is integer-issue bound (64-bit hash per base at 0.375 B/base), see `alu` and DESIGN.md",
+            "note": "nominal bound = HBM (north_star); the kernel is integer-issue bound (64-bit hash per base at 0.375 B/base), see DESIGN.md",
             "peak_source": peak_src}
 
 

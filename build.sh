@@ -1,5 +1,5 @@
 #!/bin/bash
-# Builds the product library (sm_100a only), the CPU oracle and the synthetic-input generator, in-tree.
+# Builds the product library (sm_90a only), the CPU oracle and the synthetic-input generator, in-tree.
 set -e
 cd "$(dirname "$0")"
 make -s -j8 -C skani_b200/csrc

@@ -1,5 +1,5 @@
 /* ============================================================================================
- * skani_b200.h -- C ABI of libskani_b200.so: the Blackwell (sm_100a) implementation of skani's
+ * skani_b200.h -- C ABI of libskani_b200.so: the Hopper (H100, sm_90a) implementation of skani's
  * ANI hot path (FracMinHash seeding -> marker screen -> seed intersection / chaining / ANI+AF /
  * learned-ANI regression).
  *

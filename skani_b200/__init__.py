@@ -1,4 +1,4 @@
-"""skani_b200 -- Blackwell-native (sm_100a) implementation of skani's ANI hot path.
+"""skani_b200 -- H100 (sm_90a) CUDA implementation of skani's ANI hot path.
 
 Host-side mirror of the reference's public API for the path (fastx_to_sketches -> screen -> chain_seeds,
 reference tests/tests.rs:42-60) over the C ABI in include/skani_b200.h.  No CPU fallback exists."""

@@ -794,7 +794,7 @@ int run_ingest(Opts& op) {
 
 void usage() {
   fprintf(stderr,
-          "skani-b200 (Blackwell implementation of skani v0.3.0's ANI hot path)\n"
+          "skani-b200 (H100 CUDA implementation of skani v0.3.0's ANI hot path)\n"
           "  skani-b200 triangle [fasta ... | -l list] [-i] [-E|--sparse] [-o out] [--full-matrix] [--diagonal] [--distance]\n"
           "  skani-b200 dist [query] [refs ...] [-q ...] [-r ...] [--ql list] [--rl list] [--qi] [--ri] [-n N] [-o out]\n"
           "  skani-b200 sketch [fasta ... | -l list] -o new_folder [-i] [--separate-sketches]\n"

@@ -809,7 +809,7 @@ int sketch_batch_host(sk_ctx* ctx, const HostSeq& seq, const uint64_t* contig_of
   size_t SUBBATCH = subbatch_override ? subbatch_override : subbatch_bytes(n_contigs ? contig_off[n_contigs] - contig_off[0] : 0);
   if (const char* e = getenv("SK_SUBBATCH_BYTES")) SUBBATCH = std::max<size_t>(1, (size_t)atoll(e));   // test hook: many small sub-batches
   // large sub-batches amortise the per-sub-batch launches and host synchronisations (which cost most when the GPU is shared with
-  // the chaining worker: profiles/r02_subbatch_ab.md), but nothing can be seeded before the first one is packed and uploaded:
+  // the chaining worker), but nothing can be seeded before the first one is packed and uploaded:
   // the first two are a quarter and a half of the size
   const bool ramp = (n_contigs ? contig_off[n_contigs] - contig_off[0] : 0) >= 4 * (uint64_t)SUBBATCH && getenv("SK_SUBBATCH_NO_RAMP") == nullptr;
   while (c0 < n_contigs) {

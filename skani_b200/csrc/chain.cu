@@ -120,7 +120,7 @@ constexpr int ITEMS = 4;
 // ------------------------------------------------------------------------------------------------------------
 // 1-D bulk copy (TMA, cp.async.bulk) global -> shared memory, completion signalled on an mbarrier: used to stage the whole
 // k-mer table of a SMALL ref-role genome (<= 2048 entries = 16 KB: viruses, plasmids, single contigs -- BASELINE.json
-// configs[4]) so that its probes hit shared memory instead of L2.  A/B switch SK_PROBE_TMA (profiles/r02_tma_probe.md).
+// configs[4]) so that its probes hit shared memory instead of L2.  A/B switch SK_PROBE_TMA.
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void bulk_load_to_smem(void* dst_smem, const void* src_gmem, uint32_t bytes, unsigned long long* bar) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -188,8 +188,7 @@ probe_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, const G
     uint32_t rst[ITEMS], nh[ITEMS];
     if (use_hash) {
       // one 32-byte BUCKET (4 entries = one memory sector) per record: a probe almost never needs a second access, so the
-      // lanes of a warp finish together (with one entry per step the warp waited for its longest probe chain, 3.4 steps on
-      // average: profiles/r02_ncu_full_r2a.md).  The ITEMS probes of a thread are independent.
+      // lanes of a warp finish together (with one entry per step the warp waited for its longest probe chain).  The ITEMS probes of a thread are independent.
       uint32_t kmer[ITEMS], bidx[ITEMS];
       ulonglong2 ea[ITEMS], eb[ITEMS];
       bool live[ITEMS];
@@ -1592,9 +1591,8 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
   SK_CUDA(cudaMemsetAsync(ws.pair_nchains, 0, B * 4, st));
   SK_CUDA(cudaMemsetAsync(ws.pair_tqb_ns, 0, B * 4, st));
 
-  // resident blocks per SM of the block-per-pair kernels (register caps through __launch_bounds__), measured in
-  // profiles/r02_occupancy_ab.md: probe 4 (5 blocks = 48 registers is 10 % slower, 2 blocks = 93 registers 33 % slower),
-  // anchor 6 (40 registers: 8 % faster than 72), chunk_fast 5 (indifferent)
+  // resident blocks per SM of the block-per-pair kernels (register caps through __launch_bounds__), chosen by A/B runs:
+  // probe 4, anchor 6, chunk_fast 5
   {
     // small ref-role genomes (k-mer table <= 16 KB): TMA-stage the table in shared memory when they dominate the batch
     size_t n_small = 0;
@@ -1645,7 +1643,7 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
   if (dbg) SK_LAUNCH(ctx, "dp_kernel", (dp_warp_kernel<NBV, true><<<grid, 32, 0, st>>>(TC, prm, ws)));       \
   else SK_LAUNCH(ctx, "dp_kernel", (dp_warp_kernel<NBV, false><<<grid, 32, 0, st>>>(TC, prm, ws)));
       if (prm.band <= 24 && getenv("SK_DP_WARP") == nullptr) {   // 4 chunks per warp, 8 lanes each
-        const int dp_gl = getenv("SK_DP_GL") ? atoi(getenv("SK_DP_GL")) : 4;   // lanes per chunk: 4 (default: 1.25x faster, profiles/r02_dp_lanes.md) or 8
+        const int dp_gl = getenv("SK_DP_GL") ? atoi(getenv("SK_DP_GL")) : 4;   // lanes per chunk: 4 (default, faster in A/B runs) or 8
         const int dp_minb = getenv("SK_DP_MINB") ? atoi(getenv("SK_DP_MINB")) : 25;   // register cap: 72 registers = 28 resident warps per SM (A/B: 1 = uncapped)
         const uint32_t gw = dp_gl == 4 ? 8 : 4;
         const uint32_t g4 = (uint32_t)((TC + gw - 1) / gw);

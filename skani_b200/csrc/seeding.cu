@@ -1,4 +1,4 @@
-// seeding.cu -- FracMinHash seeding + sketch assembly on the device (sm_100a).
+// seeding.cu -- FracMinHash seeding + sketch assembly on the device (sm_90a).
 //
 // Replaces avx2_seeding::avx2_fmh_seeds (reference src/avx2_seeding.rs:33-272), Sketch::add_seed_position
 // (src/types.rs:281-304) and the per-file assembly of file_io::fastx_to_sketches (src/file_io.rs:141-252).
@@ -87,7 +87,7 @@ pack_kernel(const uint8_t* __restrict__ ascii, const uint64_t* __restrict__ coff
 
 constexpr int HASH_THREADS = 128;
 
-// ---- A/B variants of the hash arithmetic (SK_HASHPASS_VARIANT=1|2, profiles/r02_hashpass_variants.md): the kernel is bound
+// ---- A/B variants of the hash arithmetic (SK_HASHPASS_VARIANT=1|2): the kernel is bound
 // by the ALU pipe (LOP3 / SHF / IADD3) while the FMA pipe (IMAD) has headroom, so the right shifts of the three xor-shift
 // steps can be issued as multiplications: x >> s == mul.hi(x, 2^(32-s)).  The multipliers arrive as kernel arguments so
 // that ptxas cannot turn them back into shifts.  V=1: the high word only; V=2: both words (low word = mul.hi(lo, c) + hi * c).
@@ -224,7 +224,7 @@ __global__ void iota_local_kernel(const uint64_t* __restrict__ seg_off, uint32_t
 
 // sort keys of the k-mer view: (genome << kbits | k-mer), value = the record's index inside its genome.  ONE device-wide radix
 // sort of these keys orders every genome of the sub-batch by (kmer, contig, pos) at once (stable), instead of a segmented
-// sort that runs one block per genome and pass (5.5 % + 1.7 % of a step in profiles/r02_launches_bench_c2.md)
+// sort that runs one block per genome and pass
 //
 // When genome, k-mer and the record's index inside its genome fit 64 bits together (ibits > 0: always, short of sub-batches of
 // thousands of multi-Gbp genomes) the index rides in the LOW bits of the key and the sort is keys-only over the bits above it:

@@ -223,8 +223,8 @@ SK_HD uint32_t funnel_r32(uint32_t lo, uint32_t hi, uint32_t sh) {  // low 32 bi
   return sh ? (lo >> sh) | (hi << (32 - sh)) : lo;
 #endif
 }
-// mm_hash64 with its shift-add steps written as multiplications (x + (x << s) == x * (2^s + 1) mod 2^64): on sm_100a
-// the 64-bit multiplies issue on the FMA pipe (IMAD) and relieve the ALU pipe (LOP3/SHF/IADD3) that bounds the kernel.
+// mm_hash64 with its shift-add steps written as multiplications (x + (x << s) == x * (2^s + 1) mod 2^64): the
+// 64-bit multiplies issue on the FMA pipe (IMAD) and relieve the ALU pipe (LOP3/SHF/IADD3) that bounds the kernel.
 SK_HD uint64_t mm_hash64_mul(uint64_t key) {
   // steps 1 + 2, x = ~(key * 0x200001); x ^= x >> 24, with the complement folded into the xors (two LOP3 fewer per window):
   //   low word : ~a ^ ~f == a ^ f                         (f = the funnel-shifted low word of the un-complemented product)

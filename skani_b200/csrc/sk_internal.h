@@ -18,7 +18,7 @@
 // large cudaMalloc'd slabs with host-side first-fit bookkeeping.  All users run on the context's single stream, so a
 // block may be handed out again as soon as the host has released it (stream order serialises the accesses).  This keeps
 // the steady state free of driver allocation calls: cudaMallocAsync's pool showed multi-100 ms stalls when multi-GB
-// blocks of changing size were recycled (profiles/r01_pipeline_trace.txt).
+// blocks of changing size were recycled.
 struct SkArena {
   struct Slab { uint8_t* base; size_t size; std::map<size_t, size_t> free_blocks; };  // offset -> size
   std::vector<Slab> slabs;
@@ -54,7 +54,7 @@ struct sk_ctx {
   cudaStream_t copy_stream = nullptr;
   std::string err;
   uint64_t launches = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   // pinned staging buffers for host->device pipelining (sk_sketch_batch)
   uint8_t* pinned[2] = {nullptr, nullptr};
   size_t pinned_bytes = 0;

@@ -111,8 +111,7 @@ int triangle_impl(sk_ctx* ctx, const sk::HostSeq& seq, const uint64_t* contig_of
   const uint64_t total_bytes = n_contigs ? contig_off[n_contigs] - contig_off[0] : 0;
   // Inputs of >= 4 GiB use the upload/seed || merge/screen/chain pipeline (SK_NO_PIPELINE=1 disables it, SK_FORCE_PIPELINE=1
   // forces it for small inputs in tests).  Two things made it work: the context arena (no driver allocations in steady
-  // state) and h2d_small (parameter uploads bypass the H2D copy engine that is saturated by the sequence upload);
-  // see profiles/r01_pipeline_trace.txt.
+  // state) and h2d_small (parameter uploads bypass the H2D copy engine that is saturated by the sequence upload).
   // memory guard: the whole sketch set stays resident (records 22 B + k-mer tables <= 32 B per seed, markers 8 B each, plus the
   // chaining workspace); refuse up front instead of failing half-way through a long run -- more genomes than one GPU holds
   // go through sk_triangle_multi (blocks per GPU), SURVEY.md section 8 config 4

@@ -1,25 +1,13 @@
 import os
 import sys
 
-import pytest
-
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-REF_TEST_FILES = "/root/reference/test_files"
-
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: takes more than ~20 s on CPU")
-
-
-def have_reference():
-    return os.path.isdir(REF_TEST_FILES)
-
-
-needs_reference = pytest.mark.skipif(not have_reference(),
-                                     reason="/root/reference fixtures not present (GPU box)")
 
 
 def db_tool():

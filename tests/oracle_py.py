@@ -34,11 +34,11 @@ def build():
     subprocess.check_call(["make", "-s", "-C", ORACLE_DIR])
 
 
-def build_native():
-    """-march=native build for the CPU baseline (oracle/_native/liboracle.so); returns its path or None."""
+def build_native(out_dir):
+    """-march=native build for the CPU baseline (out_dir/liboracle.so); returns its path or None."""
     try:
-        subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "native"])
-        return os.path.join(ORACLE_DIR, "_native", "liboracle.so")
+        subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "native", "NATIVE_DIR=" + os.path.abspath(out_dir)])
+        return os.path.join(out_dir, "liboracle.so")
     except Exception:
         return None
 

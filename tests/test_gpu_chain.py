@@ -94,7 +94,7 @@ def test_chain_debug_parity_synthetic(ctx, c, mc, learned):
 
 @pytest.mark.parametrize("lanes", ["4", "8"])
 def test_chain_debug_parity_dp_lane_groups(ctx, monkeypatch, lanes):
-    """The banded DP with 4 lanes per chunk / 8 chunks per warp (the default since the A/B of profiles/r02_dp_lanes.md) and with 8
+    """The banded DP with 4 lanes per chunk / 8 chunks per warp (the default) and with 8
     lanes / 4 chunks per warp (SK_DP_GL=8) are both held to bit-exact per-anchor score / pointer / interval parity."""
     import skani_b200 as sk
     monkeypatch.setenv("SK_DP_GL", lanes)

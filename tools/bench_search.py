@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""BASELINE.json configs[2] shape (`skani search`: many query genomes against a large pre-sketched database) on ONE B200,
+"""BASELINE.json configs[2] shape (`skani search`: many query genomes against a large pre-sketched database) on ONE H100,
 through the C ABI.  The database is sketched once (outside the timed region, as a pre-sketched `sketches.db` would be) and
 kept resident in HBM; a timed step = sketch the query genomes from host memory -> marker screen of every (query, ref) pair
 (check_markers_quickly without rescue, the `search` default, src/search.rs:127) -> chain the passing pairs -> keep ani > 0.5
