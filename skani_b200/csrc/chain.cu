@@ -316,7 +316,57 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
 // P0 / A0 of its contig (position / anchor offset of the contig's first hit, segmented "first" scan), need, and the
 // contig-local chunk of its first and last anchor (segmented prefix min, the closed form in chain_core.cuh); then the
 // chunk-start flags and chunk ids (sum).  Descriptors go to the pair's staging slice; chunk_compact_kernel packs them.
+//
+// Few memory round trips lie in series inside a tile: the records of tile i + 1 are copied to shared memory (cp.async)
+// while tile i scans and emits, and the tile's anchors are emitted anchor-parallel, one thread per anchor, so that the
+// gathers of a round are independent of each other and of the round's stores.  What remains is mostly the instruction
+// work of the four block scans (hence the branch-free FirstOp / MinOp).
 // ------------------------------------------------------------------------------------------------------------
+// 4-byte asynchronous copy global -> shared memory.  A thread waits for its own copies (wait_group); a barrier then
+// publishes them to the block.
+__device__ __forceinline__ void cp_async4(void* dst_smem, const void* src_gmem) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all_but_newest() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
+
+static_assert(TILE == 1024, "ChunkAnchorSmem::arec packs the record's index in the tile into 10 bits");
+struct __align__(16) RecTile {       // one tile of query-role records
+  uint32_t pos[TILE], cc[TILE];
+  uint32_t rs[TILE];                 // stale for records without hits: never used for them
+  uint32_t nhw[TILE / 2 + 1];        // the aligned 4-byte words holding the tile's rec_nh: record i is halfword i + nh_odd
+};
+struct ChunkAnchorSmem {
+  RecTile tile[2];                   // double buffer: tile i + 1 is in flight while tile i scans and emits
+  // per hit record of the current tile (index in the tile), read by the threads that emit its anchors
+  uint32_t clf[TILE];                // contig-local chunk of the record's first anchor
+  uint32_t need[TILE];               // need | (the first anchor starts a chunk) << 31
+  uint32_t cid[TILE];                // pair-local chunk id of the first anchor
+  uint32_t p0[TILE];                 // P0 of the record's contig
+  uint32_t arec[TILE];               // anchor of the current round -> its record | its index in the record << 10
+};
+
+// Issue the copies of records [t0, min(t0 + TILE, n_rec)) into b.  rec_nh slices start at any halfword (nh_odd = the
+// slice's start is not 4-byte aligned), so whole aligned words are copied: one halfword before and one after the tile's
+// may come along; both lie inside the allocation (the one after is at most index n_rec of the slice, and ensure()
+// over-allocates).
+__device__ __forceinline__ void stage_rec_tile(RecTile& b, uint32_t t0, uint32_t n_rec, const uint16_t* nhv, uint32_t nh_odd,
+                                               const uint32_t* rsv, const uint32_t* qpv, const uint32_t* qcv) {
+  const uint32_t n = min(TILE, n_rec - t0);
+#pragma unroll
+  for (int it = 0; it < ITEMS; it++) {
+    const uint32_t i = it * CT + threadIdx.x;
+    if (i < n) {
+      cp_async4(&b.pos[i], qpv + t0 + i);
+      cp_async4(&b.cc[i], qcv + t0 + i);
+      cp_async4(&b.rs[i], rsv + t0 + i);
+    }
+  }
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(nhv + t0 - nh_odd);
+  const uint32_t nw = (n + nh_odd + 1) >> 1;
+  for (uint32_t i = threadIdx.x; i < nw; i += CT) cp_async4(&b.nhw[i], w + i);
+}
+
 template <int MINB>
 __global__ void __launch_bounds__(CT, MINB)
 chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, const GenomeMeta* __restrict__ m0,
@@ -328,6 +378,8 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
   __shared__ typename ScanU::TempStorage tmp_a, tmp_c;
   __shared__ typename ScanF::TempStorage tmp_f;
   __shared__ typename ScanM::TempStorage tmp_m;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  ChunkAnchorSmem& S = *reinterpret_cast<ChunkAnchorSmem*>(smem_raw);
   const uint32_t p = blockIdx.x;
   const PairDesc pd = pairs[p];
   const uint32_t A_total = ws.pairA[p];
@@ -335,33 +387,46 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
     if (threadIdx.x == 0) ws.pairC[p] = 0;
     return;
   }
-  const SetView& Q = pd.qset ? s1 : s0;
-  const SetView& R = pd.rset ? s1 : s0;
   const GenomeMeta qm = (pd.qset ? m1 : m0)[pd.qg];
   const GenomeMeta rm = (pd.rset ? m1 : m0)[pd.rg];
   const uint16_t* __restrict__ nhv = ws.rec_nh + pd.rec_off;
   const uint32_t* __restrict__ rsv = ws.rec_rs + pd.rec_off;
-  const uint32_t* __restrict__ qpv = Q.pv_pos + qm.seed_off;
-  const uint32_t* __restrict__ qcv = Q.pv_cc + qm.seed_off;
-  const uint32_t* __restrict__ rpv = R.kv_pos + rm.seed_off;
-  const uint32_t* __restrict__ rcv = R.kv_cc + rm.seed_off;
+  // the fields are selected one by one (see probe_kernel)
+  const uint32_t* __restrict__ qpv = (pd.qset ? s1.pv_pos : s0.pv_pos) + qm.seed_off;
+  const uint32_t* __restrict__ qcv = (pd.qset ? s1.pv_cc : s0.pv_cc) + qm.seed_off;
+  const uint32_t* __restrict__ rpv = (pd.rset ? s1.kv_pos : s0.kv_pos) + rm.seed_off;
+  const uint32_t* __restrict__ rcv = (pd.rset ? s1.kv_cc : s0.kv_cc) + rm.seed_off;
   const uint64_t abase = ws.pairAbase[p], sbase = pd.chunk_off;
+  AnchorRec* __restrict__ anc = ws.anc + abase;
   const uint32_t cmax = pd.max_chunks;
+  const uint32_t nh_odd = (uint32_t)(reinterpret_cast<uintptr_t>(nhv) >> 1) & 1u;
   FirstState carryF; carryF.valid = 0; carryF.ctg = 0; carryF.p0 = 0; carryF.a0 = 0;
   MinState carryM; carryM.valid = 0; carryM.ctg = 0; carryM.v = 0;
   MinState identM; identM.valid = 0; identM.ctg = 0; identM.v = 0;
   uint32_t carryA = 0, carryC = 0;                  // anchors / chunk starts so far
-  bool own_last = false;                            // this thread holds the pair's last hit record
-  uint32_t last_q = 0, last_c = 0;
-  for (uint32_t t0 = 0; t0 < qm.n_rec; t0 += TILE) {
+  __shared__ uint32_t s_last_q, s_last_c;          // the pair's last hit record: its position, the chunk of its last anchor
+  stage_rec_tile(S.tile[0], 0, qm.n_rec, nhv, nh_odd, rsv, qpv, qcv);
+  cp_async_commit();
+  uint32_t buf = 0;
+  for (uint32_t t0 = 0; t0 < qm.n_rec; t0 += TILE, buf ^= 1u) {
+    // the other buffer was last read before the previous tile's final barrier
+    if (t0 + TILE < qm.n_rec) stage_rec_tile(S.tile[buf ^ 1u], t0 + TILE, qm.n_rec, nhv, nh_odd, rsv, qpv, qcv);
+    cp_async_commit();                              // possibly empty: the group before it is always this tile's
+    cp_async_wait_all_but_newest();
+    __syncthreads();
+    const RecTile& T = S.tile[buf];
     uint32_t nh[ITEMS], pos[ITEMS], cc[ITEMS];
+    {
+      const uint4 p4 = *reinterpret_cast<const uint4*>(&T.pos[threadIdx.x * ITEMS]);
+      const uint4 c4 = *reinterpret_cast<const uint4*>(&T.cc[threadIdx.x * ITEMS]);
+      pos[0] = p4.x; pos[1] = p4.y; pos[2] = p4.z; pos[3] = p4.w;
+      cc[0] = c4.x; cc[1] = c4.y; cc[2] = c4.z; cc[3] = c4.w;
+      const uint16_t* nh16 = reinterpret_cast<const uint16_t*>(T.nhw) + nh_odd;
 #pragma unroll
-    for (int it = 0; it < ITEMS; it++) {
-      const uint32_t t = t0 + threadIdx.x * ITEMS + it;
-      nh[it] = pos[it] = cc[it] = 0;
-      if (t < qm.n_rec) {
-        nh[it] = nhv[t] & 0x7FFFu;
-        if (nh[it]) { pos[it] = qpv[t]; cc[it] = qcv[t]; }
+      for (int it = 0; it < ITEMS; it++) {
+        const uint32_t i = threadIdx.x * ITEMS + it;
+        nh[it] = (t0 + i < qm.n_rec) ? nh16[i] & 0x7FFFu : 0u;
+        if (!nh[it]) pos[it] = cc[it] = 0;
       }
     }
     uint32_t aoff[ITEMS], aggA;
@@ -412,39 +477,75 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
 #pragma unroll
     for (int it = 0; it < ITEMS; it++) {
       if (!nh[it]) continue;
-      const uint32_t t = t0 + threadIdx.x * ITEMS + it;
-      const uint32_t rs = rsv[t];
+      const uint32_t r = threadIdx.x * ITEMS + it;
       const uint32_t cid = carryC + exc[it] + st[it] - 1;   // chunk id of the record's first anchor
-      const uint32_t p0 = fs[it].p0, qcc = cc[it];
-      const uint64_t x = abase + aoff[it];
-      bool start = st[it] != 0;
-      for (uint32_t u = 0; u < nh[it]; u++) {
-        const uint32_t cl = min(clf[it] + u, need[it]);     // contig-local chunk of this anchor
-        const uint32_t rpos = rpv[rs + u], rcc = rcv[rs + u];
+      S.clf[r] = clf[it];
+      S.need[r] = need[it] | (st[it] << 31);                 // need < 2^18: positions are 32-bit
+      S.cid[r] = cid;
+      S.p0[r] = fs[it].p0;
+      if (aoff[it] + nh[it] == A_total) { s_last_q = pos[it]; s_last_c = cid + (cll[it] - clf[it]); }
+    }
+    // The tile's anchors are the pair-local range [carryA, carryA + aggA), emitted in rounds of TILE: the records first
+    // mark which of the round's anchors are theirs, then thread k * CT + threadIdx.x of the round emits anchor k * CT +
+    // threadIdx.x (consecutive threads write consecutive anchors).  A record's anchors may span rounds.
+    for (uint32_t base = 0; base < aggA; base += TILE) {
+#pragma unroll
+      for (int it = 0; it < ITEMS; it++) {
+        if (!nh[it]) continue;
+        const uint32_t lo = aoff[it] - carryA, r = threadIdx.x * ITEMS + it;
+        const uint32_t j1 = min(lo + nh[it], base + TILE);
+        for (uint32_t j = max(lo, base); j < j1; j++) S.arec[j - base] = r | ((j - lo) << 10);
+      }
+      __syncthreads();
+      uint32_t ar[ITEMS], rpos[ITEMS], rcc[ITEMS];
+#pragma unroll
+      for (int k = 0; k < ITEMS; k++) {             // every gather of the round before any of its stores
+        const uint32_t j = base + k * CT + threadIdx.x;
+        ar[k] = rpos[k] = rcc[k] = 0;
+        if (j < aggA) {
+          ar[k] = S.arec[j - base];
+          const uint32_t g = T.rs[ar[k] & (TILE - 1)] + (ar[k] >> 10);
+          rpos[k] = __ldg(rpv + g);
+          rcc[k] = __ldg(rcv + g);
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < ITEMS; k++) {
+        const uint32_t j = base + k * CT + threadIdx.x;
+        if (j >= aggA) continue;
+        const uint32_t r = ar[k] & (TILE - 1), u = ar[k] >> 10;
+        const uint32_t qcc = T.cc[r], clf0 = S.clf[r], nd = S.need[r], rneed = nd & 0x7FFFFFFFu;
         AnchorRec a;
-        a.qpos = pos[it]; a.rpos = rpos;
-        a.rc = (rcc & ~1u) | ((rcc ^ qcc) & 1u);                // reverse_match = canonical differs (src/chain.rs:709)
-        ws.anc[x + u] = a;
-        const uint32_t mycid = cid + (cl - clf[it]);
-        if (start && mycid < cmax) {                           // chunk start: write its descriptor
+        a.qpos = T.pos[r]; a.rpos = rpos[k];
+        a.rc = (rcc[k] & ~1u) | ((rcc[k] ^ qcc) & 1u);          // reverse_match = canonical differs (src/chain.rs:709)
+        anc[carryA + j] = a;
+        // the record's anchor u sits in contig-local chunk cl; it starts a chunk iff it is the first anchor and the record
+        // starts one, or anchor u - 1 had not yet reached need (the chunk moves to cl + 1)
+        const uint32_t cl = min(clf0 + u, rneed);
+        const bool start = (u == 0) ? (nd >> 31) != 0 : clf0 + u - 1 < rneed;
+        const uint32_t mycid = S.cid[r] + (cl - clf0);
+        if (start && mycid < cmax) {                             // chunk start: write its descriptor
           const uint64_t c = sbase + mycid;
-          ws.stg_first[c] = x + u;
+          const uint32_t p0 = S.p0[r];
+          ws.stg_first[c] = abase + carryA + j;
           ws.stg_qctg[c] = qcc >> 1;
           ws.stg_lo[c] = (cl == 0) ? -1ll : (int64_t)p0 + (int64_t)cl * FRAGMENT_LENGTH;   // seeds with pos > lo
           ws.stg_hi[c] = (int64_t)p0 + (int64_t)(cl + 1) * FRAGMENT_LENGTH;                // and pos <= hi
         }
-        start = cl < need[it];                                 // the next anchor moves to chunk cl + 1
       }
-      if (aoff[it] + nh[it] == A_total) { own_last = true; last_q = pos[it]; last_c = cid + (cll[it] - clf[it]); }
+      __syncthreads();                              // arec, the per-record arrays and this tile buffer are reused
     }
     carryA += aggA;
     carryC += aggC;
   }
   // the pair's last chunk is never closed by the loop: it keeps seeds up to its last anchor (src/chain.rs:796-824).
-  // Patched after every descriptor of this pair has been written (same block).
+  // Patched after every descriptor of this pair has been written, whichever threads wrote them (same block; A_total > 0,
+  // so exactly one record set s_last_q / s_last_c).
   __syncthreads();
-  if (own_last && last_c < cmax) ws.stg_hi[sbase + last_c] = (int64_t)last_q;
-  if (threadIdx.x == 0) ws.pairC[p] = carryC;     // > max_chunks: run_batch reports the error, nothing was written out of range
+  if (threadIdx.x == 0) {
+    if (s_last_c < cmax) ws.stg_hi[sbase + s_last_c] = (int64_t)s_last_q;
+    ws.pairC[p] = carryC;                         // > max_chunks: run_batch reports the error, nothing was written out of range
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1503,7 +1604,9 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
   SK_CUDA(h2d_small(ctx, ws.pairIbase, ibase.data(), (B + 1) * 8));
   const size_t NA = std::max<uint64_t>(TA, 1), NI = std::max<uint64_t>(TI, 1);
   ENS(anc, c_anc, NA);
-  SK_LAUNCH(ctx, "chunk_anchor_kernel", (chunk_anchor_kernel<CHUNK_ANCHOR_MINB><<<B, CT, 0, st>>>(S.d_pairs, v0, v1, S.d_m0, S.d_m1, ws)));
+  SK_CUDA(cudaFuncSetAttribute(chunk_anchor_kernel<CHUNK_ANCHOR_MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)sizeof(ChunkAnchorSmem)));
+  SK_LAUNCH(ctx, "chunk_anchor_kernel", (chunk_anchor_kernel<CHUNK_ANCHOR_MINB><<<B, CT, sizeof(ChunkAnchorSmem), st>>>(S.d_pairs, v0, v1, S.d_m0, S.d_m1, ws)));
   SK_CUDA(cudaMemcpyAsync(hC.data(), ws.pairC, B * 4, cudaMemcpyDeviceToHost, st));
   SK_CUDA(cudaStreamSynchronize(st));
   SK_CUDA(cudaGetLastError());

@@ -34,25 +34,34 @@ struct FirstState {     // segmented "first element of the contig" scan
   uint32_t a0;          // pair-local anchor index of that record's first anchor
   uint32_t valid;       // 0 = identity
 };
+// The operators are written with selects instead of early returns: inside the block scans they run in every shuffle step,
+// and branches there cost divergence and reconvergence instructions.
 struct FirstOp {
   SK_HD FirstState operator()(const FirstState& a, const FirstState& b) const {
-    if (!b.valid) return a;
-    if (!a.valid) return b;
-    if (a.ctg == b.ctg) { FirstState r = a; return r; }  // same contig: the earlier element's values win
-    return b;                                             // b starts (or continues) a later contig
+    // b wins unless it is the identity or continues a's contig (then the earlier element's values win)
+    const bool take_b = b.valid && (!a.valid || a.ctg != b.ctg);
+    FirstState r;
+    r.ctg = take_b ? b.ctg : a.ctg;
+    r.p0 = take_b ? b.p0 : a.p0;
+    r.a0 = take_b ? b.a0 : a.a0;
+    r.valid = take_b ? b.valid : a.valid;
+    return r;
   }
 };
-struct MinState {       // segmented prefix-min of v = need - (index of the record's last anchor)
-  uint32_t ctg;
+struct MinState {       // segmented prefix-min of v = need - (index of the record's last anchor); 16 bytes, no padding
   int64_t v;
+  uint32_t ctg;
   uint32_t valid;
 };
 struct MinOp {
   SK_HD MinState operator()(const MinState& a, const MinState& b) const {
-    if (!b.valid) return a;
-    if (!a.valid) return b;
-    if (a.ctg == b.ctg) { MinState r = b; r.v = a.v < b.v ? a.v : b.v; return r; }
-    return b;
+    // b invalid: a; a invalid or another contig: b; same contig: b with the smaller v
+    const bool same = a.valid && a.ctg == b.ctg;
+    MinState r;
+    r.ctg = b.valid ? b.ctg : a.ctg;
+    r.valid = a.valid | b.valid;
+    r.v = !b.valid ? a.v : (same && a.v < b.v) ? a.v : b.v;
+    return r;
   }
 };
 SK_HD uint32_t chunk_need(uint32_t pos, uint32_t p0) {
