@@ -203,7 +203,7 @@ int sk_chain_pairs(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* 
                    uint64_t n_pairs, const sk_map_params* mp, sk_ani_result* out);
 int sk_sketch_set_set_name_ranks(sk_sketch_set* set, const uint64_t* ranks /* n_genomes */);
 
-/* parity taps for ONE pair (test use): all outputs are malloc'd (sk_free). anchors: 5 x u32 per anchor
+/* parity taps (test use), per pair: all outputs are malloc'd (sk_chain_debug_free). anchors: 5 x u32 per anchor
  * (query_contig, query_pos, ref_contig, ref_pos, reverse) in sorted order (src/chain.rs:721); chunk_first: n_chunks+1;
  * score/pointer per anchor (chunk-local pointer, src/chain.rs:881-882); intervals: 11 x i64 per interval in the
  * descending order of src/chain.rs:1012: score,num_anchors,q0,q1,r0,r1,ref_contig,query_contig,chunk,reverse,kept;
@@ -221,6 +221,11 @@ typedef struct {
   double* est;
   uint64_t* weight;
 } sk_chain_debug;
+/* sk_chain_pairs_debug runs the batching, pair descriptors and kernel instantiations of sk_chain_pairs on the same pair list
+ * (the kernels additionally store the per-anchor DP scores and pointers) and fills out[i] from pair i's slices of the batch.
+ * On error every out[i] is freed.  sk_chain_pair_debug is its one-pair call. */
+int sk_chain_pairs_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, const uint64_t* pairs,
+                         uint64_t n_pairs, const sk_map_params* mp, sk_chain_debug* out /* n_pairs */);
 int sk_chain_pair_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, uint64_t pair,
                         const sk_map_params* mp, sk_chain_debug* out);
 void sk_chain_debug_free(sk_chain_debug* d);

@@ -77,6 +77,7 @@ SYMBOLS = [
     ("sk_chain_pairs", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp]),
     ("sk_sketch_set_set_name_ranks", i32, [vp, vp]),
     ("sk_chain_pair_debug", i32, [vp, vp, vp, u64, PP(MapParams), PP(ChainDebug)]),
+    ("sk_chain_pairs_debug", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp]),
     ("sk_chain_debug_free", None, [PP(ChainDebug)]),
     ("sk_triangle", i32, [vp, vp, vp, u32, vp, u32, PP(SketchParams), PP(MapParams), PP(PP(AniResult)), PP(u64),
                           PP(TriangleStats)]),

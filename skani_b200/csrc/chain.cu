@@ -450,7 +450,7 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
         need[it] = chunk_need(pos[it], fs[it].p0);
         al[it] = aoff[it] - fs[it].a0;             // contig-local index of the record's first anchor
         ms[it].valid = 1; ms[it].ctg = cc[it] >> 1;
-        ms[it].v = (int64_t)need[it] - (int64_t)al[it] - (int64_t)(nh[it] - 1);
+        ms[it].v = record_min_key(need[it], al[it], nh[it]);
       }
     }
     carryF = FirstOp()(carryF, aggF);
@@ -465,10 +465,8 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
         const bool has_prev = e.valid && e.ctg == (cc[it] >> 1);
         clf[it] = chunk_local_of(al[it], has_prev, e.v, need[it]);
         cll[it] = chunk_local_of((uint64_t)al[it] + nh[it] - 1, has_prev, e.v, need[it]);
-        // the previous hit record's last anchor (index al - 1 of the contig) sits in chunk al - 1 + e.v: this record's
-        // first anchor starts a chunk iff it is the contig's first hit or lands in a later chunk
-        st[it] = (!has_prev || (int64_t)al[it] - 1 + e.v != (int64_t)clf[it]) ? 1u : 0u;
-        inc[it] = st[it] + (cll[it] - clf[it]);
+        st[it] = record_starts_chunk(al[it], has_prev, e.v, clf[it]);
+        inc[it] = record_chunk_starts(st[it], clf[it], cll[it]);
       }
     }
     carryM = MinOp()(carryM, aggM);
@@ -519,18 +517,16 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
         a.qpos = T.pos[r]; a.rpos = rpos[k];
         a.rc = (rcc[k] & ~1u) | ((rcc[k] ^ qcc) & 1u);          // reverse_match = canonical differs (src/chain.rs:709)
         anc[carryA + j] = a;
-        // the record's anchor u sits in contig-local chunk cl; it starts a chunk iff it is the first anchor and the record
-        // starts one, or anchor u - 1 had not yet reached need (the chunk moves to cl + 1)
-        const uint32_t cl = min(clf0 + u, rneed);
-        const bool start = (u == 0) ? (nd >> 31) != 0 : clf0 + u - 1 < rneed;
+        const uint32_t cl = anchor_chunk_local(clf0, u, rneed);
+        const bool start = anchor_starts_chunk(clf0, u, rneed, (nd >> 31) != 0);
         const uint32_t mycid = S.cid[r] + (cl - clf0);
         if (start && mycid < cmax) {                             // chunk start: write its descriptor
           const uint64_t c = sbase + mycid;
           const uint32_t p0 = S.p0[r];
           ws.stg_first[c] = abase + carryA + j;
           ws.stg_qctg[c] = qcc >> 1;
-          ws.stg_lo[c] = (cl == 0) ? -1ll : (int64_t)p0 + (int64_t)cl * FRAGMENT_LENGTH;   // seeds with pos > lo
-          ws.stg_hi[c] = (int64_t)p0 + (int64_t)(cl + 1) * FRAGMENT_LENGTH;                // and pos <= hi
+          ws.stg_lo[c] = chunk_window_lo(p0, cl);
+          ws.stg_hi[c] = chunk_window_hi(p0, cl);
         }
       }
       __syncthreads();                              // arec, the per-record arrays and this tile buffer are reused
@@ -1550,8 +1546,106 @@ struct ChainScratch {
 
 struct HostPair { uint32_t ref, query; };
 
-// Runs one batch (pairs [b0, b1) of `hp`); results -> host_out[b0..b1).  If dbg != nullptr (single pair) the
-// intermediate products are copied out as well.
+// dp_group_kernel's instantiation for the band: FULLBAND when the band fills the lanes' register sets exactly, and then the
+// 25-block register cap unless SK_DP_MINB=1.  TAPS only adds the score / pointer stores.
+template <bool TAPS, int GL, int NE>
+static int launch_dp_group(sk_ctx* ctx, uint32_t grid, uint64_t TC, const ChainParams& prm, const Workspace& ws, int dp_minb) {
+  cudaStream_t st = ctx->stream;
+  if (prm.band == GL * NE && dp_minb > 1) SK_LAUNCH(ctx, "dp_kernel", (dp_group_kernel<TAPS, GL, NE, true, 25><<<grid, 32, 0, st>>>(TC, prm, ws)));
+  else if (prm.band == GL * NE) SK_LAUNCH(ctx, "dp_kernel", (dp_group_kernel<TAPS, GL, NE, true, 1><<<grid, 32, 0, st>>>(TC, prm, ws)));
+  else SK_LAUNCH(ctx, "dp_kernel", (dp_group_kernel<TAPS, GL, NE, false, 1><<<grid, 32, 0, st>>>(TC, prm, ws)));
+  return SK_OK;
+}
+
+// Copies the intermediate products of every pair of the batch out of the batch arrays: pair i's anchors at pairAbase[i],
+// its chunks at pairCbase[i], its intervals at pairIbase[i] (pair_nint[i] of them, sorted order at iv_order + 4 ib + npow2,
+// kept flags at iv_kept + ib, both indexed by the pair-local interval index).  dbg[b0 + i] receives pair b0 + i.
+static int copy_out_debug(sk_ctx* ctx, const Workspace& ws, const std::vector<PairDesc>& descs, size_t b0, uint32_t B,
+                          const std::vector<uint64_t>& abase, const std::vector<uint64_t>& cbase, const std::vector<uint64_t>& ibase,
+                          const sk_ani_result* host_out, sk_chain_debug* dbg) {
+  const uint64_t TA = abase[B], TC = cbase[B], TI = ibase[B];
+  std::vector<AnchorRec> anc(TA);
+  std::vector<int32_t> score(TA);
+  std::vector<uint32_t> ptr(TA), cq(TC), nseeds(TC), nint(B), w(TC), order(4 * TI);
+  std::vector<uint64_t> cf(TC + 1);
+  std::vector<IntervalKey> iv(TI);
+  std::vector<uint8_t> kept(TI), valid(TC);
+  std::vector<double> est(TC);
+  if (TA) {
+    SK_CUDA(cudaMemcpy(anc.data(), ws.anc, TA * sizeof(AnchorRec), cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(score.data(), ws.score, TA * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(ptr.data(), ws.ptr, TA * 4, cudaMemcpyDeviceToHost));
+  }
+  if (TC) {
+    SK_CUDA(cudaMemcpy(cf.data(), ws.chunk_first, (TC + 1) * 8, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(cq.data(), ws.chunk_qctg, TC * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(nseeds.data(), ws.chunk_nseeds, TC * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(est.data(), ws.chunk_est, TC * 8, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(w.data(), ws.chunk_w, TC * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(valid.data(), ws.chunk_valid, TC, cudaMemcpyDeviceToHost));
+  }
+  SK_CUDA(cudaMemcpy(nint.data(), ws.pair_nint, B * 4, cudaMemcpyDeviceToHost));
+  if (TI) {
+    // a pair's sorted order ends at 4 ib + npow2 + n < 4 ib + 3 n <= 4 (ib + capacity): inside the batch's 4 TI entries
+    SK_CUDA(cudaMemcpy(iv.data(), ws.iv, TI * sizeof(IntervalKey), cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(order.data(), ws.iv_order, 4 * TI * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(kept.data(), ws.iv_kept, TI, cudaMemcpyDeviceToHost));
+  }
+  for (uint32_t i = 0; i < B; i++) {
+    sk_chain_debug* d = dbg + b0 + i;
+    memset(d, 0, sizeof(*d));
+    d->result = host_out[b0 + i];
+    d->switched = descs[b0 + i].switched;
+    const uint64_t a0 = abase[i], na = abase[i + 1] - a0, c0 = cbase[i], nc = cbase[i + 1] - c0, ib = ibase[i];
+    const uint32_t ni = nint[i];
+    if (ni > ibase[i + 1] - ib) { ctx->err = "chain debug: a pair has more intervals than its capacity"; return SK_ERR_STATE; }
+    d->n_anchors = na; d->n_chunks = nc; d->n_intervals = ni;
+    d->anchors = (uint32_t*)calloc(std::max<uint64_t>(na, 1), 20);
+    d->score = (int64_t*)calloc(std::max<uint64_t>(na, 1), 8);
+    d->pointer = (uint32_t*)calloc(std::max<uint64_t>(na, 1), 4);
+    d->chunk_first = (uint32_t*)calloc(nc + 1, 4);
+    d->chunk_nseeds = (uint32_t*)calloc(std::max<uint64_t>(nc, 1), 4);
+    d->intervals = (int64_t*)calloc(std::max<uint32_t>(ni, 1), 11 * 8);
+    if (!d->anchors || !d->score || !d->pointer || !d->chunk_first || !d->chunk_nseeds || !d->intervals) {
+      ctx->err = "chain debug: out of host memory"; return SK_ERR_STATE;
+    }
+    for (uint64_t c = 0; c < nc; c++) {
+      // chunk_first is batch-global; the pair's last chunk ends where the next pair's anchors (or the sentinel) begin
+      const uint64_t x0 = cf[c0 + c] - a0, x1 = cf[c0 + c + 1] - a0;
+      if (x0 > x1 || x1 > na) { ctx->err = "chain debug: chunk outside its pair's anchors"; return SK_ERR_STATE; }
+      d->chunk_first[c] = (uint32_t)x0; d->chunk_nseeds[c] = nseeds[c0 + c];
+      for (uint64_t x = x0; x < x1; x++) {
+        const AnchorRec& a = anc[a0 + x];
+        uint32_t* o = d->anchors + 5 * x;
+        o[0] = cq[c0 + c]; o[1] = a.qpos; o[2] = a.rc >> 1; o[3] = a.rpos; o[4] = a.rc & 1u;
+        d->score[x] = score[a0 + x]; d->pointer[x] = ptr[a0 + x];
+      }
+    }
+    d->chunk_first[nc] = (uint32_t)na;
+    uint32_t npow2 = 1;
+    while (npow2 < ni) npow2 <<= 1;
+    for (uint32_t j = 0; j < ni; j++) {
+      const uint32_t oj = order[4 * ib + npow2 + j];
+      if (oj >= ni) { ctx->err = "chain debug: interval order out of range"; return SK_ERR_STATE; }
+      const IntervalKey& x = iv[ib + oj];
+      int64_t* o = d->intervals + 11 * j;
+      o[0] = iv_score(x); o[1] = iv_num_anchors(x); o[2] = iv_q0(x); o[3] = iv_q1(x); o[4] = iv_r0(x); o[5] = iv_r1(x);
+      o[6] = iv_rctg(x); o[7] = iv_qctg(x); o[8] = iv_chunk(x); o[9] = iv_rev(x); o[10] = kept[ib + oj];
+    }
+    std::vector<std::pair<double, uint64_t>> es;
+    for (uint64_t c = c0; c < c0 + nc; c++) if (valid[c]) es.push_back({est[c], w[c]});
+    std::sort(es.begin(), es.end());
+    d->n_ests = es.size();
+    d->est = (double*)calloc(std::max<size_t>(es.size(), 1), 8);
+    d->weight = (uint64_t*)calloc(std::max<size_t>(es.size(), 1), 8);
+    if (!d->est || !d->weight) { ctx->err = "chain debug: out of host memory"; return SK_ERR_STATE; }
+    for (size_t j = 0; j < es.size(); j++) { d->est[j] = es[j].first; d->weight[j] = es[j].second; }
+  }
+  return SK_OK;
+}
+
+// Runs one batch (pairs [b0, b1) of `descs`); results -> host_out[b0..b1).  If dbg != nullptr (one entry per pair of the
+// whole list) the intermediate products of the batch's pairs are copied out as well.
 static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, const sk_sketch_set* qs, const std::vector<PairDesc>& descs,
                      size_t b0, size_t b1, uint64_t total_rec, uint64_t total_chunks, const std::vector<uint32_t>& tile_off, const ChainParams& prm, const SetView& v0, const SetView& v1,
                      sk_ani_result* host_out, sk_chain_debug* dbg) {
@@ -1648,12 +1742,11 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
         SK_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, (int)TC, 0, 32, st));
         SK_TRY(ensure(ctx, &S.sort_tmp, &S.c_sort_tmp, tb));
         SK_CUDA(cub::DeviceRadixSort::SortPairsDescending(S.sort_tmp, tb, ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, (int)TC, 0, 32, st));
+        // the debug taps run the instantiation production runs, with the score / pointer stores as the only difference
 #define DPG(GLV, NEV)                                                                                                   \
   {                                                                                                                    \
-    if (dbg) SK_LAUNCH(ctx, "dp_kernel", (dp_group_kernel<true, GLV, NEV, false, 1><<<g4, 32, 0, st>>>(TC, prm, ws)));    \
-    else if (prm.band == GLV * NEV && dp_minb > 1) SK_LAUNCH(ctx, "dp_kernel", (dp_group_kernel<false, GLV, NEV, true, 25><<<g4, 32, 0, st>>>(TC, prm, ws)));  \
-    else if (prm.band == GLV * NEV) SK_LAUNCH(ctx, "dp_kernel", (dp_group_kernel<false, GLV, NEV, true, 1><<<g4, 32, 0, st>>>(TC, prm, ws)));  \
-    else SK_LAUNCH(ctx, "dp_kernel", (dp_group_kernel<false, GLV, NEV, false, 1><<<g4, 32, 0, st>>>(TC, prm, ws)));       \
+    if (dbg) SK_TRY((launch_dp_group<true, GLV, NEV>(ctx, g4, TC, prm, ws, dp_minb)));                                \
+    else SK_TRY((launch_dp_group<false, GLV, NEV>(ctx, g4, TC, prm, ws, dp_minb)));                                   \
   }
         if (dp_gl == 4) { if (prm.band <= 20) DPG(4, 5) else DPG(4, 6) }
         else { DPG(8, 3) }
@@ -1670,75 +1763,7 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
   SK_CUDA(cudaStreamSynchronize(st));
   SK_CUDA(cudaGetLastError());
 
-  if (dbg) {  // single pair: copy the intermediate products out
-    memset(dbg, 0, sizeof(*dbg));
-    dbg->result = host_out[b0];
-    dbg->switched = descs[b0].switched;
-    dbg->n_anchors = TA; dbg->n_chunks = TC;
-    std::vector<AnchorRec> anc(TA);
-    std::vector<int32_t> score(TA);
-    std::vector<uint32_t> ptr(TA), cq(TC), nseeds(TC);
-    std::vector<uint64_t> cf(TC + 1);
-    if (TA) {
-      SK_CUDA(cudaMemcpy(anc.data(), ws.anc, TA * sizeof(AnchorRec), cudaMemcpyDeviceToHost));
-      SK_CUDA(cudaMemcpy(score.data(), ws.score, TA * 4, cudaMemcpyDeviceToHost));
-      SK_CUDA(cudaMemcpy(ptr.data(), ws.ptr, TA * 4, cudaMemcpyDeviceToHost));
-    }
-    if (TC) {
-      SK_CUDA(cudaMemcpy(cf.data(), ws.chunk_first, (TC + 1) * 8, cudaMemcpyDeviceToHost));
-      SK_CUDA(cudaMemcpy(cq.data(), ws.chunk_qctg, TC * 4, cudaMemcpyDeviceToHost));
-      SK_CUDA(cudaMemcpy(nseeds.data(), ws.chunk_nseeds, TC * 4, cudaMemcpyDeviceToHost));
-    }
-    dbg->anchors = (uint32_t*)malloc(std::max<size_t>(TA, 1) * 20);
-    dbg->score = (int64_t*)malloc(std::max<size_t>(TA, 1) * 8);
-    dbg->pointer = (uint32_t*)malloc(std::max<size_t>(TA, 1) * 4);
-    dbg->chunk_first = (uint32_t*)malloc((TC + 1) * 4);
-    dbg->chunk_nseeds = (uint32_t*)malloc(std::max<size_t>(TC, 1) * 4);
-    for (uint64_t c = 0; c < TC; c++) {
-      dbg->chunk_first[c] = (uint32_t)cf[c]; dbg->chunk_nseeds[c] = nseeds[c];
-      for (uint64_t x = cf[c]; x < cf[c + 1]; x++) {
-        dbg->anchors[5 * x] = cq[c]; dbg->anchors[5 * x + 1] = anc[x].qpos; dbg->anchors[5 * x + 2] = anc[x].rc >> 1;
-        dbg->anchors[5 * x + 3] = anc[x].rpos; dbg->anchors[5 * x + 4] = anc[x].rc & 1u;
-        dbg->score[x] = score[x]; dbg->pointer[x] = ptr[x];
-      }
-    }
-    dbg->chunk_first[TC] = (uint32_t)TA;
-    uint32_t nint = 0;
-    SK_CUDA(cudaMemcpy(&nint, ws.pair_nint, 4, cudaMemcpyDeviceToHost));
-    dbg->n_intervals = nint;
-    std::vector<IntervalKey> iv(nint);
-    std::vector<uint32_t> order(nint);
-    std::vector<uint8_t> kept(nint);
-    uint32_t npow2 = 1;
-    while (npow2 < nint) npow2 <<= 1;
-    if (nint) {
-      SK_CUDA(cudaMemcpy(iv.data(), ws.iv, nint * sizeof(IntervalKey), cudaMemcpyDeviceToHost));
-      SK_CUDA(cudaMemcpy(order.data(), ws.iv_order + npow2, nint * 4, cudaMemcpyDeviceToHost));
-      SK_CUDA(cudaMemcpy(kept.data(), ws.iv_kept, nint, cudaMemcpyDeviceToHost));
-    }
-    dbg->intervals = (int64_t*)malloc(std::max<size_t>(nint, 1) * 11 * 8);
-    for (uint32_t i = 0; i < nint; i++) {
-      const IntervalKey& x = iv[order[i]];
-      int64_t* o = dbg->intervals + 11 * i;
-      o[0] = iv_score(x); o[1] = iv_num_anchors(x); o[2] = iv_q0(x); o[3] = iv_q1(x); o[4] = iv_r0(x); o[5] = iv_r1(x);
-      o[6] = iv_rctg(x); o[7] = iv_qctg(x); o[8] = iv_chunk(x); o[9] = iv_rev(x); o[10] = kept[order[i]];
-    }
-    std::vector<double> est(TC);
-    std::vector<uint32_t> w(TC);
-    std::vector<uint8_t> valid(TC);
-    if (TC) {
-      SK_CUDA(cudaMemcpy(est.data(), ws.chunk_est, TC * 8, cudaMemcpyDeviceToHost));
-      SK_CUDA(cudaMemcpy(w.data(), ws.chunk_w, TC * 4, cudaMemcpyDeviceToHost));
-      SK_CUDA(cudaMemcpy(valid.data(), ws.chunk_valid, TC, cudaMemcpyDeviceToHost));
-    }
-    std::vector<std::pair<double, uint64_t>> es;
-    for (uint64_t c = 0; c < TC; c++) if (valid[c]) es.push_back({est[c], w[c]});
-    std::sort(es.begin(), es.end());
-    dbg->n_ests = es.size();
-    dbg->est = (double*)malloc(std::max<size_t>(es.size(), 1) * 8);
-    dbg->weight = (uint64_t*)malloc(std::max<size_t>(es.size(), 1) * 8);
-    for (size_t i = 0; i < es.size(); i++) { dbg->est[i] = es[i].first; dbg->weight[i] = es[i].second; }
-  }
+  if (dbg) SK_TRY(copy_out_debug(ctx, ws, descs, b0, B, abase, cbase, ibase, host_out, dbg));
   return SK_OK;
 }
 
@@ -1762,7 +1787,8 @@ static int chain_impl(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_se
     long d125 = std::labs((long)refs->sp.c - 125), d200 = std::labs((long)refs->sp.c - 200);
     prm.model = d125 < d200 ? 0 : 1;
   }
-  if (prm.band >= 0x7FFF) { ctx->err = "band too large"; return SK_ERR_PARAM; }
+  // dp_warp_kernel holds at most 16 register sets of 32 anchors (band / 32 + 2 <= 16): refused before anything is launched
+  if (prm.band / 32 + 2 > 16) { ctx->err = "c too small: chain band > 479 anchors is not supported"; return SK_ERR_PARAM; }
   const bool same = (refs == qs);
   if (!ctx->chain_scratch) {
     ctx->chain_scratch = new ChainScratch();
@@ -1827,18 +1853,29 @@ int sk_chain_pairs(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* 
   return sk::chain_impl(ctx, refs, queries, pairs, n_pairs, mp, out, nullptr);
 }
 
-int sk_chain_pair_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, uint64_t pair, const sk_map_params* mp,
-                        sk_chain_debug* out) {
-  if (!ctx || !refs || !queries || !mp || !out) return SK_ERR_PARAM;
-  sk_ani_result r;
-  return sk::chain_impl(ctx, refs, queries, &pair, 1, mp, &r, out);
-}
-
 void sk_chain_debug_free(sk_chain_debug* d) {
   if (!d) return;
   free(d->anchors); free(d->chunk_first); free(d->chunk_nseeds); free(d->score); free(d->pointer); free(d->intervals);
   free(d->est); free(d->weight);
   memset(d, 0, sizeof(*d));
+}
+
+int sk_chain_pairs_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, const uint64_t* pairs, uint64_t n_pairs,
+                         const sk_map_params* mp, sk_chain_debug* out) {
+  if (!ctx || !refs || !queries || !mp || (n_pairs && (!pairs || !out))) return SK_ERR_PARAM;
+  if (n_pairs == 0) return SK_OK;
+  memset(out, 0, n_pairs * sizeof(*out));
+  std::vector<sk_ani_result> res(n_pairs);
+  const int rc = sk::chain_impl(ctx, refs, queries, pairs, n_pairs, mp, res.data(), out);
+  if (rc != SK_OK)
+    for (uint64_t i = 0; i < n_pairs; i++) sk_chain_debug_free(out + i);
+  return rc;
+}
+
+int sk_chain_pair_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, uint64_t pair, const sk_map_params* mp,
+                        sk_chain_debug* out) {
+  if (!out) return SK_ERR_PARAM;
+  return sk_chain_pairs_debug(ctx, refs, queries, &pair, 1, mp, out);
 }
 
 }  // extern "C"

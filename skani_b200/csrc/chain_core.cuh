@@ -76,6 +76,38 @@ SK_HD uint32_t chunk_local_of(uint64_t al, bool has_prev, int64_t m_prev, uint32
   int64_t c = (int64_t)al + m_prev;
   return (uint32_t)(c < (int64_t)need ? c : (int64_t)need);
 }
+// the hit record's term of the segmented prefix min: need - (contig-local index of its last anchor)
+SK_HD int64_t record_min_key(uint32_t need, uint32_t al, uint32_t nh) {
+  return (int64_t)need - (int64_t)al - (int64_t)(nh - 1);
+}
+// Per hit record (al = contig-local index of its first anchor, nh anchors), given the prefix min m_prev over the earlier
+// hit records of its contig (has_prev = there are any): clf / cll = chunk_local_of(al / al + nh - 1, ...) are the
+// contig-local chunks of its first and last anchor.  The previous hit record's last anchor (index al - 1) sits in chunk
+// al - 1 + m_prev: the record's first anchor starts a chunk iff it is the contig's first hit or lands in a later chunk,
+// and the record starts that chunk (if any) plus one chunk per step from clf to cll.
+SK_HD uint32_t record_starts_chunk(uint32_t al, bool has_prev, int64_t m_prev, uint32_t clf) {
+  return (!has_prev || (int64_t)al - 1 + m_prev != (int64_t)clf) ? 1u : 0u;
+}
+SK_HD uint32_t record_chunk_starts(uint32_t st, uint32_t clf, uint32_t cll) {
+  return st + (cll - clf);
+}
+// Anchor u of a hit record whose first anchor is in contig-local chunk clf: its chunk (chunks only move forward until they
+// reach need), and whether it starts a chunk (the first anchor iff the record starts one, a later anchor iff anchor u - 1
+// had not yet reached need).
+SK_HD uint32_t anchor_chunk_local(uint32_t clf, uint32_t u, uint32_t need) {
+  return clf + u < need ? clf + u : need;
+}
+SK_HD bool anchor_starts_chunk(uint32_t clf, uint32_t u, uint32_t need, bool record_starts) {
+  return (u == 0) ? record_starts : clf + u - 1 < need;
+}
+// window of contig-local chunk cl of a contig whose first hit is at p0: it holds the seeds with lo < pos <= hi.  The pair's
+// last chunk is patched afterwards to end at its last anchor (src/chain.rs:796-824).
+SK_HD int64_t chunk_window_lo(uint32_t p0, uint32_t cl) {
+  return (cl == 0) ? -1ll : (int64_t)p0 + (int64_t)cl * FRAGMENT_LENGTH;
+}
+SK_HD int64_t chunk_window_hi(uint32_t p0, uint32_t cl) {
+  return (int64_t)p0 + (int64_t)(cl + 1) * FRAGMENT_LENGTH;
+}
 
 // ---- chain intervals: 5 x u64 keys whose lexicographic order is the derived PartialOrd of ChainInterval
 // (score, num_anchors, interval_on_query, interval_on_ref, ref_contig, query_contig, chunk_id, reverse_chain, overlap=0)

@@ -298,23 +298,38 @@ def chain_pairs(ctx, refs, queries, pairs, mp=None, as_array=False):
     return [AniResult.from_buffer_copy(out[i].tobytes()) for i in range(len(pairs))]
 
 
-def chain_pair_debug(ctx, refs, queries, ref_id, query_id, mp=None):
-    mp = mp or map_params()
-    d = ChainDebug()
-    ctx.check(ctx.L.sk_chain_pair_debug(ctx.h, refs.h, queries.h, (ref_id << 32) | query_id, C.byref(mp), C.byref(d)))
-
+def _debug_dict(d):
     def arr(p, shape, dt):
         n = int(np.prod(shape))
         return np.ctypeslib.as_array(p, shape=(n,)).astype(dt).reshape(shape).copy() if n else np.zeros(shape, dt)
-    res = dict(result=AniResult.from_buffer_copy(d.result), switched=bool(d.switched),
-               anchors=arr(d.anchors, (d.n_anchors, 5), np.uint32), score=arr(d.score, (d.n_anchors,), np.int64),
-               pointer=arr(d.pointer, (d.n_anchors,), np.uint32),
-               chunk_first=arr(d.chunk_first, (d.n_chunks + 1,), np.uint32) if d.n_chunks else np.zeros(1, np.uint32),
-               chunk_nseeds=arr(d.chunk_nseeds, (d.n_chunks,), np.uint32),
-               intervals=arr(d.intervals, (d.n_intervals, 11), np.int64),
-               est=arr(d.est, (d.n_ests,), np.float64), weight=arr(d.weight, (d.n_ests,), np.uint64))
-    ctx.L.sk_chain_debug_free(C.byref(d))
-    return res
+    return dict(result=AniResult.from_buffer_copy(d.result), switched=bool(d.switched),
+                anchors=arr(d.anchors, (d.n_anchors, 5), np.uint32), score=arr(d.score, (d.n_anchors,), np.int64),
+                pointer=arr(d.pointer, (d.n_anchors,), np.uint32),
+                chunk_first=arr(d.chunk_first, (d.n_chunks + 1,), np.uint32) if d.n_chunks else np.zeros(1, np.uint32),
+                chunk_nseeds=arr(d.chunk_nseeds, (d.n_chunks,), np.uint32),
+                intervals=arr(d.intervals, (d.n_intervals, 11), np.int64),
+                est=arr(d.est, (d.n_ests,), np.float64), weight=arr(d.weight, (d.n_ests,), np.uint64))
+
+
+def chain_pairs_debug(ctx, refs, queries, pairs, mp=None, keep=None):
+    """sk_chain_pairs_debug: the intermediate products of every pair of `pairs` (same batching and kernels as chain_pairs).
+    Returns one dict per pair, or with keep (pair indices) a {index: dict} of those pairs only."""
+    mp = mp or map_params()
+    pairs = np.ascontiguousarray(pairs, np.uint64)
+    n = len(pairs)
+    ds = (ChainDebug * max(n, 1))()
+    ctx.check(ctx.L.sk_chain_pairs_debug(ctx.h, refs.h, queries.h, pairs.ctypes.data, n, C.byref(mp), ds))
+    try:
+        if keep is None:
+            return [_debug_dict(ds[i]) for i in range(n)]
+        return {int(i): _debug_dict(ds[int(i)]) for i in keep}
+    finally:
+        for i in range(n):
+            ctx.L.sk_chain_debug_free(C.byref(ds[i]))
+
+
+def chain_pair_debug(ctx, refs, queries, ref_id, query_id, mp=None):
+    return chain_pairs_debug(ctx, refs, queries, [(ref_id << 32) | query_id], mp)[0]
 
 
 def triangle(ctx, bases, contig_off, genome_of_contig, n_genomes, sp=None, mp=None, as_array=False):

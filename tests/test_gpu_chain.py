@@ -8,11 +8,11 @@ import pytest
 
 import oracle_py as O
 from bench_support import synth
+from chain_testlib import TOL, assert_debug_equal, assert_result_close, make_sets, synth_genomes  # noqa: F401
 from fasta_py import read_fastx
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-TOL = 1e-4
 
 
 @pytest.fixture(scope="module")
@@ -25,57 +25,6 @@ def ctx():
 
 def f2(x):
     return "%.2f" % float(np.float32(x) * np.float32(100.0))
-
-
-def assert_result_close(g, o, tol=TOL):
-    if np.isnan(o.ani):
-        assert np.isnan(g.ani)
-        return
-    for f in ("ani", "af_query", "af_ref", "std", "ci_lower", "ci_upper"):
-        assert abs(getattr(g, f) - getattr(o, f)) <= tol, (f, getattr(g, f), getattr(o, f))
-    for f in ("q90_q", "q90_r", "q50_q", "q50_r", "q10_q", "q10_r", "num_contigs_q", "num_contigs_r",
-              "avg_chain_int_len", "total_bases_covered"):
-        assert getattr(g, f) == getattr(o, f), (f, getattr(g, f), getattr(o, f))
-
-
-def assert_debug_equal(gd, od):
-    assert gd["switched"] == od["switched"]
-    assert np.array_equal(gd["anchors"], od["anchors"]), "anchors"
-    assert np.array_equal(gd["chunk_first"], od["chunk_first"]), "chunk_first"
-    assert np.array_equal(gd["chunk_nseeds"], od["chunk_nseeds"]), "chunk_nseeds"
-    assert np.array_equal(gd["score"], od["score"]), "score"
-    assert np.array_equal(gd["pointer"], od["pointer"]), "pointer"
-    assert np.array_equal(gd["intervals"], od["intervals"]), "intervals"
-    assert np.array_equal(gd["weight"], od["weight"]), "weights"
-    assert np.allclose(gd["est"], od["est"], rtol=0, atol=1e-12), "ests"
-    assert_result_close(gd["result"], od["result"])
-
-
-def make_sets(ctx, genomes, sp_kw, individual=False):
-    """genomes: list of lists of contig byte arrays -> (gpu set, [oracle sketches])"""
-    import skani_b200 as sk
-    gs = sk.sketch_sequences(ctx, genomes, sk.sketch_params(**sp_kw), individual_contig=individual)
-    osk = []
-    for gi, ctgs in enumerate(genomes):
-        kept = [c for c in ctgs if len(c) >= 500]
-        if not kept:
-            continue
-        if individual:
-            for j, c in enumerate(kept):
-                osk.append(O.sketch_from_contigs("g%06d" % gi, [c], **sp_kw))
-        else:
-            osk.append(O.sketch_from_contigs("g%06d" % gi, kept, **sp_kw))
-    assert len(gs) == len(osk)
-    return gs, osk
-
-
-def synth_genomes(n, L, G):
-    bases, off, goc = synth.generate(0, n, L, G=G)
-    out = []
-    for g in range(n):
-        idx = np.nonzero(goc == g)[0]
-        out.append([bases[int(off[i]):int(off[i + 1])] for i in idx])
-    return out
 
 
 @pytest.mark.parametrize("c,mc,learned", [(125, 1000, True), (30, 200, False), (200, 1000, True)])
