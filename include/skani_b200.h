@@ -270,6 +270,32 @@ int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint8_t* bases_
                       const sk_map_params* mp, const uint64_t* name_ranks, sk_ani_result** out, uint64_t* n_out,
                       sk_triangle_stats* stats);
 
+/* ---- dist / search over several GPUs from ONE host process (src/dist.rs:98-144 screen + chain of every (ref, query) pair;
+ *      src/search.rs:119-247 the same against a sketched database).  The references are split into contiguous blocks, one
+ *      per context; the query set is copied to every context.  A pair's screen decision (its own marker counts,
+ *      src/screen.rs:84-189) and its chain result depend on that pair alone, so the results are byte-identical to the
+ *      single-context calls.  ctxs[d] may share a device.  If any context fails the call fails and sk_last_error(ctxs[0])
+ *      carries that context's message. */
+/* Copy a set (records, views, markers, contig tables, k-mer hash tables, name ranks) to another context, which may be on
+ * another device or the same one: a packed blob with the tables (no table rebuild, except the bucket index of genomes too
+ * large for a table), a peer or device copy, then an unpack.  The copy chains and screens exactly like the source. */
+int sk_sketch_set_copy(sk_ctx* dst, const sk_sketch_set* src, sk_sketch_set** out);
+/* References split into contiguous blocks: refs[d] lives on ctxs[d] and holds global refs [ref_first[d], ref_first[d] + G_d).
+ * ref_first must be ascending and the blocks disjoint.  refs[d] may be NULL or hold 0 genomes.
+ * queries[d] lives on ctxs[d] and is the same query set on every context (made with sk_sketch_set_copy).
+ * Arguments that break these rules, and sets whose sketch parameters differ, give SK_ERR_PARAM.
+ *   = sk_screen_query_ref on one set holding all refs: same modes 0-3, sorted, global ref ids. */
+int sk_screen_query_ref_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
+                              const sk_sketch_set* const* queries, const sk_map_params* mp, int mode,
+                              uint64_t** pairs_rq, uint64_t* n_pairs);
+/* pairs are global (ref << 32 | query), in any order; a pair whose ref lies in no block or whose query is out of range gives
+ * SK_ERR_PARAM.  out[i] = sk_chain_pairs(one context holding all refs, pairs[i]), with ref_id global.  Default name ranks
+ * (sk_sketch_set_set_name_ranks never called) are those of that one set: global ref ids, queries after all
+ * ref_first[n_ctx-1] + G_{n_ctx-1} refs. */
+int sk_chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
+                         const sk_sketch_set* const* queries, const uint64_t* pairs, uint64_t n_pairs,
+                         const sk_map_params* mp, sk_ani_result* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -87,6 +87,9 @@ SYMBOLS = [
                                PP(TriangleStats), PP(vp)]),
     ("sk_triangle_multi", i32, [vp, u32, vp, vp, u32, vp, u32, PP(SketchParams), PP(MapParams), vp, PP(PP(AniResult)), PP(u64),
                                 PP(TriangleStats)]),
+    ("sk_sketch_set_copy", i32, [vp, vp, PP(vp)]),
+    ("sk_screen_query_ref_multi", i32, [vp, u32, vp, vp, vp, PP(MapParams), i32, PP(PP(u64)), PP(u64)]),
+    ("sk_chain_pairs_multi", i32, [vp, u32, vp, vp, vp, vp, u64, PP(MapParams), vp]),
 ]
 
 _lib = None

@@ -12,6 +12,8 @@
 // model: instead of deserialising a reference sketch from the mmap'd database for every passing pair
 // (src/search.rs:142-166) it screens ALL queries against ALL marker sketches in one GPU pass, loads each reference sketch
 // that passed for some query exactly once, imports them to the device in one batch and chains every pair there.
+// --gpus N: dist and search split the references into contiguous blocks, one per GPU, and copy the query set to every GPU
+// (sk_screen_query_ref_multi / sk_chain_pairs_multi); the output is byte-identical to one GPU's.
 #include <dirent.h>
 #include <fcntl.h>
 #include <sys/stat.h>
@@ -245,9 +247,8 @@ bool all_sketch_files(const std::vector<std::string>& files) {
 }
 
 // file_io::sketches_from_sketch (src/file_io.rs:680-717): one (SketchParams, Sketch) blob per file, markers.bin skipped,
-// result sorted by file name; the sketches' parameters replace the command line's.  Then straight to the device.
-sk_sketch_set* load_sketch_files(sk_ctx* ctx, const std::vector<std::string>& files, skdb::DiskParams& dp, std::vector<Genome>& meta) {
-  std::vector<skdb::HostSketch> hs;
+// result sorted by file name; the sketches' parameters replace the command line's.  meta gets one Genome per sketch.
+void read_sketch_files(const std::vector<std::string>& files, skdb::DiskParams& dp, std::vector<Genome>& meta, std::vector<skdb::HostSketch>& hs) {
   for (auto& f : files) {
     if (f.find("markers.bin") != std::string::npos) continue;
     std::vector<uint8_t> b;
@@ -257,18 +258,71 @@ sk_sketch_set* load_sketch_files(sk_ctx* ctx, const std::vector<std::string>& fi
       fprintf(stderr, "ERROR %s is not a valid .sketch file or is corrupted. Skani v0.3+ is not compatible with older sketch files.\n", f.c_str());
     }
   }
-  if (hs.empty()) return nullptr;
+  if (hs.empty()) return;
   if (dp.use_aa) { fprintf(stderr, "ERROR amino-acid sketches are not supported\n"); exit(1); }
   std::stable_sort(hs.begin(), hs.end(), [](const skdb::HostSketch& x, const skdb::HostSketch& y) { return x.file_name < y.file_name; });
-  Flat f;
   for (auto& h : hs) {
-    f.add(h, true);
     Genome g; g.file_name = h.file_name; g.contigs = h.contigs; g.contig_order = h.contig_order; g.total_len = h.total_len;
     if (g.contigs.empty()) g.contigs.push_back("");
     meta.push_back(std::move(g));
   }
-  sk_sketch_params sp{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
+}
+
+// host sketches [a, b) -> one device set on ctx
+sk_sketch_set* import_sketches(sk_ctx* ctx, const std::vector<skdb::HostSketch>& hs, size_t a, size_t b, const sk_sketch_params& sp) {
+  Flat f;
+  for (size_t i = a; i < b; i++) f.add(hs[i], true);
   return f.import(ctx, sp);
+}
+
+sk_sketch_set* load_sketch_files(sk_ctx* ctx, const std::vector<std::string>& files, skdb::DiskParams& dp, std::vector<Genome>& meta) {
+  std::vector<skdb::HostSketch> hs;
+  read_sketch_files(files, dp, meta, hs);
+  if (hs.empty()) return nullptr;
+  return import_sketches(ctx, hs, 0, hs.size(), sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c});
+}
+
+// --gpus N: contexts 1..n-1 next to ctx0, on (device + d) % device count.  With fewer devices than N the contexts share
+// devices (same code path; copies between them stay on the device).
+std::vector<sk_ctx*> make_contexts(sk_ctx* ctx0, const Opts& op, size_t n) {
+  std::vector<sk_ctx*> ctxs(1, ctx0);
+  if (op.gpus <= 1) return ctxs;
+  const int ndev = sk_device_count();
+  if (ndev < op.gpus) fprintf(stderr, "WARN --gpus %d but %d CUDA device(s) visible: contexts share devices.\n", op.gpus, ndev);
+  for (size_t d = 1; d < n; d++) {
+    const int dev = (op.device + (int)d) % std::max(ndev, 1);
+    sk_ctx* c = nullptr;
+    if (sk_ctx_create(dev, &c) != 0) { fprintf(stderr, "ERROR cannot create a context on GPU %d\n", dev); exit(1); }
+    ctxs.push_back(c);
+  }
+  return ctxs;
+}
+
+// fn(d) for d < n, one host thread per context
+template <class F>
+void per_context(size_t n, F fn) {
+  if (n == 1) { fn((size_t)0); return; }
+  std::vector<std::thread> th;
+  for (size_t d = 0; d < n; d++) th.emplace_back(fn, d);
+  for (auto& t : th) t.join();
+}
+
+// [0, w.size()) cut into W contiguous blocks of about equal total weight: bounds[d], bounds[d + 1] delimit block d.  A block
+// is empty only when there are fewer items than blocks.
+std::vector<size_t> split_balanced(const std::vector<uint64_t>& w, size_t W) {
+  const size_t n = w.size();
+  uint64_t total = 0;
+  for (uint64_t x : w) total += x;
+  std::vector<size_t> b(W + 1, 0);
+  uint64_t acc = 0;
+  size_t d = 1;
+  for (size_t g = 0; g < n && d < W; g++) {
+    acc += w[g];
+    if (acc * W >= total * d || n - (g + 1) <= W - d) b[d++] = g + 1;
+  }
+  for (; d < W; d++) b[d] = b[d - 1];
+  b[W] = n;
+  return b;
 }
 
 int run_triangle(Opts& op) {
@@ -317,14 +371,7 @@ int run_triangle(Opts& op) {
   if (op.gpus > 1 && !loaded) {
     // --gpus N: one context per GPU, genome blocks + marker exchange + cross-block slices (sk_triangle_multi).  With fewer
     // physical devices than N the contexts share devices (same code path; the exchange then stays on the device).
-    const int ndev = sk_device_count();
-    if (ndev < op.gpus) fprintf(stderr, "WARN --gpus %d but %d CUDA device(s) visible: contexts share devices.\n", op.gpus, ndev);
-    std::vector<sk_ctx*> ctxs(1, ctx);
-    for (int d = 1; d < op.gpus; d++) {
-      sk_ctx* c = nullptr;
-      if (sk_ctx_create((op.device + d) % std::max(ndev, 1), &c) != 0) { fprintf(stderr, "ERROR cannot create a context on GPU %d\n", (op.device + d) % std::max(ndev, 1)); return 1; }
-      ctxs.push_back(c);
-    }
+    std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, op.gpus);
     sk_ani_result* r = nullptr; uint64_t nr = 0;
     CK(ctx, sk_triangle_multi(ctxs.data(), (uint32_t)ctxs.size(), in.bases.data(), in.contig_off.data(), (uint32_t)in.genome_of_contig.size(),
                               in.genome_of_contig.data(), (uint32_t)in.genomes.size(), &sp, &mp, ranks.data(), &r, &nr, nullptr));
@@ -421,13 +468,14 @@ int run_dist(Opts& op) {
   sk_ctx* ctx = nullptr;
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
   sk_sketch_params sp{op.c, op.k, op.m};
-  sk_sketch_set *rset = nullptr, *qset = nullptr;
-  // .sketch inputs carry their own parameters, which then also apply to FASTA inputs on the other side (src/dist.rs:17-50)
+  // .sketch inputs carry their own parameters, which then also apply to FASTA inputs on the other side (src/dist.rs:17-50).
+  // They are read on the host here and imported once the contexts exist.
+  std::vector<skdb::HostSketch> rhs, qhs;
   if (refs_are_sketch) {
     fprintf(stderr, "INFO Sketches detected.\n");
     skdb::DiskParams dp;
-    rset = load_sketch_files(ctx, op.refs, dp, rin.genomes);
-    if (rset) {
+    read_sketch_files(op.refs, dp, rin.genomes, rhs);
+    if (!rhs.empty()) {
       if (dp.c != sp.c || dp.k != sp.k || dp.marker_c != sp.marker_c)
         fprintf(stderr, "WARN Parameters from .sketch files not equal to the input parameters. Using parameters from .sketch files.\n");
       sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
@@ -435,8 +483,8 @@ int run_dist(Opts& op) {
   }
   if (queries_are_sketch) {
     skdb::DiskParams dp;
-    qset = load_sketch_files(ctx, op.queries, dp, qin.genomes);
-    if (qset && (dp.c != sp.c || dp.k != sp.k || dp.marker_c != sp.marker_c)) {
+    read_sketch_files(op.queries, dp, qin.genomes, qhs);
+    if (!qhs.empty() && (dp.c != sp.c || dp.k != sp.k || dp.marker_c != sp.marker_c)) {
       if (refs_are_sketch) { fprintf(stderr, "ERROR Query sketch parameters were not equal to reference sketch parameters. Exiting.\n"); return 1; }
       fprintf(stderr, "WARN Parameters from .sketch files not equal to the input parameters. Using parameters from .sketch files.\n");
       sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
@@ -454,25 +502,48 @@ int run_dist(Opts& op) {
   mp.learned_ani = !op.no_learned && op.c >= 70 && !op.qi && !op.ri && !op.median;
   if (mp.learned_ani) fprintf(stderr, "INFO Learned ANI mode detected. ANI may be adjusted according to a regression model trained on MAGs.\n");
   const bool use_index = (op.queries.size() > 50 || op.qi) && !op.no_marker_index;   // FULL_INDEX_THRESH (src/parse.rs:750)
-  if (!rset) rset = sketch(ctx, rin, sp);
-  if (!qset) qset = sketch(ctx, qin, sp);
   // file-name order for the switch_qr tie-break (src/chain.rs:19-21): rank all names together
+  std::vector<uint64_t> rr(rin.genomes.size()), qr(qin.genomes.size());
   {
     std::vector<std::pair<std::string, std::pair<int, size_t>>> names;
     for (size_t i = 0; i < rin.genomes.size(); i++) names.push_back({rin.genomes[i].file_name, {0, i}});
     for (size_t i = 0; i < qin.genomes.size(); i++) names.push_back({qin.genomes[i].file_name, {1, i}});
     std::sort(names.begin(), names.end(), [](auto& a, auto& b) { return a.first < b.first; });
-    std::vector<uint64_t> rr(rin.genomes.size()), qr(qin.genomes.size());
     uint64_t rank = 0;
     for (size_t i = 0; i < names.size(); i++) {
       if (i && names[i].first != names[i - 1].first) rank++;
       (names[i].second.first ? qr : rr)[names[i].second.second] = rank;
     }
-    sk_sketch_set_set_name_ranks(rset, rr.data());
-    sk_sketch_set_set_name_ranks(qset, qr.data());
   }
+  // --gpus N: the references in W contiguous blocks (genome order, balanced by bases, or by records for .sketch inputs), each
+  // sketched or imported on its own context; the queries once on context 0, then copied to the others
+  const size_t NR = rin.genomes.size(), W = std::min<size_t>(std::max(op.gpus, 1), NR);
+  std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, W);
+  std::vector<uint64_t> weight(NR);
+  for (size_t g = 0; g < NR; g++) weight[g] = refs_are_sketch ? rhs[g].kmer.size() : rin.genomes[g].total_len;
+  const std::vector<size_t> gb = split_balanced(weight, W);
+  std::vector<sk_sketch_set*> rsets(W, nullptr), qsets(W, nullptr);
+  std::vector<uint32_t> ref_first(W);
+  for (size_t d = 0; d < W; d++) ref_first[d] = (uint32_t)gb[d];
+  per_context(W, [&](size_t d) {
+    sk_ctx* c = ctxs[d];
+    if (refs_are_sketch) rsets[d] = import_sketches(c, rhs, gb[d], gb[d + 1], sp);
+    else {
+      const size_t c0 = std::lower_bound(rin.genome_of_contig.begin(), rin.genome_of_contig.end(), (uint32_t)gb[d]) - rin.genome_of_contig.begin();
+      const size_t c1 = std::lower_bound(rin.genome_of_contig.begin(), rin.genome_of_contig.end(), (uint32_t)gb[d + 1]) - rin.genome_of_contig.begin();
+      std::vector<uint32_t> gl(c1 - c0);
+      for (size_t i = c0; i < c1; i++) gl[i - c0] = rin.genome_of_contig[i] - (uint32_t)gb[d];
+      CK(c, sk_sketch_batch(c, rin.bases.data(), rin.contig_off.data() + c0, (uint32_t)(c1 - c0), gl.data(), (uint32_t)(gb[d + 1] - gb[d]), &sp, &rsets[d]));
+    }
+    sk_sketch_set_set_name_ranks(rsets[d], rr.data() + gb[d]);
+    if (d == 0) {
+      qsets[0] = queries_are_sketch ? import_sketches(c, qhs, 0, qhs.size(), sp) : sketch(c, qin, sp);
+      sk_sketch_set_set_name_ranks(qsets[0], qr.data());
+    }
+  });
+  for (size_t d = 1; d < W; d++) CK(ctxs[d], sk_sketch_set_copy(ctxs[d], qsets[0], &qsets[d]));
   uint64_t* pairs = nullptr; uint64_t np = 0;
-  CK(ctx, sk_screen_query_ref(ctx, rset, qset, &mp, use_index ? 2 : 0, &pairs, &np));
+  CK(ctx, sk_screen_query_ref_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), &mp, use_index ? 2 : 0, &pairs, &np));
   // queries are processed, and their results appended, in blocks of INTERMEDIATE_WRITE_COUNT (src/dist.rs:151-175)
   std::vector<uint64_t> byq(pairs, pairs + np);
   sk_free(pairs);
@@ -487,7 +558,7 @@ int run_dist(Opts& op) {
     size_t p1 = p0;
     while (p1 < byq.size() && (uint32_t)byq[p1] < q0 + FL) p1++;
     res.resize(p1 - p0);
-    CK(ctx, sk_chain_pairs(ctx, rset, qset, byq.data() + p0, p1 - p0, &mp, res.data()));
+    CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), byq.data() + p0, p1 - p0, &mp, res.data()));
     // write_query_ref_list (src/file_io.rs:608-678): group by the query's first contig name, sort each group by ANI desc, top n
     std::map<std::string, std::vector<const sk_ani_result*>> groups;
     for (auto& r : res) if (r.ani > 0.1f) groups[qin.genomes[r.query_id].contigs[0]].push_back(&r);
@@ -501,8 +572,8 @@ int run_dist(Opts& op) {
     p0 = p1;
   }
   if (o != stdout) fclose(o);
-  sk_sketch_set_free(rset); sk_sketch_set_free(qset);
-  sk_ctx_destroy(ctx);
+  for (size_t d = 0; d < W; d++) { sk_sketch_set_free(rsets[d]); sk_sketch_set_free(qsets[d]); }
+  for (size_t d = W; d-- > 0;) sk_ctx_destroy(ctxs[d]);
   return 0;
 }
 
@@ -679,9 +750,17 @@ int run_search(Opts& op) {
     }
     sk_sketch_set_set_name_ranks(qset, qrank.data());
   }
+  // --gpus N: the query set is copied to every context once; each query block's references are spread over them below
+  const size_t W = std::max(op.gpus, 1);
+  std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, W);
+  std::vector<sk_sketch_set*> qsets(W, qset);
+  for (size_t d = 1; d < W; d++) CK(ctxs[d], sk_sketch_set_copy(ctxs[d], qset, &qsets[d]));
   // ---- queries are processed, and their results appended, in blocks of INTERMEDIATE_WRITE_COUNT (src/search.rs:255-279).
-  //      Inside a block: the references that passed for at least one of its queries are loaded ONCE each, imported in
-  //      batches, and their pairs chained (the reference deserialises a sketch per passing PAIR, src/search.rs:142-166)
+  //      Inside a block: the references that passed for at least one of its queries ("hits") are loaded ONCE each and their
+  //      pairs chained (the reference deserialises a sketch per passing PAIR, src/search.rs:142-166).  The hits are cut into
+  //      W contiguous runs balanced by estimated records (marker counts), one per context.  Every round, each context loads
+  //      the next part of its run (-t threads split over the contexts) and imports it, then one sk_chain_pairs_multi call
+  //      chains the round's pairs on all contexts.
   FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
   if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
   write_header(o, op.ci, op.detailed);
@@ -691,69 +770,85 @@ int run_search(Opts& op) {
   for (size_t q0 = 0; q0 < NQ; q0 += FL) {
   std::vector<uint64_t> blockp;
   for (uint64_t x : all_pairs) if ((uint32_t)x >= q0 && (uint32_t)x < q0 + FL) blockp.push_back(x);   // stays sorted by (ref, query)
-  const uint64_t* pairs = blockp.data();
-  const uint64_t np = blockp.size();
   std::vector<uint32_t> hits;
-  for (uint64_t i = 0; i < np; i++) hits.push_back((uint32_t)(pairs[i] >> 32));   // pairs are sorted by (ref, query)
-  hits.erase(std::unique(hits.begin(), hits.end()), hits.end());
+  std::vector<size_t> hit_pairs;          // pairs of hits[h]: blockp[hit_pairs[h], hit_pairs[h + 1])
+  for (size_t i = 0; i < blockp.size(); i++)
+    if (hits.empty() || hits.back() != (uint32_t)(blockp[i] >> 32)) { hits.push_back((uint32_t)(blockp[i] >> 32)); hit_pairs.push_back(i); }
+  hit_pairs.push_back(blockp.size());
+  std::vector<uint64_t> est(hits.size());
+  for (size_t h = 0; h < hits.size(); h++) est[h] = ref_mk[hits[h]].markers.size() + 1;
+  const std::vector<size_t> run = split_balanced(est, W);     // context d: hits [run[d], run[d + 1])
+  std::vector<size_t> next(run.begin(), run.end() - 1);
   std::vector<sk_ani_result> kept;
-  size_t pi = 0;
-  for (size_t h0 = 0; h0 < hits.size();) {
-    size_t h1 = h0;
-    std::vector<skdb::HostSketch> loaded;
-    uint64_t recs = 0;
-    while (h1 < hits.size() && h1 - h0 < 60000 && recs < (1ull << 30)) h1++, recs += 45000;   // provisional bound, refined below
-    loaded.resize(h1 - h0);
-    std::vector<int> ok(h1 - h0, 1);
-    {
-      const int T = std::max(op.threads, 1);
-      std::vector<std::thread> pool;
-      for (int t = 0; t < T; t++) pool.emplace_back([&, t] {
-        for (size_t i = h0 + t; i < h1; i += T) {
-          const uint32_t r = hits[i];
-          std::vector<uint8_t> b;
-          bool good;
-          if (consolidated) {
-            b.resize(index[r].length);
-            good = pread(db_fd, b.data(), b.size(), (off_t)index[r].offset) == (ssize_t)b.size();
-          } else {                     // <dir>/<basename(file_name)>.sketch (src/search.rs:157-166)
-            good = skdb::read_file(op.db_dir + "/" + base_name(ref_mk[r].file_name) + ".sketch", b);
+  for (;;) {
+    std::vector<size_t> lo(next), hi(next);                   // this round: context d imports hits [lo[d], hi[d])
+    std::vector<sk_sketch_set*> rsets(W, nullptr);
+    std::atomic<bool> too_large{false};
+    per_context(W, [&](size_t d) {
+      const size_t h0 = next[d], end = run[d + 1];
+      if (h0 == end) return;
+      size_t h1 = h0;
+      std::vector<skdb::HostSketch> loaded;
+      uint64_t recs = 0;
+      while (h1 < end && h1 - h0 < 60000 && recs < (1ull << 30)) h1++, recs += 45000;   // provisional bound, refined below
+      loaded.resize(h1 - h0);
+      std::vector<int> ok(h1 - h0, 1);
+      {
+        const int T = std::max(1, std::max(op.threads, 1) / (int)W + ((int)d < std::max(op.threads, 1) % (int)W ? 1 : 0));
+        std::vector<std::thread> pool;
+        for (int t = 0; t < T; t++) pool.emplace_back([&, t] {
+          for (size_t i = h0 + t; i < h1; i += T) {
+            const uint32_t r = hits[i];
+            std::vector<uint8_t> b;
+            bool good;
+            if (consolidated) {
+              b.resize(index[r].length);
+              good = pread(db_fd, b.data(), b.size(), (off_t)index[r].offset) == (ssize_t)b.size();
+            } else {                     // <dir>/<basename(file_name)>.sketch (src/search.rs:157-166)
+              good = skdb::read_file(op.db_dir + "/" + base_name(ref_mk[r].file_name) + ".sketch", b);
+            }
+            try { if (good) loaded[i - h0] = skdb::read_blob(b.data(), b.size()); }
+            catch (const std::exception&) { good = false; }
+            if (!good) { ok[i - h0] = 0; fprintf(stderr, "ERROR Failed to load sketch %s\n", ref_mk[r].file_name.c_str()); }
           }
-          try { if (good) loaded[i - h0] = skdb::read_blob(b.data(), b.size()); }
-          catch (const std::exception&) { good = false; }
-          if (!good) { ok[i - h0] = 0; fprintf(stderr, "ERROR Failed to load sketch %s\n", ref_mk[r].file_name.c_str()); }
-        }
-      });
-      for (auto& th : pool) th.join();
-    }
-    // keep the batch under 2^31 records: shrink it if the real sizes exceed the estimate
-    uint64_t real = 0;
-    size_t cut = h0;
-    while (cut < h1 && real + loaded[cut - h0].kmer.size() < (1ull << 31) - 1) real += loaded[cut - h0].kmer.size(), cut++;
-    if (cut == h0) { fprintf(stderr, "ERROR reference sketch too large\n"); return 1; }
-    h1 = cut;
-    Flat f;
-    std::vector<uint64_t> ranks;
-    for (size_t i = h0; i < h1; i++) {
-      if (!ok[i - h0]) loaded[i - h0] = skdb::HostSketch();     // unreadable reference: chains to "no anchors", dropped below
-      f.add(loaded[i - h0], true);
-      ranks.push_back(rrank[hits[i]]);
-    }
-    sk_sketch_set* rset = f.import(ctx, sp);
-    sk_sketch_set_set_name_ranks(rset, ranks.data());
+        });
+        for (auto& th : pool) th.join();
+      }
+      // keep the batch under 2^31 records: shrink it if the real sizes exceed the estimate (the rest goes to later rounds)
+      uint64_t real = 0;
+      size_t cut = h0;
+      while (cut < h1 && real + loaded[cut - h0].kmer.size() < (1ull << 31) - 1) real += loaded[cut - h0].kmer.size(), cut++;
+      if (cut == h0) { too_large = true; return; }
+      Flat f;
+      std::vector<uint64_t> ranks;
+      for (size_t i = h0; i < cut; i++) {
+        if (!ok[i - h0]) loaded[i - h0] = skdb::HostSketch();     // unreadable reference: chains to "no anchors", dropped below
+        f.add(loaded[i - h0], true);
+        ranks.push_back(rrank[hits[i]]);
+      }
+      rsets[d] = f.import(ctxs[d], sp);
+      sk_sketch_set_set_name_ranks(rsets[d], ranks.data());
+      hi[d] = next[d] = cut;
+    });
+    if (too_large) { fprintf(stderr, "ERROR reference sketch too large\n"); return 1; }
+    // the round's refs are numbered run after run: context d's block starts at ref_first[d]
+    std::vector<uint32_t> ref_first(W), round_hit;
     std::vector<uint64_t> local;
-    while (pi < np && (uint32_t)(pairs[pi] >> 32) <= hits[h1 - 1]) {
-      const uint32_t r = (uint32_t)(pairs[pi] >> 32);
-      const size_t li = std::lower_bound(hits.begin() + h0, hits.begin() + h1, r) - (hits.begin() + h0);
-      local.push_back(((uint64_t)li << 32) | (uint32_t)pairs[pi]);
-      pi++;
+    for (size_t d = 0; d < W; d++) {
+      ref_first[d] = (uint32_t)round_hit.size();
+      for (size_t h = lo[d]; h < hi[d]; h++) {
+        for (size_t i = hit_pairs[h]; i < hit_pairs[h + 1]; i++) local.push_back(((uint64_t)round_hit.size() << 32) | (uint32_t)blockp[i]);
+        round_hit.push_back((uint32_t)h);
+      }
     }
+    if (round_hit.empty()) break;
     std::vector<sk_ani_result> res(local.size());
-    CK(ctx, sk_chain_pairs(ctx, rset, qset, local.data(), local.size(), &mp, res.data()));
-    for (auto& r : res) if (r.ani > 0.5f) { r.ref_id = hits[h0 + r.ref_id]; kept.push_back(r); }   // src/search.rs:174
-    sk_sketch_set_free(rset);
-    h0 = h1;
+    CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(), &mp, res.data()));
+    for (auto& r : res) if (r.ani > 0.5f) { r.ref_id = hits[round_hit[r.ref_id]]; kept.push_back(r); }   // src/search.rs:174
+    for (auto* s : rsets) sk_sketch_set_free(s);
   }
+  // the writer's input order: pairs sorted by (ref, query), as one context chaining the hits in order produces them
+  std::sort(kept.begin(), kept.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
   // write_query_ref_list (src/file_io.rs:608-678): group by the query's first contig name, ANI descending, top n
   std::map<std::string, std::vector<const sk_ani_result*>> groups;
   for (auto& r : kept) groups[qmeta[r.query_id].contigs[0]].push_back(&r);
@@ -771,8 +866,8 @@ int run_search(Opts& op) {
   }
   if (db_fd >= 0) close(db_fd);
   if (o != stdout) fclose(o);
-  sk_sketch_set_free(qset);
-  sk_ctx_destroy(ctx);
+  for (auto* s : qsets) sk_sketch_set_free(s);
+  for (size_t d = W; d-- > 0;) sk_ctx_destroy(ctxs[d]);
   return 0;
 }
 
@@ -800,7 +895,8 @@ void usage() {
           "  skani-b200 sketch [fasta ... | -l list] -o new_folder [-i] [--separate-sketches]\n"
           "  skani-b200 search -d sketch_folder [query ... | -q ... | --ql list] [--qi] [-n N] [-o out]\n"
           "  common: -c C -m M -k K -s SCREEN%% --min-af P --both-min-af P --robust --median --no-learned-ani --faster-small\n"
-          "          --small-genomes --fast --medium --slow --ci --detailed --short-header --no-marker-index -t THREADS --device D\n");
+          "          --small-genomes --fast --medium --slow --ci --detailed --short-header --no-marker-index -t THREADS --device D\n"
+          "          --gpus N (triangle, dist, search: one context per GPU, devices D, D+1, ...)\n");
 }
 
 }  // namespace

@@ -48,6 +48,18 @@ struct Blob { void* d = nullptr; uint64_t bytes = 0; std::vector<uint64_t> meta;
 
 double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
+// peer access between the distinct devices of ctxs[0..n) (ignored when unsupported: copies then stage through the host)
+void enable_peer_access(sk_ctx* const* ctxs, uint32_t n) {
+  for (uint32_t a = 0; a < n; a++)
+    for (uint32_t b = 0; b < n; b++)
+      if (ctxs[a]->device != ctxs[b]->device) {
+        cudaSetDevice(ctxs[a]->device);
+        int can = 0;
+        if (cudaDeviceCanAccessPeer(&can, ctxs[a]->device, ctxs[b]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[b]->device, 0);
+        cudaGetLastError();
+      }
+}
+
 }  // namespace
 
 // Cross-block pairs -> one list per device.  The pairs of one connected component of the pair graph (a cluster of related
@@ -129,15 +141,7 @@ extern "C" int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint
     for (uint32_t k = 1; k <= W; k++) gb[k] = std::max(gb[k], gb[k - 1]);
   }
   for (uint32_t d = 0; d <= W; d++) cb[d] = (uint32_t)(std::lower_bound(genome_of_contig, genome_of_contig + n_contigs, gb[d]) - genome_of_contig);
-  // peer access between distinct devices (ignored when unsupported: the copies then stage through the host)
-  for (uint32_t a = 0; a < W; a++)
-    for (uint32_t b = 0; b < W; b++)
-      if (ctxs[a]->device != ctxs[b]->device) {
-        cudaSetDevice(ctxs[a]->device);
-        int can = 0;
-        if (cudaDeviceCanAccessPeer(&can, ctxs[a]->device, ctxs[b]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[b]->device, 0);
-        cudaGetLastError();
-      }
+  enable_peer_access(ctxs, W);
 
   PhaseBarrier bar(W);
   std::vector<sk_sketch_set*> local(W, nullptr);
@@ -320,4 +324,167 @@ extern "C" int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint
     stats->n_pairs_kept = nres;
   }
   return SK_OK;
+}
+
+// ---- query x ref work over several contexts (`skani dist` / `skani search` with --gpus N, src/dist.rs:98-144,
+//      src/search.rs:119-247).  The references are split into contiguous blocks, one per context; the query set is copied
+//      to every context.  A (ref, query) pair's screen decision and chain result depend on that pair alone, so each context
+//      screens / chains its own block and the per-block results are put back in the caller's order with global ref ids.
+
+extern "C" int sk_sketch_set_copy(sk_ctx* dst, const sk_sketch_set* src, sk_sketch_set** out) {
+  if (!dst || !src || !out) return SK_ERR_PARAM;
+  *out = nullptr;
+  sk_ctx* sc = src->ctx;
+  if (dst != sc) { sk_ctx* pair[2] = {sc, dst}; enable_peer_access(pair, 2); }
+  // the source set's own blob, k-mer tables included (no rebuild on the destination), copied device to device
+  uint64_t bytes = 0, words = 0;
+  int rc = sk_sketch_set_subset_blob_size(src, nullptr, 0, SK_PACK_TABLES, &bytes, &words);
+  std::vector<uint64_t> meta(words);
+  void *sblob = nullptr, *dblob = nullptr;
+  if (rc == SK_OK && (cudaSetDevice(sc->device) != cudaSuccess || sc->arena.alloc(&sblob, bytes) != cudaSuccess)) { sc->err = "sk_sketch_set_copy: out of device memory (source)"; rc = SK_ERR_NOMEM; }
+  if (rc == SK_OK) rc = sk_sketch_set_pack_subset(src, nullptr, 0, SK_PACK_TABLES, sblob, meta.data());   // synchronises the source stream
+  if (rc != SK_OK && dst != sc) dst->err = sc->err;
+  const void* from = sblob;
+  if (rc == SK_OK && dst != sc) {
+    cudaError_t e = cudaSetDevice(dst->device);
+    if (e == cudaSuccess && dst->arena.alloc(&dblob, bytes) != cudaSuccess) { dst->err = "sk_sketch_set_copy: out of device memory (destination)"; rc = SK_ERR_NOMEM; }
+    if (rc == SK_OK && e == cudaSuccess) e = cudaMemcpyAsync(dblob, sblob, bytes, cudaMemcpyDefault, dst->stream);
+    if (rc == SK_OK && e == cudaSuccess) e = cudaStreamSynchronize(dst->stream);
+    if (rc == SK_OK && e != cudaSuccess) { dst->err = std::string("sk_sketch_set_copy: ") + cudaGetErrorString(e); rc = SK_ERR_CUDA; }
+    from = dblob;
+  }
+  const uint64_t* mp = meta.data();
+  if (rc == SK_OK) rc = sk_sketch_set_unpack(dst, 1, &from, &mp, out);
+  if (rc == SK_OK) { (*out)->name_rank = src->name_rank; (*out)->ranks_user_set = src->ranks_user_set; }   // host-side state
+  if (dblob) { cudaSetDevice(dst->device); dst->arena.release(dblob); }
+  if (sblob) { cudaSetDevice(sc->device); sc->arena.release(sblob); }
+  cudaSetDevice(dst->device);
+  return rc;
+}
+
+namespace {
+
+struct QrBlocks {
+  std::vector<uint32_t> G;   // references held by each context (0 for a NULL set)
+  uint64_t n_refs = 0;       // end of the last block: the size of the one set the blocks stand for
+  uint32_t n_queries = 0;
+};
+
+// the arguments shared by the two query x ref calls; every violation is the caller's and is reported on ctxs[0]
+int check_qr_args(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
+                  const sk_sketch_set* const* queries, const sk_map_params* mp, QrBlocks& qb) {
+  if (!ctxs || n_ctx == 0 || !ctxs[0]) return SK_ERR_PARAM;
+  sk_ctx* ctx = ctxs[0];
+  auto fail = [&](const std::string& m) { ctx->err = m; return SK_ERR_PARAM; };
+  if (!refs || !ref_first || !queries || !mp) return fail("NULL argument");
+  if (!queries[0]) return fail("queries[0] is NULL");
+  const sk_sketch_set* q0 = queries[0];
+  auto same_params = [](const sk_sketch_params& a, const sk_sketch_params& b) { return a.c == b.c && a.k == b.k && a.marker_c == b.marker_c; };
+  qb.G.assign(n_ctx, 0);
+  for (uint32_t d = 0; d < n_ctx; d++) {
+    const std::string at = "context " + std::to_string(d) + ": ";
+    if (!ctxs[d]) return fail(at + "NULL context");
+    for (uint32_t e = 0; e < d; e++) if (ctxs[e] == ctxs[d]) return fail(at + "the same context appears twice (one host thread per context)");
+    const sk_sketch_set* q = queries[d];
+    if (!q || q->ctx != ctxs[d]) return fail(at + "queries[d] must be a set of ctxs[d]");
+    if (q->G != q0->G || q->seed_off != q0->seed_off || q->mk_off != q0->mk_off || q->ctg_off != q0->ctg_off)
+      return fail(at + "queries[d] is not the query set of context 0 (copy it with sk_sketch_set_copy)");
+    if (!same_params(q->sp, q0->sp)) return fail(at + "sketch parameters differ");
+    if (refs[d]) {
+      if (refs[d]->ctx != ctxs[d]) return fail(at + "refs[d] must be a set of ctxs[d]");
+      if (!same_params(refs[d]->sp, q0->sp)) return fail(at + "sketch parameters differ");
+      qb.G[d] = refs[d]->G;
+    }
+    if (d && (uint64_t)ref_first[d] < (uint64_t)ref_first[d - 1] + qb.G[d - 1]) return fail(at + "ref_first must be ascending and the blocks disjoint");
+    if ((uint64_t)ref_first[d] + qb.G[d] > (1ull << 32)) return fail(at + "global ref ids must fit 32 bits");
+  }
+  qb.n_refs = (uint64_t)ref_first[n_ctx - 1] + qb.G[n_ctx - 1];
+  qb.n_queries = q0->G;
+  return SK_OK;
+}
+
+// fn(d) on one host thread per context, device d current.  The calls touch only their own context's memory, so they need
+// neither peer access nor barriers; the call fails if any context failed, with the first failure's message on ctxs[0].
+int run_per_context(sk_ctx* const* ctxs, uint32_t n, const std::function<int(uint32_t)>& fn) {
+  std::vector<int> rcs(n, SK_OK);
+  auto one = [&](uint32_t d) { rcs[d] = cudaSetDevice(ctxs[d]->device) == cudaSuccess ? fn(d) : SK_ERR_CUDA; };
+  if (n == 1) one(0);
+  else {
+    std::vector<std::thread> th;
+    for (uint32_t d = 0; d < n; d++) th.emplace_back(one, d);
+    for (auto& t : th) t.join();
+  }
+  int rc = SK_OK;
+  for (uint32_t d = 0; d < n && rc == SK_OK; d++)
+    if (rcs[d] != SK_OK) { rc = rcs[d]; if (d) ctxs[0]->err = "context " + std::to_string(d) + ": " + ctxs[d]->err; }
+  cudaSetDevice(ctxs[0]->device);
+  return rc;
+}
+
+}  // namespace
+
+extern "C" int sk_screen_query_ref_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
+                                         const sk_sketch_set* const* queries, const sk_map_params* mp, int mode,
+                                         uint64_t** pairs_rq, uint64_t* n_pairs) {
+  if (!pairs_rq || !n_pairs) return SK_ERR_PARAM;
+  *pairs_rq = nullptr; *n_pairs = 0;
+  QrBlocks qb;
+  SK_TRY(check_qr_args(ctxs, n_ctx, refs, ref_first, queries, mp, qb));
+  if (mode < 0 || mode > 3) { ctxs[0]->err = "mode must be 0..3"; return SK_ERR_PARAM; }
+  std::vector<std::vector<uint64_t>> part(n_ctx);
+  SK_TRY(run_per_context(ctxs, n_ctx, [&](uint32_t d) -> int {
+    if (qb.G[d] == 0) return SK_OK;
+    uint64_t* p = nullptr; uint64_t n = 0;
+    const int rc = sk_screen_query_ref(ctxs[d], refs[d], queries[d], mp, mode, &p, &n);
+    if (rc == SK_OK) {
+      const uint64_t shift = (uint64_t)ref_first[d] << 32;     // (local ref << 32 | query) -> global ref
+      part[d].resize(n);
+      for (uint64_t i = 0; i < n; i++) part[d][i] = p[i] + shift;
+    }
+    if (p) sk_free(p);
+    return rc;
+  }));
+  // every block's list is sorted and the blocks ascend: their concatenation is sorted
+  size_t total = 0;
+  for (auto& v : part) total += v.size();
+  uint64_t* o = (uint64_t*)malloc(std::max<size_t>(total, 1) * 8);
+  if (!o) { ctxs[0]->err = "out of host memory"; return SK_ERR_NOMEM; }
+  size_t k = 0;
+  for (auto& v : part) { if (!v.empty()) memcpy(o + k, v.data(), v.size() * 8); k += v.size(); }
+  *pairs_rq = o; *n_pairs = total;
+  return SK_OK;
+}
+
+extern "C" int sk_chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
+                                    const sk_sketch_set* const* queries, const uint64_t* pairs, uint64_t n_pairs,
+                                    const sk_map_params* mp, sk_ani_result* out) {
+  QrBlocks qb;
+  SK_TRY(check_qr_args(ctxs, n_ctx, refs, ref_first, queries, mp, qb));
+  if (n_pairs && (!pairs || !out)) { ctxs[0]->err = "NULL pairs / out"; return SK_ERR_PARAM; }
+  // route every pair to the block holding its ref (pairs may come in any order)
+  std::vector<std::vector<uint64_t>> local(n_ctx);
+  std::vector<std::vector<uint64_t>> where(n_ctx);      // index of the pair in the caller's list
+  for (uint64_t i = 0; i < n_pairs; i++) {
+    const uint32_t r = (uint32_t)(pairs[i] >> 32), q = (uint32_t)pairs[i];
+    if (q >= qb.n_queries) { ctxs[0]->err = "pair " + std::to_string(i) + ": query index out of range"; return SK_ERR_PARAM; }
+    const uint32_t* it = std::upper_bound(ref_first, ref_first + n_ctx, r);
+    const uint32_t d = (uint32_t)(it - ref_first) - 1;
+    if (it == ref_first || r - ref_first[d] >= qb.G[d]) { ctxs[0]->err = "pair " + std::to_string(i) + ": ref " + std::to_string(r) + " lies in no block"; return SK_ERR_PARAM; }
+    local[d].push_back(((uint64_t)(r - ref_first[d]) << 32) | q);
+    where[d].push_back(i);
+  }
+  return run_per_context(ctxs, n_ctx, [&](uint32_t d) -> int {
+    if (local[d].empty()) return SK_OK;
+    // switch_qr's file-name tie-break (src/chain.rs:19-21) as in the one set of all refs: default ranks are global ref ids,
+    // and default query ranks follow all n_refs refs.  Applied on non-owning views; the caller's sets are not touched.
+    sk_sketch_set rv = *refs[d], qv = *queries[d];
+    if (!rv.ranks_user_set) for (uint32_t g = 0; g < rv.G; g++) rv.name_rank[g] = (uint64_t)ref_first[d] + g;
+    if (!qv.ranks_user_set) for (uint32_t g = 0; g < qv.G; g++) qv.name_rank[g] += qb.n_refs;
+    rv.ranks_user_set = qv.ranks_user_set = true;
+    std::vector<sk_ani_result> res(local[d].size());
+    const int rc = sk_chain_pairs(ctxs[d], &rv, &qv, local[d].data(), local[d].size(), mp, res.data());
+    if (rc != SK_OK) return rc;
+    for (size_t k = 0; k < res.size(); k++) { res[k].ref_id += ref_first[d]; out[where[d][k]] = res[k]; }
+    return SK_OK;
+  });
 }

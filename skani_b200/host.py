@@ -136,6 +136,12 @@ class SketchSet:
     def append(self, other):
         self.ctx.check(self.ctx.L.sk_sketch_set_append(self.h, other.h))
 
+    def copy_to(self, ctx):
+        """sk_sketch_set_copy: the same set (k-mer tables and name ranks included) on another context, which may share the device."""
+        h = C.c_void_p()
+        ctx.check(ctx.L.sk_sketch_set_copy(ctx.h, self.h, C.byref(h)))
+        return SketchSet(ctx, h, self.names)
+
     def free(self):
         if self.h and self.ctx.h:      # the set's storage lives in its context's arena
             self.ctx.L.sk_sketch_set_free(self.h)
@@ -292,6 +298,39 @@ def chain_pairs(ctx, refs, queries, pairs, mp=None, as_array=False):
     pairs = np.ascontiguousarray(pairs, np.uint64)
     out = np.zeros(max(len(pairs), 1), RESULT_DTYPE)
     ctx.check(ctx.L.sk_chain_pairs(ctx.h, refs.h, queries.h, pairs.ctypes.data, len(pairs), C.byref(mp), out.ctypes.data))
+    out = out[:len(pairs)]
+    if as_array:
+        return out
+    return [AniResult.from_buffer_copy(out[i].tobytes()) for i in range(len(pairs))]
+
+
+def _multi_args(ctxs, refs, ref_first, queries):
+    hs = (C.c_void_p * len(ctxs))(*[c.h for c in ctxs])
+    rh = (C.c_void_p * len(ctxs))(*[None if r is None else r.h for r in refs])
+    qh = (C.c_void_p * len(ctxs))(*[q.h for q in queries])
+    rf = np.ascontiguousarray(ref_first, np.uint32)
+    assert len(refs) == len(queries) == len(rf) == len(ctxs)
+    return hs, rh, rf, qh
+
+
+def screen_query_ref_multi(ctxs, refs, ref_first, queries, mp=None, mode=0):
+    """sk_screen_query_ref_multi: refs[d] (None or a set on ctxs[d]) holds the global refs [ref_first[d], ref_first[d] + len);
+    queries[d] is the query set on ctxs[d].  Same pair list as screen_query_ref on one set of all refs."""
+    mp = mp or map_params()
+    hs, rh, rf, qh = _multi_args(ctxs, refs, ref_first, queries)
+    c0 = ctxs[0]
+    return _pairs_out(c0, c0.L.sk_screen_query_ref_multi, hs, len(ctxs), rh, rf.ctypes.data, qh, C.byref(mp), mode)
+
+
+def chain_pairs_multi(ctxs, refs, ref_first, queries, pairs, mp=None, as_array=False):
+    """sk_chain_pairs_multi: global (ref << 32 | query) pairs in any order, each chained on the context holding its ref.
+    Same results as chain_pairs on one set of all refs, ref_id global."""
+    mp = mp or map_params()
+    hs, rh, rf, qh = _multi_args(ctxs, refs, ref_first, queries)
+    pairs = np.ascontiguousarray(pairs, np.uint64)
+    out = np.zeros(max(len(pairs), 1), RESULT_DTYPE)
+    c0 = ctxs[0]
+    c0.check(c0.L.sk_chain_pairs_multi(hs, len(ctxs), rh, rf.ctypes.data, qh, pairs.ctypes.data, len(pairs), C.byref(mp), out.ctypes.data))
     out = out[:len(pairs)]
     if as_array:
         return out
