@@ -62,6 +62,8 @@ typedef struct {
 
 /* ---- context ------------------------------------------------------------------------------- */
 int sk_device_count(void);   /* usable CUDA devices (0 = none: nothing in this library can run) */
+/* free and total memory of a device in bytes (cudaMemGetInfo), e.g. to decide whether a triangle's sketches fit it */
+int sk_device_memory(int device, uint64_t* free_bytes, uint64_t* total_bytes);
 int sk_ctx_create(int device, sk_ctx** out);
 int sk_ctx_destroy(sk_ctx* ctx);
 const char* sk_last_error(const sk_ctx* ctx);
@@ -295,6 +297,48 @@ int sk_screen_query_ref_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sket
 int sk_chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
                          const sk_sketch_set* const* queries, const uint64_t* pairs, uint64_t n_pairs,
                          const sk_map_params* mp, sk_ani_result* out);
+
+/* ---- triangle beyond one GPU's memory: sketches live in pinned HOST memory and come back to the device in working sets --
+ * A store holds sketches with their k-mer tables, genome-indexed, in fixed-size pinned, device-mapped host slabs.
+ * sk_sketch_store_add     : appends set's genomes (ids continue after the store's; name ranks continue after its largest
+ *                           rank, as sk_sketch_set_append does).  Different sketch parameters give SK_ERR_PARAM.  The caller
+ *                           may free the set afterwards: device memory then holds one batch of sketches at a time.
+ * sk_sketch_store_genome_bytes : device bytes genome g takes in a working set (records, k-mer groups, markers, contig
+ *                           tables and its k-mer hash table).
+ * sk_sketch_store_set_name_ranks : file-name order of every genome (switch_qr tie-break, see sk_sketch_set_set_name_ranks).
+ * sk_sketch_store_gather  : a device set on ctx holding genomes[0..n) in list order (ascending, no duplicates, < n_genomes;
+ *                           anything else gives SK_ERR_PARAM), with the store's name ranks.  One batched copy pulls the
+ *                           genomes' slices from the mapped host slabs over PCIe; the k-mer tables come along (genomes of
+ *                           2^20 or more records carry none and get the bucket index rebuilt, as sk_sketch_set_unpack does).
+ *                           flags = SK_PACK_MARKERS_ONLY gathers the markers only (enough for sk_screen_*).  A gathered set
+ *                           chains, screens and exports exactly like the set that was added. */
+typedef struct sk_sketch_store sk_sketch_store;
+int sk_sketch_store_create(const sk_sketch_params* sp, sk_sketch_store** out);
+int sk_sketch_store_add(sk_sketch_store* st, const sk_sketch_set* set);
+uint32_t sk_sketch_store_n_genomes(const sk_sketch_store* st);
+uint64_t sk_sketch_store_genome_bytes(const sk_sketch_store* st, uint32_t g);
+int sk_sketch_store_set_name_ranks(sk_sketch_store* st, const uint64_t* ranks /* n_genomes */);
+int sk_sketch_store_gather(sk_ctx* ctx, const sk_sketch_store* st, const uint32_t* genomes, uint32_t n, int flags,
+                           sk_sketch_set** out);
+int sk_sketch_store_free(sk_sketch_store* st);
+
+/* sk_triangle_store: the triangle (src/triangle.rs:71-105) of every genome of a store.  The markers of all genomes are gathered
+ * on ctxs[0] and screened (sk_screen_triangle); the pairs are planned into working sets whose genomes fit device_budget bytes
+ * (per context; 0 = derived from the free device memory) -- components of the pair graph packed first-fit decreasing, a
+ * component over budget cut into chunks of budget / 2 and chained chunk pair by chunk pair -- and the contexts take the
+ * working sets in plan order: gather, sk_chain_pairs, keep ani > 0.1.  Two contexts on one device overlap one's gather with
+ * the other's chaining.  Results (malloc'd, sk_free) are sorted by (ref_id, query_id) and equal sk_triangle's on the same
+ * genomes and name ranks.  A genome over budget / 2 gives SK_ERR_NOMEM before any device work.  If any context fails the
+ * call fails and sk_last_error(ctxs[0]) carries that context's message.  SK_TRACE=1 prints one line per working set.
+ * stats (optional): t_screen = marker gather + screen; t_gather / t_chain = seconds spent gathering / chaining working sets,
+ * summed over contexts; gathered_bytes = working-set bytes pulled from the store. */
+typedef struct {
+  uint32_t n_working_sets, n_split_components;
+  uint64_t gathered_bytes, max_working_set_bytes;
+  double t_screen, t_gather, t_chain;
+} sk_store_stats;
+int sk_triangle_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp,
+                      uint64_t device_budget, sk_ani_result** out, uint64_t* n_out, sk_store_stats* stats);
 
 #ifdef __cplusplus
 }

@@ -38,11 +38,17 @@ class TriangleStats(C.Structure):
                 ("n_pairs_screened", C.c_uint64), ("n_pairs_kept", C.c_uint64)]
 
 
+class StoreStats(C.Structure):
+    _fields_ = [("n_working_sets", C.c_uint32), ("n_split_components", C.c_uint32), ("gathered_bytes", C.c_uint64),
+                ("max_working_set_bytes", C.c_uint64), ("t_screen", C.c_double), ("t_gather", C.c_double), ("t_chain", C.c_double)]
+
+
 # every symbol include/skani_b200.h declares: (name, restype, argtypes)
 vp, u64, u32, i32 = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int
 PP = C.POINTER
 SYMBOLS = [
     ("sk_device_count", i32, []),
+    ("sk_device_memory", i32, [i32, PP(u64), PP(u64)]),
     ("sk_ctx_create", i32, [i32, PP(vp)]),
     ("sk_ctx_destroy", i32, [vp]),
     ("sk_ctx_set_seeding_semantics", i32, [vp, i32]),
@@ -90,6 +96,14 @@ SYMBOLS = [
     ("sk_sketch_set_copy", i32, [vp, vp, PP(vp)]),
     ("sk_screen_query_ref_multi", i32, [vp, u32, vp, vp, vp, PP(MapParams), i32, PP(PP(u64)), PP(u64)]),
     ("sk_chain_pairs_multi", i32, [vp, u32, vp, vp, vp, vp, u64, PP(MapParams), vp]),
+    ("sk_sketch_store_create", i32, [PP(SketchParams), PP(vp)]),
+    ("sk_sketch_store_add", i32, [vp, vp]),
+    ("sk_sketch_store_n_genomes", u32, [vp]),
+    ("sk_sketch_store_genome_bytes", u64, [vp, u32]),
+    ("sk_sketch_store_set_name_ranks", i32, [vp, vp]),
+    ("sk_sketch_store_gather", i32, [vp, vp, vp, u32, i32, PP(vp)]),
+    ("sk_sketch_store_free", i32, [vp]),
+    ("sk_triangle_store", i32, [vp, u32, vp, PP(MapParams), u64, PP(PP(AniResult)), PP(u64), PP(StoreStats)]),
 ]
 
 _lib = None

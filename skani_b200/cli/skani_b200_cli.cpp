@@ -325,12 +325,96 @@ std::vector<size_t> split_balanced(const std::vector<uint64_t>& w, size_t W) {
   return b;
 }
 
+// sorted files [f0, end) form the next group that goes through the GPU at once: at most 4096 files and about 8 GiB of
+// sequence (file sizes x 4, as gz inflates ~4x), at least one file
+size_t file_group_end(const std::vector<std::string>& files, size_t f0) {
+  size_t f1 = f0;
+  uint64_t bytes = 0;
+  while (f1 < files.size() && (f1 == f0 || (f1 - f0 < 4096 && bytes < (8ull << 30)))) {
+    struct stat st;
+    bytes += stat(files[f1].c_str(), &st) == 0 ? (uint64_t)st.st_size * 4 : 0;
+    f1++;
+  }
+  return f1;
+}
+
+// triangle: whether the sketches are expected to exceed the device (the estimate of sk_triangle's memory guard: 56 B per
+// seed, 24 B per marker and 6 GB of workspace against 92 % of the device, from the file sizes, x 4 for .gz; .sketch files
+// about triple on the device) or SK_DEVICE_BUDGET_MB asks for the store path.  --gpus N with FASTA inputs keeps
+// sk_triangle_multi.
+bool triangle_needs_store(const Opts& op, bool sketches, double* need_gb) {
+  *need_gb = 0;
+  if (op.gpus > 1 && !sketches) return false;
+  uint64_t bytes = 0;
+  for (auto& f : op.files) {
+    struct stat st;
+    if (stat(f.c_str(), &st) != 0) continue;
+    const bool gz = f.size() > 3 && f.compare(f.size() - 3, 3, ".gz") == 0;
+    bytes += (uint64_t)st.st_size * (gz ? 4 : 1);
+  }
+  const double need = sketches ? 3.0 * bytes + 6.0e9 : (double)bytes / op.c * 56.0 + (double)bytes / op.m * 24.0 + 6.0e9;
+  *need_gb = need / 1e9;
+  if (getenv("SK_DEVICE_BUDGET_MB")) return true;
+  uint64_t free_b = 0, total_b = 0;
+  if (sk_device_memory(op.device, &free_b, &total_b) != 0) return false;
+  return need > 0.92 * (double)total_b;
+}
+
+// The store path of triangle: files are sketched (or .sketch files imported) in groups, each group's set is added to a host
+// sketch store and freed, so device memory holds one group at a time and host memory one group of sequence plus the
+// sketches.  genomes gets the metadata of every genome in store order (= the order of the in-memory path).
+sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, bool sketches, std::vector<Genome>& genomes, sk_sketch_params& sp) {
+  if (sketches) {
+    fprintf(stderr, "INFO Sketches detected.\n");
+    skdb::DiskParams dp;
+    std::vector<skdb::HostSketch> hs;
+    read_sketch_files(op.files, dp, genomes, hs);
+    if (hs.empty()) return nullptr;
+    if (dp.c != op.c || dp.marker_c != op.m)
+      fprintf(stderr, "WARN Input parameter c = %u, m = %u is not equal to the sketch parameter c = %llu,m = %llu. Using sketch parameters.\n", op.c, op.m,
+              (unsigned long long)dp.c, (unsigned long long)dp.marker_c);
+    sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
+    sk_sketch_store* st = nullptr;
+    CK(ctx, sk_sketch_store_create(&sp, &st));
+    for (size_t a = 0; a < hs.size();) {      // import groups of < 2^28 records
+      size_t b = a;
+      uint64_t recs = 0;
+      while (b < hs.size() && (b == a || recs + hs[b].kmer.size() < (1ull << 28))) recs += hs[b++].kmer.size();
+      sk_sketch_set* set = import_sketches(ctx, hs, a, b, sp);
+      CK(ctx, sk_sketch_store_add(st, set));
+      sk_sketch_set_free(set);
+      for (size_t i = a; i < b; i++) hs[i] = skdb::HostSketch();
+      a = b;
+    }
+    return st;
+  }
+  sk_sketch_store* st = nullptr;
+  CK(ctx, sk_sketch_store_create(&sp, &st));
+  std::vector<std::string> files = op.files;
+  std::sort(files.begin(), files.end());
+  for (size_t f0 = 0; f0 < files.size();) {
+    const size_t f1 = file_group_end(files, f0);
+    Inputs in;
+    load_inputs(std::vector<std::string>(files.begin() + f0, files.begin() + f1), op.individual, std::max(op.threads, 1), in);
+    f0 = f1;
+    if (in.genomes.empty()) continue;
+    sk_sketch_set* set = sketch(ctx, in, sp);
+    CK(ctx, sk_sketch_store_add(st, set));
+    sk_sketch_set_free(set);
+    for (auto& g : in.genomes) genomes.push_back(std::move(g));
+  }
+  if (genomes.empty()) { sk_sketch_store_free(st); return nullptr; }
+  return st;
+}
+
 int run_triangle(Opts& op) {
   resolve_presets(op);
   if (op.files.empty()) { fprintf(stderr, "ERROR No reference inputs found.\n"); return 1; }
   Inputs in;
   const bool refs_are_sketch = all_sketch_files(op.files);
-  if (!refs_are_sketch) {
+  double need_gb = 0;
+  const bool use_store = triangle_needs_store(op, refs_are_sketch, &need_gb);
+  if (!refs_are_sketch && !use_store) {
     load_inputs(op.files, op.individual, std::max(op.threads, 1), in);
     if (in.genomes.empty()) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }   // src/triangle.rs:46-49
   }
@@ -338,7 +422,13 @@ int run_triangle(Opts& op) {
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
   sk_sketch_params sp{op.c, op.k, op.m};
   sk_sketch_set* loaded = nullptr;
-  if (refs_are_sketch) {      // src/triangle.rs:16-24
+  sk_sketch_store* store = nullptr;
+  if (use_store) {
+    fprintf(stderr, "INFO Store path: sketches (~%.1f GB estimated) are kept in a host sketch store and chained in working sets on GPU %d%s.\n", need_gb,
+            op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
+    store = fill_store(ctx, op, refs_are_sketch, in.genomes, sp);
+    if (!store) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }
+  } else if (refs_are_sketch) {      // src/triangle.rs:16-24
     fprintf(stderr, "INFO Sketches detected.\n");
     skdb::DiskParams dp;
     loaded = load_sketch_files(ctx, op.files, dp, in.genomes);
@@ -368,7 +458,22 @@ int run_triangle(Opts& op) {
   }
   std::vector<sk_ani_result> res;
   sk_sketch_set* set = nullptr;
-  if (op.gpus > 1 && !loaded) {
+  if (store) {
+    // two contexts on the device: one gathers its next working set over PCIe while the other chains; every row is written at
+    // the end (no intermediate "Writing results" flushes in sparse mode)
+    CK(ctx, sk_sketch_store_set_name_ranks(store, ranks.data()));
+    sk_ctx* ctx2 = nullptr;
+    if (sk_ctx_create(op.device, &ctx2) != 0) { fprintf(stderr, "ERROR cannot create a second context on GPU %d\n", op.device); return 1; }
+    sk_ctx* ctxs[2] = {ctx, ctx2};
+    uint64_t budget = 0;
+    if (const char* e = getenv("SK_DEVICE_BUDGET_MB")) budget = (uint64_t)std::max(1ll, atoll(e)) << 20;
+    sk_ani_result* r = nullptr; uint64_t nr = 0;
+    CK(ctx, sk_triangle_store(ctxs, 2, store, &mp, budget, &r, &nr, nullptr));
+    res.assign(r, r + nr);                  // sorted by (ref_id, query_id)
+    sk_free(r);
+    sk_ctx_destroy(ctx2);
+    sk_sketch_store_free(store);
+  } else if (op.gpus > 1 && !loaded) {
     // --gpus N: one context per GPU, genome blocks + marker exchange + cross-block slices (sk_triangle_multi).  With fewer
     // physical devices than N the contexts share devices (same code path; the exchange then stays on the device).
     std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, op.gpus);
@@ -618,13 +723,7 @@ int run_sketch(Opts& op) {
   size_t total = 0;
   // files go through the GPU in groups (bounds the host copy of the sequences); database order = (file_name, contig_order)
   for (size_t f0 = 0; f0 < files.size();) {
-    size_t f1 = f0;
-    uint64_t bytes = 0;
-    while (f1 < files.size() && (f1 == f0 || (f1 - f0 < 4096 && bytes < (8ull << 30)))) {
-      struct stat st;
-      bytes += stat(files[f1].c_str(), &st) == 0 ? (uint64_t)st.st_size * 4 : 0;   // gz inflates ~4x
-      f1++;
-    }
+    const size_t f1 = file_group_end(files, f0);
     Inputs in;
     load_inputs(std::vector<std::string>(files.begin() + f0, files.begin() + f1), op.individual, std::max(op.threads, 1), in);
     f0 = f1;

@@ -354,6 +354,18 @@ int sk_device_count(void) {
   return n;
 }
 
+int sk_device_memory(int device, uint64_t* free_bytes, uint64_t* total_bytes) {
+  if (!free_bytes || !total_bytes || device < 0 || device >= sk_device_count()) return SK_ERR_PARAM;
+  int prev = 0;
+  size_t f = 0, t = 0;
+  if (cudaGetDevice(&prev) != cudaSuccess || cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return SK_ERR_CUDA; }
+  const cudaError_t e = cudaMemGetInfo(&f, &t);
+  cudaSetDevice(prev);
+  if (e != cudaSuccess) { cudaGetLastError(); return SK_ERR_CUDA; }
+  *free_bytes = f; *total_bytes = t;
+  return SK_OK;
+}
+
 int sk_ctx_set_seeding_semantics(sk_ctx* ctx, int semantics) {
   if (!ctx || (semantics != SK_SEED_AVX2 && semantics != SK_SEED_SCALAR)) return SK_ERR_PARAM;
   ctx->seed_scalar = semantics == SK_SEED_SCALAR;
@@ -471,23 +483,6 @@ int sk_sketch_set_append(sk_sketch_set* dst, const sk_sketch_set* src) {
 }
 
 namespace {
-constexpr int BLOB_ARRAYS = 12;     // 11 set arrays + the k-mer hash tables (present only with SK_PACK_TABLES)
-constexpr int META_HEADER = 10;     // G S U M C c k marker_c HT flags
-struct BlobLayout {
-  size_t off[BLOB_ARRAYS];
-  size_t bytes[BLOB_ARRAYS];
-  size_t total;
-};
-inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
-BlobLayout blob_layout(size_t G, size_t S, size_t U, size_t M, size_t Cn, size_t HT = 0) {
-  BlobLayout b;
-  const size_t n[BLOB_ARRAYS] = {S * 4, S * 4, S * 4, S * 2, S * 4, S * 4, U * 4, (U + G) * 4, M * 8, (Cn + G) * 4, Cn * 4, HT * 8};
-  size_t o = 0;
-  for (int i = 0; i < BLOB_ARRAYS; i++) { b.off[i] = o; b.bytes[i] = n[i]; o += al256(n[i]); }
-  b.total = o ? o : 256;
-  return b;
-}
-inline uint64_t meta_words(uint64_t G, uint64_t C, bool tables) { return META_HEADER + 4 * (G + 1) + G + C + (tables ? G + 1 : 0); }
 inline const void* set_array(const sk_sketch_set* s, int i) {
   const void* p[BLOB_ARRAYS] = {s->pv_kmer, s->pv_pos, s->pv_cc, s->pv_mult, s->kv_pos, s->kv_cc, s->ukmer, s->ustart, s->markers, s->ctg_rec_off,
                                  s->d_ctg_len, s->htab};

@@ -223,6 +223,27 @@ int tri_screen_create(sk_ctx* ctx, size_t marker_hint, TriScreen** out);
 int tri_screen_add(TriScreen* ts, const sk_sketch_set* set, uint32_t g_end, uint32_t row_begin, const sk_map_params* mp, uint64_t** pairs, uint64_t* n);
 void tri_screen_free(TriScreen* ts);
 bool tri_screen_supports(uint32_t n_genomes, uint64_t n_markers);
+// sketch-set blob (sk_sketch_set_pack / pack_subset / unpack, and the host sketch store of store.cu): 12 arrays, each
+// 256-byte aligned, in the order pv_kmer pv_pos pv_cc pv_mult kv_pos kv_cc ukmer ustart markers ctg_rec_off d_ctg_len htab
+// (the k-mer hash tables are present only with SK_PACK_TABLES); host metadata = META_HEADER words G S U M C c k marker_c HT
+// flags, then seed_off uk_off mk_off ctg_off [G+1 each], total_len [G], contig lengths [C] and, with tables, ht_off [G+1]
+constexpr int BLOB_ARRAYS = 12;
+constexpr int META_HEADER = 10;
+struct BlobLayout {
+  size_t off[BLOB_ARRAYS];
+  size_t bytes[BLOB_ARRAYS];
+  size_t total;
+};
+inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
+inline BlobLayout blob_layout(size_t G, size_t S, size_t U, size_t M, size_t Cn, size_t HT = 0) {
+  BlobLayout b;
+  const size_t n[BLOB_ARRAYS] = {S * 4, S * 4, S * 4, S * 2, S * 4, S * 4, U * 4, (U + G) * 4, M * 8, (Cn + G) * 4, Cn * 4, HT * 8};
+  size_t o = 0;
+  for (int i = 0; i < BLOB_ARRAYS; i++) { b.off[i] = o; b.bytes[i] = n[i]; o += al256(n[i]); }
+  b.total = o ? o : 256;
+  return b;
+}
+inline uint64_t meta_words(uint64_t G, uint64_t C, bool tables) { return META_HEADER + 4 * (G + 1) + G + C + (tables ? G + 1 : 0); }
 // screen.cu / chain.cu
 uint64_t count_launch(sk_ctx* ctx, uint64_t n = 1);
 cudaError_t h2d_small(sk_ctx* ctx, void* dst, const void* src, size_t bytes);  // api.cu

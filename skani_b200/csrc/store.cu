@@ -1,0 +1,398 @@
+// store.cu -- the triangle beyond one GPU's memory: a host-resident sketch store and working-set chaining.
+//
+// sk_sketch_store keeps every genome's sketch (the 12 blob arrays of sk_internal.h, k-mer hash table included) as one
+// contiguous record in pinned, device-mapped host slabs of a fixed size.  Adding a set packs it into a device blob with its
+// tables and scatters the blob's per-genome slices into their records with ONE batched device memcpy whose destinations are
+// mapped host memory.  Gathering is the mirror image: ONE batched memcpy whose sources are the records of the listed genomes
+// pulls them over PCIe straight into a device blob in the layout sk_sketch_set_unpack reads (no host-side copy, no staging
+// buffer), and the existing unpack builds the set without rebuilding the tables.
+// sk_triangle_store screens the markers of every genome, plans working sets (ws_plan.hpp) and lets one host thread per
+// context gather and chain them in plan order.
+#include <cub/cub.cuh>
+
+#include <algorithm>
+#include <atomic>
+#include <chrono>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <thread>
+#include <vector>
+
+#include "sk_internal.h"
+#include "ws_plan.hpp"
+
+using namespace sk;
+
+struct sk_sketch_store {
+  sk_sketch_params sp{};
+  struct Slab { uint8_t* host = nullptr; uint8_t* dev = nullptr; size_t size = 0, used = 0; };
+  std::vector<Slab> slabs;
+  size_t slab_bytes = 1ull << 30;
+  struct Genome {
+    uint32_t slab = 0;
+    uint64_t off = 0;                   // record offset inside the slab
+    uint64_t S = 0, U = 0, M = 0, C = 0, HT = 0, total_len = 0;
+    uint64_t ctg0 = 0;                  // first contig length in ctg_len
+    uint64_t slice[BLOB_ARRAYS] = {};   // slice offsets inside the record
+  };
+  std::vector<Genome> g;
+  std::vector<uint32_t> ctg_len;
+  std::vector<uint64_t> name_rank;
+};
+
+namespace {
+
+double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+// element counts of a genome's 12 arrays (one sentinel per genome in the k-mer group starts and contig record tables)
+void genome_counts(const sk_sketch_store::Genome& e, uint64_t n[BLOB_ARRAYS]) {
+  const uint64_t v[BLOB_ARRAYS] = {e.S, e.S, e.S, e.S, e.S, e.S, e.U, e.U + 1, e.M, e.C + 1, e.C, e.HT};
+  for (int a = 0; a < BLOB_ARRAYS; a++) n[a] = v[a];
+}
+constexpr uint64_t ESZ[BLOB_ARRAYS] = {4, 4, 4, 2, 4, 4, 4, 4, 8, 4, 4, 8};
+
+// one cub::DeviceMemcpy::Batched on ctx->stream (sources and destinations may be device or mapped host memory), synchronised
+int batched_copy(sk_ctx* ctx, const std::vector<const void*>& src, const std::vector<void*>& dst, const std::vector<size_t>& n) {
+  const size_t ns = n.size();
+  if (ns == 0) return SK_OK;
+  if (ns >= (1ull << 32)) { ctx->err = "too many copy segments"; return SK_ERR_PARAM; }
+  cudaStream_t st = ctx->stream;
+  DTmp<const void*> d_src; DTmp<void*> d_dst; DTmp<size_t> d_n;
+  SK_CUDA(d_src.alloc(ns, ctx)); SK_CUDA(d_dst.alloc(ns, ctx)); SK_CUDA(d_n.alloc(ns, ctx));
+  SK_CUDA(cudaMemcpyAsync(d_src.p, src.data(), ns * sizeof(void*), cudaMemcpyHostToDevice, st));
+  SK_CUDA(cudaMemcpyAsync(d_dst.p, dst.data(), ns * sizeof(void*), cudaMemcpyHostToDevice, st));
+  SK_CUDA(cudaMemcpyAsync(d_n.p, n.data(), ns * sizeof(size_t), cudaMemcpyHostToDevice, st));
+  size_t tb = 0;
+  SK_CUDA(cub::DeviceMemcpy::Batched(nullptr, tb, d_src.p, d_dst.p, d_n.p, (uint32_t)ns, st));
+  DTmp<uint8_t> tmp;
+  SK_CUDA(tmp.alloc(tb, ctx));
+  SK_CUDA(cub::DeviceMemcpy::Batched(tmp.p, tb, d_src.p, d_dst.p, d_n.p, (uint32_t)ns, st));
+  count_launch(ctx);
+  SK_CUDA(cudaStreamSynchronize(st));   // the host-side lists and the temporaries are released on return
+  return SK_OK;
+}
+
+bool same_params(const sk_sketch_params& a, const sk_sketch_params& b) { return a.c == b.c && a.k == b.k && a.marker_c == b.marker_c; }
+
+}  // namespace
+
+extern "C" {
+
+int sk_sketch_store_create(const sk_sketch_params* sp, sk_sketch_store** out) {
+  if (!sp || !out) return SK_ERR_PARAM;
+  sk_sketch_store* st = new sk_sketch_store();
+  st->sp = *sp;
+  if (const char* e = getenv("SK_STORE_SLAB_MB")) st->slab_bytes = std::max<size_t>(1, (size_t)atoll(e)) << 20;   // test hook: many slabs
+  *out = st;
+  return SK_OK;
+}
+
+int sk_sketch_store_free(sk_sketch_store* st) {
+  if (!st) return SK_OK;
+  for (auto& s : st->slabs) cudaFreeHost(s.host);
+  delete st;
+  return SK_OK;
+}
+
+uint32_t sk_sketch_store_n_genomes(const sk_sketch_store* st) { return st ? (uint32_t)st->g.size() : 0; }
+
+uint64_t sk_sketch_store_genome_bytes(const sk_sketch_store* st, uint32_t g) {
+  if (!st || g >= st->g.size()) return 0;
+  uint64_t n[BLOB_ARRAYS], b = 0;
+  genome_counts(st->g[g], n);
+  for (int a = 0; a < BLOB_ARRAYS; a++) b += n[a] * ESZ[a];
+  return b;
+}
+
+int sk_sketch_store_set_name_ranks(sk_sketch_store* st, const uint64_t* ranks) {
+  if (!st || (!ranks && !st->g.empty())) return SK_ERR_PARAM;
+  for (size_t g = 0; g < st->g.size(); g++) st->name_rank[g] = ranks[g];
+  return SK_OK;
+}
+
+int sk_sketch_store_add(sk_sketch_store* st, const sk_sketch_set* set) {
+  if (!st || !set) return SK_ERR_PARAM;
+  sk_ctx* ctx = set->ctx;
+  if (!same_params(set->sp, st->sp)) { ctx->err = "sk_sketch_store_add: the set's sketch parameters differ from the store's"; return SK_ERR_PARAM; }
+  if ((uint64_t)st->g.size() + set->G >= (1ull << 32)) { ctx->err = "sk_sketch_store_add: more than 2^32 genomes"; return SK_ERR_PARAM; }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  if (set->G == 0) return SK_OK;
+  // the set's own blob with its k-mer tables
+  uint64_t bytes = 0, words = 0;
+  SK_TRY(sk_sketch_set_subset_blob_size(set, nullptr, 0, SK_PACK_TABLES, &bytes, &words));
+  DTmp<uint8_t> blob;
+  if (blob.alloc(bytes, ctx) != cudaSuccess) { ctx->err = "sk_sketch_store_add: out of device memory for the blob"; return SK_ERR_NOMEM; }
+  std::vector<uint64_t> meta(words);
+  SK_TRY(sk_sketch_set_pack_subset(set, nullptr, 0, SK_PACK_TABLES, blob.p, meta.data()));
+  const uint64_t* m = meta.data();
+  const uint32_t G = (uint32_t)m[0];
+  const uint64_t HT = m[8];
+  const bool tables = m[9] != 0;
+  const BlobLayout b = blob_layout(G, m[1], m[2], m[3], m[4], HT);
+  const uint64_t *seed_off = m + META_HEADER, *uk_off = seed_off + G + 1, *mk_off = uk_off + G + 1, *ctg_off = mk_off + G + 1;
+  const uint64_t* total_len = ctg_off + G + 1;
+  const uint64_t* clen = total_len + G;
+  const uint64_t* ht_off = tables ? clen + m[4] : nullptr;
+  // records in the slabs (host-side bookkeeping first, so that a failed slab allocation leaves the store unchanged)
+  std::vector<sk_sketch_store::Genome> add(G);
+  std::vector<sk_sketch_store::Slab> new_slabs;
+  auto slab_at = [&](uint32_t i) -> sk_sketch_store::Slab& { return i < st->slabs.size() ? st->slabs[i] : new_slabs[i - st->slabs.size()]; };
+  uint32_t cur = st->slabs.empty() ? 0 : (uint32_t)st->slabs.size() - 1;
+  std::vector<size_t> used;
+  for (auto& s : st->slabs) used.push_back(s.used);
+  auto fail_slabs = [&](int rc) { for (auto& s : new_slabs) cudaFreeHost(s.host); return rc; };
+  for (uint32_t i = 0; i < G; i++) {
+    sk_sketch_store::Genome& e = add[i];
+    e.S = seed_off[i + 1] - seed_off[i]; e.U = uk_off[i + 1] - uk_off[i]; e.M = mk_off[i + 1] - mk_off[i]; e.C = ctg_off[i + 1] - ctg_off[i];
+    e.HT = tables ? ht_off[i + 1] - ht_off[i] : 0;
+    e.total_len = total_len[i];
+    uint64_t n[BLOB_ARRAYS], o = 0;
+    genome_counts(e, n);
+    for (int a = 0; a < BLOB_ARRAYS; a++) { e.slice[a] = o; o += (n[a] * ESZ[a] + 15) & ~15ull; }
+    const size_t need = std::max<uint64_t>(al256(o), 256);
+    const uint32_t n_slabs = (uint32_t)(st->slabs.size() + new_slabs.size());
+    if (n_slabs == 0 || used[cur] + need > slab_at(cur).size) {
+      sk_sketch_store::Slab s;
+      s.size = std::max(st->slab_bytes, need);
+      cudaError_t err = cudaHostAlloc((void**)&s.host, s.size, cudaHostAllocMapped | cudaHostAllocPortable);
+      if (err == cudaSuccess) err = cudaHostGetDevicePointer((void**)&s.dev, s.host, 0);
+      if (err != cudaSuccess) {
+        cudaGetLastError();
+        if (s.host) cudaFreeHost(s.host);
+        ctx->err = "sk_sketch_store_add: cannot allocate " + std::to_string(s.size >> 20) + " MiB of pinned host memory: " + cudaGetErrorString(err);
+        return fail_slabs(SK_ERR_NOMEM);
+      }
+      new_slabs.push_back(s);
+      used.push_back(0);
+      cur = n_slabs;
+    }
+    e.slab = cur; e.off = used[cur];
+    used[cur] += need;
+  }
+  // one batched copy: blob slices -> records in mapped host memory
+  std::vector<const void*> src;
+  std::vector<void*> dst;
+  std::vector<size_t> nb;
+  for (uint32_t i = 0; i < G; i++) {
+    const sk_sketch_store::Genome& e = add[i];
+    const uint64_t first[BLOB_ARRAYS] = {seed_off[i], seed_off[i], seed_off[i], seed_off[i], seed_off[i], seed_off[i], uk_off[i], uk_off[i] + i,
+                                         mk_off[i], ctg_off[i] + i, ctg_off[i], tables ? ht_off[i] : 0};
+    uint64_t n[BLOB_ARRAYS];
+    genome_counts(e, n);
+    for (int a = 0; a < BLOB_ARRAYS; a++) {
+      if (n[a] == 0) continue;
+      src.push_back(blob.p + b.off[a] + first[a] * ESZ[a]);
+      dst.push_back(slab_at(e.slab).dev + e.off + e.slice[a]);
+      nb.push_back(n[a] * ESZ[a]);
+    }
+  }
+  const int rc = batched_copy(ctx, src, dst, nb);
+  if (rc != SK_OK) return fail_slabs(rc);
+  // commit
+  for (auto& s : new_slabs) st->slabs.push_back(s);
+  for (size_t i = 0; i < st->slabs.size(); i++) st->slabs[i].used = used[i];
+  uint64_t mx = 0;
+  for (uint64_t r : st->name_rank) mx = std::max(mx, r + 1);
+  for (uint32_t i = 0; i < G; i++) {
+    add[i].ctg0 = st->ctg_len.size();
+    for (uint64_t c = ctg_off[i]; c < ctg_off[i + 1]; c++) st->ctg_len.push_back((uint32_t)clen[c]);
+    st->g.push_back(add[i]);
+    st->name_rank.push_back(mx + set->name_rank[i]);
+  }
+  return SK_OK;
+}
+
+int sk_sketch_store_gather(sk_ctx* ctx, const sk_sketch_store* st, const uint32_t* genomes, uint32_t n, int flags, sk_sketch_set** out) {
+  if (!ctx || !out) return SK_ERR_PARAM;
+  *out = nullptr;
+  if (!st || (n && !genomes)) { ctx->err = "sk_sketch_store_gather: NULL store or genome list"; return SK_ERR_PARAM; }
+  if (flags != 0 && flags != SK_PACK_MARKERS_ONLY) { ctx->err = "sk_sketch_store_gather: flags must be 0 or SK_PACK_MARKERS_ONLY"; return SK_ERR_PARAM; }
+  for (uint32_t i = 0; i < n; i++) {
+    if (genomes[i] >= st->g.size()) { ctx->err = "sk_sketch_store_gather: genome " + std::to_string(genomes[i]) + " out of range"; return SK_ERR_PARAM; }
+    if (i && genomes[i] <= genomes[i - 1]) { ctx->err = "sk_sketch_store_gather: genomes must be ascending without duplicates"; return SK_ERR_PARAM; }
+  }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  const bool mo = flags == SK_PACK_MARKERS_ONLY;
+  // output offsets (the subset plan of sk_sketch_set_pack_subset, over the store's records)
+  std::vector<uint64_t> seed_off(n + 1, 0), uk_off(n + 1, 0), mk_off(n + 1, 0), ctg_off(n + 1, 0), ht_off(n + 1, 0);
+  for (uint32_t i = 0; i < n; i++) {
+    const sk_sketch_store::Genome& e = st->g[genomes[i]];
+    seed_off[i + 1] = seed_off[i] + (mo ? 0 : e.S);
+    uk_off[i + 1] = uk_off[i] + (mo ? 0 : e.U);
+    ctg_off[i + 1] = ctg_off[i] + (mo ? 0 : e.C);
+    ht_off[i + 1] = ht_off[i] + (mo ? 0 : e.HT);
+    mk_off[i + 1] = mk_off[i] + e.M;
+  }
+  const bool tables = !mo;
+  const BlobLayout b = blob_layout(n, seed_off[n], uk_off[n], mk_off[n], ctg_off[n], ht_off[n]);
+  DTmp<uint8_t> blob;
+  if (blob.alloc(b.total, ctx) != cudaSuccess) { ctx->err = "sk_sketch_store_gather: out of device memory (" + std::to_string(b.total >> 20) + " MiB blob)"; return SK_ERR_NOMEM; }
+  if (mo && n) {   // one zero sentinel per genome in the group-start and contig-record tables
+    SK_CUDA(cudaMemsetAsync(blob.p + b.off[7], 0, (size_t)n * 4, ctx->stream));
+    SK_CUDA(cudaMemsetAsync(blob.p + b.off[9], 0, (size_t)n * 4, ctx->stream));
+  }
+  std::vector<const void*> src;
+  std::vector<void*> dst;
+  std::vector<size_t> nb;
+  for (uint32_t i = 0; i < n; i++) {
+    const sk_sketch_store::Genome& e = st->g[genomes[i]];
+    const uint8_t* rec = st->slabs[e.slab].dev + e.off;
+    const uint64_t first[BLOB_ARRAYS] = {seed_off[i], seed_off[i], seed_off[i], seed_off[i], seed_off[i], seed_off[i], uk_off[i], uk_off[i] + i,
+                                         mk_off[i], ctg_off[i] + i, ctg_off[i], ht_off[i]};
+    uint64_t cnt[BLOB_ARRAYS];
+    genome_counts(e, cnt);
+    for (int a = 0; a < BLOB_ARRAYS; a++) {
+      if (cnt[a] == 0 || (mo && a != 8)) continue;
+      src.push_back(rec + e.slice[a]);
+      dst.push_back(blob.p + b.off[a] + first[a] * ESZ[a]);
+      nb.push_back(cnt[a] * ESZ[a]);
+    }
+  }
+  SK_TRY(batched_copy(ctx, src, dst, nb));
+  if (mo && n) SK_CUDA(cudaStreamSynchronize(ctx->stream));
+  // metadata in sk_sketch_set_pack_subset's format
+  std::vector<uint64_t> meta;
+  meta.reserve(meta_words(n, ctg_off[n], tables));
+  for (uint64_t w : {(uint64_t)n, seed_off[n], uk_off[n], mk_off[n], ctg_off[n], (uint64_t)st->sp.c, (uint64_t)st->sp.k, (uint64_t)st->sp.marker_c,
+                     ht_off[n], (uint64_t)(tables ? 1 : 0)})
+    meta.push_back(w);
+  for (auto* v : {&seed_off, &uk_off, &mk_off, &ctg_off}) meta.insert(meta.end(), v->begin(), v->end());
+  for (uint32_t i = 0; i < n; i++) meta.push_back(st->g[genomes[i]].total_len);
+  if (!mo)
+    for (uint32_t i = 0; i < n; i++) {
+      const sk_sketch_store::Genome& e = st->g[genomes[i]];
+      for (uint64_t c = 0; c < e.C; c++) meta.push_back(st->ctg_len[e.ctg0 + c]);
+    }
+  if (tables) meta.insert(meta.end(), ht_off.begin(), ht_off.end());
+  const void* bp = blob.p;
+  const uint64_t* mp = meta.data();
+  SK_TRY(sk_sketch_set_unpack(ctx, 1, &bp, &mp, out));
+  for (uint32_t i = 0; i < n; i++) (*out)->name_rank[i] = st->name_rank[genomes[i]];
+  (*out)->ranks_user_set = true;
+  return SK_OK;
+}
+
+int sk_triangle_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp, uint64_t device_budget,
+                      sk_ani_result** out, uint64_t* n_out, sk_store_stats* stats) {
+  if (!ctxs || n_ctx == 0 || !ctxs[0]) return SK_ERR_PARAM;
+  sk_ctx* ctx = ctxs[0];
+  if (!st || !mp || !out || !n_out) { ctx->err = "sk_triangle_store: NULL argument"; return SK_ERR_PARAM; }
+  *out = nullptr; *n_out = 0;
+  for (uint32_t d = 0; d < n_ctx; d++) {
+    if (!ctxs[d]) { ctx->err = "context " + std::to_string(d) + ": NULL context"; return SK_ERR_PARAM; }
+    for (uint32_t e = 0; e < d; e++)
+      if (ctxs[e] == ctxs[d]) { ctx->err = "context " + std::to_string(d) + ": the same context appears twice (one host thread per context)"; return SK_ERR_PARAM; }
+  }
+  const uint32_t N = (uint32_t)st->g.size();
+  // budget per context: a working set's sketches, its gather blob (as large) and the chaining workspace share the device with
+  // the other contexts on it, so a third of each context's share of the free memory (80 % of it)
+  uint64_t budget = device_budget;
+  if (budget == 0) {
+    budget = ~0ull;
+    for (uint32_t d = 0; d < n_ctx; d++) {
+      uint32_t same = 0;
+      for (uint32_t e = 0; e < n_ctx; e++) same += ctxs[e]->device == ctxs[d]->device;
+      size_t free_b = 0, total_b = 0;
+      SK_CUDA(cudaSetDevice(ctxs[d]->device));
+      SK_CUDA(cudaMemGetInfo(&free_b, &total_b));
+      budget = std::min<uint64_t>(budget, (uint64_t)(0.8 * (double)free_b / (3.0 * same)));
+    }
+    SK_CUDA(cudaSetDevice(ctx->device));
+  }
+  std::vector<uint64_t> gbytes(N);
+  for (uint32_t g = 0; g < N; g++) gbytes[g] = sk_sketch_store_genome_bytes(st, g);
+  for (uint32_t g = 0; g < N; g++)
+    if (gbytes[g] > budget / 2) {
+      ctx->err = "sk_triangle_store: genome " + std::to_string(g) + " needs " + std::to_string(gbytes[g]) + " device bytes, more than half the working-set budget of " +
+                 std::to_string(budget) + " bytes";
+      return SK_ERR_NOMEM;
+    }
+  // ---- 1. screen: markers of every genome on context 0
+  const double t0 = now_s();
+  std::vector<uint64_t> pairs;
+  {
+    SK_CUDA(cudaSetDevice(ctx->device));
+    std::vector<uint32_t> all(N);
+    for (uint32_t g = 0; g < N; g++) all[g] = g;
+    sk_sketch_set* mk = nullptr;
+    SK_TRY(sk_sketch_store_gather(ctx, st, all.data(), N, SK_PACK_MARKERS_ONLY, &mk));
+    uint64_t* p = nullptr; uint64_t np = 0;
+    const int rc = sk_screen_triangle(ctx, mk, mp, &p, &np);
+    sk_sketch_set_free(mk);
+    SK_TRY(rc);
+    pairs.assign(p, p + np);
+    sk_free(p);
+  }
+  const double t_screen = now_s() - t0;
+  // ---- 2. plan
+  skws::Plan plan;
+  std::string perr;
+  if (!skws::plan_working_sets(pairs, gbytes, budget, plan, perr)) { ctx->err = "sk_triangle_store: " + perr; return SK_ERR_NOMEM; }
+  // ---- 3. contexts take the working sets in plan order
+  const bool trace = getenv("SK_TRACE") != nullptr;
+  std::atomic<size_t> next{0};
+  std::atomic<bool> failed{false};
+  std::vector<std::vector<sk_ani_result>> kept(n_ctx);
+  std::vector<double> tg(n_ctx, 0), tc(n_ctx, 0);
+  std::vector<uint64_t> gathered(n_ctx, 0);
+  std::vector<int> rcs(n_ctx, SK_OK);
+  auto run = [&](uint32_t d) {
+    sk_ctx* c = ctxs[d];
+    if (cudaSetDevice(c->device) != cudaSuccess) { c->err = "cudaSetDevice failed"; rcs[d] = SK_ERR_CUDA; failed = true; return; }
+    for (size_t w; !failed && (w = next.fetch_add(1)) < plan.sets.size();) {
+      const skws::WorkingSet& ws = plan.sets[w];
+      const double a = now_s();
+      sk_sketch_set* set = nullptr;
+      int rc = sk_sketch_store_gather(c, st, ws.genomes.data(), (uint32_t)ws.genomes.size(), 0, &set);
+      const double bt = now_s();
+      if (rc == SK_OK) {
+        std::vector<uint64_t> lp(ws.pairs.size());
+        for (size_t i = 0; i < lp.size(); i++) {
+          const uint64_t x = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)(ws.pairs[i] >> 32)) - ws.genomes.begin();
+          const uint64_t y = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)ws.pairs[i]) - ws.genomes.begin();
+          lp[i] = (x << 32) | y;
+        }
+        std::vector<sk_ani_result> res(lp.size());
+        rc = sk_chain_pairs(c, set, set, lp.data(), lp.size(), mp, res.data());
+        if (rc == SK_OK)
+          for (auto& r : res)
+            if (r.ani > 0.1f) { r.ref_id = ws.genomes[r.ref_id]; r.query_id = ws.genomes[r.query_id]; kept[d].push_back(r); }   // src/triangle.rs:99
+      }
+      if (set) sk_sketch_set_free(set);
+      const double ct = now_s();
+      tg[d] += bt - a; tc[d] += ct - bt; gathered[d] += ws.bytes;
+      if (trace)
+        fprintf(stderr, "[sk_triangle_store] context %u: working set %zu/%zu%s: %zu genomes, %zu pairs, %.1f MB gathered in %.1f ms, chain %.1f ms\n", d, w + 1,
+                plan.sets.size(), ws.chunk_pair ? " (chunk pair)" : "", ws.genomes.size(), ws.pairs.size(), ws.bytes / 1e6, (bt - a) * 1e3, (ct - bt) * 1e3);
+      if (rc != SK_OK) { rcs[d] = rc; failed = true; }
+    }
+  };
+  if (n_ctx == 1) run(0);
+  else {
+    std::vector<std::thread> th;
+    for (uint32_t d = 0; d < n_ctx; d++) th.emplace_back(run, d);
+    for (auto& t : th) t.join();
+  }
+  cudaSetDevice(ctx->device);
+  for (uint32_t d = 0; d < n_ctx; d++)
+    if (rcs[d] != SK_OK) { if (d) ctx->err = "context " + std::to_string(d) + ": " + ctxs[d]->err; return rcs[d]; }
+  std::vector<sk_ani_result> res;
+  for (auto& v : kept) res.insert(res.end(), v.begin(), v.end());
+  std::sort(res.begin(), res.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
+  sk_ani_result* o = (sk_ani_result*)malloc(sizeof(sk_ani_result) * std::max<size_t>(res.size(), 1));
+  if (!o) { ctx->err = "out of host memory"; return SK_ERR_NOMEM; }
+  if (!res.empty()) memcpy(o, res.data(), res.size() * sizeof(sk_ani_result));
+  *out = o; *n_out = res.size();
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_working_sets = (uint32_t)plan.sets.size();
+    stats->n_split_components = plan.n_split_components;
+    for (auto& ws : plan.sets) stats->max_working_set_bytes = std::max(stats->max_working_set_bytes, ws.bytes);
+    stats->t_screen = t_screen;
+    for (uint32_t d = 0; d < n_ctx; d++) { stats->gathered_bytes += gathered[d]; stats->t_gather += tg[d]; stats->t_chain += tc[d]; }
+  }
+  return SK_OK;
+}
+
+}  // extern "C"

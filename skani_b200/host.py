@@ -4,7 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import AniResult, ChainDebug, MapParams, SketchParams, TriangleStats
+from ._lib import AniResult, ChainDebug, MapParams, SketchParams, StoreStats, TriangleStats
 
 # numpy view of sk_ani_result (include/skani_b200.h): lets callers take 10^5..10^6 results without per-row Python objects
 RESULT_DTYPE = np.dtype([(n, np.float32) for n in ("ani", "af_query", "af_ref", "ci_lower", "ci_upper", "std", "q90_q", "q90_r", "q50_q",
@@ -444,4 +444,70 @@ def triangle_multi(ctxs, bases, contig_off, genome_of_contig, n_genomes, sp=None
     c0 = ctxs[0]
     c0.check(c0.L.sk_triangle_multi(hs, len(ctxs), ptr, contig_off.ctypes.data, len(goc), goc.ctypes.data, n_genomes, C.byref(sp), C.byref(mp),
                                     None if nr is None else nr.ctypes.data, C.byref(out), C.byref(n), C.byref(st)))
+    return _take_results(c0, out, n, as_array), st
+
+
+class SketchStore:
+    """sk_sketch_store: sketches (with their k-mer tables) in pinned host memory, genome-indexed.  Sets added to it may be freed
+    afterwards; gather() brings any ascending list of genomes back to a device set that chains, screens and exports exactly
+    like the set that was added."""
+
+    def __init__(self, sp=None):
+        self.L = _lib.load()
+        self.sp = sp or sketch_params()
+        h = C.c_void_p()
+        if self.L.sk_sketch_store_create(C.byref(self.sp), C.byref(h)) != 0:
+            raise SkaniError("sk_sketch_store_create failed")
+        self.h = h
+
+    def add(self, sset):
+        """Append the genomes of a device set (ids continue; name ranks continue after the store's largest)."""
+        sset.ctx.check(self.L.sk_sketch_store_add(self.h, sset.h))
+
+    def n_genomes(self):
+        return self.L.sk_sketch_store_n_genomes(self.h)
+
+    def __len__(self):
+        return self.n_genomes()
+
+    def genome_bytes(self, g):
+        """Device bytes genome g takes in a working set."""
+        return self.L.sk_sketch_store_genome_bytes(self.h, int(g))
+
+    def set_name_ranks(self, ranks):
+        r = np.ascontiguousarray(ranks, np.uint64)
+        assert len(r) == self.n_genomes()
+        if self.L.sk_sketch_store_set_name_ranks(self.h, r.ctypes.data if len(r) else None) != 0:
+            raise SkaniError("sk_sketch_store_set_name_ranks failed")
+
+    def gather(self, ctx, genomes=None, markers_only=False):
+        """Device set on ctx holding `genomes` (ascending, no duplicates; None = all) in list order."""
+        g = np.arange(self.n_genomes(), dtype=np.uint32) if genomes is None else np.ascontiguousarray(genomes, np.uint32)
+        keep = g if len(g) else np.zeros(1, np.uint32)
+        h = C.c_void_p()
+        ctx.check(self.L.sk_sketch_store_gather(ctx.h, self.h, keep.ctypes.data, len(g), 1 if markers_only else 0, C.byref(h)))
+        return SketchSet(ctx, h)
+
+    def free(self):
+        if self.h:
+            self.L.sk_sketch_store_free(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
+def triangle_store(ctxs, store, mp=None, device_budget=0, as_array=True):
+    """sk_triangle_store: the triangle of every genome of `store`, chained in working sets of at most device_budget bytes per
+    context (0 = derived from free device memory).  ctxs: one Context or a list (two on one device overlap gather and chain).
+    Returns (results sorted by (ref_id, query_id), StoreStats)."""
+    ctxs = list(ctxs) if isinstance(ctxs, (list, tuple)) else [ctxs]
+    mp = mp or map_params()
+    hs = (C.c_void_p * len(ctxs))(*[c.h for c in ctxs])
+    out = C.POINTER(AniResult)(); n = C.c_uint64(); st = StoreStats()
+    c0 = ctxs[0]
+    c0.check(c0.L.sk_triangle_store(hs, len(ctxs), store.h, C.byref(mp), int(device_budget), C.byref(out), C.byref(n), C.byref(st)))
     return _take_results(c0, out, n, as_array), st
