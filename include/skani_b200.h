@@ -144,7 +144,8 @@ int sk_sketch_set_import(sk_ctx* ctx, const sk_sketch_params* params, const uint
  * [mk_off[g], mk_off[g+1]) and contigs [ctg_off[g], ctg_off[g+1]) of the concatenated arrays (offset arrays have
  * n_genomes + 1 entries, n_genomes >= 1).  total_len: Sketch.total_sequence_length per genome, or NULL = sum of the
  * genome's contig lengths (marker-only sketches carry no contig lengths).  A batch is limited to < 2^31 records and
- * markers; larger databases are imported in several batches joined with sk_sketch_set_append. */
+ * markers; larger databases are imported in several batches joined with sk_sketch_set_append.  Markers must be < 2^42
+ * and seed k-mers < 4^k (a k-mer hash of a DNA sketch always is); SK_ERR_PARAM otherwise. */
 int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* params, uint32_t n_genomes, const uint64_t* rec_off,
                                const uint32_t* kmer, const uint32_t* pos, const uint32_t* contig_canon,
                                const uint64_t* mk_off, const uint64_t* markers, const uint64_t* ctg_off,

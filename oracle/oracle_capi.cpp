@@ -173,6 +173,45 @@ int orc_screen_triangle(void** sk, int n, double screen_val, int rescue_small, u
   *row_off = ro; *cols = cs;
   return 0;
 }
+// markers-only sketches (Sketch::get_markers_only): genome g holds markers[mk_off[g] .. mk_off[g+1]), inserted through
+// MarkerSet::insert (duplicates collapse as in the reference's HashSet); handles are written to out[0..n)
+int orc_sketches_from_markers(int n, const uint64_t* mk_off, const uint64_t* markers, void** out) {
+  for (int g = 0; g < n; g++) {
+    Sketch* s = new Sketch();
+    for (uint64_t i = mk_off[g]; i < mk_off[g + 1]; i++) s->marker_seeds.insert(markers[i]);
+    out[g] = s;
+  }
+  return 0;
+}
+// query x ref screen as the drivers pick it (orc_dist / orc_search): mode 0 check_markers_quickly(rescue_small), 1 the same
+// without rescue, 2 screen_refs, 3 screen_refs_indices.  Output: ascending (ref << 32 | query), malloc'd.
+int orc_screen_query_ref(void** refs, int nr, void** queries, int nq, double screen_val, int mode, int rescue_small,
+                         uint64_t** pairs, uint64_t* n) {
+  if (mode < 0 || mode > 3) return -1;
+  std::vector<const Sketch*> r, q;
+  for (int i = 0; i < nr; i++) r.push_back((Sketch*)refs[i]);
+  for (int i = 0; i < nq; i++) q.push_back((Sketch*)queries[i]);
+  const double sv = screen_val == 0. ? SEARCH_ANI_CUTOFF_DEFAULT : screen_val;   // dist.rs:68-77
+  std::vector<uint64_t> out;
+  if (mode <= 1) {
+    const bool rescue = mode == 0 && rescue_small != 0;
+    for (int j = 0; j < nq; j++)
+      for (int i = 0; i < nr; i++)
+        if (check_markers_quickly(*q[j], *r[i], sv, rescue)) out.push_back(((uint64_t)i << 32) | (uint32_t)j);
+  } else {
+    KmerToSketch* idx = kmer_to_sketch_from_refs(r);
+    for (int j = 0; j < nq; j++) {
+      auto pass = mode == 3 ? screen_refs_indices(sv, *idx, *q[j], r) : screen_refs(sv, *idx, *q[j], r, rescue_small != 0);
+      for (uint32_t i : pass) out.push_back(((uint64_t)i << 32) | (uint32_t)j);
+    }
+    kmer_to_sketch_free(idx);
+  }
+  std::sort(out.begin(), out.end());
+  uint64_t* o = (uint64_t*)malloc(sizeof(uint64_t) * (out.size() + 1));
+  if (!out.empty()) memcpy(o, out.data(), out.size() * 8);
+  *pairs = o; *n = out.size();
+  return 0;
+}
 
 // ---- chain ------------------------------------------------------------------------------------------
 int orc_chain(void* ref, void* query, const orc_cmd* cmd, orc_result* out) {

@@ -166,7 +166,16 @@ __global__ void import_ctab_kernel(const uint64_t* __restrict__ rec_off, const u
   const uint64_t want = (uint64_t)c << 32;
   while (a < z) { const uint64_t m = (a + z) >> 1; if (skeys[m] < want) a = m + 1; else z = m; }
   ctab[t] = (uint32_t)(a - b);
-  if (c == nc && a != e) atomicExch(bad, 1u);                              // a record names a contig the sketch does not have
+  if (c == nc && a != e) atomicOr(bad, 1u);                                // a record names a contig the sketch does not have
+}
+
+// flags `bad` when some v[i] >= limit.  Imported markers must be < 2^42 and seed k-mers < 4^k: the views build their sort
+// keys as (genome << 42 | marker) and (genome << 2k | k-mer), so a larger value would land in another genome's list.
+template <typename T>
+__global__ void import_range_kernel(const T* __restrict__ v, uint64_t n, uint64_t limit, uint32_t* __restrict__ bad, uint32_t flag) {
+  bool over = false;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)blockDim.x * gridDim.x) over |= (uint64_t)v[i] >= limit;
+  if (over) atomicOr(bad, flag);
 }
 
 __global__ void stage_copy_kernel(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src, size_t n_words) {
@@ -1263,6 +1272,7 @@ int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* sp, uint32_t
   cudaStream_t st = ctx->stream;
   SK_CUDA(cudaStreamSynchronize(st));
   if (n_contigs) SK_CUDA(cudaMemcpyAsync(s->d_ctg_len, contig_lengths + c0, n_contigs * 4, cudaMemcpyHostToDevice, st));
+  DTmp<uint64_t> mraw;
   {
     DTmp<uint64_t> d_ro, d_co;
     SK_CUDA(d_ro.alloc(G + 1, ctx)); SK_CUDA(d_co.alloc(G + 1, ctx));
@@ -1271,6 +1281,14 @@ int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* sp, uint32_t
     DTmp<uint32_t> d_bad;
     SK_CUDA(d_bad.alloc(1, ctx));
     SK_CUDA(cudaMemsetAsync(d_bad.p, 0, 4, st));
+    enum { BAD_CONTIG = 1, BAD_MARKER = 2, BAD_KMER = 4 };
+    auto range_blocks = [](uint64_t n) { return (unsigned)std::min<uint64_t>((n + 255) / 256, 1024); };
+    SK_CUDA(mraw.alloc(n_markers, ctx));
+    if (n_markers) {
+      SK_CUDA(cudaMemcpyAsync(mraw.p, markers + m0, n_markers * 8, cudaMemcpyHostToDevice, st));
+      import_range_kernel<uint64_t><<<range_blocks(n_markers), 256, 0, st>>>(mraw.p, n_markers, 1ull << (2 * MARKER_K), d_bad.p, BAD_MARKER);
+      count_launch(ctx);
+    }
     if (n_records) {
       DTmp<uint32_t> rk, rp, rc, vals, perm;
       DTmp<uint64_t> keys, skeys;
@@ -1279,6 +1297,10 @@ int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* sp, uint32_t
       SK_CUDA(cudaMemcpyAsync(rk.p, kmer + r0, n_records * 4, cudaMemcpyHostToDevice, st));
       SK_CUDA(cudaMemcpyAsync(rp.p, pos + r0, n_records * 4, cudaMemcpyHostToDevice, st));
       SK_CUDA(cudaMemcpyAsync(rc.p, cc + r0, n_records * 4, cudaMemcpyHostToDevice, st));
+      if (2 * sp->k < 32) {
+        import_range_kernel<uint32_t><<<range_blocks(n_records), 256, 0, st>>>(rk.p, n_records, 1ull << (2 * sp->k), d_bad.p, BAD_KMER);
+        count_launch(ctx);
+      }
       import_keys_kernel<<<dim3(G, 8), 256, 0, st>>>(d_ro.p, rp.p, rc.p, keys.p, vals.p); count_launch(ctx);
       size_t tb = 0;
       SK_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb, keys.p, skeys.p, vals.p, perm.p, (int)n_records, (int)G, d_ro.p, d_ro.p + 1, 0, 62, st));
@@ -1295,11 +1317,10 @@ int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* sp, uint32_t
     uint32_t bad = 0;
     SK_CUDA(cudaMemcpyAsync(&bad, d_bad.p, 4, cudaMemcpyDeviceToHost, st));
     SK_CUDA(cudaStreamSynchronize(st));
-    if (bad) { ctx->err = "record contig index out of range"; return SK_ERR_PARAM; }
+    if (bad & BAD_MARKER) { ctx->err = "marker out of range (markers must be < 2^42)"; return SK_ERR_PARAM; }
+    if (bad & BAD_KMER) { ctx->err = "seed k-mer out of range (k-mers must be < 4^k)"; return SK_ERR_PARAM; }
+    if (bad & BAD_CONTIG) { ctx->err = "record contig index out of range"; return SK_ERR_PARAM; }
   }
-  DTmp<uint64_t> mraw;
-  SK_CUDA(mraw.alloc(n_markers, ctx));
-  if (n_markers) SK_CUDA(cudaMemcpy(mraw.p, markers + m0, n_markers * 8, cudaMemcpyHostToDevice));
   std::vector<uint64_t> raw_off(G + 1);
   for (uint32_t g = 0; g <= G; g++) raw_off[g] = mk_off[g] - m0;
   mbox_reset(ctx);                 // build_views takes pinned read-back space from the context's mailbox

@@ -95,8 +95,6 @@ __global__ void qr_ranges_kernel(const uint32_t* __restrict__ sval, const uint32
   }
 }
 
-enum ScreenMode { MODE_QUICK = 0, MODE_QUICK_NORESCUE = 1, MODE_INDEX = 2, MODE_INDEX_NORESCUE = 3, MODE_TRIANGLE = 4 };
-
 // One block per row genome.  counts[] lives in dynamic shared memory (tile of `tile` columns).
 __global__ void __launch_bounds__(256)
 screen_rows_kernel(const uint64_t* __restrict__ row_mk_off, const uint64_t* __restrict__ col_mk_off, uint32_t n_rows,
@@ -111,8 +109,8 @@ screen_rows_kernel(const uint64_t* __restrict__ row_mk_off, const uint64_t* __re
   const uint64_t card_i = me - mb;
   const bool tri = (mode == MODE_TRIANGLE);
   const uint32_t col_begin = tri ? i + 1 : 0;
-  // screen_refs: a row with < 20 markers passes everything when rescue is on (src/screen.rs:158-160)
-  const bool row_rescue = (mode == MODE_TRIANGLE || mode == MODE_INDEX) && rescue_small && card_i < 20;
+  // a rescued row passes every column: nothing to count
+  const bool row_rescue = screen_row_rescued(mode, rescue_small, card_i);
   for (uint32_t t0 = col_begin; t0 < n_cols; t0 += tile) {
     const uint32_t t1 = min(n_cols, t0 + tile);
     for (uint32_t c = threadIdx.x; c < t1 - t0; c += blockDim.x) counts[c] = 0;
@@ -130,31 +128,7 @@ screen_rows_kernel(const uint64_t* __restrict__ row_mk_off, const uint64_t* __re
     for (uint32_t c = threadIdx.x; c < t1 - t0; c += blockDim.x) {
       const uint32_t j = t0 + c;
       const uint64_t card_j = col_mk_off[j + 1] - col_mk_off[j];
-      const uint64_t mn = card_i < card_j ? card_i : card_j;
-      const uint64_t cnt = counts[c];
-      bool pass;
-      if (all_pass) pass = true;
-      else if (mode == MODE_TRIANGLE || mode == MODE_INDEX || mode == MODE_INDEX_NORESCUE) {
-        // screen_refs / screen_refs_indices (src/screen.rs:177-187, 63-73): only columns with >= 1 shared marker are
-        // candidates; pass iff count > max((usize)(cutoff * min(|Mj|,|Mi|)), 1)
-        if (row_rescue) pass = true;
-        else {
-          unsigned long long thr = (unsigned long long)(cutoff * (double)mn);
-          if (thr < 1) thr = 1;
-          pass = cnt > thr;
-        }
-      } else {
-        // check_markers_quickly (src/screen.rs:84-142)
-        const bool rescue = (mode == MODE_QUICK) && rescue_small;
-        if (mn < 20 && rescue) pass = true;
-        else if (mn == 0) pass = rescue;
-        else {
-          unsigned long long ratio = (unsigned long long)(cutoff * (double)mn);
-          if (ratio == 0) ratio = 1;
-          pass = cnt >= ratio;
-        }
-      }
-      if (pass) {
+      if (all_pass || screen_pass(mode, rescue_small, card_i, card_j, counts[c], cutoff)) {
         unsigned long long slot = atomicAdd(n_pairs, 1ull);
         // triangle: (i, j); query x ref: (ref = column, query = row)
         if (slot < cap) pairs[slot] = tri ? (((uint64_t)i << 32) | j) : (((uint64_t)j << 32) | i);
@@ -334,16 +308,8 @@ ts_rows_kernel(const uint64_t* __restrict__ markers, const uint64_t* __restrict_
     for (uint32_t c = threadIdx.x; c < t1 - t0; c += blockDim.x) {
       const uint32_t i = t0 + c;
       const uint64_t card_i = off[i + 1] - off[i];
-      bool pass;
-      // screen_refs with row i (src/screen.rs:158-160, 177-187): a row with < 20 markers passes every column when rescue is on
-      if (rescue_small && card_i < 20) pass = true;
-      else {
-        const uint64_t mn = card_i < card_j ? card_i : card_j;
-        unsigned long long thr = (unsigned long long)(cutoff * (double)mn);
-        if (thr < 1) thr = 1;
-        pass = counts[c] > thr;
-      }
-      if (pass) {
+      // screen_refs with the smaller index i as its row (the rescue follows i, src/screen.rs:158-160)
+      if (screen_pass(MODE_TRIANGLE, rescue_small, card_i, card_j, counts[c], cutoff)) {
         unsigned long long slot = atomicAdd(n_pairs, 1ull);
         if (slot < cap) pairs[slot] = ((uint64_t)i << 32) | j;
       }

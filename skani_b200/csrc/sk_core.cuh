@@ -273,3 +273,39 @@ SK_HD uint32_t unit_pass_mask_fast(uint64_t lo, uint64_t hi, uint32_t nm_lo, uin
 
 }  // namespace sk
 
+namespace sk {
+
+// ---- marker screen predicate (screen_rows_kernel, ts_rows_kernel) -----------------------------------------------------
+// Modes 0-3 are the query x ref screens of sk_screen_query_ref; the triangle screens with screen_refs' rule.
+enum ScreenMode { MODE_QUICK = 0, MODE_QUICK_NORESCUE = 1, MODE_INDEX = 2, MODE_INDEX_NORESCUE = 3, MODE_TRIANGLE = 4 };
+constexpr uint64_t SCREEN_MINIMUM_KMERS = 20;   // reference src/params.rs:49
+
+// screen_refs (triangle, mode 2): a row (the screen_refs query) with < 20 markers passes every column when rescue is on
+// (src/screen.rs:158-160).  Only the row's own count decides; a small column never rescues its row.
+SK_HD bool screen_row_rescued(int mode, bool rescue_small, uint64_t card_row) {
+  return (mode == MODE_TRIANGLE || mode == MODE_INDEX) && rescue_small && card_row < SCREEN_MINIMUM_KMERS;
+}
+
+// Whether the pair (row, column) passes, given the markers they share (`count`) and cutoff = screen_val^21 (screen_val 0
+// already replaced by 0.80, as every caller of the reference does).
+SK_HD bool screen_pass(int mode, bool rescue_small, uint64_t card_row, uint64_t card_col, uint64_t count, double cutoff) {
+  const uint64_t mn = card_row < card_col ? card_row : card_col;
+  if (mode == MODE_TRIANGLE || mode == MODE_INDEX || mode == MODE_INDEX_NORESCUE) {
+    // screen_refs / screen_refs_indices (src/screen.rs:177-187, 63-73): only columns with >= 1 shared marker are candidates;
+    // pass iff count > max((usize)(cutoff * min(|Mj|,|Mi|)), 1)
+    if (screen_row_rescued(mode, rescue_small, card_row)) return true;
+    unsigned long long thr = (unsigned long long)(cutoff * (double)mn);
+    if (thr < 1) thr = 1;
+    return count > thr;
+  }
+  // check_markers_quickly (src/screen.rs:84-142): symmetric in its two sketches, rescue only in mode 0
+  const bool rescue = (mode == MODE_QUICK) && rescue_small;
+  if (mn < SCREEN_MINIMUM_KMERS && rescue) return true;
+  if (mn == 0) return rescue;
+  unsigned long long ratio = (unsigned long long)(cutoff * (double)mn);
+  if (ratio == 0) ratio = 1;
+  return count >= ratio;
+}
+
+}  // namespace sk
+

@@ -273,6 +273,12 @@ def screen_triangle(ctx, sset, mp=None):
     return _pairs_out(ctx, ctx.L.sk_screen_triangle, ctx.h, sset.h, C.byref(mp))
 
 
+def screen_triangle_rows(ctx, sset, row_mod, row_rem, mp=None):
+    """Pairs (i, j), i < j, of the triangle screen whose row i satisfies i % row_mod == row_rem."""
+    mp = mp or map_params()
+    return _pairs_out(ctx, ctx.L.sk_screen_triangle_rows, ctx.h, sset.h, C.byref(mp), int(row_mod), int(row_rem))
+
+
 def screen_triangle_block(ctx, sset, g_begin, g_end, mp=None):
     """Pairs (i, j), i < j, g_begin <= j < g_end of the triangle screen (sharded screen: one block of rows)."""
     mp = mp or map_params()

@@ -85,6 +85,10 @@ def lib():
     L.orc_check_markers_quickly.restype = i32; L.orc_check_markers_quickly.argtypes = [vp, vp, dbl, i32]
     L.orc_screen_triangle.restype = i32
     L.orc_screen_triangle.argtypes = [C.POINTER(vp), i32, dbl, i32, C.POINTER(C.POINTER(u64)), C.POINTER(C.POINTER(u32))]
+    L.orc_sketches_from_markers.restype = i32
+    L.orc_sketches_from_markers.argtypes = [i32, vp, vp, C.POINTER(vp)]
+    L.orc_screen_query_ref.restype = i32
+    L.orc_screen_query_ref.argtypes = [C.POINTER(vp), i32, C.POINTER(vp), i32, dbl, i32, i32, C.POINTER(C.POINTER(u64)), C.POINTER(u64)]
     L.orc_chain.restype = i32; L.orc_chain.argtypes = [vp, vp, C.POINTER(OrcCmd), C.POINTER(OrcResult)]
     L.orc_chain_debug.restype = vp; L.orc_chain_debug.argtypes = [vp, vp, C.POINTER(OrcCmd)]
     L.orc_debug_free.argtypes = [vp]
@@ -240,7 +244,38 @@ def screen_triangle(sketches, screen_val=0.0, rescue_small=True):
     ro = C.POINTER(C.c_uint64)(); cols = C.POINTER(C.c_uint32)()
     L.orc_screen_triangle(hs, len(sketches), screen_val, int(rescue_small), C.byref(ro), C.byref(cols))
     n = len(sketches)
-    row_off = np.array([ro[i] for i in range(n + 1)], np.uint64)
-    c = np.array([cols[i] for i in range(int(row_off[-1]))], np.uint32)
+    row_off = np.ctypeslib.as_array(ro, shape=(n + 1,)).astype(np.uint64)
+    c = np.ctypeslib.as_array(cols, shape=(int(row_off[-1]),)).astype(np.uint32) if row_off[-1] else np.zeros(0, np.uint32)
     L.orc_free_array(ro); L.orc_free_array(cols)
     return row_off, c
+
+
+def sketches_from_markers(mk_off, markers):
+    """Markers-only oracle sketches, built in one call: genome g holds markers[mk_off[g]:mk_off[g + 1]]."""
+    n = len(mk_off) - 1
+    off = np.ascontiguousarray(mk_off, np.uint64)
+    mk = np.ascontiguousarray(np.concatenate([np.asarray(markers, np.uint64), np.zeros(1, np.uint64)]))
+    out = (C.c_void_p * max(n, 1))()
+    lib().orc_sketches_from_markers(n, off.ctypes.data, mk.ctypes.data, out)
+    return [Sketch(out[i]) for i in range(n)]
+
+
+def screen_query_ref(refs, queries, screen_val=0.0, mode=0, rescue_small=True):
+    """Sorted (ref << 32 | query) list of the query x ref screen in mode 0-3 (see orc_screen_query_ref)."""
+    L = lib()
+    hr = (C.c_void_p * max(len(refs), 1))(*[s.h for s in refs])
+    hq = (C.c_void_p * max(len(queries), 1))(*[s.h for s in queries])
+    pp = C.POINTER(C.c_uint64)(); n = C.c_uint64()
+    rc = L.orc_screen_query_ref(hr, len(refs), hq, len(queries), screen_val, mode, int(rescue_small), C.byref(pp), C.byref(n))
+    if rc != 0:
+        raise ValueError("orc_screen_query_ref rc=%d" % rc)
+    arr = np.ctypeslib.as_array(pp, shape=(n.value,)).copy() if n.value else np.zeros(0, np.uint64)
+    L.orc_free_array(pp)
+    return arr
+
+
+def screen_triangle_pairs(sketches, screen_val=0.0, rescue_small=True):
+    """screen_triangle as a sorted (i << 32 | j) list, the form sk_screen_triangle returns."""
+    row_off, cols = screen_triangle(sketches, screen_val, rescue_small)
+    rows = np.repeat(np.arange(len(sketches), dtype=np.uint64), np.diff(row_off).astype(np.int64))
+    return np.sort((rows << np.uint64(32)) | cols.astype(np.uint64))
