@@ -341,6 +341,24 @@ typedef struct {
 int sk_triangle_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp,
                       uint64_t device_budget, sk_ani_result** out, uint64_t* n_out, sk_store_stats* stats);
 
+/* sk_query_ref_store: dist (src/dist.rs:98-144) of every (reference, query) pair of two stores.  Returns what one context
+ * computes from sets R and Q holding every genome of refs and queries with the stores' name ranks:
+ * sk_screen_query_ref(R, Q, mode), sk_chain_pairs(R, Q, pairs), keep ani > 0.1 (src/dist.rs:115,139).  ref_id / query_id are
+ * store genome ids; results (malloc'd, sk_free) are sorted by (ref_id, query_id).  The markers of both stores are gathered on
+ * ctxs[0] and screened; the pairs are planned into working sets that each hold some references and some queries within
+ * device_budget bytes per context (0 = derived as in sk_triangle_store); the contexts, on one device or several, take the
+ * working sets in plan order and gather each one's references from refs and queries from queries.  refs == queries (a set
+ * against itself) is allowed.  A genome over budget / 2 on either side gives SK_ERR_NOMEM before any device work; stores with
+ * different sketch parameters, a mode outside 0-3, NULL arguments or a context listed twice give SK_ERR_PARAM.  If any
+ * context fails the call fails and sk_last_error(ctxs[0]) carries that context's message.  SK_TRACE=1 prints one line per
+ * working set.  stats as in sk_triangle_store.
+ * Name ranks: both stores' ranks are used exactly as stored, so the caller ranks both sides in one file-name order (set both
+ * with sk_sketch_store_set_name_ranks).  Two stores left at their default ranks do NOT reproduce sk_chain_pairs' default for
+ * two sets, where the queries rank after the references: both stores then rank from 0. */
+int sk_query_ref_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* refs, const sk_sketch_store* queries,
+                       const sk_map_params* mp, int mode, uint64_t device_budget, sk_ani_result** out, uint64_t* n_out,
+                       sk_store_stats* stats);
+
 #ifdef __cplusplus
 }
 #endif

@@ -104,6 +104,7 @@ SYMBOLS = [
     ("sk_sketch_store_gather", i32, [vp, vp, vp, u32, i32, PP(vp)]),
     ("sk_sketch_store_free", i32, [vp]),
     ("sk_triangle_store", i32, [vp, u32, vp, PP(MapParams), u64, PP(PP(AniResult)), PP(u64), PP(StoreStats)]),
+    ("sk_query_ref_store", i32, [vp, u32, vp, vp, PP(MapParams), i32, u64, PP(PP(AniResult)), PP(u64), PP(StoreStats)]),
 ]
 
 _lib = None

@@ -342,60 +342,82 @@ size_t file_group_end(const std::vector<std::string>& files, size_t f0) {
 // seed, 24 B per marker and 6 GB of workspace against 92 % of the device, from the file sizes, x 4 for .gz; .sketch files
 // about triple on the device) or SK_DEVICE_BUDGET_MB asks for the store path.  --gpus N with FASTA inputs keeps
 // sk_triangle_multi.
-bool triangle_needs_store(const Opts& op, bool sketches, double* need_gb) {
-  *need_gb = 0;
-  if (op.gpus > 1 && !sketches) return false;
+double sketch_bytes_estimate(const Opts& op, const std::vector<std::string>& files, bool sketches) {
   uint64_t bytes = 0;
-  for (auto& f : op.files) {
+  for (auto& f : files) {
     struct stat st;
     if (stat(f.c_str(), &st) != 0) continue;
     const bool gz = f.size() > 3 && f.compare(f.size() - 3, 3, ".gz") == 0;
     bytes += (uint64_t)st.st_size * (gz ? 4 : 1);
   }
-  const double need = sketches ? 3.0 * bytes + 6.0e9 : (double)bytes / op.c * 56.0 + (double)bytes / op.m * 24.0 + 6.0e9;
-  *need_gb = need / 1e9;
+  return sketches ? 3.0 * bytes : (double)bytes / op.c * 56.0 + (double)bytes / op.m * 24.0;
+}
+// need bytes against 92 % of the device, or SK_DEVICE_BUDGET_MB asks for the store path
+bool exceeds_device(const Opts& op, double need) {
   if (getenv("SK_DEVICE_BUDGET_MB")) return true;
   uint64_t free_b = 0, total_b = 0;
   if (sk_device_memory(op.device, &free_b, &total_b) != 0) return false;
   return need > 0.92 * (double)total_b;
 }
+bool triangle_needs_store(const Opts& op, bool sketches, double* need_gb) {
+  *need_gb = 0;
+  if (op.gpus > 1 && !sketches) return false;
+  const double need = sketch_bytes_estimate(op, op.files, sketches) + 6.0e9;
+  *need_gb = need / 1e9;
+  return exceeds_device(op, need);
+}
 
-// The store path of triangle: files are sketched (or .sketch files imported) in groups, each group's set is added to a host
-// sketch store and freed, so device memory holds one group at a time and host memory one group of sequence plus the
+// dist: the same estimate per context, where the references are split over --gpus contexts and every context holds the
+// whole query set
+bool dist_needs_store(const Opts& op, bool refs_sketch, bool queries_sketch, double* need_gb) {
+  const double need = sketch_bytes_estimate(op, op.refs, refs_sketch) / std::max(op.gpus, 1) + sketch_bytes_estimate(op, op.queries, queries_sketch) + 6.0e9;
+  *need_gb = need / 1e9;
+  return exceeds_device(op, need);
+}
+
+// Host sketches (read_sketch_files' order) imported in groups of < 2^28 records, each group added to a new store and freed;
+// hs is emptied along the way.
+sk_sketch_store* store_from_sketches(sk_ctx* ctx, std::vector<skdb::HostSketch>& hs, const sk_sketch_params& sp) {
+  sk_sketch_store* st = nullptr;
+  CK(ctx, sk_sketch_store_create(&sp, &st));
+  for (size_t a = 0; a < hs.size();) {
+    size_t b = a;
+    uint64_t recs = 0;
+    while (b < hs.size() && (b == a || recs + hs[b].kmer.size() < (1ull << 28))) recs += hs[b++].kmer.size();
+    sk_sketch_set* set = import_sketches(ctx, hs, a, b, sp);
+    CK(ctx, sk_sketch_store_add(st, set));
+    sk_sketch_set_free(set);
+    for (size_t i = a; i < b; i++) hs[i] = skdb::HostSketch();
+    a = b;
+  }
+  return st;
+}
+
+// The store path of triangle and dist: files are sketched (or .sketch files imported) in groups, each group's set is added to a
+// host sketch store and freed, so device memory holds one group at a time and host memory one group of sequence plus the
 // sketches.  genomes gets the metadata of every genome in store order (= the order of the in-memory path).
-sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, bool sketches, std::vector<Genome>& genomes, sk_sketch_params& sp) {
+sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, const std::vector<std::string>& input_files, bool individual, bool sketches,
+                            std::vector<Genome>& genomes, sk_sketch_params& sp) {
   if (sketches) {
     fprintf(stderr, "INFO Sketches detected.\n");
     skdb::DiskParams dp;
     std::vector<skdb::HostSketch> hs;
-    read_sketch_files(op.files, dp, genomes, hs);
+    read_sketch_files(input_files, dp, genomes, hs);
     if (hs.empty()) return nullptr;
     if (dp.c != op.c || dp.marker_c != op.m)
       fprintf(stderr, "WARN Input parameter c = %u, m = %u is not equal to the sketch parameter c = %llu,m = %llu. Using sketch parameters.\n", op.c, op.m,
               (unsigned long long)dp.c, (unsigned long long)dp.marker_c);
     sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
-    sk_sketch_store* st = nullptr;
-    CK(ctx, sk_sketch_store_create(&sp, &st));
-    for (size_t a = 0; a < hs.size();) {      // import groups of < 2^28 records
-      size_t b = a;
-      uint64_t recs = 0;
-      while (b < hs.size() && (b == a || recs + hs[b].kmer.size() < (1ull << 28))) recs += hs[b++].kmer.size();
-      sk_sketch_set* set = import_sketches(ctx, hs, a, b, sp);
-      CK(ctx, sk_sketch_store_add(st, set));
-      sk_sketch_set_free(set);
-      for (size_t i = a; i < b; i++) hs[i] = skdb::HostSketch();
-      a = b;
-    }
-    return st;
+    return store_from_sketches(ctx, hs, sp);
   }
   sk_sketch_store* st = nullptr;
   CK(ctx, sk_sketch_store_create(&sp, &st));
-  std::vector<std::string> files = op.files;
+  std::vector<std::string> files = input_files;
   std::sort(files.begin(), files.end());
   for (size_t f0 = 0; f0 < files.size();) {
     const size_t f1 = file_group_end(files, f0);
     Inputs in;
-    load_inputs(std::vector<std::string>(files.begin() + f0, files.begin() + f1), op.individual, std::max(op.threads, 1), in);
+    load_inputs(std::vector<std::string>(files.begin() + f0, files.begin() + f1), individual, std::max(op.threads, 1), in);
     f0 = f1;
     if (in.genomes.empty()) continue;
     sk_sketch_set* set = sketch(ctx, in, sp);
@@ -426,7 +448,7 @@ int run_triangle(Opts& op) {
   if (use_store) {
     fprintf(stderr, "INFO Store path: sketches (~%.1f GB estimated) are kept in a host sketch store and chained in working sets on GPU %d%s.\n", need_gb,
             op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
-    store = fill_store(ctx, op, refs_are_sketch, in.genomes, sp);
+    store = fill_store(ctx, op, op.files, op.individual, refs_are_sketch, in.genomes, sp);
     if (!store) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }
   } else if (refs_are_sketch) {      // src/triangle.rs:16-24
     fprintf(stderr, "INFO Sketches detected.\n");
@@ -565,6 +587,32 @@ int run_triangle(Opts& op) {
   return 0;
 }
 
+// write_query_ref_list (src/file_io.rs:608-678) of dist: queries in blocks of INTERMEDIATE_WRITE_COUNT (src/dist.rs:151-175).
+// block(q0, q1, res) fills res with the results of the queries [q0, q1) in (query, ref) order; each block is grouped by the
+// query's first contig name, each group sorted by ANI (descending, stable) and its top n written, then flushed.
+template <class F>
+int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vector<Genome>& queries, F block) {
+  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
+  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
+  write_header(o, op.ci, op.detailed);
+  const size_t FL = intermediate_write_count(), NQ = queries.size();
+  std::vector<sk_ani_result> res;
+  for (size_t q0 = 0; q0 < NQ; q0 += FL) {
+    block(q0, std::min(q0 + FL, NQ), res);
+    std::map<std::string, std::vector<const sk_ani_result*>> groups;
+    for (auto& r : res) if (r.ani > 0.1f) groups[queries[r.query_id].contigs[0]].push_back(&r);
+    for (auto& kv : groups) {
+      auto v = kv.second;
+      std::stable_sort(v.begin(), v.end(), [](const sk_ani_result* a, const sk_ani_result* b) { return a->ani > b->ani; });
+      for (size_t i = 0; i < v.size() && i < op.n; i++) write_row(o, *v[i], refs[v[i]->ref_id], queries[v[i]->query_id], op);
+    }
+    fflush(o);
+    if (q0 + FL < NQ) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", FL);
+  }
+  if (o != stdout) fclose(o);
+  return 0;
+}
+
 int run_dist(Opts& op) {
   resolve_presets(op);
   if (op.refs.empty() || op.queries.empty()) { fprintf(stderr, "ERROR No reference sketches/genomes or query sketches/genomes found.\n"); return 1; }
@@ -595,8 +643,19 @@ int run_dist(Opts& op) {
       sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
     }
   }
-  if (!refs_are_sketch) load_inputs(op.refs, op.ri, std::max(op.threads, 1), rin);
-  if (!queries_are_sketch) load_inputs(op.queries, op.qi, std::max(op.threads, 1), qin);
+  // store path: both sides go into host sketch stores in groups and are chained in working sets (sk_query_ref_store)
+  double need_gb = 0;
+  const bool use_store = dist_needs_store(op, refs_are_sketch, queries_are_sketch, &need_gb);
+  sk_sketch_store *rstore = nullptr, *qstore = nullptr;
+  if (use_store) {
+    fprintf(stderr, "INFO Store path: sketches (~%.1f GB per context estimated) are kept in host sketch stores and chained in working sets on %d GPU(s) from GPU %d%s.\n",
+            need_gb, std::max(op.gpus, 1), op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
+    rstore = refs_are_sketch ? store_from_sketches(ctx, rhs, sp) : fill_store(ctx, op, op.refs, op.ri, false, rin.genomes, sp);
+    qstore = queries_are_sketch ? store_from_sketches(ctx, qhs, sp) : fill_store(ctx, op, op.queries, op.qi, false, qin.genomes, sp);
+  } else {
+    if (!refs_are_sketch) load_inputs(op.refs, op.ri, std::max(op.threads, 1), rin);
+    if (!queries_are_sketch) load_inputs(op.queries, op.qi, std::max(op.threads, 1), qin);
+  }
   if (rin.genomes.empty() || qin.genomes.empty()) { fprintf(stderr, "ERROR No reference sketches/genomes or query sketches/genomes found.\n"); return 1; }
   sk_map_params mp{};
   mp.screen_val = op.s / 100.0;
@@ -619,6 +678,40 @@ int run_dist(Opts& op) {
       if (i && names[i].first != names[i - 1].first) rank++;
       (names[i].second.first ? qr : rr)[names[i].second.second] = rank;
     }
+  }
+  if (use_store) {
+    // two contexts on each of the --gpus devices: one gathers its next working set over PCIe while the other chains.  Every
+    // block of queries is written at the end, through the same writer as the in-memory path.
+    CK(ctx, sk_sketch_store_set_name_ranks(rstore, rr.data()));
+    CK(ctx, sk_sketch_store_set_name_ranks(qstore, qr.data()));
+    const int ndev = std::max(sk_device_count(), 1), gpus = std::max(op.gpus, 1);
+    if (ndev < gpus) fprintf(stderr, "WARN --gpus %d but %d CUDA device(s) visible: contexts share devices.\n", gpus, ndev);
+    std::vector<sk_ctx*> sctx(1, ctx);
+    for (int d = 0; d < gpus; d++)
+      for (int k = d == 0; k < 2; k++) {
+        const int dev = (op.device + d) % ndev;
+        sk_ctx* c = nullptr;
+        if (sk_ctx_create(dev, &c) != 0) { fprintf(stderr, "ERROR cannot create a context on GPU %d\n", dev); return 1; }
+        sctx.push_back(c);
+      }
+    uint64_t budget = 0;
+    if (const char* e = getenv("SK_DEVICE_BUDGET_MB")) budget = (uint64_t)std::max(1ll, atoll(e)) << 20;
+    sk_ani_result* r = nullptr; uint64_t nr = 0;
+    CK(ctx, sk_query_ref_store(sctx.data(), (uint32_t)sctx.size(), rstore, qstore, &mp, use_index ? 2 : 0, budget, &r, &nr, nullptr));
+    std::vector<sk_ani_result> all(r, r + nr);
+    sk_free(r);
+    std::sort(all.begin(), all.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.query_id != b.query_id ? a.query_id < b.query_id : a.ref_id < b.ref_id; });
+    size_t p0 = 0;
+    const int rc = write_dist(op, rin.genomes, qin.genomes, [&](size_t, size_t q1, std::vector<sk_ani_result>& res) {
+      size_t p1 = p0;
+      while (p1 < all.size() && all[p1].query_id < q1) p1++;
+      res.assign(all.begin() + p0, all.begin() + p1);
+      p0 = p1;
+    });
+    sk_sketch_store_free(rstore);
+    sk_sketch_store_free(qstore);
+    for (size_t d = sctx.size(); d-- > 0;) sk_ctx_destroy(sctx[d]);
+    return rc;
   }
   // --gpus N: the references in W contiguous blocks (genome order, balanced by bases, or by records for .sketch inputs), each
   // sketched or imported on its own context; the queries once on context 0, then copied to the others
@@ -653,33 +746,17 @@ int run_dist(Opts& op) {
   std::vector<uint64_t> byq(pairs, pairs + np);
   sk_free(pairs);
   std::sort(byq.begin(), byq.end(), [](uint64_t a, uint64_t b) { return (uint32_t)a != (uint32_t)b ? (uint32_t)a < (uint32_t)b : a < b; });
-  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
-  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
-  write_header(o, op.ci, op.detailed);
-  const size_t FL = intermediate_write_count(), NQ = qin.genomes.size();
   size_t p0 = 0;
-  std::vector<sk_ani_result> res;
-  for (size_t q0 = 0; q0 < NQ; q0 += FL) {
+  const int rc = write_dist(op, rin.genomes, qin.genomes, [&](size_t, size_t q1, std::vector<sk_ani_result>& res) {
     size_t p1 = p0;
-    while (p1 < byq.size() && (uint32_t)byq[p1] < q0 + FL) p1++;
+    while (p1 < byq.size() && (uint32_t)byq[p1] < q1) p1++;
     res.resize(p1 - p0);
     CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), byq.data() + p0, p1 - p0, &mp, res.data()));
-    // write_query_ref_list (src/file_io.rs:608-678): group by the query's first contig name, sort each group by ANI desc, top n
-    std::map<std::string, std::vector<const sk_ani_result*>> groups;
-    for (auto& r : res) if (r.ani > 0.1f) groups[qin.genomes[r.query_id].contigs[0]].push_back(&r);
-    for (auto& kv : groups) {
-      auto v = kv.second;
-      std::stable_sort(v.begin(), v.end(), [](const sk_ani_result* a, const sk_ani_result* b) { return a->ani > b->ani; });
-      for (size_t i = 0; i < v.size() && i < op.n; i++) write_row(o, *v[i], rin.genomes[v[i]->ref_id], qin.genomes[v[i]->query_id], op);
-    }
-    fflush(o);
-    if (q0 + FL < NQ) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", FL);
     p0 = p1;
-  }
-  if (o != stdout) fclose(o);
+  });
   for (size_t d = 0; d < W; d++) { sk_sketch_set_free(rsets[d]); sk_sketch_set_free(qsets[d]); }
   for (size_t d = W; d-- > 0;) sk_ctx_destroy(ctxs[d]);
-  return 0;
+  return rc;
 }
 
 // ---- sketch / search (src/sketch.rs, src/search.rs) --------------------------------------------------------------

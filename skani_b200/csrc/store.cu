@@ -7,7 +7,9 @@
 // pulls them over PCIe straight into a device blob in the layout sk_sketch_set_unpack reads (no host-side copy, no staging
 // buffer), and the existing unpack builds the set without rebuilding the tables.
 // sk_triangle_store screens the markers of every genome, plans working sets (ws_plan.hpp) and lets one host thread per
-// context gather and chain them in plan order.
+// context gather and chain them in plan order.  sk_query_ref_store does the same for every (reference, query) pair of two
+// stores: one marker screen of all references against all queries, working sets that each hold some references and some
+// queries, gathered from their own stores.
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -74,6 +76,83 @@ int batched_copy(sk_ctx* ctx, const std::vector<const void*>& src, const std::ve
 }
 
 bool same_params(const sk_sketch_params& a, const sk_sketch_params& b) { return a.c == b.c && a.k == b.k && a.marker_c == b.marker_c; }
+
+// NULL or repeated contexts (each context gets its own host thread) give SK_ERR_PARAM with the message on ctxs[0]
+int check_contexts(sk_ctx* const* ctxs, uint32_t n_ctx) {
+  for (uint32_t d = 0; d < n_ctx; d++) {
+    if (!ctxs[d]) { ctxs[0]->err = "context " + std::to_string(d) + ": NULL context"; return SK_ERR_PARAM; }
+    for (uint32_t e = 0; e < d; e++)
+      if (ctxs[e] == ctxs[d]) { ctxs[0]->err = "context " + std::to_string(d) + ": the same context appears twice (one host thread per context)"; return SK_ERR_PARAM; }
+  }
+  return SK_OK;
+}
+
+// budget per context: a working set's sketches, its gather blob (as large) and the chaining workspace share the device with
+// the other contexts on it, so a third of each context's share of the free memory (80 % of it)
+int working_set_budget(sk_ctx* const* ctxs, uint32_t n_ctx, uint64_t device_budget, uint64_t* budget) {
+  *budget = device_budget;
+  if (device_budget) return SK_OK;
+  sk_ctx* ctx = ctxs[0];
+  uint64_t b = ~0ull;
+  for (uint32_t d = 0; d < n_ctx; d++) {
+    uint32_t same = 0;
+    for (uint32_t e = 0; e < n_ctx; e++) same += ctxs[e]->device == ctxs[d]->device;
+    size_t free_b = 0, total_b = 0;
+    SK_CUDA(cudaSetDevice(ctxs[d]->device));
+    SK_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    b = std::min<uint64_t>(b, (uint64_t)(0.8 * (double)free_b / (3.0 * same)));
+  }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  *budget = b;
+  return SK_OK;
+}
+
+struct WsTimes { double gather = 0, chain = 0; uint64_t bytes = 0; };
+
+// One host thread per context takes the working sets [0, n_sets) in plan order through an atomic counter;
+// work(c, d, w, kept, times) gathers and chains working set w on context c = ctxs[d] and appends the results it keeps.  The
+// first failure stops every context and its message goes to ctxs[0].  res: every kept result, sorted by (ref_id, query_id).
+template <class F>
+int run_working_sets(sk_ctx* const* ctxs, uint32_t n_ctx, size_t n_sets, F work, std::vector<sk_ani_result>& res, WsTimes& total) {
+  sk_ctx* ctx = ctxs[0];
+  std::atomic<size_t> next{0};
+  std::atomic<bool> failed{false};
+  std::vector<std::vector<sk_ani_result>> kept(n_ctx);
+  std::vector<WsTimes> times(n_ctx);
+  std::vector<int> rcs(n_ctx, SK_OK);
+  auto run = [&](uint32_t d) {
+    sk_ctx* c = ctxs[d];
+    if (cudaSetDevice(c->device) != cudaSuccess) { c->err = "cudaSetDevice failed"; rcs[d] = SK_ERR_CUDA; failed = true; return; }
+    for (size_t w; !failed && (w = next.fetch_add(1)) < n_sets;) {
+      const int rc = work(c, d, w, kept[d], times[d]);
+      if (rc != SK_OK) { rcs[d] = rc; failed = true; }
+    }
+  };
+  if (n_ctx == 1) run(0);
+  else {
+    std::vector<std::thread> th;
+    for (uint32_t d = 0; d < n_ctx; d++) th.emplace_back(run, d);
+    for (auto& t : th) t.join();
+  }
+  cudaSetDevice(ctx->device);
+  for (uint32_t d = 0; d < n_ctx; d++)
+    if (rcs[d] != SK_OK) { if (d) ctx->err = "context " + std::to_string(d) + ": " + ctxs[d]->err; return rcs[d]; }
+  for (uint32_t d = 0; d < n_ctx; d++) {
+    res.insert(res.end(), kept[d].begin(), kept[d].end());
+    total.gather += times[d].gather; total.chain += times[d].chain; total.bytes += times[d].bytes;
+  }
+  std::sort(res.begin(), res.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
+  return SK_OK;
+}
+
+// results as a malloc'd array (sk_free)
+int hand_out(sk_ctx* ctx, const std::vector<sk_ani_result>& res, sk_ani_result** out, uint64_t* n_out) {
+  sk_ani_result* o = (sk_ani_result*)malloc(sizeof(sk_ani_result) * std::max<size_t>(res.size(), 1));
+  if (!o) { ctx->err = "out of host memory"; return SK_ERR_NOMEM; }
+  if (!res.empty()) memcpy(o, res.data(), res.size() * sizeof(sk_ani_result));
+  *out = o; *n_out = res.size();
+  return SK_OK;
+}
 
 }  // namespace
 
@@ -279,27 +358,10 @@ int sk_triangle_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store
   sk_ctx* ctx = ctxs[0];
   if (!st || !mp || !out || !n_out) { ctx->err = "sk_triangle_store: NULL argument"; return SK_ERR_PARAM; }
   *out = nullptr; *n_out = 0;
-  for (uint32_t d = 0; d < n_ctx; d++) {
-    if (!ctxs[d]) { ctx->err = "context " + std::to_string(d) + ": NULL context"; return SK_ERR_PARAM; }
-    for (uint32_t e = 0; e < d; e++)
-      if (ctxs[e] == ctxs[d]) { ctx->err = "context " + std::to_string(d) + ": the same context appears twice (one host thread per context)"; return SK_ERR_PARAM; }
-  }
+  SK_TRY(check_contexts(ctxs, n_ctx));
   const uint32_t N = (uint32_t)st->g.size();
-  // budget per context: a working set's sketches, its gather blob (as large) and the chaining workspace share the device with
-  // the other contexts on it, so a third of each context's share of the free memory (80 % of it)
-  uint64_t budget = device_budget;
-  if (budget == 0) {
-    budget = ~0ull;
-    for (uint32_t d = 0; d < n_ctx; d++) {
-      uint32_t same = 0;
-      for (uint32_t e = 0; e < n_ctx; e++) same += ctxs[e]->device == ctxs[d]->device;
-      size_t free_b = 0, total_b = 0;
-      SK_CUDA(cudaSetDevice(ctxs[d]->device));
-      SK_CUDA(cudaMemGetInfo(&free_b, &total_b));
-      budget = std::min<uint64_t>(budget, (uint64_t)(0.8 * (double)free_b / (3.0 * same)));
-    }
-    SK_CUDA(cudaSetDevice(ctx->device));
-  }
+  uint64_t budget = 0;
+  SK_TRY(working_set_budget(ctxs, n_ctx, device_budget, &budget));
   std::vector<uint64_t> gbytes(N);
   for (uint32_t g = 0; g < N; g++) gbytes[g] = sk_sketch_store_genome_bytes(st, g);
   for (uint32_t g = 0; g < N; g++)
@@ -331,66 +393,138 @@ int sk_triangle_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store
   if (!skws::plan_working_sets(pairs, gbytes, budget, plan, perr)) { ctx->err = "sk_triangle_store: " + perr; return SK_ERR_NOMEM; }
   // ---- 3. contexts take the working sets in plan order
   const bool trace = getenv("SK_TRACE") != nullptr;
-  std::atomic<size_t> next{0};
-  std::atomic<bool> failed{false};
-  std::vector<std::vector<sk_ani_result>> kept(n_ctx);
-  std::vector<double> tg(n_ctx, 0), tc(n_ctx, 0);
-  std::vector<uint64_t> gathered(n_ctx, 0);
-  std::vector<int> rcs(n_ctx, SK_OK);
-  auto run = [&](uint32_t d) {
-    sk_ctx* c = ctxs[d];
-    if (cudaSetDevice(c->device) != cudaSuccess) { c->err = "cudaSetDevice failed"; rcs[d] = SK_ERR_CUDA; failed = true; return; }
-    for (size_t w; !failed && (w = next.fetch_add(1)) < plan.sets.size();) {
-      const skws::WorkingSet& ws = plan.sets[w];
-      const double a = now_s();
-      sk_sketch_set* set = nullptr;
-      int rc = sk_sketch_store_gather(c, st, ws.genomes.data(), (uint32_t)ws.genomes.size(), 0, &set);
-      const double bt = now_s();
-      if (rc == SK_OK) {
-        std::vector<uint64_t> lp(ws.pairs.size());
-        for (size_t i = 0; i < lp.size(); i++) {
-          const uint64_t x = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)(ws.pairs[i] >> 32)) - ws.genomes.begin();
-          const uint64_t y = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)ws.pairs[i]) - ws.genomes.begin();
-          lp[i] = (x << 32) | y;
-        }
-        std::vector<sk_ani_result> res(lp.size());
-        rc = sk_chain_pairs(c, set, set, lp.data(), lp.size(), mp, res.data());
-        if (rc == SK_OK)
-          for (auto& r : res)
-            if (r.ani > 0.1f) { r.ref_id = ws.genomes[r.ref_id]; r.query_id = ws.genomes[r.query_id]; kept[d].push_back(r); }   // src/triangle.rs:99
+  auto work = [&](sk_ctx* c, uint32_t d, size_t w, std::vector<sk_ani_result>& kept, WsTimes& t) {
+    const skws::WorkingSet& ws = plan.sets[w];
+    const double a = now_s();
+    sk_sketch_set* set = nullptr;
+    int rc = sk_sketch_store_gather(c, st, ws.genomes.data(), (uint32_t)ws.genomes.size(), 0, &set);
+    const double bt = now_s();
+    if (rc == SK_OK) {
+      std::vector<uint64_t> lp(ws.pairs.size());
+      for (size_t i = 0; i < lp.size(); i++) {
+        const uint64_t x = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)(ws.pairs[i] >> 32)) - ws.genomes.begin();
+        const uint64_t y = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)ws.pairs[i]) - ws.genomes.begin();
+        lp[i] = (x << 32) | y;
       }
-      if (set) sk_sketch_set_free(set);
-      const double ct = now_s();
-      tg[d] += bt - a; tc[d] += ct - bt; gathered[d] += ws.bytes;
-      if (trace)
-        fprintf(stderr, "[sk_triangle_store] context %u: working set %zu/%zu%s: %zu genomes, %zu pairs, %.1f MB gathered in %.1f ms, chain %.1f ms\n", d, w + 1,
-                plan.sets.size(), ws.chunk_pair ? " (chunk pair)" : "", ws.genomes.size(), ws.pairs.size(), ws.bytes / 1e6, (bt - a) * 1e3, (ct - bt) * 1e3);
-      if (rc != SK_OK) { rcs[d] = rc; failed = true; }
+      std::vector<sk_ani_result> res(lp.size());
+      rc = sk_chain_pairs(c, set, set, lp.data(), lp.size(), mp, res.data());
+      if (rc == SK_OK)
+        for (auto& r : res)
+          if (r.ani > 0.1f) { r.ref_id = ws.genomes[r.ref_id]; r.query_id = ws.genomes[r.query_id]; kept.push_back(r); }   // src/triangle.rs:99
     }
+    if (set) sk_sketch_set_free(set);
+    const double ct = now_s();
+    t.gather += bt - a; t.chain += ct - bt; t.bytes += ws.bytes;
+    if (trace)
+      fprintf(stderr, "[sk_triangle_store] context %u: working set %zu/%zu%s: %zu genomes, %zu pairs, %.1f MB gathered in %.1f ms, chain %.1f ms\n", d, w + 1,
+              plan.sets.size(), ws.chunk_pair ? " (chunk pair)" : "", ws.genomes.size(), ws.pairs.size(), ws.bytes / 1e6, (bt - a) * 1e3, (ct - bt) * 1e3);
+    return rc;
   };
-  if (n_ctx == 1) run(0);
-  else {
-    std::vector<std::thread> th;
-    for (uint32_t d = 0; d < n_ctx; d++) th.emplace_back(run, d);
-    for (auto& t : th) t.join();
-  }
-  cudaSetDevice(ctx->device);
-  for (uint32_t d = 0; d < n_ctx; d++)
-    if (rcs[d] != SK_OK) { if (d) ctx->err = "context " + std::to_string(d) + ": " + ctxs[d]->err; return rcs[d]; }
   std::vector<sk_ani_result> res;
-  for (auto& v : kept) res.insert(res.end(), v.begin(), v.end());
-  std::sort(res.begin(), res.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
-  sk_ani_result* o = (sk_ani_result*)malloc(sizeof(sk_ani_result) * std::max<size_t>(res.size(), 1));
-  if (!o) { ctx->err = "out of host memory"; return SK_ERR_NOMEM; }
-  if (!res.empty()) memcpy(o, res.data(), res.size() * sizeof(sk_ani_result));
-  *out = o; *n_out = res.size();
+  WsTimes t;
+  SK_TRY(run_working_sets(ctxs, n_ctx, plan.sets.size(), work, res, t));
+  SK_TRY(hand_out(ctx, res, out, n_out));
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->n_working_sets = (uint32_t)plan.sets.size();
     stats->n_split_components = plan.n_split_components;
     for (auto& ws : plan.sets) stats->max_working_set_bytes = std::max(stats->max_working_set_bytes, ws.bytes);
     stats->t_screen = t_screen;
-    for (uint32_t d = 0; d < n_ctx; d++) { stats->gathered_bytes += gathered[d]; stats->t_gather += tg[d]; stats->t_chain += tc[d]; }
+    stats->gathered_bytes = t.bytes; stats->t_gather = t.gather; stats->t_chain = t.chain;
+  }
+  return SK_OK;
+}
+
+int sk_query_ref_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* refs, const sk_sketch_store* queries, const sk_map_params* mp,
+                       int mode, uint64_t device_budget, sk_ani_result** out, uint64_t* n_out, sk_store_stats* stats) {
+  if (!ctxs || n_ctx == 0 || !ctxs[0]) return SK_ERR_PARAM;
+  sk_ctx* ctx = ctxs[0];
+  if (!refs || !queries || !mp || !out || !n_out) { ctx->err = "sk_query_ref_store: NULL argument"; return SK_ERR_PARAM; }
+  *out = nullptr; *n_out = 0;
+  if (mode < 0 || mode > 3) { ctx->err = "sk_query_ref_store: mode " + std::to_string(mode) + " is not 0-3"; return SK_ERR_PARAM; }
+  if (!same_params(refs->sp, queries->sp)) { ctx->err = "sk_query_ref_store: the stores' sketch parameters differ"; return SK_ERR_PARAM; }
+  SK_TRY(check_contexts(ctxs, n_ctx));
+  const uint32_t NR = (uint32_t)refs->g.size(), NQ = (uint32_t)queries->g.size();
+  uint64_t budget = 0;
+  SK_TRY(working_set_budget(ctxs, n_ctx, device_budget, &budget));
+  std::vector<uint64_t> rbytes(NR), qbytes(NQ);
+  for (uint32_t g = 0; g < NR; g++) rbytes[g] = sk_sketch_store_genome_bytes(refs, g);
+  for (uint32_t g = 0; g < NQ; g++) qbytes[g] = sk_sketch_store_genome_bytes(queries, g);
+  for (int side = 0; side < 2; side++) {
+    const std::vector<uint64_t>& b = side ? qbytes : rbytes;
+    for (size_t g = 0; g < b.size(); g++)
+      if (b[g] > budget / 2) {
+        ctx->err = std::string("sk_query_ref_store: ") + (side ? "query " : "reference ") + std::to_string(g) + " needs " + std::to_string(b[g]) +
+                   " device bytes, more than half the working-set budget of " + std::to_string(budget) + " bytes";
+        return SK_ERR_NOMEM;
+      }
+  }
+  // ---- 1. screen: markers of every reference and every query on context 0
+  const double t0 = now_s();
+  std::vector<uint64_t> pairs;
+  if (NR && NQ) {
+    SK_CUDA(cudaSetDevice(ctx->device));
+    sk_sketch_set *rm = nullptr, *qm = nullptr;
+    std::vector<uint32_t> all(std::max(NR, NQ));
+    for (uint32_t g = 0; g < all.size(); g++) all[g] = g;
+    int rc = sk_sketch_store_gather(ctx, refs, all.data(), NR, SK_PACK_MARKERS_ONLY, &rm);
+    if (rc == SK_OK) rc = sk_sketch_store_gather(ctx, queries, all.data(), NQ, SK_PACK_MARKERS_ONLY, &qm);
+    uint64_t* p = nullptr; uint64_t np = 0;
+    if (rc == SK_OK) rc = sk_screen_query_ref(ctx, rm, qm, mp, mode, &p, &np);
+    if (rm) sk_sketch_set_free(rm);
+    if (qm) sk_sketch_set_free(qm);
+    SK_TRY(rc);
+    pairs.assign(p, p + np);    // sorted (r << 32 | q)
+    sk_free(p);
+  }
+  const double t_screen = now_s() - t0;
+  // ---- 2. plan
+  skws::QrPlan plan;
+  std::string perr;
+  if (!skws::plan_query_ref_working_sets(pairs, rbytes, qbytes, budget, plan, perr)) { ctx->err = "sk_query_ref_store: " + perr; return SK_ERR_NOMEM; }
+  // ---- 3. contexts take the working sets in plan order: gather the references and the queries, chain, keep ani > 0.1
+  const bool trace = getenv("SK_TRACE") != nullptr;
+  auto work = [&](sk_ctx* c, uint32_t d, size_t w, std::vector<sk_ani_result>& kept, WsTimes& t) {
+    const skws::QrWorkingSet& ws = plan.sets[w];
+    const double a = now_s();
+    sk_sketch_set *R = nullptr, *Q = nullptr;
+    int rc = sk_sketch_store_gather(c, refs, ws.refs.data(), (uint32_t)ws.refs.size(), 0, &R);
+    if (rc == SK_OK) rc = sk_sketch_store_gather(c, queries, ws.queries.data(), (uint32_t)ws.queries.size(), 0, &Q);
+    const double bt = now_s();
+    if (rc == SK_OK) {
+      std::vector<uint64_t> lp(ws.pairs.size());
+      for (size_t i = 0; i < lp.size(); i++) {
+        const uint64_t x = std::lower_bound(ws.refs.begin(), ws.refs.end(), (uint32_t)(ws.pairs[i] >> 32)) - ws.refs.begin();
+        const uint64_t y = std::lower_bound(ws.queries.begin(), ws.queries.end(), (uint32_t)ws.pairs[i]) - ws.queries.begin();
+        lp[i] = (x << 32) | y;
+      }
+      std::vector<sk_ani_result> res(lp.size());
+      rc = sk_chain_pairs(c, R, Q, lp.data(), lp.size(), mp, res.data());
+      if (rc == SK_OK)
+        for (auto& r : res)
+          if (r.ani > 0.1f) { r.ref_id = ws.refs[r.ref_id]; r.query_id = ws.queries[r.query_id]; kept.push_back(r); }   // src/dist.rs:115,139
+    }
+    if (R) sk_sketch_set_free(R);
+    if (Q) sk_sketch_set_free(Q);
+    const double ct = now_s();
+    t.gather += bt - a; t.chain += ct - bt; t.bytes += ws.bytes;
+    if (trace)
+      fprintf(stderr, "[sk_query_ref_store] context %u: working set %zu/%zu%s: %zu references, %zu queries, %zu pairs, %.1f MB gathered in %.1f ms, chain %.1f ms\n",
+              d, w + 1, plan.sets.size(), ws.chunk_pair ? " (chunk pair)" : "", ws.refs.size(), ws.queries.size(), ws.pairs.size(), ws.bytes / 1e6,
+              (bt - a) * 1e3, (ct - bt) * 1e3);
+    return rc;
+  };
+  std::vector<sk_ani_result> res;
+  WsTimes t;
+  SK_TRY(run_working_sets(ctxs, n_ctx, plan.sets.size(), work, res, t));
+  SK_TRY(hand_out(ctx, res, out, n_out));
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->n_working_sets = (uint32_t)plan.sets.size();
+    stats->n_split_components = plan.n_split_components;
+    for (auto& ws : plan.sets) stats->max_working_set_bytes = std::max(stats->max_working_set_bytes, ws.bytes);
+    stats->t_screen = t_screen;
+    stats->gathered_bytes = t.bytes; stats->t_gather = t.gather; stats->t_chain = t.chain;
   }
   return SK_OK;
 }

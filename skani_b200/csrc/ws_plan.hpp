@@ -1,4 +1,5 @@
-// ws_plan.hpp -- working-set planner of sk_triangle_store (host only, no CUDA: tests/emu/emu_ws_plan.cpp runs it on the CPU).
+// ws_plan.hpp -- working-set planner of sk_triangle_store and sk_query_ref_store (host only, no CUDA: tests/emu/emu_ws_plan.cpp
+// and tests/emu/emu_qr_plan.cpp run it on the CPU).
 //
 // The triangle's screened pairs are cut into working sets: groups of pairs whose genomes, gathered from the host sketch
 // store, fit a device budget.  A pair's chain result depends only on its two sketches, so every pair is chained in exactly
@@ -128,6 +129,56 @@ inline bool plan_working_sets(const std::vector<uint64_t>& sorted_pairs, const s
       plan.sets.push_back(std::move(ws));
       i = j;
     }
+  }
+  return true;
+}
+
+// ---- query x reference (sk_query_ref_store) ----------------------------------------------------------------------------
+struct QrWorkingSet {
+  std::vector<uint32_t> refs;      // ascending reference ids
+  std::vector<uint32_t> queries;   // ascending query ids
+  std::vector<uint64_t> pairs;     // global (r << 32 | q), sorted
+  uint64_t bytes = 0;              // sum of the genomes' bytes
+  bool chunk_pair = false;
+};
+
+struct QrPlan {
+  std::vector<QrWorkingSet> sets;
+  uint32_t n_split_components = 0;
+};
+
+// The bipartite pair graph as one genome graph: reference r is genome r, query q is genome NR + q, so pairs sorted by (r, q)
+// stay sorted and keep i < j.  plan_working_sets cuts it; each working set's genome list splits at NR.  References come first
+// in id order, so a component over budget with few queries and many references is cut into reference chunks plus a last chunk
+// holding the queries: every reference is gathered once.
+inline bool plan_query_ref_working_sets(const std::vector<uint64_t>& sorted_pairs_rq, const std::vector<uint64_t>& ref_bytes,
+                                        const std::vector<uint64_t>& query_bytes, uint64_t budget, QrPlan& plan, std::string& err) {
+  plan = QrPlan();
+  const uint64_t NR = ref_bytes.size();
+  if (NR + query_bytes.size() >= (1ull << 32)) { err = "more than 2^32 references and queries together"; return false; }
+  std::vector<uint64_t> bytes(ref_bytes);
+  bytes.insert(bytes.end(), query_bytes.begin(), query_bytes.end());
+  for (uint64_t g = 0; g < bytes.size(); g++)
+    if (bytes[g] > budget / 2) {
+      err = (g < NR ? "reference " + std::to_string(g) : "query " + std::to_string(g - NR)) + " needs " + std::to_string(bytes[g]) +
+            " device bytes, more than half the working-set budget of " + std::to_string(budget) + " bytes";
+      return false;
+    }
+  std::vector<uint64_t> pairs(sorted_pairs_rq.size());
+  for (size_t i = 0; i < pairs.size(); i++) pairs[i] = sorted_pairs_rq[i] + NR;   // (r << 32) | (NR + q)
+  Plan p;
+  if (!plan_working_sets(pairs, bytes, budget, p, err)) return false;
+  plan.n_split_components = p.n_split_components;
+  for (WorkingSet& ws : p.sets) {
+    QrWorkingSet q;
+    const size_t cut = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)NR) - ws.genomes.begin();
+    q.refs.assign(ws.genomes.begin(), ws.genomes.begin() + cut);
+    for (size_t i = cut; i < ws.genomes.size(); i++) q.queries.push_back(ws.genomes[i] - (uint32_t)NR);
+    q.pairs.resize(ws.pairs.size());
+    for (size_t i = 0; i < ws.pairs.size(); i++) q.pairs[i] = ws.pairs[i] - NR;
+    q.bytes = ws.bytes;
+    q.chunk_pair = ws.chunk_pair;
+    plan.sets.push_back(std::move(q));
   }
   return true;
 }

@@ -517,3 +517,18 @@ def triangle_store(ctxs, store, mp=None, device_budget=0, as_array=True):
     c0 = ctxs[0]
     c0.check(c0.L.sk_triangle_store(hs, len(ctxs), store.h, C.byref(mp), int(device_budget), C.byref(out), C.byref(n), C.byref(st)))
     return _take_results(c0, out, n, as_array), st
+
+
+def query_ref_store(ctxs, ref_store, query_store, mp=None, mode=0, device_budget=0, as_array=True):
+    """sk_query_ref_store: screen_query_ref (mode 0-3) + chain_pairs of every reference of ref_store against every query of
+    query_store (the same store may be both), chained in working sets of at most device_budget bytes per context (0 = derived
+    from free device memory).  Both stores' name ranks are used as stored: rank both sides in one file-name order.
+    Returns (results with ani > 0.1 sorted by (ref_id, query_id), StoreStats)."""
+    ctxs = list(ctxs) if isinstance(ctxs, (list, tuple)) else [ctxs]
+    mp = mp or map_params()
+    hs = (C.c_void_p * len(ctxs))(*[None if c is None else c.h for c in ctxs])
+    out = C.POINTER(AniResult)(); n = C.c_uint64(); st = StoreStats()
+    c0 = ctxs[0]
+    c0.check(c0.L.sk_query_ref_store(hs, len(ctxs), None if ref_store is None else ref_store.h, None if query_store is None else query_store.h,
+                                     C.byref(mp), int(mode), int(device_budget), C.byref(out), C.byref(n), C.byref(st)))
+    return _take_results(c0, out, n, as_array), st
