@@ -277,6 +277,21 @@ void orc_debug_ests(void* dd, double* est, uint64_t* weight) {
 
 float orc_gbdt_predict(int model, const float* x) { return gbdt_predict(model, x); }
 
+// final_estimate on a sorted (est, weight) list of n entries; quant_q / quant_r = {q10, q50, q90}; model -1 none, 0 C125,
+// 1 C200.  The cutoffs and trim mode come from cmd as map_params_from_sketch takes them.
+int orc_final_estimate(const double* est, const uint64_t* weight, uint64_t n, uint32_t total_query_bases,
+                       uint32_t avg_chain_int_len, uint64_t query_total_len, uint64_t ref_total_len, const float* quant_q,
+                       const float* quant_r, const orc_cmd* cmd, int model, orc_result* out) {
+  std::vector<std::pair<double, size_t>> ests(n);
+  for (uint64_t i = 0; i < n; i++) ests[i] = {est[i], (size_t)weight[i]};
+  Sketch unit;
+  unit.c = 125; unit.k = 15;
+  MapParams mp = map_params_from_sketch(unit, to_cp(cmd), model);
+  to_res(final_estimate(ests, total_query_bases, avg_chain_int_len, query_total_len, ref_total_len, quant_q, quant_r, mp),
+         0, 0, out);
+  return 0;
+}
+
 // ---- drivers ----------------------------------------------------------------------------------------
 static int emit(const std::vector<PairResult>& v, orc_result** out, uint64_t* n) {
   orc_result* arr = (orc_result*)malloc(sizeof(orc_result) * (v.size() + 1));

@@ -972,6 +972,80 @@ static void bootstrap_interval(const std::vector<std::pair<double, size_t>>& ani
   hi = res[iters * 95 / 100 - 1];
 }
 
+static void predict_from_ani_res(AniEstResult& a, int model) {  // regression.rs:30-64
+  if (a.ani > 0.9f && a.total_bases_covered > TOTAL_BASES_REGRESS_CUTOFF) {
+    float x[5];
+    x[0] = a.ani * 100.f;
+    x[1] = a.std;
+    if (a.quant_50_contig_len_r > a.quant_50_contig_len_q) { x[2] = a.quant_90_contig_len_r; x[3] = a.quant_90_contig_len_q; }
+    else { x[2] = a.quant_90_contig_len_q; x[3] = a.quant_90_contig_len_r; }
+    x[4] = (float)a.avg_chain_int_len;
+    float pred = gbdt_predict(model, x);
+    if (pred < 100.f) {
+      a.ci_upper = (a.ci_upper - a.ani) + pred / 100.f;
+      a.ci_lower = (a.ci_lower - a.ani) + pred / 100.f;
+      a.ani = pred / 100.f;
+    }
+  }
+}
+
+AniEstResult final_estimate(const std::vector<std::pair<double, size_t>>& ani_ests, uint32_t total_query_bases,
+                            uint32_t avg_chain_int_len, uint64_t query_total_len, uint64_t ref_total_len,
+                            const float quant_q[3], const float quant_r[3], const MapParams& mp) {  // chain.rs:422-555
+  if (ani_ests.empty()) {  // :416-420
+    AniEstResult r;
+    r.ani = std::numeric_limits<float>::quiet_NaN();
+    return r;
+  }
+  size_t total_mult = 0;
+  for (auto& e : ani_ests) total_mult += e.second;
+  double lower, upper;
+  if (mp.median) { lower = 0.499; upper = 0.501; }
+  else if (mp.robust) { lower = 0.10; upper = 0.90; }
+  else { lower = 0.; upper = 1.; }
+  size_t lower_i = 0, upper_i = ani_ests.size() - 1;
+  bool changed_l = false, changed_u = false;
+  size_t curr = 0;
+  for (size_t i = 0; i < ani_ests.size(); i++) {  // :448-460
+    curr += ani_ests[i].second;
+    if (curr >= (size_t)((double)total_mult * lower) && !changed_l) { lower_i = i; changed_l = true; }
+    if (curr >= (size_t)((double)total_mult * upper) && !changed_u) { upper_i = i + 1; changed_u = true; break; }
+  }
+  size_t tm2 = 0;
+  double weighted = 0.;
+  for (size_t i = lower_i; i < upper_i; i++) {  // :462-469
+    weighted += ani_ests[i].first * (double)ani_ests[i].second;
+    tm2 += ani_ests[i].second;
+  }
+  double final_ani = weighted / (double)tm2;
+  double ci_lo, ci_hi, sd;
+  bootstrap_interval(ani_ests, ci_lo, ci_hi, sd);
+  double covered_query = std::min(1., (double)total_query_bases / (double)query_total_len);  // :477-480
+  double covered_ref = std::min(1., (double)total_query_bases / (double)ref_total_len);      // :481-484
+  if (mp.both_frac_cover_cutoff > 0.0) {  // :500-505
+    if (covered_query < mp.both_frac_cover_cutoff || covered_ref < mp.both_frac_cover_cutoff) final_ani = -1.;
+  } else if (covered_query < mp.frac_cover_cutoff && covered_ref < mp.frac_cover_cutoff) {  // :513-516
+    final_ani = -1.;
+  }
+  AniEstResult r;
+  r.ani = (float)final_ani;
+  r.align_fraction_query = (float)covered_query;
+  r.align_fraction_ref = (float)covered_ref;
+  r.ci_upper = (float)ci_hi;
+  r.ci_lower = (float)ci_lo;
+  r.quant_10_contig_len_q = quant_q[0];
+  r.quant_50_contig_len_q = quant_q[1];
+  r.quant_90_contig_len_q = quant_q[2];
+  r.quant_10_contig_len_r = quant_r[0];
+  r.quant_50_contig_len_r = quant_r[1];
+  r.quant_90_contig_len_r = quant_r[2];
+  r.std = (float)sd;
+  r.avg_chain_int_len = avg_chain_int_len;
+  r.total_bases_covered = total_query_bases;
+  if (mp.model >= 0) predict_from_ani_res(r, mp.model);
+  return r;
+}
+
 static AniEstResult calculate_ani(const std::vector<std::vector<ChainInterval>>& int_chunks, const Sketch& ref_sketch,
                                   const Sketch& query_sketch, const AnchorChunks& ac, const MapParams& mp, bool switched,
                                   ChainDebug* dbg) {  // chain.rs:173-555
@@ -1033,75 +1107,18 @@ static AniEstResult calculate_ani(const std::vector<std::vector<ChainInterval>>&
     return r;
   }
   avg_chain_int_len /= num_chains;  // :421
-  size_t total_mult = 0;
-  for (auto& e : ani_ests) total_mult += e.second;
-  double lower, upper;
-  if (mp.median) { lower = 0.499; upper = 0.501; }
-  else if (mp.robust) { lower = 0.10; upper = 0.90; }
-  else { lower = 0.; upper = 1.; }
-  size_t lower_i = 0, upper_i = ani_ests.size() - 1;
-  bool changed_l = false, changed_u = false;
-  size_t curr = 0;
-  for (size_t i = 0; i < ani_ests.size(); i++) {  // :448-460
-    curr += ani_ests[i].second;
-    if (curr >= (size_t)((double)total_mult * lower) && !changed_l) { lower_i = i; changed_l = true; }
-    if (curr >= (size_t)((double)total_mult * upper) && !changed_u) { upper_i = i + 1; changed_u = true; break; }
-  }
-  size_t tm2 = 0;
-  double weighted = 0.;
-  for (size_t i = lower_i; i < upper_i; i++) {  // :462-469
-    weighted += ani_ests[i].first * (double)ani_ests[i].second;
-    tm2 += ani_ests[i].second;
-  }
-  double final_ani = weighted / (double)tm2;
-  double ci_lo, ci_hi, sd;
-  bootstrap_interval(ani_ests, ci_lo, ci_hi, sd);
-  double covered_query = std::min(1., (double)total_query_bases / (double)query_sketch.total_sequence_length);  // :477-480
-  double covered_ref = std::min(1., (double)total_ref_range / (double)ref_sketch.total_sequence_length);        // :481-484
-  if (mp.both_frac_cover_cutoff > 0.0) {  // :500-505
-    if (covered_query < mp.both_frac_cover_cutoff || covered_ref < mp.both_frac_cover_cutoff) final_ani = -1.;
-  } else if (covered_query < mp.frac_cover_cutoff && covered_ref < mp.frac_cover_cutoff) {  // :513-516
-    final_ani = -1.;
-  }
+  // total_ref_range == total_query_bases: both grow by the same amounts above
   std::vector<uint32_t> sq = query_sketch.contig_lengths, sr = ref_sketch.contig_lengths;
   std::sort(sq.begin(), sq.end());
   std::sort(sr.begin(), sr.end());
-  size_t ql = sq.size(), rl = sr.size();
-  AniEstResult r;
-  r.ani = (float)final_ani;
-  r.align_fraction_query = (float)covered_query;
-  r.align_fraction_ref = (float)covered_ref;
+  const size_t ql = sq.size(), rl = sr.size();
+  const float quant_q[3] = {(float)sq[ql * 10 / 100], (float)sq[ql * 50 / 100], (float)sq[ql * 90 / 100]};
+  const float quant_r[3] = {(float)sr[rl * 10 / 100], (float)sr[rl * 50 / 100], (float)sr[rl * 90 / 100]};
+  AniEstResult r = final_estimate(ani_ests, total_query_bases, avg_chain_int_len, query_sketch.total_sequence_length,
+                                  ref_sketch.total_sequence_length, quant_q, quant_r, mp);
   r.num_contigs_r = (uint32_t)ref_sketch.contigs.size();
   r.num_contigs_q = (uint32_t)query_sketch.contigs.size();
-  r.ci_upper = (float)ci_hi;
-  r.ci_lower = (float)ci_lo;
-  r.quant_10_contig_len_q = (float)sq[ql * 10 / 100];
-  r.quant_50_contig_len_q = (float)sq[ql * 50 / 100];
-  r.quant_90_contig_len_q = (float)sq[ql * 90 / 100];
-  r.quant_10_contig_len_r = (float)sr[rl * 10 / 100];
-  r.quant_50_contig_len_r = (float)sr[rl * 50 / 100];
-  r.quant_90_contig_len_r = (float)sr[rl * 90 / 100];
-  r.std = (float)sd;
-  r.avg_chain_int_len = avg_chain_int_len;
-  r.total_bases_covered = total_query_bases;
   return r;
-}
-
-static void predict_from_ani_res(AniEstResult& a, int model) {  // regression.rs:30-64
-  if (a.ani > 0.9f && a.total_bases_covered > TOTAL_BASES_REGRESS_CUTOFF) {
-    float x[5];
-    x[0] = a.ani * 100.f;
-    x[1] = a.std;
-    if (a.quant_50_contig_len_r > a.quant_50_contig_len_q) { x[2] = a.quant_90_contig_len_r; x[3] = a.quant_90_contig_len_q; }
-    else { x[2] = a.quant_90_contig_len_q; x[3] = a.quant_90_contig_len_r; }
-    x[4] = (float)a.avg_chain_int_len;
-    float pred = gbdt_predict(model, x);
-    if (pred < 100.f) {
-      a.ci_upper = (a.ci_upper - a.ani) + pred / 100.f;
-      a.ci_lower = (a.ci_lower - a.ani) + pred / 100.f;
-      a.ani = pred / 100.f;
-    }
-  }
 }
 
 AniEstResult chain_seeds(const Sketch& ref, const Sketch& query, const MapParams& mp, ChainDebug* dbg) {  // chain.rs:144-171
@@ -1128,9 +1145,7 @@ AniEstResult chain_seeds(const Sketch& ref, const Sketch& query, const MapParams
     dbg->intervals_all = good;
     dbg->interval_kept = kept;
   }
-  AniEstResult r = calculate_ani(good_chunks, ref, query, ac, mp, switched, dbg);
-  if (mp.model >= 0) predict_from_ani_res(r, mp.model);
-  return r;
+  return calculate_ani(good_chunks, ref, query, ac, mp, switched, dbg);
 }
 
 // ------------------------------------------------------------------------------------------------

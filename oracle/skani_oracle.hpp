@@ -197,6 +197,12 @@ int get_model_id(uint64_t c, bool learned_ani);  // regression.rs:12-28
 MapParams map_params_from_sketch(const Sketch& ref, const CommandParams& cp, int model);  // chain.rs:88-142
 AniEstResult chain_seeds(const Sketch& ref, const Sketch& query, const MapParams& mp, ChainDebug* dbg = nullptr);  // chain.rs:144-171
 float gbdt_predict(int model, const float x[5]);  // gbdt 0.1.1 GBDT::predict, LAD
+// the tail of calculate_ani plus predict_from_ani_res (chain.rs:422-555, regression.rs:30-64): trimmed weighted mean, std,
+// bootstrap CI, AF cutoffs and learned ANI (mp.model >= 0) from the sorted (est, weight) list; quantiles are {q10, q50, q90}
+// of each genome's contig lengths.  An empty list gives ani = NaN.  num_contigs_* are left 0 for the caller.
+AniEstResult final_estimate(const std::vector<std::pair<double, size_t>>& ani_ests, uint32_t total_query_bases,
+                            uint32_t avg_chain_int_len, uint64_t query_total_len, uint64_t ref_total_len,
+                            const float quant_q[3], const float quant_r[3], const MapParams& mp);
 
 // ---- drivers (pair loops of triangle.rs:71-105 / dist.rs:98-144 / search.rs:119-247) -------------
 struct PairResult { uint32_t ref_id, query_id; AniEstResult r; };

@@ -1151,23 +1151,26 @@ __device__ __forceinline__ bool est_less(double ea, uint32_t wa, double eb, uint
   return wa < wb;
 }
 
-constexpr int FT = 128;
+constexpr int FT = 128;                      // >= BOOT_ITERS: one replicate per thread
 constexpr uint32_t FIN_SMEM_MAX = 1024;
+constexpr uint32_t GBDT_TREES = SK_GBDT_C125_NTREES;   // one tree per thread
+static_assert(SK_GBDT_C125_NTREES == SK_GBDT_C200_NTREES, "both models have the same number of trees");
+static_assert(FT >= (int)BOOT_ITERS, "final_kernel runs one bootstrap replicate per thread");
 
 __global__ void __launch_bounds__(FT)
 final_kernel(const PairDesc* __restrict__ pairs, const GenomeMeta* __restrict__ m0, const GenomeMeta* __restrict__ m1,
-             ChainParams prm, Workspace ws, sk_ani_result* __restrict__ out) {
+             ChainParams prm, Workspace ws, sk_ani_result* __restrict__ out, int force_redo) {
   __shared__ double s_e[FIN_SMEM_MAX];
   __shared__ uint32_t s_w[FIN_SMEM_MAX];
   __shared__ uint64_t s_cum[FIN_SMEM_MAX];
   __shared__ uint32_t s_n;
-  __shared__ double s_boot[128];
+  __shared__ double s_boot[BOOT_ITERS];
   __shared__ double s_ci[2];
-  __shared__ uint16_t s_guide[1028];
-  __shared__ float s_term[200];
+  __shared__ uint16_t s_guide[GUIDE_BUCKETS];
+  __shared__ float s_term[GBDT_TREES];
   __shared__ float s_x[5];
   __shared__ int s_do_reg;
-  __shared__ uint32_t s_lower_i, s_upper_i, s_reject;
+  __shared__ uint32_t s_reject;
   __shared__ double s_final, s_std;
   __shared__ uint64_t s_pool;
   const uint32_t p = blockIdx.x;
@@ -1224,124 +1227,50 @@ final_kernel(const PairDesc* __restrict__ pairs, const GenomeMeta* __restrict__ 
     uint64_t total_mult = 0;
     for (uint32_t i = 0; i < n; i++) total_mult += gw[i];
     double lower, upper;
-    if (prm.median) { lower = 0.499; upper = 0.501; }
-    else if (prm.robust) { lower = 0.10; upper = 0.90; }
-    else { lower = 0.; upper = 1.; }
-    uint32_t lower_i = 0, upper_i = n - 1;
-    bool cl = false, cu = false;
-    uint64_t curr = 0;
-    const uint64_t tl = (uint64_t)((double)total_mult * lower), tu = (uint64_t)((double)total_mult * upper);
-    for (uint32_t i = 0; i < n; i++) {                   // src/chain.rs:448-460
-      curr += gw[i];
-      if (curr >= tl && !cl) { lower_i = i; cl = true; }
-      if (curr >= tu && !cu) { upper_i = i + 1; cu = true; break; }
-    }
-    double weighted = 0.;
-    uint64_t tm2 = 0;
-    for (uint32_t i = lower_i; i < upper_i; i++) { weighted += ge[i] * (double)gw[i]; tm2 += gw[i]; }
-    s_final = weighted / (double)tm2;
-    // population std of the unweighted estimates (src/chain.rs:28-55)
-    double sum = 0.;
-    for (uint32_t i = 0; i < n; i++) sum += ge[i];
-    double mean = sum / (double)n, var = 0.;
-    for (uint32_t i = 0; i < n; i++) { double d = mean - ge[i]; var += d * d; }
-    s_std = sqrt(var / (double)n);
-    s_lower_i = lower_i; s_upper_i = upper_i;
-    s_reject = 0;
+    trim_fractions(prm.median != 0, prm.robust != 0, &lower, &upper);
+    uint32_t lower_i, upper_i;
+    trim_bounds(gw, n, total_mult, lower, upper, &lower_i, &upper_i);
+    s_final = trimmed_mean(ge, gw, lower_i, upper_i);
+    s_std = pop_std(ge, n);
+    s_reject = force_redo ? 1u : 0u;
     s_pool = total_mult;
   }
   __syncthreads();
-  // bootstrap (src/chain.rs:57-86): 100 replicates x n draws from the weight-expanded pool; replicate r uses draws
-  // [r*n, (r+1)*n) of the WyRand stream seeded with 7, each replicate summed sequentially by one thread.
+  // bootstrap (src/chain.rs:57-86): BOOT_ITERS replicates x n draws from the weight-expanded pool; replicate r uses draws
+  // [r*n, (r+1)*n) of the WyRand stream, each replicate summed sequentially by one thread.
   double ci_lo = 0., ci_hi = 1.;
-  if (n >= 10) {
+  if (boot_enabled(n)) {
     const uint64_t pool = s_pool;
-    // prefix sums of weights for idx -> estimate lookup: reuse gw? keep separate: binary search over running sums
-    // (n <= a few thousand; compute cumulative on the fly per thread is O(n) per draw -> too slow; build once)
+    // inclusive running weights for the idx -> estimate lookup, built once
     uint64_t* cum = (nc <= FIN_SMEM_MAX) ? s_cum : (uint64_t*)(ws.est_sorted + 4 * cb + npow2);  // global scratch: 8 B per chunk available
     if (threadIdx.x == 0) {
       uint64_t run = 0;
       for (uint32_t i = 0; i < n; i++) { run += gw[i]; cum[i] = run; }
     }
     __syncthreads();
-    // guide table for the draws: bucket b = idx >> gshift (<= 1024 buckets) -> first chunk i with cum[i] > (b << gshift); a draw then
-    // walks forward from there (0-1 steps) instead of a 8-12 step binary search per draw (100 x n draws per pair)
-    uint32_t gshift = 0;
-    while ((pool >> gshift) >= 1024) gshift++;
-    const uint32_t nbuck = (uint32_t)(pool >> gshift) + 1;
-    for (uint32_t bk = threadIdx.x; bk < nbuck; bk += blockDim.x) {
-      const uint64_t lo = (uint64_t)bk << gshift;
-      uint32_t a = 0, b = n;
-      while (a < b) { uint32_t m = (a + b) >> 1; if (cum[m] <= lo) a = m + 1; else b = m; }
-      s_guide[bk] = (uint16_t)min(a, 0xFFFFu);
-    }
+    const uint32_t gshift = guide_shift(pool);
+    const uint32_t nbuck = guide_buckets(pool, gshift);
+    for (uint32_t bk = threadIdx.x; bk < nbuck; bk += blockDim.x) s_guide[bk] = guide_entry(cum, n, bk, gshift);
     __syncthreads();
-    auto replicate = [&](const uint64_t* cumv, const double* gev) {
-      const uint32_t rep = threadIdx.x;
-      double ssum = 0.;
-      bool rej = false;
-      for (uint32_t s = 0; s < n; s++) {
-        bool nr;
-        const uint64_t idx = lemire_below(wyrand_at(7, (uint64_t)rep * n + s), pool, &nr);
-        rej |= nr;
-        uint32_t a = s_guide[(uint32_t)(idx >> gshift)];   // first i with cum[i] > idx
-        while (a + 1 < n && cumv[a] <= idx) a++;           // idx < pool = cum[n-1]: ends inside the array (bounded anyway)
-        ssum += gev[a];
-      }
-      s_boot[rep] = ssum / (double)n;
+    if (threadIdx.x < BOOT_ITERS) {
+      bool rej;
+      double m;
+      if (nc <= FIN_SMEM_MAX && n < GUIDE_MAX_N) m = boot_replicate<true>(s_cum, s_e, n, pool, s_guide, gshift, threadIdx.x, &rej);   // shared-memory operands (LDS), the common case
+      else if (n < GUIDE_MAX_N) m = boot_replicate<true>(cum, ge, n, pool, s_guide, gshift, threadIdx.x, &rej);
+      else m = boot_replicate<false>(cum, ge, n, pool, nullptr, 0, threadIdx.x, &rej);                 // 65535 estimates or more: plain search
+      s_boot[threadIdx.x] = m;
       if (rej) atomicOr(&s_reject, 1u);
-    };
-    if (threadIdx.x < 100) {
-      if (nc <= FIN_SMEM_MAX && n < 0xFFFFu) replicate(s_cum, s_e);   // shared-memory operands (LDS), the common case
-      else if (n < 0xFFFFu) replicate(cum, ge);
-      else {                                              // more than 65535 chunks: plain binary search
-        const uint32_t rep = threadIdx.x;
-        double ssum = 0.;
-        bool rej = false;
-        for (uint32_t s = 0; s < n; s++) {
-          bool nr;
-          uint64_t idx = lemire_below(wyrand_at(7, (uint64_t)rep * n + s), pool, &nr);
-          rej |= nr;
-          uint32_t a = 0, b = n;
-          while (a < b) { uint32_t m = (a + b) >> 1; if (cum[m] <= idx) a = m + 1; else b = m; }
-          ssum += ge[a];
-        }
-        s_boot[rep] = ssum / (double)n;
-        if (rej) atomicOr(&s_reject, 1u);
-      }
     }
     __syncthreads();
-    if (threadIdx.x == 0) {
-      if (s_reject) {
-        // a Lemire rejection shifts the stream: redo sequentially (probability ~ n*100*pool / 2^64)
-        uint64_t draws = 0;
-        for (uint32_t rep = 0; rep < 100; rep++) {
-          double ssum = 0.;
-          // the reference draws all n indices first, then sums: same stream order
-          for (uint32_t s = 0; s < n; s++) {
-            uint64_t rr = wyrand_at(7, draws++);
-            uint64_t hi = __umul64hi(rr, pool), lo = rr * pool;
-            if (lo < pool) {
-              uint64_t thr = (0 - pool) % pool;
-              while (lo < thr) { rr = wyrand_at(7, draws++); hi = __umul64hi(rr, pool); lo = rr * pool; }
-            }
-            uint32_t a = 0, b = n;
-            while (a < b) { uint32_t m = (a + b) >> 1; if (cum[m] <= hi) a = m + 1; else b = m; }
-            ssum += ge[a];
-          }
-          s_boot[rep] = ssum / (double)n;
-        }
-      }
-    }
+    // a Lemire rejection shifts the stream: redo sequentially (probability ~ n * 100 * pool / 2^64)
+    if (threadIdx.x == 0 && s_reject) boot_redo(cum, ge, n, pool, s_boot);
     __syncthreads();
-    // order statistics [4] and [94] of the 100 replicate means (src/chain.rs:80-85 sorts them): every thread ranks its own
-    // value (ties broken by index, so the ranks are a permutation) instead of one thread sorting serially
-    if (threadIdx.x < 100) {
-      const double v = s_boot[threadIdx.x];
-      uint32_t rank = 0;
-      for (uint32_t j = 0; j < 100; j++) { const double u = s_boot[j]; rank += (u < v || (u == v && j < threadIdx.x)) ? 1u : 0u; }
-      if (rank == 4) s_ci[0] = v;
-      if (rank == 94) s_ci[1] = v;
+    // order statistics of the replicate means (src/chain.rs:80-85 sorts them): every thread ranks its own value instead of
+    // one thread sorting serially
+    if (threadIdx.x < BOOT_ITERS) {
+      const uint32_t rank = boot_rank(s_boot, threadIdx.x);
+      if (rank == CI_LO_RANK) s_ci[0] = s_boot[threadIdx.x];
+      if (rank == CI_HI_RANK) s_ci[1] = s_boot[threadIdx.x];
     }
     __syncthreads();
     ci_lo = s_ci[0]; ci_hi = s_ci[1];
@@ -1350,13 +1279,8 @@ final_kernel(const PairDesc* __restrict__ pairs, const GenomeMeta* __restrict__ 
     double final_ani = s_final;
     const uint32_t sumlen = ws.pair_sumlen[p];
     const uint32_t tqb = (prm.c < 200) ? sumlen : ws.pair_tqb_ns[p];      // sensitive_af (:183-190, 244-247, 261-264)
-    double covered_query = (double)tqb / (double)qrym.total_len; if (covered_query > 1.) covered_query = 1.;
-    double covered_ref = (double)tqb / (double)refm.total_len; if (covered_ref > 1.) covered_ref = 1.;
-    if (prm.both_frac_cover_cutoff > 0.0) {
-      if (covered_query < prm.both_frac_cover_cutoff || covered_ref < prm.both_frac_cover_cutoff) final_ani = -1.;
-    } else if (covered_query < prm.frac_cover_cutoff && covered_ref < prm.frac_cover_cutoff) {
-      final_ani = -1.;
-    }
+    const double covered_query = covered_frac(tqb, qrym.total_len), covered_ref = covered_frac(tqb, refm.total_len);
+    if (af_cut(covered_query, covered_ref, prm.frac_cover_cutoff, prm.both_frac_cover_cutoff)) final_ani = -1.;
     r.ani = (float)final_ani;
     r.af_query = (float)covered_query; r.af_ref = (float)covered_ref;
     r.ci_lower = (float)ci_lo; r.ci_upper = (float)ci_hi; r.std = (float)s_std;
@@ -1367,35 +1291,24 @@ final_kernel(const PairDesc* __restrict__ pairs, const GenomeMeta* __restrict__ 
     r.total_bases_covered = tqb;
     // learned-ANI regression (src/regression.rs:30-64): features now, the 195 trees are walked by all threads below
     s_do_reg = 0;
-    if (prm.model >= 0 && r.ani > 0.9f && r.total_bases_covered > REGRESS_CUTOFF) {
-      s_x[0] = r.ani * 100.f; s_x[1] = r.std;
-      if (r.q50_r > r.q50_q) { s_x[2] = r.q90_r; s_x[3] = r.q90_q; } else { s_x[2] = r.q90_q; s_x[3] = r.q90_r; }
-      s_x[4] = (float)r.avg_chain_int_len;
+    if (prm.model >= 0 && regress_gate(r.ani, r.total_bases_covered)) {
+      regress_features(r.ani, r.std, r.q50_q, r.q90_q, r.q50_r, r.q90_r, r.avg_chain_int_len, s_x);
       s_do_reg = 1;
     }
   }
   __syncthreads();
   if (s_do_reg) {   // uniform
-    // gbdt 0.1.1 predict: bias + sum_t shrink * leaf_t(x), the sum taken in tree order in f32 (SURVEY App. D.5): the per-tree
-    // terms are independent -> one tree per thread, then thread 0 adds them in order
+    // gbdt_eval with the per-tree terms (independent) one per thread, then summed in tree order by thread 0
     const unsigned char* feat = c_gbdt_feat[prm.model];
     const float* thr = c_gbdt_thr[prm.model];
     const float* leaf = c_gbdt_leaf[prm.model];
     const float shrink = c_gbdt_shrink[prm.model];
-    for (uint32_t t = threadIdx.x; t < 195; t += blockDim.x) {
-      int node = 0;
-      for (int d = 0; d < 3; d++) node = 2 * node + ((s_x[feat[7 * t + node]] < thr[7 * t + node]) ? 1 : 2);
-      s_term[t] = __fmul_rn(shrink, leaf[8 * t + (node - 7)]);
-    }
+    for (uint32_t t = threadIdx.x; t < GBDT_TREES; t += blockDim.x) s_term[t] = gbdt_tree_term(feat, thr, leaf, (int)t, shrink, s_x);
     __syncthreads();
     if (threadIdx.x == 0) {
       float pred = c_gbdt_bias[prm.model];
-      for (int t = 0; t < 195; t++) pred = __fadd_rn(pred, s_term[t]);
-      if (pred < 100.f) {
-        r.ci_upper = (r.ci_upper - r.ani) + pred / 100.f;
-        r.ci_lower = (r.ci_lower - r.ani) + pred / 100.f;
-        r.ani = pred / 100.f;
-      }
+      for (uint32_t t = 0; t < GBDT_TREES; t++) pred = fadd_rn(pred, s_term[t]);
+      regress_apply(pred, &r.ani, &r.ci_lower, &r.ci_upper);
     }
   }
   if (threadIdx.x == 0) out[p] = r;
@@ -1758,7 +1671,10 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
     SK_LAUNCH(ctx, "select_kernel", (select_kernel<<<B, CT, 0, st>>>(S.d_pairs, prm, ws)));
     SK_LAUNCH(ctx, "chunkstat_kernel", (chunkstat_kernel<<<(uint32_t)((TC + CS_WARPS * CS_PER_WARP - 1) / (CS_WARPS * CS_PER_WARP)), CS_WARPS * 32, 0, st>>>(TC, S.d_pairs, v0, v1, S.d_m0, S.d_m1, prm, ws)));
   }
-  SK_LAUNCH(ctx, "final_kernel", (final_kernel<<<B, FT, 0, st>>>(S.d_pairs, S.d_m0, S.d_m1, prm, ws, S.d_out)));
+  // test hook: SK_FINAL_FORCE_REDO=1 takes the sequential bootstrap redo for every pair, as if some draw had been rejected
+  const char* fr = getenv("SK_FINAL_FORCE_REDO");
+  const int force_redo = (fr && atoi(fr) != 0) ? 1 : 0;
+  SK_LAUNCH(ctx, "final_kernel", (final_kernel<<<B, FT, 0, st>>>(S.d_pairs, S.d_m0, S.d_m1, prm, ws, S.d_out, force_redo)));
   SK_CUDA(cudaMemcpyAsync(host_out + b0, S.d_out, B * sizeof(sk_ani_result), cudaMemcpyDeviceToHost, st));
   SK_CUDA(cudaStreamSynchronize(st));
   SK_CUDA(cudaGetLastError());

@@ -216,23 +216,209 @@ SK_HD uint64_t lemire_below(uint64_t r, uint64_t n, bool* needs_reject) {
   return hi;
 }
 
-// ---- gbdt 0.1.1 predict (LAD), SURVEY App. D.5; tables from gbdt_tables.inc (complete depth-3 trees, heap order)
+// ---- final estimate (src/chain.rs:414-555, src/regression.rs:30-64): the per-item pieces of final_kernel, on the pair's
+// (est, weight) list sorted by the (f64, usize) tuple order.  The reference never fuses a multiply into an add; nvcc would
+// contract `s += a * b` into one DFMA under the default --fmad=true, so products and their sums go through the _rn helpers.
+constexpr uint32_t BOOT_ITERS = 100;          // src/chain.rs:68
+constexpr uint32_t BOOT_MIN_N = 10;           // fewer estimates: CI = [0, 1] (:65-67)
+constexpr uint64_t BOOT_SEED = 7;             // fastrand::seed(7) (:63)
+constexpr uint32_t CI_LO_RANK = BOOT_ITERS * 5 / 100 - 1, CI_HI_RANK = BOOT_ITERS * 95 / 100 - 1;   // res[4], res[94] (:80-85)
+constexpr uint32_t GUIDE_BUCKETS = 1024;      // bootstrap guide table: at most this many buckets of the pool
+constexpr uint32_t GUIDE_MAX_N = 0xFFFFu;     // guide entries are u16: lists of this many estimates or more search instead
+
+// the bootstrap runs on lists of BOOT_MIN_N estimates or more
+SK_HD bool boot_enabled(uint32_t n) { return n >= BOOT_MIN_N; }
+
+SK_HD double dmul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(a, b);
+#else
+  volatile double p = a * b;
+  return p;
+#endif
+}
+SK_HD double dadd_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dadd_rn(a, b);
+#else
+  volatile double s = a + b;
+  return s;
+#endif
+}
+SK_HD float fmul_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_rn(a, b);
+#else
+  volatile float p = a * b;
+  return p;
+#endif
+}
+SK_HD float fadd_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fadd_rn(a, b);
+#else
+  volatile float s = a + b;
+  return s;
+#endif
+}
+
+// trim fractions of the weight mass: --median, --robust, plain (src/chain.rs:424-446)
+SK_HD void trim_fractions(bool median, bool robust, double* lower, double* upper) {
+  if (median) { *lower = 0.499; *upper = 0.501; }
+  else if (robust) { *lower = 0.10; *upper = 0.90; }
+  else { *lower = 0.; *upper = 1.; }
+}
+// the estimates [lower_i, upper_i) the mean keeps (src/chain.rs:448-460): lower_i is the first index whose running weight
+// reaches floor(total * lower), upper_i one past the first that reaches floor(total * upper)
+SK_HD void trim_bounds(const uint32_t* w, uint32_t n, uint64_t total, double lower, double upper, uint32_t* lower_i,
+                       uint32_t* upper_i) {
+  uint32_t lo = 0, hi = n - 1;
+  bool cl = false;
+  uint64_t curr = 0;
+  const uint64_t tl = (uint64_t)((double)total * lower), tu = (uint64_t)((double)total * upper);
+  for (uint32_t i = 0; i < n; i++) {
+    curr += w[i];
+    if (curr >= tl && !cl) { lo = i; cl = true; }
+    if (curr >= tu) { hi = i + 1; break; }
+  }
+  *lower_i = lo; *upper_i = hi;
+}
+// weighted mean of the kept estimates, summed left to right (src/chain.rs:462-471)
+SK_HD double trimmed_mean(const double* e, const uint32_t* w, uint32_t lower_i, uint32_t upper_i) {
+  double weighted = 0.;
+  uint64_t tm = 0;
+  for (uint32_t i = lower_i; i < upper_i; i++) { weighted = dadd_rn(weighted, dmul_rn(e[i], (double)w[i])); tm += w[i]; }
+  return weighted / (double)tm;
+}
+// population std of the unweighted estimates (src/chain.rs:28-55)
+SK_HD double pop_std(const double* e, uint32_t n) {
+  double sum = 0.;
+  for (uint32_t i = 0; i < n; i++) sum += e[i];
+  const double mean = sum / (double)n;
+  double var = 0.;
+  for (uint32_t i = 0; i < n; i++) { const double d = mean - e[i]; var = dadd_rn(var, dmul_rn(d, d)); }
+  return sqrt(var / (double)n);
+}
+
+SK_HD void mul64_wide(uint64_t a, uint64_t b, uint64_t* hi, uint64_t* lo) {
+#if defined(__CUDA_ARCH__)
+  *hi = __umul64hi(a, b); *lo = a * b;
+#else
+  const __uint128_t t = (__uint128_t)a * b;
+  *hi = (uint64_t)(t >> 64); *lo = (uint64_t)t;
+#endif
+}
+// bootstrap lookups: a draw idx < pool of the weight-expanded pool picks the first estimate i with cum[i] > idx, where
+// cum holds the inclusive running weights (pool = cum[n - 1])
+SK_HD uint32_t cum_search(const uint64_t* cum, uint32_t n, uint64_t idx) {
+  uint32_t a = 0, b = n;
+  while (a < b) { const uint32_t m = (a + b) >> 1; if (cum[m] <= idx) a = m + 1; else b = m; }
+  return a;
+}
+// guide table: bucket bk = idx >> gshift (at most GUIDE_BUCKETS buckets) holds the lookup of its first draw value, so a
+// draw walks forward from there (0-1 steps) instead of searching
+SK_HD uint32_t guide_shift(uint64_t pool) {
+  uint32_t g = 0;
+  while ((pool >> g) >= GUIDE_BUCKETS) g++;
+  return g;
+}
+SK_HD uint32_t guide_buckets(uint64_t pool, uint32_t gshift) { return (uint32_t)(pool >> gshift) + 1; }
+SK_HD uint16_t guide_entry(const uint64_t* cum, uint32_t n, uint32_t bk, uint32_t gshift) {
+  const uint32_t a = cum_search(cum, n, (uint64_t)bk << gshift);
+  return (uint16_t)(a < 0xFFFFu ? a : 0xFFFFu);
+}
+// replicate `rep` of the bootstrap (src/chain.rs:57-86): the mean of the estimates picked by draws [rep * n, (rep + 1) * n)
+// of the WyRand stream, summed in draw order.  GUIDE: the lookups start at the guide table (n < GUIDE_MAX_N); otherwise they
+// search.  *rej reports a draw Lemire's loop would have rejected: the stream then shifts and boot_redo takes over.
+template <bool GUIDE>
+SK_HD double boot_replicate(const uint64_t* cum, const double* e, uint32_t n, uint64_t pool, const uint16_t* guide,
+                            uint32_t gshift, uint32_t rep, bool* rej) {
+  double ssum = 0.;
+  bool any = false;
+  for (uint32_t s = 0; s < n; s++) {
+    bool nr;
+    const uint64_t idx = lemire_below(wyrand_at(BOOT_SEED, (uint64_t)rep * n + s), pool, &nr);
+    any |= nr;
+    uint32_t a;
+    if (GUIDE) {
+      a = guide[(uint32_t)(idx >> gshift)];
+      while (a + 1 < n && cum[a] <= idx) a++;           // idx < pool = cum[n - 1]: ends inside the array (bounded anyway)
+    } else {
+      a = cum_search(cum, n, idx);
+    }
+    ssum += e[a];
+  }
+  *rej = any;
+  return ssum / (double)n;
+}
+// all BOOT_ITERS replicates drawn one after another as the reference draws them, Lemire's rejection loop included (a
+// rejected draw is replaced by the next one, shifting the rest of the stream): boot[rep] for every replicate
+SK_HD void boot_redo(const uint64_t* cum, const double* e, uint32_t n, uint64_t pool, double* boot) {
+  uint64_t draws = 0;
+  for (uint32_t rep = 0; rep < BOOT_ITERS; rep++) {
+    double ssum = 0.;
+    for (uint32_t s = 0; s < n; s++) {               // all n indices of a replicate are drawn before it is summed: same order
+      uint64_t hi, lo;
+      mul64_wide(wyrand_at(BOOT_SEED, draws++), pool, &hi, &lo);
+      if (lo < pool) {
+        const uint64_t thr = (0 - pool) % pool;
+        while (lo < thr) mul64_wide(wyrand_at(BOOT_SEED, draws++), pool, &hi, &lo);
+      }
+      ssum += e[cum_search(cum, n, hi)];
+    }
+    boot[rep] = ssum / (double)n;
+  }
+}
+// rank of replicate i among the BOOT_ITERS means, ties broken by index (the ranks are a permutation): the reference's
+// sorted res[CI_LO_RANK] / res[CI_HI_RANK] are the replicates of those ranks
+SK_HD uint32_t boot_rank(const double* boot, uint32_t i) {
+  const double v = boot[i];
+  uint32_t rank = 0;
+  for (uint32_t j = 0; j < BOOT_ITERS; j++) { const double u = boot[j]; rank += (u < v || (u == v && j < i)) ? 1u : 0u; }
+  return rank;
+}
+
+// aligned fraction of one genome, capped at 1 (src/chain.rs:477-484)
+SK_HD double covered_frac(uint32_t total_bases_covered, uint64_t total_len) {
+  const double c = (double)total_bases_covered / (double)total_len;
+  return c > 1. ? 1. : c;
+}
+// true if the AF cutoffs void the estimate (ani = -1, src/chain.rs:500-516)
+SK_HD bool af_cut(double covered_query, double covered_ref, double frac_cover_cutoff, double both_frac_cover_cutoff) {
+  if (both_frac_cover_cutoff > 0.0) return covered_query < both_frac_cover_cutoff || covered_ref < both_frac_cover_cutoff;
+  return covered_query < frac_cover_cutoff && covered_ref < frac_cover_cutoff;
+}
+
+// ---- learned ANI (src/regression.rs:30-64): gate, features, gbdt 0.1.1 predict (LAD, SURVEY App. D.5) on the tables of
+// gbdt_tables.inc (complete depth-3 trees, heap order), and the correction of ani / CI
+SK_HD bool regress_gate(float ani, uint32_t total_bases_covered) { return ani > 0.9f && total_bases_covered > REGRESS_CUTOFF; }
+SK_HD void regress_features(float ani, float std, float q50_q, float q90_q, float q50_r, float q90_r, uint32_t avg_chain_int_len,
+                            float x[5]) {
+  x[0] = ani * 100.f; x[1] = std;
+  if (q50_r > q50_q) { x[2] = q90_r; x[3] = q90_q; } else { x[2] = q90_q; x[3] = q90_r; }
+  x[4] = (float)avg_chain_int_len;
+}
+// tree t's term shrink * leaf(x), an f32 product never fused into the sum
+SK_HD float gbdt_tree_term(const unsigned char* feat, const float* thr, const float* leaf, int t, float shrink, const float* x) {
+  const unsigned char* f = feat + 7 * t;
+  const float* th = thr + 7 * t;
+  int node = 0;
+  for (int d = 0; d < 3; d++) node = 2 * node + ((x[f[node]] < th[node]) ? 1 : 2);   // children of i: 2i+1 (x < thr), 2i+2
+  return fmul_rn(shrink, leaf[8 * t + (node - 7)]);
+}
+// bias + the terms, summed in tree order in f32 (final_kernel computes the terms in parallel and sums them the same way)
 SK_HD float gbdt_eval(const unsigned char* feat, const float* thr, const float* leaf, int ntrees, float shrink, float bias,
                       const float x[5]) {
   float v = bias;
-  for (int t = 0; t < ntrees; t++) {
-    const unsigned char* f = feat + 7 * t;
-    const float* th = thr + 7 * t;
-    int node = 0;
-    for (int d = 0; d < 3; d++) node = 2 * node + ((x[f[node]] < th[node]) ? 1 : 2);
-#if defined(__CUDA_ARCH__)
-    v = __fadd_rn(v, __fmul_rn(shrink, leaf[8 * t + (node - 7)]));  // f32 multiply then add, never fused
-#else
-    volatile float prod = shrink * leaf[8 * t + (node - 7)];
-    v = v + prod;
-#endif
-  }
+  for (int t = 0; t < ntrees; t++) v = fadd_rn(v, gbdt_tree_term(feat, thr, leaf, t, shrink, x));
   return v;
+}
+SK_HD void regress_apply(float pred, float* ani, float* ci_lower, float* ci_upper) {
+  if (pred < 100.f) {
+    *ci_upper = (*ci_upper - *ani) + pred / 100.f;
+    *ci_lower = (*ci_lower - *ani) + pred / 100.f;
+    *ani = pred / 100.f;
+  }
 }
 
 }  // namespace sk

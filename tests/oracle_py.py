@@ -101,6 +101,8 @@ def lib():
     L.orc_debug_intervals.argtypes = [vp] * 2
     L.orc_debug_ests.argtypes = [vp] * 3
     L.orc_gbdt_predict.restype = C.c_float; L.orc_gbdt_predict.argtypes = [i32, vp]
+    L.orc_final_estimate.restype = i32
+    L.orc_final_estimate.argtypes = [vp, vp, u64, u32, u32, u64, u64, vp, vp, C.POINTER(OrcCmd), i32, C.POINTER(OrcResult)]
     L.orc_triangle.restype = i32
     L.orc_triangle.argtypes = [C.POINTER(vp), i32, C.POINTER(OrcCmd), i32, C.POINTER(C.POINTER(OrcResult)),
                                C.POINTER(u64), C.POINTER(u64), C.POINTER(dbl), C.POINTER(dbl)]
@@ -204,6 +206,23 @@ def chain_debug(ref, query, cp=None):
                     chunk_first=first, chunk_nseeds=nseeds, intervals=iv, est=est, weight=w)
     finally:
         L.orc_debug_free(d)
+
+
+def final_estimate(est, weight, total_bases_covered, avg_chain_int_len, query_total_len, ref_total_len, quant_q, quant_r,
+                   cp=None, model=0):
+    """The final estimate (trimmed mean, std, bootstrap CI, AF cutoffs, learned ANI) of a sorted (est, weight) list, as
+    calculate_ani + predict_from_ani_res compute it; quant_q / quant_r = (q10, q50, q90); model -1 none, 0 C125, 1 C200.
+    num_contigs_* of the result are 0."""
+    cp = cp or cmd()
+    e = np.ascontiguousarray(est, np.float64)
+    w = np.ascontiguousarray(weight, np.uint64)
+    assert len(e) == len(w)
+    qq = np.ascontiguousarray(quant_q, np.float32); qr = np.ascontiguousarray(quant_r, np.float32)
+    r = OrcResult()
+    lib().orc_final_estimate(e.ctypes.data, w.ctypes.data, len(e), int(total_bases_covered), int(avg_chain_int_len),
+                             int(query_total_len), int(ref_total_len), qq.ctypes.data, qr.ctypes.data, C.byref(cp), model,
+                             C.byref(r))
+    return r
 
 
 def _results(out, n):
