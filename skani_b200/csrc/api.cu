@@ -204,6 +204,40 @@ cudaError_t h2d_small(sk_ctx* ctx, void* dst, const void* src, size_t bytes) {
   ctx->stage_pos = pos + bytes;
   return cudaGetLastError();
 }
+
+int SegmentCopy::run(sk_ctx* ctx) {
+  cudaStream_t st = ctx->stream;
+  const size_t ns = bytes.size();
+  if (!batched) {
+    for (size_t i = 0; i < ns; i++) SK_CUDA(cudaMemcpyAsync(dst[i], src[i], bytes[i], cudaMemcpyDeviceToDevice, st));
+    return SK_OK;
+  }
+  if (ns == 0) return SK_OK;
+  if (ns >= (1ull << 32)) { ctx->err = "too many copy segments"; return SK_ERR_PARAM; }
+  DTmp<const void*> d_src; DTmp<void*> d_dst; DTmp<size_t> d_n;
+  SK_CUDA(d_src.alloc(ns, ctx)); SK_CUDA(d_dst.alloc(ns, ctx)); SK_CUDA(d_n.alloc(ns, ctx));
+  SK_CUDA(cudaMemcpyAsync(d_src.p, src.data(), ns * sizeof(void*), cudaMemcpyHostToDevice, st));
+  SK_CUDA(cudaMemcpyAsync(d_dst.p, dst.data(), ns * sizeof(void*), cudaMemcpyHostToDevice, st));
+  SK_CUDA(cudaMemcpyAsync(d_n.p, bytes.data(), ns * sizeof(size_t), cudaMemcpyHostToDevice, st));
+  size_t tb = 0;
+  auto copy = [&](void* tmp) { return cub::DeviceMemcpy::Batched(tmp, tb, d_src.p, d_dst.p, d_n.p, (uint32_t)ns, st); };
+  SK_CUDA(copy(nullptr));
+  DTmp<uint8_t> tmp;
+  SK_CUDA(tmp.alloc(tb, ctx));
+  SK_CUDA(copy(tmp.p));
+  count_launch(ctx);
+  SK_CUDA(cudaStreamSynchronize(st));   // the host-side lists and the temporaries are released on return
+  return SK_OK;
+}
+
+cudaError_t zero_absent_arrays(sk_ctx* ctx, uint8_t* blob, const BlobLayout& b, bool markers_only, bool tables) {
+  for (int a = 0; a < BLOB_ARRAYS; a++) {
+    if (array_travels(a, markers_only, tables) || b.bytes[a] == 0) continue;
+    const cudaError_t e = cudaMemsetAsync(blob + b.off[a], 0, b.bytes[a], ctx->stream);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
 }  // namespace sk
 
 namespace {
@@ -224,19 +258,10 @@ void parallel_memcpy(sk_ctx* ctx, void* dst, const void* src, size_t n) {
   ctx_pool(ctx)->run(nt, [&](size_t t) { const size_t b = t * chunk; memcpy((uint8_t*)dst + b, (const uint8_t*)src + b, std::min(chunk, n - b)); });
 }
 
-template <typename T>
-int concat_dev(sk_ctx* ctx, const std::vector<const T*>& parts, const std::vector<size_t>& counts, T** out) {
-  size_t total = 0;
-  for (size_t c : counts) total += c;
-  T* p = nullptr;
-  SK_CUDA(ctx->arena.alloc((void**)&p, std::max<size_t>(total, 1) * sizeof(T)));
-  size_t o = 0;
-  for (size_t i = 0; i < parts.size(); i++) {
-    if (counts[i]) SK_CUDA(cudaMemcpyAsync(p + o, parts[i], counts[i] * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
-    o += counts[i];
-  }
-  *out = p;
-  return SK_OK;
+// elements of blob array a in set s (ht_off is read for the table array only: a set growing in place extends it last)
+uint64_t set_elems(const sk_sketch_set* s, int a) {
+  const uint64_t n[N_COUNTS] = {s->S, s->U, s->M, s->C, SET_ARRAYS[a].by == CNT_HT ? s->ht_off[s->G] : 0};
+  return array_elems(a, s->G, n);
 }
 
 // concatenate sketch sets (genome-local indexing everywhere, so only the prefix offsets shift).  with_tables: the parts
@@ -247,42 +272,35 @@ int concat_sets(sk_ctx* ctx, const std::vector<const sk_sketch_set*>& parts, sk_
   s->sp = parts.empty() ? sk_sketch_params{125, 15, 1000} : parts[0]->sp;
   struct Guard { sk_sketch_set* s; ~Guard() { if (s) { free_set_device(s); delete s; } } } guard{s};
   s->seed_off = {0}; s->uk_off = {0}; s->mk_off = {0}; s->ctg_off = {0};
-  std::vector<size_t> nS, nU, nM, nC, nUG, nCG, nB;
+  if (with_tables) s->ht_off = {0};
   for (auto* p : parts) {
-    if (p->sp.c != s->sp.c || p->sp.k != s->sp.k || p->sp.marker_c != s->sp.marker_c) { ctx->err = "sketch parameter mismatch"; return SK_ERR_PARAM; }
+    if (!same_params(p->sp, s->sp)) { ctx->err = "sketch parameter mismatch"; return SK_ERR_PARAM; }
     for (uint32_t g = 0; g < p->G; g++) {
       s->seed_off.push_back(s->seed_off.back() + (p->seed_off[g + 1] - p->seed_off[g]));
       s->uk_off.push_back(s->uk_off.back() + (p->uk_off[g + 1] - p->uk_off[g]));
       s->mk_off.push_back(s->mk_off.back() + (p->mk_off[g + 1] - p->mk_off[g]));
       s->ctg_off.push_back(s->ctg_off.back() + (p->ctg_off[g + 1] - p->ctg_off[g]));
+      if (with_tables) s->ht_off.push_back(s->ht_off.back() + (p->ht_off[g + 1] - p->ht_off[g]));
       s->total_len.push_back(p->total_len[g]);
       s->name_rank.push_back(s->G + g);
     }
     s->ctg_len.insert(s->ctg_len.end(), p->ctg_len.begin(), p->ctg_len.end());
     s->G += p->G;
-    nS.push_back(p->S); nU.push_back(p->U); nM.push_back(p->M); nC.push_back(p->C);
-    nUG.push_back(p->U + p->G); nCG.push_back(p->C + p->G); nB.push_back((size_t)p->G * (UBUCKETS + 1));
   }
   s->S = s->seed_off.back(); s->U = s->uk_off.back(); s->M = s->mk_off.back(); s->C = s->ctg_off.back();
-#define CAT(field, T, counts)                                         \
-  {                                                                   \
-    std::vector<const T*> v;                                          \
-    for (auto* p : parts) v.push_back(p->field);                      \
-    SK_TRY(concat_dev<T>(ctx, v, counts, &s->field));                 \
-  }
-  CAT(pv_kmer, uint32_t, nS) CAT(pv_pos, uint32_t, nS) CAT(pv_cc, uint32_t, nS) CAT(pv_mult, uint16_t, nS)
-  CAT(kv_pos, uint32_t, nS) CAT(kv_cc, uint32_t, nS) CAT(ukmer, uint32_t, nU) CAT(ustart, uint32_t, nUG)
-  CAT(markers, uint64_t, nM) CAT(ctg_rec_off, uint32_t, nCG) CAT(d_ctg_len, uint32_t, nC)
-  if (with_tables) {
-    std::vector<size_t> nH;
-    s->ht_off = {0};
+  for (int a = 0; a < BLOB_ARRAYS; a++) {
+    if (!array_travels(a, false, with_tables)) continue;
+    const size_t esz = SET_ARRAYS[a].esz;
+    uint64_t total = 0;
+    for (auto* p : parts) total += set_elems(p, a);
+    SK_CUDA(ctx->arena.alloc(&set_array(s, a), std::max<uint64_t>(total, 1) * esz));
+    uint8_t* dst = (uint8_t*)set_array(s, a);
     for (auto* p : parts) {
-      for (uint32_t g = 0; g < p->G; g++) s->ht_off.push_back(s->ht_off.back() + (p->ht_off[g + 1] - p->ht_off[g]));
-      nH.push_back(p->ht_off[p->G]);
+      const uint64_t n = set_elems(p, a);
+      if (n) SK_CUDA(cudaMemcpyAsync(dst, set_array(p, a), n * esz, cudaMemcpyDeviceToDevice, ctx->stream));
+      dst += n * esz;
     }
-    CAT(htab, unsigned long long, nH)
   }
-#undef CAT
   SK_CUDA(cudaStreamSynchronize(ctx->stream));
   guard.s = nullptr;
   *out = s;
@@ -491,64 +509,26 @@ int sk_sketch_set_append(sk_sketch_set* dst, const sk_sketch_set* src) {
   return SK_OK;
 }
 
-namespace {
-inline const void* set_array(const sk_sketch_set* s, int i) {
-  const void* p[BLOB_ARRAYS] = {s->pv_kmer, s->pv_pos, s->pv_cc, s->pv_mult, s->kv_pos, s->kv_cc, s->ukmer, s->ustart, s->markers, s->ctg_rec_off,
-                                 s->d_ctg_len, s->htab};
-  return p[i];
-}
-}  // namespace
-
 int sk_sketch_set_blob_size(const sk_sketch_set* s, uint64_t* device_bytes, uint64_t* host_meta_words) {
-  if (!s || !device_bytes || !host_meta_words) return SK_ERR_PARAM;
-  *device_bytes = blob_layout(s->G, s->S, s->U, s->M, s->C).total;
-  *host_meta_words = meta_words(s->G, s->C, false);
-  return SK_OK;
+  return sk_sketch_set_subset_blob_size(s, nullptr, 0, 0, device_bytes, host_meta_words);
 }
 
-int sk_sketch_set_pack(const sk_sketch_set* s, void* d_blob, uint64_t* meta) {
-  if (!s || !d_blob || !meta) return SK_ERR_PARAM;
-  sk_ctx* ctx = s->ctx;
-  SK_CUDA(cudaSetDevice(ctx->device));
-  BlobLayout b = blob_layout(s->G, s->S, s->U, s->M, s->C);
-  for (int i = 0; i < 11; i++)
-    if (b.bytes[i]) SK_CUDA(cudaMemcpyAsync((uint8_t*)d_blob + b.off[i], set_array(s, i), b.bytes[i], cudaMemcpyDeviceToDevice, ctx->stream));
-  uint64_t* m = meta;
-  *m++ = s->G; *m++ = s->S; *m++ = s->U; *m++ = s->M; *m++ = s->C; *m++ = s->sp.c; *m++ = s->sp.k; *m++ = s->sp.marker_c; *m++ = 0; *m++ = 0;
-  for (uint32_t g = 0; g <= s->G; g++) *m++ = s->seed_off[g];
-  for (uint32_t g = 0; g <= s->G; g++) *m++ = s->uk_off[g];
-  for (uint32_t g = 0; g <= s->G; g++) *m++ = s->mk_off[g];
-  for (uint32_t g = 0; g <= s->G; g++) *m++ = s->ctg_off[g];
-  for (uint32_t g = 0; g < s->G; g++) *m++ = s->total_len[g];
-  for (size_t c = 0; c < s->C; c++) *m++ = s->ctg_len[c];
-  SK_CUDA(cudaStreamSynchronize(ctx->stream));
-  return SK_OK;
-}
+int sk_sketch_set_pack(const sk_sketch_set* s, void* d_blob, uint64_t* meta) { return sk_sketch_set_pack_subset(s, nullptr, 0, 0, d_blob, meta); }
 
 namespace {
-// host-side plan of a subset blob: maximal runs of consecutive genomes are copied with one memcpy per array
-struct SubsetPlan {
-  std::vector<uint32_t> idx;                        // selected genomes, in output order
-  std::vector<uint64_t> seed_off, uk_off, mk_off, ctg_off, ht_off;
-  size_t S = 0, U = 0, M = 0, C = 0, HT = 0;
-  bool tables = false;
-};
-int plan_subset(const sk_sketch_set* s, const uint32_t* genomes, uint32_t n, int flags, SubsetPlan& pl) {
+// metadata of a subset blob: the selected genomes (genomes = NULL: all) in output order
+int plan_subset(const sk_sketch_set* s, const uint32_t* genomes, uint32_t n, int flags, std::vector<uint32_t>& idx, SetMeta& m) {
   const bool mo = (flags & SK_PACK_MARKERS_ONLY) != 0;
-  if (!genomes) { n = s->G; pl.idx.resize(n); for (uint32_t i = 0; i < n; i++) pl.idx[i] = i; }
-  else pl.idx.assign(genomes, genomes + n);
-  pl.seed_off.assign(n + 1, 0); pl.uk_off.assign(n + 1, 0); pl.mk_off.assign(n + 1, 0); pl.ctg_off.assign(n + 1, 0); pl.ht_off.assign(n + 1, 0);
-  pl.tables = !mo && (flags & SK_PACK_TABLES) != 0 && s->htab != nullptr && s->ht_off.size() == (size_t)s->G + 1;
-  for (uint32_t i = 0; i < n; i++) {
-    const uint32_t g = pl.idx[i];
+  if (!genomes) { n = s->G; idx.resize(n); for (uint32_t i = 0; i < n; i++) idx[i] = i; }
+  else idx.assign(genomes, genomes + n);
+  m.c = s->sp.c; m.k = s->sp.k; m.marker_c = s->sp.marker_c;
+  m.tables = !mo && (flags & SK_PACK_TABLES) != 0 && s->htab != nullptr && s->ht_off.size() == (size_t)s->G + 1;
+  for (uint32_t g : idx) {
     if (g >= s->G) { s->ctx->err = "subset genome index out of range"; return SK_ERR_PARAM; }
-    pl.ht_off[i + 1] = pl.ht_off[i] + (pl.tables ? s->ht_off[g + 1] - s->ht_off[g] : 0);
-    pl.seed_off[i + 1] = pl.seed_off[i] + (mo ? 0 : s->seed_off[g + 1] - s->seed_off[g]);
-    pl.uk_off[i + 1] = pl.uk_off[i] + (mo ? 0 : s->uk_off[g + 1] - s->uk_off[g]);
-    pl.ctg_off[i + 1] = pl.ctg_off[i] + (mo ? 0 : s->ctg_off[g + 1] - s->ctg_off[g]);
-    pl.mk_off[i + 1] = pl.mk_off[i] + (s->mk_off[g + 1] - s->mk_off[g]);
+    const uint64_t cnt[N_COUNTS] = {s->seed_off[g + 1] - s->seed_off[g], s->uk_off[g + 1] - s->uk_off[g], s->mk_off[g + 1] - s->mk_off[g],
+                                    s->ctg_off[g + 1] - s->ctg_off[g], m.tables ? s->ht_off[g + 1] - s->ht_off[g] : 0};
+    meta_push(m, cnt, mo, s->total_len[g], s->ctg_len.begin() + s->ctg_off[g], s->ctg_len.begin() + s->ctg_off[g + 1]);
   }
-  pl.S = pl.seed_off[n]; pl.U = pl.uk_off[n]; pl.M = pl.mk_off[n]; pl.C = pl.ctg_off[n]; pl.HT = pl.ht_off[n];
   return SK_OK;
 }
 }  // namespace
@@ -556,11 +536,11 @@ int plan_subset(const sk_sketch_set* s, const uint32_t* genomes, uint32_t n, int
 int sk_sketch_set_subset_blob_size(const sk_sketch_set* s, const uint32_t* genomes, uint32_t n, int flags, uint64_t* device_bytes,
                                    uint64_t* host_meta_words) {
   if (!s || !device_bytes || !host_meta_words) return SK_ERR_PARAM;
-  SubsetPlan pl;
-  SK_TRY(plan_subset(s, genomes, n, flags, pl));
-  const size_t G = pl.idx.size();
-  *device_bytes = blob_layout(G, pl.S, pl.U, pl.M, pl.C, pl.HT).total;
-  *host_meta_words = meta_words(G, pl.C, pl.tables);
+  std::vector<uint32_t> idx;
+  SetMeta m;
+  SK_TRY(plan_subset(s, genomes, n, flags, idx, m));
+  *device_bytes = blob_layout(m.G, m.n).total;
+  *host_meta_words = meta_words(m.G, m.n[CNT_C], m.tables);
   return SK_OK;
 }
 
@@ -568,81 +548,40 @@ int sk_sketch_set_pack_subset(const sk_sketch_set* s, const uint32_t* genomes, u
   if (!s || !d_blob || !meta) return SK_ERR_PARAM;
   sk_ctx* ctx = s->ctx;
   SK_CUDA(cudaSetDevice(ctx->device));
-  SubsetPlan pl;
-  SK_TRY(plan_subset(s, genomes, n, flags, pl));
+  std::vector<uint32_t> idx;
+  SetMeta m;
+  SK_TRY(plan_subset(s, genomes, n, flags, idx, m));
   const bool mo = (flags & SK_PACK_MARKERS_ONLY) != 0;
-  const uint32_t G = (uint32_t)pl.idx.size();
-  const BlobLayout b = blob_layout(G, pl.S, pl.U, pl.M, pl.C, pl.HT);
+  const uint32_t G = (uint32_t)m.G;
+  const BlobLayout b = blob_layout(G, m.n);
   uint8_t* base = (uint8_t*)d_blob;
-  cudaStream_t st = ctx->stream;
-  // A scattered subset (the cross-block fetch of a genome order unrelated to relatedness asks for thousands of separate runs,
-  // 12 arrays each) would cost tens of thousands of cudaMemcpyAsync calls (150 ms measured for 5 000 genomes): beyond a few
-  // runs the segments are collected and copied by ONE batched device memcpy (cub::DeviceMemcpy::Batched).
-  uint32_t n_runs = 0;
-  for (uint32_t i = 0; i < G;) { uint32_t j = i + 1; while (j < G && pl.idx[j] == pl.idx[j - 1] + 1) j++; n_runs++; i = j; }
-  const bool batched = n_runs > 8;
-  std::vector<const void*> seg_src;
-  std::vector<void*> seg_dst;
-  std::vector<size_t> seg_n;
-  auto cp = [&](int arr, size_t dst_elem, const void* src, size_t src_elem, size_t count, size_t esz) -> cudaError_t {
-    if (count == 0) return cudaSuccess;
-    if (batched) {
-      seg_src.push_back((const uint8_t*)src + src_elem * esz); seg_dst.push_back(base + b.off[arr] + dst_elem * esz); seg_n.push_back(count * esz);
-      return cudaSuccess;
-    }
-    return cudaMemcpyAsync(base + b.off[arr] + dst_elem * esz, (const uint8_t*)src + src_elem * esz, count * esz, cudaMemcpyDeviceToDevice, st);
-  };
-  if (mo) {   // one zero sentinel per genome in the group-start and contig-record tables
-    if (G) SK_CUDA(cudaMemsetAsync(base + b.off[7], 0, (size_t)G * 4, st));
-    if (G) SK_CUDA(cudaMemsetAsync(base + b.off[9], 0, (size_t)G * 4, st));
-  }
+  SK_CUDA(zero_absent_arrays(ctx, base, b, mo, m.tables));
+  // maximal runs of consecutive source genomes [a, e) -> one segment per array; a scattered subset (the cross-block fetch of a
+  // genome order unrelated to relatedness asks for thousands of runs: 150 ms measured for 5 000 genomes as separate calls)
+  // goes through the batched copy beyond a few runs
+  const std::vector<uint64_t>* src[N_COUNTS] = {&s->seed_off, &s->uk_off, &s->mk_off, &s->ctg_off, &s->ht_off};
+  std::vector<std::pair<uint32_t, uint32_t>> runs;   // [i, j) of the output
   for (uint32_t i = 0; i < G;) {
     uint32_t j = i + 1;
-    while (j < G && pl.idx[j] == pl.idx[j - 1] + 1) j++;       // run [i, j) = source genomes [a, e)
-    const uint32_t a = pl.idx[i], e = pl.idx[j - 1] + 1;
-    if (!mo) {
-      const size_t so = s->seed_off[a], ns = s->seed_off[e] - so, uo = s->uk_off[a], nu = s->uk_off[e] - uo;
-      const size_t co = s->ctg_off[a], nc = s->ctg_off[e] - co;
-      SK_CUDA(cp(0, pl.seed_off[i], s->pv_kmer, so, ns, 4)); SK_CUDA(cp(1, pl.seed_off[i], s->pv_pos, so, ns, 4));
-      SK_CUDA(cp(2, pl.seed_off[i], s->pv_cc, so, ns, 4));   SK_CUDA(cp(3, pl.seed_off[i], s->pv_mult, so, ns, 2));
-      SK_CUDA(cp(4, pl.seed_off[i], s->kv_pos, so, ns, 4));  SK_CUDA(cp(5, pl.seed_off[i], s->kv_cc, so, ns, 4));
-      SK_CUDA(cp(6, pl.uk_off[i], s->ukmer, uo, nu, 4));
-      SK_CUDA(cp(7, pl.uk_off[i] + i, s->ustart, uo + a, nu + (e - a), 4));          // + one sentinel per genome
-      SK_CUDA(cp(9, pl.ctg_off[i] + i, s->ctg_rec_off, co + a, nc + (e - a), 4));
-      SK_CUDA(cp(10, pl.ctg_off[i], s->d_ctg_len, co, nc, 4));
-      if (pl.tables) SK_CUDA(cp(11, pl.ht_off[i], s->htab, s->ht_off[a], s->ht_off[e] - s->ht_off[a], 8));
-    }
-    SK_CUDA(cp(8, pl.mk_off[i], s->markers, s->mk_off[a], s->mk_off[e] - s->mk_off[a], 8));
+    while (j < G && idx[j] == idx[j - 1] + 1) j++;
+    runs.push_back({i, j});
     i = j;
   }
-  if (batched && !seg_n.empty()) {
-    const size_t ns = seg_n.size();
-    DTmp<const void*> d_src; DTmp<void*> d_dst; DTmp<size_t> d_n;
-    SK_CUDA(d_src.alloc(ns, ctx)); SK_CUDA(d_dst.alloc(ns, ctx)); SK_CUDA(d_n.alloc(ns, ctx));
-    SK_CUDA(cudaMemcpyAsync(d_src.p, seg_src.data(), ns * sizeof(void*), cudaMemcpyHostToDevice, st));
-    SK_CUDA(cudaMemcpyAsync(d_dst.p, seg_dst.data(), ns * sizeof(void*), cudaMemcpyHostToDevice, st));
-    SK_CUDA(cudaMemcpyAsync(d_n.p, seg_n.data(), ns * sizeof(size_t), cudaMemcpyHostToDevice, st));
-    size_t tb = 0;
-    SK_CUDA(cub::DeviceMemcpy::Batched(nullptr, tb, d_src.p, d_dst.p, d_n.p, (uint32_t)ns, st));
-    DTmp<uint8_t> tmp;
-    SK_CUDA(tmp.alloc(tb, ctx));
-    SK_CUDA(cub::DeviceMemcpy::Batched(tmp.p, tb, d_src.p, d_dst.p, d_n.p, (uint32_t)ns, st));
-    sk::count_launch(ctx);
-    SK_CUDA(cudaStreamSynchronize(st));      // the host-side segment lists and the temporaries are released below
+  SegmentCopy cp;
+  cp.batched = runs.size() > 8;
+  for (auto [i, j] : runs) {
+    const uint32_t a0 = idx[i], e = idx[j - 1] + 1;
+    for (int a = 0; a < BLOB_ARRAYS; a++) {
+      if (!array_travels(a, mo, m.tables)) continue;
+      const ArrayDesc& d = SET_ARRAYS[a];
+      const std::vector<uint64_t>& so = *src[d.by];
+      const uint64_t first = array_index(a, a0, so[a0]), count = array_index(a, e, so[e]) - first;
+      cp.add((const uint8_t*)set_array(s, a) + first * d.esz, base + b.off[a] + array_index(a, i, m.off[d.by][i]) * d.esz, count * d.esz);
+    }
   }
-  uint64_t* m = meta;
-  *m++ = G; *m++ = pl.S; *m++ = pl.U; *m++ = pl.M; *m++ = pl.C; *m++ = s->sp.c; *m++ = s->sp.k; *m++ = s->sp.marker_c;
-  *m++ = pl.HT; *m++ = pl.tables ? 1 : 0;
-  for (uint32_t g = 0; g <= G; g++) *m++ = pl.seed_off[g];
-  for (uint32_t g = 0; g <= G; g++) *m++ = pl.uk_off[g];
-  for (uint32_t g = 0; g <= G; g++) *m++ = pl.mk_off[g];
-  for (uint32_t g = 0; g <= G; g++) *m++ = pl.ctg_off[g];
-  for (uint32_t g = 0; g < G; g++) *m++ = s->total_len[pl.idx[g]];
-  if (!mo)
-    for (uint32_t g = 0; g < G; g++)
-      for (uint64_t c = s->ctg_off[pl.idx[g]]; c < s->ctg_off[pl.idx[g] + 1]; c++) *m++ = s->ctg_len[c];
-  if (pl.tables) for (uint32_t g = 0; g <= G; g++) *m++ = pl.ht_off[g];
-  SK_CUDA(cudaStreamSynchronize(st));
+  SK_TRY(cp.run(ctx));
+  encode_meta(m, meta);
+  SK_CUDA(cudaStreamSynchronize(ctx->stream));
   return SK_OK;
 }
 
@@ -654,32 +593,19 @@ int sk_sketch_set_unpack(sk_ctx* ctx, uint32_t n_parts, const void* const* d_blo
   std::vector<sk_sketch_set> views(n_parts);
   std::vector<const sk_sketch_set*> vp;
   for (uint32_t i = 0; i < n_parts; i++) {
-    const uint64_t* m = metas[i];
+    SetMeta m = decode_meta(metas[i]);
     sk_sketch_set& v = views[i];
     v.ctx = ctx;
-    v.G = (uint32_t)m[0]; v.S = m[1]; v.U = m[2]; v.M = m[3]; v.C = m[4];
-    v.sp.c = (uint32_t)m[5]; v.sp.k = (uint32_t)m[6]; v.sp.marker_c = (uint32_t)m[7];
-    const uint64_t HT = m[8];
-    const bool tables = m[9] != 0;
-    all_tables = all_tables && (tables || v.U == 0);
-    m += META_HEADER;
-    v.seed_off.assign(m, m + v.G + 1); m += v.G + 1;
-    v.uk_off.assign(m, m + v.G + 1); m += v.G + 1;
-    v.mk_off.assign(m, m + v.G + 1); m += v.G + 1;
-    v.ctg_off.assign(m, m + v.G + 1); m += v.G + 1;
-    v.total_len.assign(m, m + v.G); m += v.G;
-    v.ctg_len.resize(v.C);
-    for (size_t c = 0; c < v.C; c++) v.ctg_len[c] = (uint32_t)m[c];
+    v.G = (uint32_t)m.G; v.S = m.n[CNT_S]; v.U = m.n[CNT_U]; v.M = m.n[CNT_M]; v.C = m.n[CNT_C];
+    v.sp = sk_sketch_params{(uint32_t)m.c, (uint32_t)m.k, (uint32_t)m.marker_c};
+    all_tables = all_tables && (m.tables || v.U == 0);
+    v.seed_off = std::move(m.off[CNT_S]); v.uk_off = std::move(m.off[CNT_U]); v.mk_off = std::move(m.off[CNT_M]);
+    v.ctg_off = std::move(m.off[CNT_C]); v.ht_off = std::move(m.off[CNT_HT]);
+    v.total_len = std::move(m.total_len);
+    v.ctg_len.assign(m.ctg_len.begin(), m.ctg_len.end());
     v.name_rank.resize(v.G);
-    if (tables) { v.ht_off.assign(m + v.C, m + v.C + v.G + 1); }
-    else v.ht_off.assign((size_t)v.G + 1, 0);
-    BlobLayout b = blob_layout(v.G, v.S, v.U, v.M, v.C, HT);
-    uint8_t* base = (uint8_t*)d_blobs[i];
-    v.htab = (unsigned long long*)(base + b.off[11]);
-    v.pv_kmer = (uint32_t*)(base + b.off[0]); v.pv_pos = (uint32_t*)(base + b.off[1]); v.pv_cc = (uint32_t*)(base + b.off[2]);
-    v.pv_mult = (uint16_t*)(base + b.off[3]); v.kv_pos = (uint32_t*)(base + b.off[4]); v.kv_cc = (uint32_t*)(base + b.off[5]);
-    v.ukmer = (uint32_t*)(base + b.off[6]); v.ustart = (uint32_t*)(base + b.off[7]); v.markers = (uint64_t*)(base + b.off[8]);
-    v.ctg_rec_off = (uint32_t*)(base + b.off[9]); v.d_ctg_len = (uint32_t*)(base + b.off[10]);
+    const BlobLayout b = blob_layout(m.G, m.n);
+    for (int a = 0; a < BLOB_ARRAYS; a++) set_array(&v, a) = (uint8_t*)d_blobs[i] + b.off[a];
     vp.push_back(&v);
   }
   // blobs packed with SK_PACK_TABLES bring their k-mer hash tables along: no rebuild (genomes too large for a table, which
@@ -690,7 +616,6 @@ int sk_sketch_set_unpack(sk_ctx* ctx, uint32_t n_parts, const void* const* d_blo
         if (v.uk_off[g + 1] > v.uk_off[g] && v.ht_off[g + 1] == v.ht_off[g]) all_tables = false;
   }
   SK_TRY(concat_sets(ctx, vp, out, all_tables));
-  for (auto& v : views) v.htab = nullptr;
   if (all_tables) return SK_OK;
   return build_hash(ctx, *out);
 }
@@ -1117,20 +1042,19 @@ int sketch_batch_host(sk_ctx* ctx, const HostSeq& seq, const uint64_t* contig_of
 }
 
 namespace {
-template <typename T>
-int grow_append(sk_ctx* ctx, T** arr, size_t* cap, size_t used_alloc, size_t used, const T* src, size_t add) {
-  // *cap == 0: the array was allocated at exactly `used_alloc` elements
-  const size_t have = *cap ? *cap : std::max<size_t>(used_alloc, 1);
+// appends `add` elements of esz bytes at element `used` of *arr, growing it by 1.5x when its capacity (0: exactly `used`) is short
+int grow_append(sk_ctx* ctx, void*& arr, size_t& cap, size_t used, const void* src, size_t add, size_t esz) {
+  const size_t have = cap ? cap : std::max<size_t>(used, 1);
   if (used + add > have) {
     const size_t ncap = std::max<size_t>(used + add, have + have / 2);
-    T* n = nullptr;
-    SK_CUDA(ctx->arena.alloc((void**)&n, ncap * sizeof(T)));
-    if (used) SK_CUDA(cudaMemcpyAsync(n, *arr, used * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
+    void* n = nullptr;
+    SK_CUDA(ctx->arena.alloc(&n, ncap * esz));
+    if (used) SK_CUDA(cudaMemcpyAsync(n, arr, used * esz, cudaMemcpyDeviceToDevice, ctx->stream));
     SK_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (*arr) ctx->arena.release(*arr);
-    *arr = n; *cap = ncap;
+    if (arr) ctx->arena.release(arr);
+    arr = n; cap = ncap;
   }
-  if (add) SK_CUDA(cudaMemcpyAsync(*arr + used, src, add * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
+  if (add) SK_CUDA(cudaMemcpyAsync((uint8_t*)arr + used * esz, src, add * esz, cudaMemcpyDeviceToDevice, ctx->stream));
   return SK_OK;
 }
 }  // namespace
@@ -1144,34 +1068,24 @@ int append_sets_inplace(sk_ctx* ctx, sk_sketch_set** dstp, const std::vector<sk_
     d->seed_off = {0}; d->uk_off = {0}; d->mk_off = {0}; d->ctg_off = {0}; d->ht_off = {0};
     const uint64_t S = (uint64_t)((double)hint.bases / d->sp.c * 1.06) + 64 * hint.genomes + 1024;
     const uint64_t M = (uint64_t)((double)hint.bases / d->sp.marker_c * 1.10) + 16 * hint.genomes + 1024;
-    d->capS = S; d->capU = S; d->capUG = S + hint.genomes + 1; d->capM = M; d->capC = hint.contigs + 1; d->capCG = hint.contigs + hint.genomes + 1;
-    d->capHT = 4 * S + 16 * hint.genomes;   // table capacity = power of two >= 2 x distinct k-mers: between 2 and 4 entries per k-mer
+    // distinct k-mers <= records; table capacity = power of two >= 2 x distinct k-mers: between 2 and 4 entries per k-mer.
+    // Sized for one genome and one contig more than the hint, so ctg_rec_off (contig + genome counted) holds one element more
+    // than the hint can need
+    const uint64_t reserve[N_COUNTS] = {S, S, M, hint.contigs + 1, 4 * S + 16 * hint.genomes};
     struct G0 { sk_sketch_set* s; ~G0() { if (s) { free_set_device(s); delete s; } } } g0{d};
-    SK_CUDA(ctx->arena.alloc((void**)&d->pv_kmer, d->capS * 4)); SK_CUDA(ctx->arena.alloc((void**)&d->pv_pos, d->capS * 4));
-    SK_CUDA(ctx->arena.alloc((void**)&d->pv_cc, d->capS * 4));   SK_CUDA(ctx->arena.alloc((void**)&d->pv_mult, d->capS * 2));
-    SK_CUDA(ctx->arena.alloc((void**)&d->kv_pos, d->capS * 4));  SK_CUDA(ctx->arena.alloc((void**)&d->kv_cc, d->capS * 4));
-    SK_CUDA(ctx->arena.alloc((void**)&d->ukmer, d->capU * 4));   SK_CUDA(ctx->arena.alloc((void**)&d->ustart, d->capUG * 4));
-    SK_CUDA(ctx->arena.alloc((void**)&d->markers, d->capM * 8)); SK_CUDA(ctx->arena.alloc((void**)&d->ctg_rec_off, d->capCG * 4));
-    SK_CUDA(ctx->arena.alloc((void**)&d->d_ctg_len, d->capC * 4)); SK_CUDA(ctx->arena.alloc((void**)&d->htab, d->capHT * 8));
+    for (int a = 0; a < BLOB_ARRAYS; a++) {
+      d->cap[a] = array_elems(a, hint.genomes + 1, reserve);
+      SK_CUDA(ctx->arena.alloc(&set_array(d, a), d->cap[a] * SET_ARRAYS[a].esz));
+    }
     g0.s = nullptr;
     *dstp = d;
   }
   const uint32_t g_begin = d->G;
   for (auto* p : parts) {
-    if (p->sp.c != d->sp.c || p->sp.k != d->sp.k || p->sp.marker_c != d->sp.marker_c) { ctx->err = "sketch parameter mismatch"; return SK_ERR_PARAM; }
-    size_t cS;   // the six record arrays share one capacity
-    cS = d->capS; SK_TRY(grow_append(ctx, &d->pv_kmer, &cS, d->S, d->S, p->pv_kmer, p->S));
-    cS = d->capS; SK_TRY(grow_append(ctx, &d->pv_pos, &cS, d->S, d->S, p->pv_pos, p->S));
-    cS = d->capS; SK_TRY(grow_append(ctx, &d->pv_cc, &cS, d->S, d->S, p->pv_cc, p->S));
-    cS = d->capS; SK_TRY(grow_append(ctx, &d->pv_mult, &cS, d->S, d->S, p->pv_mult, p->S));
-    cS = d->capS; SK_TRY(grow_append(ctx, &d->kv_pos, &cS, d->S, d->S, p->kv_pos, p->S));
-    cS = d->capS; SK_TRY(grow_append(ctx, &d->kv_cc, &cS, d->S, d->S, p->kv_cc, p->S));
-    d->capS = cS;
-    SK_TRY(grow_append(ctx, &d->ukmer, &d->capU, d->U, d->U, p->ukmer, p->U));
-    SK_TRY(grow_append(ctx, &d->ustart, &d->capUG, d->U + d->G, d->U + d->G, p->ustart, p->U + p->G));
-    SK_TRY(grow_append(ctx, &d->markers, &d->capM, d->M, d->M, p->markers, p->M));
-    SK_TRY(grow_append(ctx, &d->ctg_rec_off, &d->capCG, d->C + d->G, d->C + d->G, p->ctg_rec_off, p->C + p->G));
-    SK_TRY(grow_append(ctx, &d->d_ctg_len, &d->capC, d->C, d->C, p->d_ctg_len, p->C));
+    if (!same_params(p->sp, d->sp)) { ctx->err = "sketch parameter mismatch"; return SK_ERR_PARAM; }
+    for (int a = 0; a < BLOB_ARRAYS; a++)   // every array but the k-mer tables, which build_hash_range appends
+      if (array_travels(a, false, false))
+        SK_TRY(grow_append(ctx, set_array(d, a), d->cap[a], set_elems(d, a), set_array(p, a), set_elems(p, a), SET_ARRAYS[a].esz));
     for (uint32_t g = 0; g < p->G; g++) {
       d->seed_off.push_back(d->seed_off.back() + (p->seed_off[g + 1] - p->seed_off[g]));
       d->uk_off.push_back(d->uk_off.back() + (p->uk_off[g + 1] - p->uk_off[g]));
@@ -1185,15 +1099,6 @@ int append_sets_inplace(sk_ctx* ctx, sk_sketch_set** dstp, const std::vector<sk_
   }
   SK_CUDA(cudaStreamSynchronize(ctx->stream));   // the parts may be released by the caller now
   return build_hash_range(ctx, d, g_begin);
-}
-
-// concatenate `parts` after `base` (may be null) into a fresh set owned by ctx, with hash tables; inputs stay valid
-int merge_sets(sk_ctx* ctx, const sk_sketch_set* base, const std::vector<sk_sketch_set*>& parts, sk_sketch_set** out) {
-  std::vector<const sk_sketch_set*> v;
-  if (base) v.push_back(base);
-  for (auto* p : parts) v.push_back(p);
-  SK_TRY(concat_sets(ctx, v, out));
-  return build_hash(ctx, *out);
 }
 }  // namespace sk
 

@@ -46,6 +46,43 @@ struct PhaseBarrier {   // all threads meet; a failure reported by any of them m
 
 struct Blob { void* d = nullptr; uint64_t bytes = 0; std::vector<uint64_t> meta; };
 
+// packs the genomes of s (NULL: all of them) with these flags into a blob in the arena of s's context; errors name `who`
+int pack_blob(const char* who, const sk_sketch_set* s, const std::vector<uint32_t>* genomes, int flags, Blob& b) {
+  sk_ctx* c = s->ctx;
+  const uint32_t none = 0;
+  const uint32_t* g = genomes ? (genomes->empty() ? &none : genomes->data()) : nullptr;
+  const uint32_t n = genomes ? (uint32_t)genomes->size() : 0;
+  uint64_t words = 0;
+  SK_TRY(sk_sketch_set_subset_blob_size(s, g, n, flags, &b.bytes, &words));
+  if (cudaSetDevice(c->device) != cudaSuccess || c->arena.alloc(&b.d, b.bytes) != cudaSuccess) {
+    c->err = std::string(who) + ": out of device memory (source)";
+    return SK_ERR_NOMEM;
+  }
+  b.meta.resize(words);
+  return sk_sketch_set_pack_subset(s, g, n, flags, b.d, b.meta.data());
+}
+
+// copies the blobs (which may lie on other devices) into one buffer on ctx and unpacks them into one set, in list order;
+// errors name `who`
+int unpack_blobs(const char* who, sk_ctx* ctx, const std::vector<const Blob*>& blobs, sk_sketch_set** out) {
+  const size_t n = blobs.size();
+  std::vector<uint64_t> offs(n + 1, 0);
+  for (size_t r = 0; r < n; r++) offs[r + 1] = offs[r] + sk::al256(blobs[r]->bytes);
+  DTmp<uint8_t> all;
+  if (all.alloc(std::max<uint64_t>(offs[n], 256), ctx) != cudaSuccess) { ctx->err = std::string(who) + ": out of device memory (destination)"; return SK_ERR_NOMEM; }
+  std::vector<const void*> bp(n);
+  std::vector<const uint64_t*> mp(n);
+  cudaError_t e = cudaSuccess;
+  for (size_t r = 0; r < n && e == cudaSuccess; r++) {
+    bp[r] = all.p + offs[r];
+    mp[r] = blobs[r]->meta.data();
+    e = cudaMemcpyAsync(all.p + offs[r], blobs[r]->d, blobs[r]->bytes, cudaMemcpyDefault, ctx->stream);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) { ctx->err = std::string(who) + ": " + cudaGetErrorString(e); return SK_ERR_CUDA; }
+  return sk_sketch_set_unpack(ctx, (uint32_t)n, bp.data(), mp.data(), out);
+}
+
 double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 
 // peer access between the distinct devices of ctxs[0..n) (ignored when unsupported: copies then stage through the host)
@@ -175,29 +212,13 @@ extern "C" int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint
     }
     const double t1 = now_s();
     // ---- 2. markers of every block -> every device
-    if (rc == SK_OK) {
-      uint64_t words = 0;
-      rc = sk_sketch_set_subset_blob_size(local[d], nullptr, 0, SK_PACK_MARKERS_ONLY, &mk[d].bytes, &words);
-      if (rc == SK_OK && c->arena.alloc(&mk[d].d, mk[d].bytes) != cudaSuccess) rc = SK_ERR_NOMEM;
-      if (rc == SK_OK) { mk[d].meta.resize(words); rc = sk_sketch_set_pack_subset(local[d], nullptr, 0, SK_PACK_MARKERS_ONLY, mk[d].d, mk[d].meta.data()); }
-    }
+    if (rc == SK_OK) rc = pack_blob("sk_triangle_multi", local[d], nullptr, SK_PACK_MARKERS_ONLY, mk[d]);
     if (!bar.sync(rc == SK_OK)) return rc;
     sk_sketch_set* mkset = nullptr;
     {
-      std::vector<uint64_t> offs(W + 1, 0);
-      for (uint32_t r = 0; r < W; r++) offs[r + 1] = offs[r] + ((mk[r].bytes + 255) & ~255ull);
-      void* all = nullptr;
-      if (c->arena.alloc(&all, std::max<uint64_t>(offs[W], 256)) != cudaSuccess) rc = SK_ERR_NOMEM;
-      for (uint32_t r = 0; r < W && rc == SK_OK; r++)
-        if (cudaMemcpyAsync((uint8_t*)all + offs[r], mk[r].d, mk[r].bytes, cudaMemcpyDefault, c->stream) != cudaSuccess) rc = SK_ERR_CUDA;
-      if (rc == SK_OK && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = SK_ERR_CUDA;
-      if (rc == SK_OK) {
-        std::vector<const void*> bp(W);
-        std::vector<const uint64_t*> mp_(W);
-        for (uint32_t r = 0; r < W; r++) { bp[r] = (uint8_t*)all + offs[r]; mp_[r] = mk[r].meta.data(); }
-        rc = sk_sketch_set_unpack(c, W, bp.data(), mp_.data(), &mkset);
-      }
-      if (all) c->arena.release(all);
+      std::vector<const Blob*> from(W);
+      for (uint32_t r = 0; r < W; r++) from[r] = &mk[r];
+      rc = unpack_blobs("sk_triangle_multi", c, from, &mkset);
     }
     if (!bar.sync(rc == SK_OK)) { if (mkset) sk_sketch_set_free(mkset); return rc; }   // every peer has copied: the marker blobs may go
     c->arena.release(mk[d].d); mk[d].d = nullptr;
@@ -233,33 +254,18 @@ extern "C" int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint
       if (r == d) mine = need;
       std::vector<uint32_t> loc;
       for (uint32_t g : need) if (g >= gb[d] && g < gb[d + 1]) loc.push_back(g - gb[d]);
-      Blob& b = sub[d][r];
-      uint64_t words = 0;
-      uint32_t dummy = 0;
-      rc = sk_sketch_set_subset_blob_size(local[d], loc.empty() ? &dummy : loc.data(), (uint32_t)loc.size(), SK_PACK_TABLES, &b.bytes, &words);
-      if (rc == SK_OK && c->arena.alloc(&b.d, b.bytes) != cudaSuccess) rc = SK_ERR_NOMEM;
-      if (rc == SK_OK) { b.meta.resize(words); rc = sk_sketch_set_pack_subset(local[d], loc.empty() ? &dummy : loc.data(), (uint32_t)loc.size(), SK_PACK_TABLES, b.d, b.meta.data()); }
+      rc = pack_blob("sk_triangle_multi", local[d], &loc, SK_PACK_TABLES, sub[d][r]);
     }
     if (!bar.sync(rc == SK_OK)) return rc;
     sk_sketch_set* work = nullptr;
     uint64_t remote_bytes = 0;
     {
-      std::vector<uint64_t> offs(W + 1, 0);
-      for (uint32_t r = 0; r < W; r++) offs[r + 1] = offs[r] + ((sub[r][d].bytes + 255) & ~255ull);
-      void* all = nullptr;
-      if (c->arena.alloc(&all, std::max<uint64_t>(offs[W], 256)) != cudaSuccess) rc = SK_ERR_NOMEM;
-      for (uint32_t r = 0; r < W && rc == SK_OK; r++) {
-        if (cudaMemcpyAsync((uint8_t*)all + offs[r], sub[r][d].d, sub[r][d].bytes, cudaMemcpyDefault, c->stream) != cudaSuccess) rc = SK_ERR_CUDA;
+      std::vector<const Blob*> from(W);
+      for (uint32_t r = 0; r < W; r++) {
+        from[r] = &sub[r][d];
         if (r != d) remote_bytes += sub[r][d].bytes;
       }
-      if (rc == SK_OK && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = SK_ERR_CUDA;
-      if (rc == SK_OK) {
-        std::vector<const void*> bp(W);
-        std::vector<const uint64_t*> mp_(W);
-        for (uint32_t r = 0; r < W; r++) { bp[r] = (uint8_t*)all + offs[r]; mp_[r] = sub[r][d].meta.data(); }
-        rc = sk_sketch_set_unpack(c, W, bp.data(), mp_.data(), &work);     // source-block order = ascending global ids
-      }
-      if (all) c->arena.release(all);
+      rc = unpack_blobs("sk_triangle_multi", c, from, &work);     // source-block order = ascending global ids
     }
     if (!bar.sync(rc == SK_OK)) { if (work) sk_sketch_set_free(work); return rc; }     // every peer has copied its sub-blobs
     for (uint32_t r = 0; r < W; r++) if (sub[d][r].d) { c->arena.release(sub[d][r].d); sub[d][r].d = nullptr; }
@@ -337,27 +343,21 @@ extern "C" int sk_sketch_set_copy(sk_ctx* dst, const sk_sketch_set* src, sk_sket
   sk_ctx* sc = src->ctx;
   if (dst != sc) { sk_ctx* pair[2] = {sc, dst}; enable_peer_access(pair, 2); }
   // the source set's own blob, k-mer tables included (no rebuild on the destination), copied device to device
-  uint64_t bytes = 0, words = 0;
-  int rc = sk_sketch_set_subset_blob_size(src, nullptr, 0, SK_PACK_TABLES, &bytes, &words);
-  std::vector<uint64_t> meta(words);
-  void *sblob = nullptr, *dblob = nullptr;
-  if (rc == SK_OK && (cudaSetDevice(sc->device) != cudaSuccess || sc->arena.alloc(&sblob, bytes) != cudaSuccess)) { sc->err = "sk_sketch_set_copy: out of device memory (source)"; rc = SK_ERR_NOMEM; }
-  if (rc == SK_OK) rc = sk_sketch_set_pack_subset(src, nullptr, 0, SK_PACK_TABLES, sblob, meta.data());   // synchronises the source stream
-  if (rc != SK_OK && dst != sc) dst->err = sc->err;
-  const void* from = sblob;
-  if (rc == SK_OK && dst != sc) {
-    cudaError_t e = cudaSetDevice(dst->device);
-    if (e == cudaSuccess && dst->arena.alloc(&dblob, bytes) != cudaSuccess) { dst->err = "sk_sketch_set_copy: out of device memory (destination)"; rc = SK_ERR_NOMEM; }
-    if (rc == SK_OK && e == cudaSuccess) e = cudaMemcpyAsync(dblob, sblob, bytes, cudaMemcpyDefault, dst->stream);
-    if (rc == SK_OK && e == cudaSuccess) e = cudaStreamSynchronize(dst->stream);
-    if (rc == SK_OK && e != cudaSuccess) { dst->err = std::string("sk_sketch_set_copy: ") + cudaGetErrorString(e); rc = SK_ERR_CUDA; }
-    from = dblob;
+  Blob blob;
+  int rc = pack_blob("sk_sketch_set_copy", src, nullptr, SK_PACK_TABLES, blob);   // synchronises the source stream
+  if (rc == SK_OK && dst == sc) {
+    const void* bp = blob.d;
+    const uint64_t* mp = blob.meta.data();
+    rc = sk_sketch_set_unpack(dst, 1, &bp, &mp, out);
+  } else if (rc == SK_OK) {
+    const cudaError_t e = cudaSetDevice(dst->device);
+    if (e == cudaSuccess) rc = unpack_blobs("sk_sketch_set_copy", dst, {&blob}, out);
+    else { dst->err = std::string("sk_sketch_set_copy: ") + cudaGetErrorString(e); rc = SK_ERR_CUDA; }
+  } else if (dst != sc) {
+    dst->err = sc->err;
   }
-  const uint64_t* mp = meta.data();
-  if (rc == SK_OK) rc = sk_sketch_set_unpack(dst, 1, &from, &mp, out);
   if (rc == SK_OK) { (*out)->name_rank = src->name_rank; (*out)->ranks_user_set = src->ranks_user_set; }   // host-side state
-  if (dblob) { cudaSetDevice(dst->device); dst->arena.release(dblob); }
-  if (sblob) { cudaSetDevice(sc->device); sc->arena.release(sblob); }
+  if (blob.d) { cudaSetDevice(sc->device); sc->arena.release(blob.d); }
   cudaSetDevice(dst->device);
   return rc;
 }
@@ -379,7 +379,6 @@ int check_qr_args(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* cons
   if (!refs || !ref_first || !queries || !mp) return fail("NULL argument");
   if (!queries[0]) return fail("queries[0] is NULL");
   const sk_sketch_set* q0 = queries[0];
-  auto same_params = [](const sk_sketch_params& a, const sk_sketch_params& b) { return a.c == b.c && a.k == b.k && a.marker_c == b.marker_c; };
   qb.G.assign(n_ctx, 0);
   for (uint32_t d = 0; d < n_ctx; d++) {
     const std::string at = "context " + std::to_string(d) + ": ";
@@ -389,10 +388,10 @@ int check_qr_args(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* cons
     if (!q || q->ctx != ctxs[d]) return fail(at + "queries[d] must be a set of ctxs[d]");
     if (q->G != q0->G || q->seed_off != q0->seed_off || q->mk_off != q0->mk_off || q->ctg_off != q0->ctg_off)
       return fail(at + "queries[d] is not the query set of context 0 (copy it with sk_sketch_set_copy)");
-    if (!same_params(q->sp, q0->sp)) return fail(at + "sketch parameters differ");
+    if (!sk::same_params(q->sp, q0->sp)) return fail(at + "sketch parameters differ");
     if (refs[d]) {
       if (refs[d]->ctx != ctxs[d]) return fail(at + "refs[d] must be a set of ctxs[d]");
-      if (!same_params(refs[d]->sp, q0->sp)) return fail(at + "sketch parameters differ");
+      if (!sk::same_params(refs[d]->sp, q0->sp)) return fail(at + "sketch parameters differ");
       qb.G[d] = refs[d]->G;
     }
     if (d && (uint64_t)ref_first[d] < (uint64_t)ref_first[d - 1] + qb.G[d - 1]) return fail(at + "ref_first must be ascending and the blocks disjoint");

@@ -373,14 +373,13 @@ static int scan_exclusive(sk_ctx* ctx, const T* in, T* out, size_t n) {
 }
 
 void free_set_device(sk_sketch_set* s) {
-  void* ptrs[] = {s->pv_kmer, s->pv_pos, s->pv_cc, s->pv_mult, s->kv_pos, s->kv_cc, s->ukmer, s->ustart,
-                  s->markers, s->ctg_rec_off, s->d_ctg_len, s->ubucket, s->htab};
-  for (void* p : ptrs) if (p) s->ctx->arena.release(p);
-  s->pv_kmer = s->pv_pos = s->pv_cc = s->kv_pos = s->kv_cc = s->ukmer = s->ustart = s->ctg_rec_off = s->d_ctg_len = nullptr;
-  s->pv_mult = nullptr;
-  s->markers = nullptr;
+  for (int a = 0; a < BLOB_ARRAYS; a++) {
+    void*& p = set_array(s, a);
+    if (p) s->ctx->arena.release(p);
+    p = nullptr;
+  }
+  if (s->ubucket) s->ctx->arena.release(s->ubucket);
   s->ubucket = nullptr;
-  s->htab = nullptr;
 }
 
 // per-genome k-mer hash table for the probe kernel: one 8-byte entry holds key, group start and (saturated) group size,
@@ -458,19 +457,19 @@ int build_hash(sk_ctx* ctx, sk_sketch_set* set) {
 int build_hash_range(sk_ctx* ctx, sk_sketch_set* set, uint32_t g_begin) {
   cudaStream_t st = ctx->stream;
   const uint32_t G = set->G;
-  if (set->ht_off.size() != (size_t)g_begin + 1 || set->ubucket || getenv("SK_FORCE_BUCKET_PROBE")) { set->capHT = 0; return build_hash(ctx, set); }
+  if (set->ht_off.size() != (size_t)g_begin + 1 || set->ubucket || getenv("SK_FORCE_BUCKET_PROBE")) { set->cap[HTAB_ARRAY] = 0; return build_hash(ctx, set); }
   std::vector<uint64_t> ht(set->ht_off);
   for (uint32_t g = g_begin; g < G; g++) {
     const uint64_t nuk = set->uk_off[g + 1] - set->uk_off[g], nrec = set->seed_off[g + 1] - set->seed_off[g];
     uint64_t cap = 0;
     if (nuk > 0) {
-      if (nrec >= (1ull << 20)) { set->capHT = 0; return build_hash(ctx, set); }
+      if (nrec >= (1ull << 20)) { set->cap[HTAB_ARRAY] = 0; return build_hash(ctx, set); }
       cap = 16; while (cap < 2 * nuk) cap <<= 1;
     }
     ht.push_back(ht.back() + cap);
   }
   const uint64_t old_total = ht[g_begin], total = ht[G];
-  const size_t have = set->capHT ? set->capHT : std::max<uint64_t>(old_total, 1);
+  const size_t have = set->cap[HTAB_ARRAY] ? set->cap[HTAB_ARRAY] : std::max<uint64_t>(old_total, 1);
   if (total > have) {
     const size_t ncap = std::max<size_t>(total, have + have / 2);
     unsigned long long* nt = nullptr;
@@ -478,7 +477,7 @@ int build_hash_range(sk_ctx* ctx, sk_sketch_set* set, uint32_t g_begin) {
     if (old_total) SK_CUDA(cudaMemcpyAsync(nt, set->htab, old_total * 8, cudaMemcpyDeviceToDevice, st));
     SK_CUDA(cudaStreamSynchronize(st));
     ctx->arena.release(set->htab);
-    set->htab = nt; set->capHT = ncap;
+    set->htab = nt; set->cap[HTAB_ARRAY] = ncap;
   }
   set->ht_off = ht;
   if (total == old_total) return SK_OK;

@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "../../include/skani_b200.h"
+#include "set_layout.hpp"
 
 // Context-owned device arena: every sketch-set array and every temporary of this library is sub-allocated from a few
 // large cudaMalloc'd slabs with host-side first-fit bookkeeping.  All users run on the context's single stream, so a
@@ -136,10 +137,21 @@ struct sk_sketch_set {
   uint32_t* d_ctg_len = nullptr;                                      // [C]
   unsigned long long* htab = nullptr;                                 // [ht_off[G]] per-genome open-addressing table: kmer<<32 | start<<12 | min(count,4095); 0 = empty
   std::vector<uint64_t> ht_off;                                       // [G+1] table offsets (capacity = power of two, >= 2 * distinct k-mers); capacity 0 => use ubucket search
-  // element capacities of the device arrays when the set grows in place (append_sets_inplace); 0 = allocated at exact size
-  size_t capS = 0, capU = 0, capUG = 0, capM = 0, capC = 0, capCG = 0, capHT = 0;
+  // element capacities of the blob arrays (SET_ARRAYS order) when the set grows in place (append_sets_inplace); 0 = exact size
+  size_t cap[sk::BLOB_ARRAYS] = {};
   uint32_t* ubucket = nullptr;                                        // [G * (UBUCKETS + 1)] first ukmer index of each top-bits bucket, per genome
 };
+
+namespace sk {
+// the member pointer of blob array a (SET_ARRAYS order), untyped
+inline void*& set_array(sk_sketch_set* s, int a) {
+  void** p[BLOB_ARRAYS] = {(void**)&s->pv_kmer, (void**)&s->pv_pos, (void**)&s->pv_cc, (void**)&s->pv_mult, (void**)&s->kv_pos, (void**)&s->kv_cc,
+                           (void**)&s->ukmer,   (void**)&s->ustart, (void**)&s->markers, (void**)&s->ctg_rec_off, (void**)&s->d_ctg_len, (void**)&s->htab};
+  return *p[a];
+}
+inline const void* set_array(const sk_sketch_set* s, int a) { return set_array(const_cast<sk_sketch_set*>(s), a); }
+inline bool same_params(const sk_sketch_params& a, const sk_sketch_params& b) { return a.c == b.c && a.k == b.k && a.marker_c == b.marker_c; }
+}  // namespace sk
 
 #define SK_CUDA(call)                                                                         \
   do {                                                                                        \
@@ -216,34 +228,28 @@ SkPool* ctx_pool(sk_ctx* ctx);
 struct SetReserve { uint64_t bases = 0, contigs = 0, genomes = 0; };
 int append_sets_inplace(sk_ctx* ctx, sk_sketch_set** dst, const std::vector<sk_sketch_set*>& parts, const SetReserve& hint);
 int build_hash_range(sk_ctx* ctx, sk_sketch_set* set, uint32_t g_begin);   // tables of the genomes [g_begin, G) appended to set->htab
-int merge_sets(sk_ctx* ctx, const sk_sketch_set* base, const std::vector<sk_sketch_set*>& parts, sk_sketch_set** out);  // (re)builds set->htab from ukmer/ustart; call on every finished set
 // screen.cu: incremental triangle screen of a growing set (pipelined sk_triangle)
 struct TriScreen;
 int tri_screen_create(sk_ctx* ctx, size_t marker_hint, TriScreen** out);
 int tri_screen_add(TriScreen* ts, const sk_sketch_set* set, uint32_t g_end, uint32_t row_begin, const sk_map_params* mp, uint64_t** pairs, uint64_t* n);
 void tri_screen_free(TriScreen* ts);
 bool tri_screen_supports(uint32_t n_genomes, uint64_t n_markers);
-// sketch-set blob (sk_sketch_set_pack / pack_subset / unpack, and the host sketch store of store.cu): 12 arrays, each
-// 256-byte aligned, in the order pv_kmer pv_pos pv_cc pv_mult kv_pos kv_cc ukmer ustart markers ctg_rec_off d_ctg_len htab
-// (the k-mer hash tables are present only with SK_PACK_TABLES); host metadata = META_HEADER words G S U M C c k marker_c HT
-// flags, then seed_off uk_off mk_off ctg_off [G+1 each], total_len [G], contig lengths [C] and, with tables, ht_off [G+1]
-constexpr int BLOB_ARRAYS = 12;
-constexpr int META_HEADER = 10;
-struct BlobLayout {
-  size_t off[BLOB_ARRAYS];
-  size_t bytes[BLOB_ARRAYS];
-  size_t total;
+// sketch-set blobs (sk_sketch_set_pack_subset / unpack, the host sketch store): layout and metadata words are derived from
+// SET_ARRAYS in set_layout.hpp
+
+// (src, dst, bytes) copies on ctx->stream (device or mapped host memory on either side), issued one cudaMemcpyAsync each or,
+// batched, as ONE cub::DeviceMemcpy::Batched that is synchronised (the segment lists and temporaries go on return).  A
+// scattered subset of thousands of genomes would otherwise cost tens of thousands of cudaMemcpyAsync calls.
+struct SegmentCopy {
+  bool batched = false;
+  std::vector<const void*> src;
+  std::vector<void*> dst;
+  std::vector<size_t> bytes;
+  void add(const void* s, void* d, size_t n) { if (n) { src.push_back(s); dst.push_back(d); bytes.push_back(n); } }
+  int run(sk_ctx* ctx);
 };
-inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
-inline BlobLayout blob_layout(size_t G, size_t S, size_t U, size_t M, size_t Cn, size_t HT = 0) {
-  BlobLayout b;
-  const size_t n[BLOB_ARRAYS] = {S * 4, S * 4, S * 4, S * 2, S * 4, S * 4, U * 4, (U + G) * 4, M * 8, (Cn + G) * 4, Cn * 4, HT * 8};
-  size_t o = 0;
-  for (int i = 0; i < BLOB_ARRAYS; i++) { b.off[i] = o; b.bytes[i] = n[i]; o += al256(n[i]); }
-  b.total = o ? o : 256;
-  return b;
-}
-inline uint64_t meta_words(uint64_t G, uint64_t C, bool tables) { return META_HEADER + 4 * (G + 1) + G + C + (tables ? G + 1 : 0); }
+// zeros for the arrays of a blob that do not travel with these flags: in a markers-only blob, one zero sentinel per genome
+cudaError_t zero_absent_arrays(sk_ctx* ctx, uint8_t* blob, const BlobLayout& b, bool markers_only, bool tables);
 // screen.cu / chain.cu
 uint64_t count_launch(sk_ctx* ctx, uint64_t n = 1);
 cudaError_t h2d_small(sk_ctx* ctx, void* dst, const void* src, size_t bytes);  // api.cu

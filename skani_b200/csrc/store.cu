@@ -10,8 +10,6 @@
 // context gather and chain them in plan order.  sk_query_ref_store does the same for every (reference, query) pair of two
 // stores: one marker screen of all references against all queries, working sets that each hold some references and some
 // queries, gathered from their own stores.
-#include <cub/cub.cuh>
-
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -34,7 +32,8 @@ struct sk_sketch_store {
   struct Genome {
     uint32_t slab = 0;
     uint64_t off = 0;                   // record offset inside the slab
-    uint64_t S = 0, U = 0, M = 0, C = 0, HT = 0, total_len = 0;
+    uint64_t n[N_COUNTS] = {};          // S U M C HT
+    uint64_t total_len = 0;
     uint64_t ctg0 = 0;                  // first contig length in ctg_len
     uint64_t slice[BLOB_ARRAYS] = {};   // slice offsets inside the record
   };
@@ -46,36 +45,6 @@ struct sk_sketch_store {
 namespace {
 
 double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
-// element counts of a genome's 12 arrays (one sentinel per genome in the k-mer group starts and contig record tables)
-void genome_counts(const sk_sketch_store::Genome& e, uint64_t n[BLOB_ARRAYS]) {
-  const uint64_t v[BLOB_ARRAYS] = {e.S, e.S, e.S, e.S, e.S, e.S, e.U, e.U + 1, e.M, e.C + 1, e.C, e.HT};
-  for (int a = 0; a < BLOB_ARRAYS; a++) n[a] = v[a];
-}
-constexpr uint64_t ESZ[BLOB_ARRAYS] = {4, 4, 4, 2, 4, 4, 4, 4, 8, 4, 4, 8};
-
-// one cub::DeviceMemcpy::Batched on ctx->stream (sources and destinations may be device or mapped host memory), synchronised
-int batched_copy(sk_ctx* ctx, const std::vector<const void*>& src, const std::vector<void*>& dst, const std::vector<size_t>& n) {
-  const size_t ns = n.size();
-  if (ns == 0) return SK_OK;
-  if (ns >= (1ull << 32)) { ctx->err = "too many copy segments"; return SK_ERR_PARAM; }
-  cudaStream_t st = ctx->stream;
-  DTmp<const void*> d_src; DTmp<void*> d_dst; DTmp<size_t> d_n;
-  SK_CUDA(d_src.alloc(ns, ctx)); SK_CUDA(d_dst.alloc(ns, ctx)); SK_CUDA(d_n.alloc(ns, ctx));
-  SK_CUDA(cudaMemcpyAsync(d_src.p, src.data(), ns * sizeof(void*), cudaMemcpyHostToDevice, st));
-  SK_CUDA(cudaMemcpyAsync(d_dst.p, dst.data(), ns * sizeof(void*), cudaMemcpyHostToDevice, st));
-  SK_CUDA(cudaMemcpyAsync(d_n.p, n.data(), ns * sizeof(size_t), cudaMemcpyHostToDevice, st));
-  size_t tb = 0;
-  SK_CUDA(cub::DeviceMemcpy::Batched(nullptr, tb, d_src.p, d_dst.p, d_n.p, (uint32_t)ns, st));
-  DTmp<uint8_t> tmp;
-  SK_CUDA(tmp.alloc(tb, ctx));
-  SK_CUDA(cub::DeviceMemcpy::Batched(tmp.p, tb, d_src.p, d_dst.p, d_n.p, (uint32_t)ns, st));
-  count_launch(ctx);
-  SK_CUDA(cudaStreamSynchronize(st));   // the host-side lists and the temporaries are released on return
-  return SK_OK;
-}
-
-bool same_params(const sk_sketch_params& a, const sk_sketch_params& b) { return a.c == b.c && a.k == b.k && a.marker_c == b.marker_c; }
 
 // NULL or repeated contexts (each context gets its own host thread) give SK_ERR_PARAM with the message on ctxs[0]
 int check_contexts(sk_ctx* const* ctxs, uint32_t n_ctx) {
@@ -178,10 +147,7 @@ uint32_t sk_sketch_store_n_genomes(const sk_sketch_store* st) { return st ? (uin
 
 uint64_t sk_sketch_store_genome_bytes(const sk_sketch_store* st, uint32_t g) {
   if (!st || g >= st->g.size()) return 0;
-  uint64_t n[BLOB_ARRAYS], b = 0;
-  genome_counts(st->g[g], n);
-  for (int a = 0; a < BLOB_ARRAYS; a++) b += n[a] * ESZ[a];
-  return b;
+  return genome_bytes(st->g[g].n);
 }
 
 int sk_sketch_store_set_name_ranks(sk_sketch_store* st, const uint64_t* ranks) {
@@ -202,17 +168,11 @@ int sk_sketch_store_add(sk_sketch_store* st, const sk_sketch_set* set) {
   SK_TRY(sk_sketch_set_subset_blob_size(set, nullptr, 0, SK_PACK_TABLES, &bytes, &words));
   DTmp<uint8_t> blob;
   if (blob.alloc(bytes, ctx) != cudaSuccess) { ctx->err = "sk_sketch_store_add: out of device memory for the blob"; return SK_ERR_NOMEM; }
-  std::vector<uint64_t> meta(words);
-  SK_TRY(sk_sketch_set_pack_subset(set, nullptr, 0, SK_PACK_TABLES, blob.p, meta.data()));
-  const uint64_t* m = meta.data();
-  const uint32_t G = (uint32_t)m[0];
-  const uint64_t HT = m[8];
-  const bool tables = m[9] != 0;
-  const BlobLayout b = blob_layout(G, m[1], m[2], m[3], m[4], HT);
-  const uint64_t *seed_off = m + META_HEADER, *uk_off = seed_off + G + 1, *mk_off = uk_off + G + 1, *ctg_off = mk_off + G + 1;
-  const uint64_t* total_len = ctg_off + G + 1;
-  const uint64_t* clen = total_len + G;
-  const uint64_t* ht_off = tables ? clen + m[4] : nullptr;
+  std::vector<uint64_t> words_v(words);
+  SK_TRY(sk_sketch_set_pack_subset(set, nullptr, 0, SK_PACK_TABLES, blob.p, words_v.data()));
+  const SetMeta m = decode_meta(words_v.data());
+  const uint32_t G = (uint32_t)m.G;
+  const BlobLayout b = blob_layout(G, m.n);
   // records in the slabs (host-side bookkeeping first, so that a failed slab allocation leaves the store unchanged)
   std::vector<sk_sketch_store::Genome> add(G);
   std::vector<sk_sketch_store::Slab> new_slabs;
@@ -223,13 +183,9 @@ int sk_sketch_store_add(sk_sketch_store* st, const sk_sketch_set* set) {
   auto fail_slabs = [&](int rc) { for (auto& s : new_slabs) cudaFreeHost(s.host); return rc; };
   for (uint32_t i = 0; i < G; i++) {
     sk_sketch_store::Genome& e = add[i];
-    e.S = seed_off[i + 1] - seed_off[i]; e.U = uk_off[i + 1] - uk_off[i]; e.M = mk_off[i + 1] - mk_off[i]; e.C = ctg_off[i + 1] - ctg_off[i];
-    e.HT = tables ? ht_off[i + 1] - ht_off[i] : 0;
-    e.total_len = total_len[i];
-    uint64_t n[BLOB_ARRAYS], o = 0;
-    genome_counts(e, n);
-    for (int a = 0; a < BLOB_ARRAYS; a++) { e.slice[a] = o; o += (n[a] * ESZ[a] + 15) & ~15ull; }
-    const size_t need = std::max<uint64_t>(al256(o), 256);
+    for (int x = 0; x < N_COUNTS; x++) e.n[x] = m.off[x][i + 1] - m.off[x][i];
+    e.total_len = m.total_len[i];
+    const size_t need = std::max<uint64_t>(al256(genome_slices(e.n, e.slice)), 256);
     const uint32_t n_slabs = (uint32_t)(st->slabs.size() + new_slabs.size());
     if (n_slabs == 0 || used[cur] + need > slab_at(cur).size) {
       sk_sketch_store::Slab s;
@@ -250,23 +206,15 @@ int sk_sketch_store_add(sk_sketch_store* st, const sk_sketch_set* set) {
     used[cur] += need;
   }
   // one batched copy: blob slices -> records in mapped host memory
-  std::vector<const void*> src;
-  std::vector<void*> dst;
-  std::vector<size_t> nb;
-  for (uint32_t i = 0; i < G; i++) {
-    const sk_sketch_store::Genome& e = add[i];
-    const uint64_t first[BLOB_ARRAYS] = {seed_off[i], seed_off[i], seed_off[i], seed_off[i], seed_off[i], seed_off[i], uk_off[i], uk_off[i] + i,
-                                         mk_off[i], ctg_off[i] + i, ctg_off[i], tables ? ht_off[i] : 0};
-    uint64_t n[BLOB_ARRAYS];
-    genome_counts(e, n);
+  SegmentCopy cp;
+  cp.batched = true;
+  for (uint32_t i = 0; i < G; i++)
     for (int a = 0; a < BLOB_ARRAYS; a++) {
-      if (n[a] == 0) continue;
-      src.push_back(blob.p + b.off[a] + first[a] * ESZ[a]);
-      dst.push_back(slab_at(e.slab).dev + e.off + e.slice[a]);
-      nb.push_back(n[a] * ESZ[a]);
+      const ArrayDesc& d = SET_ARRAYS[a];
+      cp.add(blob.p + b.off[a] + array_index(a, i, m.off[d.by][i]) * d.esz, slab_at(add[i].slab).dev + add[i].off + add[i].slice[a],
+             array_elems(a, 1, add[i].n) * d.esz);
     }
-  }
-  const int rc = batched_copy(ctx, src, dst, nb);
+  const int rc = cp.run(ctx);
   if (rc != SK_OK) return fail_slabs(rc);
   // commit
   for (auto& s : new_slabs) st->slabs.push_back(s);
@@ -275,7 +223,7 @@ int sk_sketch_store_add(sk_sketch_store* st, const sk_sketch_set* set) {
   for (uint64_t r : st->name_rank) mx = std::max(mx, r + 1);
   for (uint32_t i = 0; i < G; i++) {
     add[i].ctg0 = st->ctg_len.size();
-    for (uint64_t c = ctg_off[i]; c < ctg_off[i + 1]; c++) st->ctg_len.push_back((uint32_t)clen[c]);
+    for (uint64_t c = m.off[CNT_C][i]; c < m.off[CNT_C][i + 1]; c++) st->ctg_len.push_back((uint32_t)m.ctg_len[c]);
     st->g.push_back(add[i]);
     st->name_rank.push_back(mx + set->name_rank[i]);
   }
@@ -293,57 +241,31 @@ int sk_sketch_store_gather(sk_ctx* ctx, const sk_sketch_store* st, const uint32_
   }
   SK_CUDA(cudaSetDevice(ctx->device));
   const bool mo = flags == SK_PACK_MARKERS_ONLY;
-  // output offsets (the subset plan of sk_sketch_set_pack_subset, over the store's records)
-  std::vector<uint64_t> seed_off(n + 1, 0), uk_off(n + 1, 0), mk_off(n + 1, 0), ctg_off(n + 1, 0), ht_off(n + 1, 0);
+  // the metadata sk_sketch_set_pack_subset would write for these genomes, over the store's records
+  SetMeta m;
+  m.c = st->sp.c; m.k = st->sp.k; m.marker_c = st->sp.marker_c; m.tables = !mo;
   for (uint32_t i = 0; i < n; i++) {
     const sk_sketch_store::Genome& e = st->g[genomes[i]];
-    seed_off[i + 1] = seed_off[i] + (mo ? 0 : e.S);
-    uk_off[i + 1] = uk_off[i] + (mo ? 0 : e.U);
-    ctg_off[i + 1] = ctg_off[i] + (mo ? 0 : e.C);
-    ht_off[i + 1] = ht_off[i] + (mo ? 0 : e.HT);
-    mk_off[i + 1] = mk_off[i] + e.M;
+    meta_push(m, e.n, mo, e.total_len, st->ctg_len.begin() + e.ctg0, st->ctg_len.begin() + e.ctg0 + e.n[CNT_C]);
   }
-  const bool tables = !mo;
-  const BlobLayout b = blob_layout(n, seed_off[n], uk_off[n], mk_off[n], ctg_off[n], ht_off[n]);
+  const BlobLayout b = blob_layout(n, m.n);
   DTmp<uint8_t> blob;
   if (blob.alloc(b.total, ctx) != cudaSuccess) { ctx->err = "sk_sketch_store_gather: out of device memory (" + std::to_string(b.total >> 20) + " MiB blob)"; return SK_ERR_NOMEM; }
-  if (mo && n) {   // one zero sentinel per genome in the group-start and contig-record tables
-    SK_CUDA(cudaMemsetAsync(blob.p + b.off[7], 0, (size_t)n * 4, ctx->stream));
-    SK_CUDA(cudaMemsetAsync(blob.p + b.off[9], 0, (size_t)n * 4, ctx->stream));
-  }
-  std::vector<const void*> src;
-  std::vector<void*> dst;
-  std::vector<size_t> nb;
+  SK_CUDA(zero_absent_arrays(ctx, blob.p, b, mo, m.tables));
+  SegmentCopy cp;
+  cp.batched = true;
   for (uint32_t i = 0; i < n; i++) {
     const sk_sketch_store::Genome& e = st->g[genomes[i]];
     const uint8_t* rec = st->slabs[e.slab].dev + e.off;
-    const uint64_t first[BLOB_ARRAYS] = {seed_off[i], seed_off[i], seed_off[i], seed_off[i], seed_off[i], seed_off[i], uk_off[i], uk_off[i] + i,
-                                         mk_off[i], ctg_off[i] + i, ctg_off[i], ht_off[i]};
-    uint64_t cnt[BLOB_ARRAYS];
-    genome_counts(e, cnt);
     for (int a = 0; a < BLOB_ARRAYS; a++) {
-      if (cnt[a] == 0 || (mo && a != 8)) continue;
-      src.push_back(rec + e.slice[a]);
-      dst.push_back(blob.p + b.off[a] + first[a] * ESZ[a]);
-      nb.push_back(cnt[a] * ESZ[a]);
+      const ArrayDesc& d = SET_ARRAYS[a];
+      if (array_travels(a, mo, m.tables)) cp.add(rec + e.slice[a], blob.p + b.off[a] + array_index(a, i, m.off[d.by][i]) * d.esz, array_elems(a, 1, e.n) * d.esz);
     }
   }
-  SK_TRY(batched_copy(ctx, src, dst, nb));
+  SK_TRY(cp.run(ctx));
   if (mo && n) SK_CUDA(cudaStreamSynchronize(ctx->stream));
-  // metadata in sk_sketch_set_pack_subset's format
-  std::vector<uint64_t> meta;
-  meta.reserve(meta_words(n, ctg_off[n], tables));
-  for (uint64_t w : {(uint64_t)n, seed_off[n], uk_off[n], mk_off[n], ctg_off[n], (uint64_t)st->sp.c, (uint64_t)st->sp.k, (uint64_t)st->sp.marker_c,
-                     ht_off[n], (uint64_t)(tables ? 1 : 0)})
-    meta.push_back(w);
-  for (auto* v : {&seed_off, &uk_off, &mk_off, &ctg_off}) meta.insert(meta.end(), v->begin(), v->end());
-  for (uint32_t i = 0; i < n; i++) meta.push_back(st->g[genomes[i]].total_len);
-  if (!mo)
-    for (uint32_t i = 0; i < n; i++) {
-      const sk_sketch_store::Genome& e = st->g[genomes[i]];
-      for (uint64_t c = 0; c < e.C; c++) meta.push_back(st->ctg_len[e.ctg0 + c]);
-    }
-  if (tables) meta.insert(meta.end(), ht_off.begin(), ht_off.end());
+  std::vector<uint64_t> meta(meta_words(n, m.n[CNT_C], m.tables));
+  encode_meta(m, meta.data());
   const void* bp = blob.p;
   const uint64_t* mp = meta.data();
   SK_TRY(sk_sketch_set_unpack(ctx, 1, &bp, &mp, out));
