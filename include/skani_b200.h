@@ -210,7 +210,10 @@ int sk_sketch_set_set_name_ranks(sk_sketch_set* set, const uint64_t* ranks /* n_
  * (query_contig, query_pos, ref_contig, ref_pos, reverse) in sorted order (src/chain.rs:721); chunk_first: n_chunks+1;
  * score/pointer per anchor (chunk-local pointer, src/chain.rs:881-882); intervals: 11 x i64 per interval in the
  * descending order of src/chain.rs:1012: score,num_anchors,q0,q1,r0,r1,ref_contig,query_contig,chunk,reverse,kept;
- * ests: sorted (est, weight) of src/chain.rs:414. */
+ * ests: sorted (est, weight) of src/chain.rs:414; chunk_stats: 9 x u32 per chunk (src/chain.rs:204-394): total_anchors, rq0,
+ * rq1 (min q0 / max q1 of the kept intervals; 0xFFFFFFFF / 0 without one), tbcq (total_bases_contained_query, wrapping),
+ * n_int (kept intervals), n_seeds, num_in (seeds inside the intervals padded by c), upper_lower (seeds in [rq0, rq1]),
+ * filtered (1 = the putative-ANI filter replaced the weight n_seeds by upper_lower). */
 typedef struct {
   sk_ani_result result;
   int32_t switched;
@@ -223,6 +226,7 @@ typedef struct {
   int64_t* intervals;
   double* est;
   uint64_t* weight;
+  uint32_t* chunk_stats;
 } sk_chain_debug;
 /* sk_chain_pairs_debug runs the batching, pair descriptors and kernel instantiations of sk_chain_pairs on the same pair list
  * (the kernels additionally store the per-anchor DP scores and pointers) and fills out[i] from pair i's slices of the batch.
@@ -232,6 +236,11 @@ int sk_chain_pairs_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch
 int sk_chain_pair_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, uint64_t pair,
                         const sk_map_params* mp, sk_chain_debug* out);
 void sk_chain_debug_free(sk_chain_debug* d);
+/* (test use) the device's per-chunk identity, chunk_estimate of chunkstat_kernel, over n chunks given as 8 x u32 each:
+ * total_anchors, rq0, rq1, tbcq, n_int, n_seeds, num_in, upper_lower (host arrays).  Per chunk: est, weight, and valid =
+ * 0 (no estimate), 1 (estimate) or 3 (estimate, the putative-ANI filter applied). */
+int sk_debug_chunk_estimate(sk_ctx* ctx, uint64_t n, const uint32_t* inputs, uint32_t c, uint32_t k, double* est,
+                            uint32_t* weight, uint32_t* valid);
 
 /* ---- whole triangle (src/triangle.rs:13-105: sketch -> screen -> chain -> keep ani > 0.1) from HOST sequence
  *      buffers; results malloc'd (sk_free).  Timing breakdown (seconds, device events) optional. -------------- */

@@ -270,6 +270,11 @@ void orc_debug_intervals(void* dd, int64_t* f) {
     o[10] = d.interval_kept[i];
   }
 }
+// 9 x u32 per chunk: total_anchors, rq0, rq1, tbcq, n_int, n_seeds, num_in, upper_lower, filtered
+void orc_debug_chunk_stats(void* dd, uint32_t* out) {
+  auto& d = ((orc_debug*)dd)->d;
+  if (!d.chunk_stats.empty()) memcpy(out, d.chunk_stats.data(), d.chunk_stats.size() * 4);
+}
 void orc_debug_ests(void* dd, double* est, uint64_t* weight) {
   auto& d = ((orc_debug*)dd)->d;
   for (size_t i = 0; i < d.ani_ests.size(); i++) { est[i] = d.ani_ests[i].first; weight[i] = d.ani_ests[i].second; }
@@ -289,6 +294,20 @@ int orc_final_estimate(const double* est, const uint64_t* weight, uint64_t n, ui
   MapParams mp = map_params_from_sketch(unit, to_cp(cmd), model);
   to_res(final_estimate(ests, total_query_bases, avg_chain_int_len, query_total_len, ref_total_len, quant_q, quant_r, mp),
          0, 0, out);
+  return 0;
+}
+
+// chunk_estimate over n chunks of 8 x u32 each (total_anchors, rq0, rq1, tbcq, n_int, n_seeds, num_in, upper_lower), the form of
+// sk_debug_chunk_estimate: est, weight and valid = 0 (no estimate), 1 (estimate) or 3 (estimate, filter applied)
+int orc_chunk_estimate(uint64_t n, const uint32_t* in, uint32_t c, uint32_t k, double* est, uint32_t* weight, uint32_t* valid) {
+  for (uint64_t i = 0; i < n; i++) {
+    const uint32_t* x = in + 8 * i;
+    ChunkStats s;
+    s.total_anchors = x[0]; s.rq0 = x[1]; s.rq1 = x[2]; s.tbcq = x[3]; s.n_int = x[4];
+    s.n_seeds = x[5]; s.num_in = x[6]; s.upper_lower = x[7];
+    chunk_estimate(s, c, k, MIN_LENGTH_COVER);
+    est[i] = s.est; weight[i] = (uint32_t)s.weight; valid[i] = s.valid ? (s.filtered ? 3u : 1u) : 0u;
+  }
   return 0;
 }
 

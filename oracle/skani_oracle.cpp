@@ -1046,6 +1046,55 @@ AniEstResult final_estimate(const std::vector<std::pair<double, size_t>>& ani_es
   return r;
 }
 
+uint32_t padded_start(uint32_t q0, uint32_t c) {  // chain.rs:239-240: i32::max(q0 as i32 - c as i32, 0), wrapping i32 subtraction
+  const uint32_t d = q0 - c;                       // the same wrap in u32 (no signed overflow)
+  return (int32_t)d > 0 ? d : 0u;
+}
+
+void chunk_estimate(ChunkStats& s, uint32_t c, size_t k, uint32_t min_length_cover) {  // chain.rs:253-394
+  s.valid = s.filtered = false;
+  s.est = 0.; s.weight = 0;
+  if (s.total_anchors == 0) return;                  // :253-255
+  if (s.rq1 - s.rq0 < min_length_cover) return;      // :257-259
+  size_t considered = s.n_seeds;
+  double putative = std::pow((double)s.total_anchors / (double)s.num_in, 1. / (double)k);  // :331-335
+  if (putative > 0.950 && s.tbcq > c * 4 && s.rq1 - s.rq0 < (uint32_t)(CHUNK_SIZE_DNA * 9 / 10) &&
+      (double)considered > 1.05 * (double)s.upper_lower) {  // :336-347
+    considered = s.upper_lower;
+    s.filtered = true;
+  }
+  double ml_hits = std::min(1., (double)s.total_anchors / (double)considered);  // :368-372
+  s.est = std::pow(ml_hits, 1. / (double)k);                                     // :373-377
+  s.weight = considered;                                                         // :394
+  s.valid = true;
+}
+
+ChunkStats chunk_stats(const std::vector<ChainInterval>& intervals, const std::vector<uint32_t>& seeds, uint32_t c, size_t k,
+                       uint32_t min_length_cover, bool switched) {  // chain.rs:204-394
+  ChunkStats s;
+  std::vector<std::pair<uint32_t, uint32_t>> all_intervals;  // closed intervals; union realised lazily (only contains() matters)
+  for (const auto& in : intervals) {
+    s.total_anchors += in.num_anchors;
+    if (in.q0 < s.rq0) s.rq0 = in.q0;
+    if (in.q1 > s.rq1) s.rq1 = in.q1;
+    if (!switched) s.tbcq += in.q1 - in.q0 + (uint32_t)k + 2 * c;  // :223-237
+    else s.tbcq += in.r1 - in.r0 + (uint32_t)k + 2 * c;
+    all_intervals.push_back({padded_start(in.q0, c), in.q1 + c});  // :239-240
+    s.n_int++;
+  }
+  s.n_seeds = seeds.size();
+  if (s.n_int) {
+    for (uint32_t pos : seeds) {
+      bool in = false;
+      for (auto& iv : all_intervals) if (iv.first <= pos && pos <= iv.second) { in = true; break; }
+      if (in) s.num_in++;
+      if (pos >= s.rq0 && pos <= s.rq1) s.upper_lower++;  // :322-328 with both spacing estimates 0 (extend = 0, :295)
+    }
+  }
+  chunk_estimate(s, c, k, min_length_cover);
+  return s;
+}
+
 static AniEstResult calculate_ani(const std::vector<std::vector<ChainInterval>>& int_chunks, const Sketch& ref_sketch,
                                   const Sketch& query_sketch, const AnchorChunks& ac, const MapParams& mp, bool switched,
                                   ChainDebug* dbg) {  // chain.rs:173-555
@@ -1056,48 +1105,24 @@ static AniEstResult calculate_ani(const std::vector<std::vector<ChainInterval>>&
   uint32_t total_query_bases = 0, total_ref_range = 0;
   uint32_t avg_chain_int_len = 0, num_chains = 0;
   for (size_t i = 0; i < int_chunks.size(); i++) {
-    const auto& intervals = int_chunks[i];
-    std::vector<std::pair<uint32_t, uint32_t>> all_intervals;  // closed intervals; union realised lazily (only contains() matters)
-    size_t total_anchors = 0;
-    uint32_t tbcq = 0;
-    uint32_t rq0 = UINT32_MAX, rq1 = 0;
-    for (const auto& in : intervals) {
-      total_anchors += in.num_anchors;
-      if (in.q0 < rq0) rq0 = in.q0;
-      if (in.q1 > rq1) rq1 = in.q1;
-      if (!switched) tbcq += in.q1 - in.q0 + (uint32_t)k + 2 * c;  // :223-237
-      else tbcq += in.r1 - in.r0 + (uint32_t)k + 2 * c;
-      uint32_t start = (uint32_t)std::max((int32_t)in.q0 - (int32_t)c, 0);  // :239-240 (i32 arithmetic as in the reference)
-      uint32_t stop = in.q1 + c;
-      all_intervals.push_back({start, stop});
+    for (const auto& in : int_chunks[i]) {
       uint32_t add = (in.q1 - in.q0) - in.overlap + 2 * c + (uint32_t)k;
       if (sensitive_af) { total_query_bases += add; total_ref_range += add; }  // :244-247
       avg_chain_int_len += add;  // :249
       num_chains += 1;
     }
-    if (total_anchors == 0) continue;                    // :253-255
-    if (rq1 - rq0 < mp.min_length_cover) continue;       // :257-259
+    const ChunkStats cs = chunk_stats(int_chunks[i], ac.seeds_in_chunk[i], c, k, mp.min_length_cover, switched);
+    if (dbg) {
+      const uint32_t row[9] = {(uint32_t)cs.total_anchors, cs.rq0, cs.rq1, cs.tbcq, cs.n_int, (uint32_t)cs.n_seeds,
+                               (uint32_t)cs.num_in, (uint32_t)cs.upper_lower, cs.filtered ? 1u : 0u};
+      dbg->chunk_stats.insert(dbg->chunk_stats.end(), row, row + 9);
+    }
+    if (!cs.valid) continue;                             // :253-259
     if (!sensitive_af) {                                 // :261-264
-      total_query_bases += rq1 - rq0 + 2 * c + (uint32_t)k;
-      total_ref_range += rq1 - rq0 + 2 * c + (uint32_t)k;
+      total_query_bases += cs.rq1 - cs.rq0 + 2 * c + (uint32_t)k;
+      total_ref_range += cs.rq1 - cs.rq0 + 2 * c + (uint32_t)k;
     }
-    size_t num_seeds_in_intervals = 0, upper_lower_seeds = 0;
-    const auto& seeds = ac.seeds_in_chunk[i];
-    for (uint32_t pos : seeds) {
-      bool in = false;
-      for (auto& iv : all_intervals) if (iv.first <= pos && pos <= iv.second) { in = true; break; }
-      if (in) num_seeds_in_intervals++;
-      if (pos >= rq0 && pos <= rq1) upper_lower_seeds++;  // :322-328 with both spacing estimates 0 (extend = 0, :295)
-    }
-    size_t considered = seeds.size();
-    double putative = std::pow((double)total_anchors / (double)num_seeds_in_intervals, 1. / (double)k);  // :331-335
-    if (putative > 0.950 && tbcq > c * 4 && rq1 - rq0 < (uint32_t)(CHUNK_SIZE_DNA * 9 / 10) &&
-        (double)considered > 1.05 * (double)upper_lower_seeds) {  // :336-347
-      considered = upper_lower_seeds;
-    }
-    double ml_hits = std::min(1., (double)total_anchors / (double)considered);  // :368-372
-    double ani_est = std::pow(ml_hits, 1. / (double)k);                          // :373-377
-    ani_ests.push_back({ani_est, considered});                                   // :394
+    ani_ests.push_back({cs.est, cs.weight});             // :394
   }
   std::sort(ani_ests.begin(), ani_ests.end());  // :414 (f64, usize) lexicographic
   if (dbg) dbg->ani_ests = ani_ests;

@@ -191,7 +191,27 @@ struct ChainDebug {  // parity taps (not in the reference): intermediate product
   std::vector<ChainInterval> intervals_all;    // after the descending sort (chain.rs:1012)
   std::vector<uint8_t> interval_kept;          // greedy decision per sorted interval
   std::vector<std::pair<double, size_t>> ani_ests;  // sorted (est, weight) (chain.rs:414)
+  std::vector<uint32_t> chunk_stats;           // 9 per chunk: the fields of ChunkStats up to `filtered`
 };
+
+// one chunk of calculate_ani (chain.rs:204-394): the kept intervals' sums, the seed counts and the chunk's identity.  The seed
+// counts are taken for every chunk with an interval (the reference counts them only for chunks that pass :253-259).
+struct ChunkStats {
+  size_t total_anchors = 0;
+  uint32_t rq0 = UINT32_MAX, rq1 = 0;   // total_range_query
+  uint32_t tbcq = 0;                    // total_bases_contained_query (wrapping u32)
+  uint32_t n_int = 0;
+  size_t n_seeds = 0, num_in = 0, upper_lower = 0;
+  bool filtered = false;                // the putative-ANI filter replaced n_seeds by upper_lower (:336-347)
+  bool valid = false;                   // the chunk yields an estimate
+  double est = 0.;
+  size_t weight = 0;
+};
+uint32_t padded_start(uint32_t q0, uint32_t c);  // chain.rs:239-240, i32 arithmetic wrapping as in a release build
+// filtered / valid / est / weight from the other fields
+void chunk_estimate(ChunkStats& s, uint32_t c, size_t k, uint32_t min_length_cover);
+ChunkStats chunk_stats(const std::vector<ChainInterval>& intervals, const std::vector<uint32_t>& seeds, uint32_t c, size_t k,
+                       uint32_t min_length_cover, bool switched);
 
 int get_model_id(uint64_t c, bool learned_ani);  // regression.rs:12-28
 MapParams map_params_from_sketch(const Sketch& ref, const CommandParams& cp, int model);  // chain.rs:88-142

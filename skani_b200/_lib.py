@@ -30,7 +30,7 @@ class ChainDebug(C.Structure):
                 ("anchors", C.POINTER(C.c_uint32)), ("chunk_first", C.POINTER(C.c_uint32)),
                 ("chunk_nseeds", C.POINTER(C.c_uint32)), ("score", C.POINTER(C.c_int64)),
                 ("pointer", C.POINTER(C.c_uint32)), ("intervals", C.POINTER(C.c_int64)),
-                ("est", C.POINTER(C.c_double)), ("weight", C.POINTER(C.c_uint64))]
+                ("est", C.POINTER(C.c_double)), ("weight", C.POINTER(C.c_uint64)), ("chunk_stats", C.POINTER(C.c_uint32))]
 
 
 class TriangleStats(C.Structure):
@@ -85,6 +85,7 @@ SYMBOLS = [
     ("sk_chain_pair_debug", i32, [vp, vp, vp, u64, PP(MapParams), PP(ChainDebug)]),
     ("sk_chain_pairs_debug", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp]),
     ("sk_chain_debug_free", None, [PP(ChainDebug)]),
+    ("sk_debug_chunk_estimate", i32, [vp, u64, vp, u32, u32, vp, vp, vp]),
     ("sk_triangle", i32, [vp, vp, vp, u32, vp, u32, PP(SketchParams), PP(MapParams), PP(PP(AniResult)), PP(u64),
                           PP(TriangleStats)]),
     ("sk_triangle_local", i32, [vp, vp, vp, u32, vp, u32, PP(SketchParams), PP(MapParams), vp, PP(PP(AniResult)), PP(u64),

@@ -1052,7 +1052,8 @@ __device__ __forceinline__ uint32_t warp_first_greater(const uint32_t* __restric
 
 __global__ void __launch_bounds__(CS_WARPS * 32)
 chunkstat_kernel(uint64_t n_chunks, const PairDesc* __restrict__ pairs, SetView s0, SetView s1,
-                 const GenomeMeta* __restrict__ m0, const GenomeMeta* __restrict__ m1, ChainParams prm, Workspace ws) {
+                 const GenomeMeta* __restrict__ m0, const GenomeMeta* __restrict__ m1, ChainParams prm, Workspace ws,
+                 uint32_t* __restrict__ dbg_counts) {
   __shared__ uint32_t s_start[CS_WARPS][CS_IV_MAX], s_stop[CS_WARPS][CS_IV_MAX];
   __shared__ uint32_t s_nseeds[CS_WARPS * CS_PER_WARP], s_numin[CS_WARPS * CS_PER_WARP], s_ul[CS_WARPS * CS_PER_WARP];
   const unsigned FULL = 0xFFFFFFFFu;
@@ -1090,7 +1091,7 @@ chunkstat_kernel(uint64_t n_chunks, const PairDesc* __restrict__ pairs, SetView 
         while (i != 0xFFFFFFFFu && n_iv < CS_IV_MAX) {
           const IntervalKey x = ws.iv[ib + i];
           const uint32_t q0 = iv_q0(x), q1 = iv_q1(x);
-          s_start[w][n_iv] = q0 > prm.c ? q0 - prm.c : 0;       // max(q0 - c, 0) in i32
+          s_start[w][n_iv] = padded_start(q0, prm.c);
           s_stop[w][n_iv] = q1 + prm.c;
           n_iv++;
           i = ws.iv_next[ib + i];
@@ -1111,8 +1112,7 @@ chunkstat_kernel(uint64_t n_chunks, const PairDesc* __restrict__ pairs, SetView 
       for (uint32_t i = 0; i < n_iv; i++) if (s_start[w][i] <= ps && ps <= s_stop[w][i]) { in = true; break; }
       for (uint32_t i = more; !in && i != 0xFFFFFFFFu; i = ws.iv_next[ib + i]) {
         const IntervalKey x = ws.iv[ib + i];
-        const uint32_t q0 = iv_q0(x), q1 = iv_q1(x);
-        if ((q0 > prm.c ? q0 - prm.c : 0) <= ps && ps <= q1 + prm.c) in = true;
+        if (seed_in_padded(ps, iv_q0(x), iv_q1(x), prm.c)) in = true;
       }
       if (in) num_in++;
       if (ps >= rq0 && ps <= rq1) upper_lower++;              // :322-328 with both spacing estimates 0
@@ -1133,13 +1133,30 @@ chunkstat_kernel(uint64_t n_chunks, const PairDesc* __restrict__ pairs, SetView 
       ws.chunk_nseeds[c] = s_nseeds[threadIdx.x];
       double est; uint32_t wgt;
       uint8_t valid = 0;
-      if (chunk_estimate(acc, prm.c, prm.k, s_nseeds[threadIdx.x], s_numin[threadIdx.x], s_ul[threadIdx.x], &est, &wgt)) {
+      bool filtered;
+      if (chunk_estimate(acc, prm.c, prm.k, s_nseeds[threadIdx.x], s_numin[threadIdx.x], s_ul[threadIdx.x], &est, &wgt, &filtered)) {
         ws.chunk_est[c] = est; ws.chunk_w[c] = wgt; valid = 1;
         if (prm.c >= 200) atomicAdd(&ws.pair_tqb_ns[ws.chunk_pair[c]], acc.rq1 - acc.rq0 + 2 * prm.c + prm.k);  // !sensitive_af (:261-264)
       }
       ws.chunk_valid[c] = valid;
+      if (dbg_counts) {                                        // debug runs: the warp-reduced counts and the filter decision
+        dbg_counts[3 * c] = s_numin[threadIdx.x]; dbg_counts[3 * c + 1] = s_ul[threadIdx.x]; dbg_counts[3 * c + 2] = filtered ? 1u : 0u;
+      }
     }
   }
+}
+
+// test use (sk_debug_chunk_estimate): chunk_estimate on given accumulations and counts, 8 x u32 per chunk
+__global__ void debug_chunk_estimate_kernel(uint64_t n, const uint32_t* __restrict__ in, uint32_t c, uint32_t k, double* est,
+                                            uint32_t* weight, uint32_t* valid) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t* x = in + 8 * i;
+  ChunkAcc acc;
+  acc.total_anchors = x[0]; acc.rq0 = x[1]; acc.rq1 = x[2]; acc.tbcq = x[3]; acc.n_int = x[4];
+  double e = 0.; uint32_t w = 0; bool f = false;
+  const bool ok = chunk_estimate(acc, c, k, x[5], x[6], x[7], &e, &w, &f);
+  est[i] = ok ? e : 0.; weight[i] = ok ? w : 0u; valid[i] = ok ? (f ? 3u : 1u) : 0u;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1440,6 +1457,7 @@ struct ChainScratch {
   size_t c_anc = 0, c_score = 0, c_ptr = 0, c_rootkey = 0, c_depth = 0;
   size_t c_chunk_size = 0, c_chunk_size_sorted = 0, c_chunk_id = 0, c_chunk_perm = 0, c_sort_tmp = 0;
   uint8_t* sort_tmp = nullptr;
+  uint32_t* dbg_counts = nullptr; size_t c_dbg_counts = 0;   // debug runs: chunkstat_kernel's num_in, upper_lower, filtered
   size_t c_chunk_first = 0, c_chunk_pair = 0, c_chunk_qctg = 0, c_chunk_lo = 0, c_chunk_hi = 0, c_acc_total = 0, c_acc_rq0 = 0,
          c_acc_rq1 = 0, c_acc_tbcq = 0, c_acc_nint = 0, c_chunk_head = 0, c_chunk_est = 0, c_chunk_w = 0, c_chunk_valid = 0, c_chunk_nseeds = 0;
   size_t c_iv = 0, c_iv_keys = 0, c_iv_order = 0, c_iv_kept = 0, c_iv_next = 0, c_acc_list = 0, c_est_sorted = 0, c_w_sorted = 0;
@@ -1448,7 +1466,7 @@ struct ChainScratch {
   GenomeMeta *d_m0 = nullptr, *d_m1 = nullptr;
   size_t c_m0 = 0, c_m1 = 0;
   void free_all() {
-    void* ptrs[] = {ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, sort_tmp, ws.rec_nh, ws.rec_rs, ws.tile_off, ws.stg_first, ws.stg_qctg, ws.stg_lo, ws.stg_hi,
+    void* ptrs[] = {ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, sort_tmp, dbg_counts, ws.rec_nh, ws.rec_rs, ws.tile_off, ws.stg_first, ws.stg_qctg, ws.stg_lo, ws.stg_hi,
                     ws.pairA, ws.pairC, ws.pairAbase, ws.pairCbase, ws.pairIbase, ws.pair_nint, ws.pair_sumlen, ws.pair_nchains, ws.pair_tqb_ns, ws.anc,
                     ws.score, ws.ptr, ws.rootkey, ws.depth, ws.chunk_first, ws.chunk_pair, ws.chunk_qctg, ws.chunk_lo, ws.chunk_hi,
                     ws.acc_total, ws.acc_rq0, ws.acc_rq1, ws.acc_tbcq, ws.acc_nint, ws.chunk_head, ws.chunk_est, ws.chunk_w, ws.chunk_valid,
@@ -1475,7 +1493,7 @@ static int launch_dp_group(sk_ctx* ctx, uint32_t grid, uint64_t TC, const ChainP
 // kept flags at iv_kept + ib, both indexed by the pair-local interval index).  dbg[b0 + i] receives pair b0 + i.
 static int copy_out_debug(sk_ctx* ctx, const Workspace& ws, const std::vector<PairDesc>& descs, size_t b0, uint32_t B,
                           const std::vector<uint64_t>& abase, const std::vector<uint64_t>& cbase, const std::vector<uint64_t>& ibase,
-                          const sk_ani_result* host_out, sk_chain_debug* dbg) {
+                          const uint32_t* dbg_counts, const sk_ani_result* host_out, sk_chain_debug* dbg) {
   const uint64_t TA = abase[B], TC = cbase[B], TI = ibase[B];
   std::vector<AnchorRec> anc(TA);
   std::vector<int32_t> score(TA);
@@ -1484,6 +1502,7 @@ static int copy_out_debug(sk_ctx* ctx, const Workspace& ws, const std::vector<Pa
   std::vector<IntervalKey> iv(TI);
   std::vector<uint8_t> kept(TI), valid(TC);
   std::vector<double> est(TC);
+  std::vector<uint32_t> a_total(TC), a_rq0(TC), a_rq1(TC), a_tbcq(TC), a_nint(TC), counts(3 * TC);
   if (TA) {
     SK_CUDA(cudaMemcpy(anc.data(), ws.anc, TA * sizeof(AnchorRec), cudaMemcpyDeviceToHost));
     SK_CUDA(cudaMemcpy(score.data(), ws.score, TA * 4, cudaMemcpyDeviceToHost));
@@ -1496,6 +1515,12 @@ static int copy_out_debug(sk_ctx* ctx, const Workspace& ws, const std::vector<Pa
     SK_CUDA(cudaMemcpy(est.data(), ws.chunk_est, TC * 8, cudaMemcpyDeviceToHost));
     SK_CUDA(cudaMemcpy(w.data(), ws.chunk_w, TC * 4, cudaMemcpyDeviceToHost));
     SK_CUDA(cudaMemcpy(valid.data(), ws.chunk_valid, TC, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(a_total.data(), ws.acc_total, TC * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(a_rq0.data(), ws.acc_rq0, TC * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(a_rq1.data(), ws.acc_rq1, TC * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(a_tbcq.data(), ws.acc_tbcq, TC * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(a_nint.data(), ws.acc_nint, TC * 4, cudaMemcpyDeviceToHost));
+    SK_CUDA(cudaMemcpy(counts.data(), dbg_counts, TC * 12, cudaMemcpyDeviceToHost));
   }
   SK_CUDA(cudaMemcpy(nint.data(), ws.pair_nint, B * 4, cudaMemcpyDeviceToHost));
   if (TI) {
@@ -1519,7 +1544,8 @@ static int copy_out_debug(sk_ctx* ctx, const Workspace& ws, const std::vector<Pa
     d->chunk_first = (uint32_t*)calloc(nc + 1, 4);
     d->chunk_nseeds = (uint32_t*)calloc(std::max<uint64_t>(nc, 1), 4);
     d->intervals = (int64_t*)calloc(std::max<uint32_t>(ni, 1), 11 * 8);
-    if (!d->anchors || !d->score || !d->pointer || !d->chunk_first || !d->chunk_nseeds || !d->intervals) {
+    d->chunk_stats = (uint32_t*)calloc(std::max<uint64_t>(nc, 1), 9 * 4);
+    if (!d->anchors || !d->score || !d->pointer || !d->chunk_first || !d->chunk_nseeds || !d->intervals || !d->chunk_stats) {
       ctx->err = "chain debug: out of host memory"; return SK_ERR_STATE;
     }
     for (uint64_t c = 0; c < nc; c++) {
@@ -1527,6 +1553,10 @@ static int copy_out_debug(sk_ctx* ctx, const Workspace& ws, const std::vector<Pa
       const uint64_t x0 = cf[c0 + c] - a0, x1 = cf[c0 + c + 1] - a0;
       if (x0 > x1 || x1 > na) { ctx->err = "chain debug: chunk outside its pair's anchors"; return SK_ERR_STATE; }
       d->chunk_first[c] = (uint32_t)x0; d->chunk_nseeds[c] = nseeds[c0 + c];
+      const uint64_t g = c0 + c;
+      const uint32_t st[9] = {a_total[g], a_rq0[g], a_rq1[g], a_tbcq[g], a_nint[g], nseeds[g], counts[3 * g], counts[3 * g + 1],
+                              counts[3 * g + 2]};
+      memcpy(d->chunk_stats + 9 * c, st, sizeof(st));
       for (uint64_t x = x0; x < x1; x++) {
         const AnchorRec& a = anc[a0 + x];
         uint32_t* o = d->anchors + 5 * x;
@@ -1632,6 +1662,8 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
   ENS(iv, c_iv, NI); ENS(iv_keys, c_iv_keys, 2 * NI + 8); ENS(iv_order, c_iv_order, 4 * NI + 8); ENS(iv_kept, c_iv_kept, NI); ENS(iv_next, c_iv_next, NI); ENS(acc_list, c_acc_list, NI);
   ENS(est_sorted, c_est_sorted, 4 * NCH + 8); ENS(w_sorted, c_w_sorted, 4 * NCH + 8);
 #undef ENS
+  if (dbg) SK_TRY(ensure(ctx, &S.dbg_counts, &S.c_dbg_counts, 3 * NCH));
+  uint32_t* const dbg_counts = dbg ? S.dbg_counts : nullptr;
   if (TC > 0) {
     SK_CUDA(h2d_small(ctx, ws.chunk_first + TC, &TA, 8));
     SK_LAUNCH(ctx, "chunk_compact_kernel", (chunk_compact_kernel<<<B, CT, 0, st>>>(S.d_pairs, ws)));
@@ -1669,7 +1701,7 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
 #undef DP_LAUNCH
     }
     SK_LAUNCH(ctx, "select_kernel", (select_kernel<<<B, CT, 0, st>>>(S.d_pairs, prm, ws)));
-    SK_LAUNCH(ctx, "chunkstat_kernel", (chunkstat_kernel<<<(uint32_t)((TC + CS_WARPS * CS_PER_WARP - 1) / (CS_WARPS * CS_PER_WARP)), CS_WARPS * 32, 0, st>>>(TC, S.d_pairs, v0, v1, S.d_m0, S.d_m1, prm, ws)));
+    SK_LAUNCH(ctx, "chunkstat_kernel", (chunkstat_kernel<<<(uint32_t)((TC + CS_WARPS * CS_PER_WARP - 1) / (CS_WARPS * CS_PER_WARP)), CS_WARPS * 32, 0, st>>>(TC, S.d_pairs, v0, v1, S.d_m0, S.d_m1, prm, ws, dbg_counts)));
   }
   // test hook: SK_FINAL_FORCE_REDO=1 takes the sequential bootstrap redo for every pair, as if some draw had been rejected
   const char* fr = getenv("SK_FINAL_FORCE_REDO");
@@ -1679,7 +1711,7 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
   SK_CUDA(cudaStreamSynchronize(st));
   SK_CUDA(cudaGetLastError());
 
-  if (dbg) SK_TRY(copy_out_debug(ctx, ws, descs, b0, B, abase, cbase, ibase, host_out, dbg));
+  if (dbg) SK_TRY(copy_out_debug(ctx, ws, descs, b0, B, abase, cbase, ibase, dbg_counts, host_out, dbg));
   return SK_OK;
 }
 
@@ -1772,8 +1804,36 @@ int sk_chain_pairs(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* 
 void sk_chain_debug_free(sk_chain_debug* d) {
   if (!d) return;
   free(d->anchors); free(d->chunk_first); free(d->chunk_nseeds); free(d->score); free(d->pointer); free(d->intervals);
-  free(d->est); free(d->weight);
+  free(d->est); free(d->weight); free(d->chunk_stats);
   memset(d, 0, sizeof(*d));
+}
+
+int sk_debug_chunk_estimate(sk_ctx* ctx, uint64_t n, const uint32_t* inputs, uint32_t c, uint32_t k, double* est, uint32_t* weight,
+                            uint32_t* valid) {
+  if (!ctx || (n && (!inputs || !est || !weight || !valid)) || k == 0) return SK_ERR_PARAM;
+  if (n == 0) return SK_OK;
+  SK_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  uint32_t *d_in = nullptr, *d_w = nullptr, *d_v = nullptr;
+  double* d_e = nullptr;
+  int rc = SK_OK;
+  cudaError_t e = cudaMalloc(&d_in, n * 32);
+  if (e == cudaSuccess) e = cudaMalloc(&d_e, n * 8);
+  if (e == cudaSuccess) e = cudaMalloc(&d_w, n * 4);
+  if (e == cudaSuccess) e = cudaMalloc(&d_v, n * 4);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_in, inputs, n * 32, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) {
+    sk::debug_chunk_estimate_kernel<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>(n, d_in, c, k, d_e, d_w, d_v);
+    sk::count_launch(ctx);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(est, d_e, n * 8, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(weight, d_w, n * 4, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(valid, d_v, n * 4, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); rc = SK_ERR_CUDA; }
+  cudaFree(d_in); cudaFree(d_e); cudaFree(d_w); cudaFree(d_v);
+  return rc;
 }
 
 int sk_chain_pairs_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, const uint64_t* pairs, uint64_t n_pairs,

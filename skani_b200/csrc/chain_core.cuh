@@ -170,9 +170,22 @@ struct ChunkAcc {
   uint32_t tbcq;           // total_bases_contained_query (wrapping u32)
   uint32_t n_int;
 };
-// returns false if the chunk yields no estimate; else est / weight
+// start of a kept interval padded by c (src/chain.rs:239-240): i32::max(q0 as i32 - c as i32, 0) as u32, where the i32
+// subtraction wraps (release build).  So q0 < c gives 0, and so does q0 >= 2^31 + c (negative as i32): such an interval
+// covers its contig from position 0.  Subtracted in u32 here, which wraps the same way without signed overflow.
+SK_HD uint32_t padded_start(uint32_t q0, uint32_t c) {
+  const uint32_t d = q0 - c;
+  return (int32_t)d > 0 ? d : 0u;
+}
+// seed position pos inside the kept interval [q0, q1] padded by c on both sides (closed at both ends)
+SK_HD bool seed_in_padded(uint32_t pos, uint32_t q0, uint32_t q1, uint32_t c) {
+  return padded_start(q0, c) <= pos && pos <= q1 + c;
+}
+// returns false if the chunk yields no estimate; else est / weight, and *filtered = the putative-ANI filter replaced the
+// chunk's seed count by upper_lower (if filtered != nullptr)
 SK_HD bool chunk_estimate(const ChunkAcc& acc, uint32_t c, uint32_t k, uint32_t n_seeds, uint32_t num_in, uint32_t upper_lower,
-                          double* est, uint32_t* weight) {
+                          double* est, uint32_t* weight, bool* filtered = nullptr) {
+  if (filtered) *filtered = false;
   if (acc.n_int == 0 || acc.total_anchors == 0) return false;        // :253-255
   if (acc.rq1 - acc.rq0 < MIN_LENGTH_COVER) return false;            // :257-259
   uint32_t considered = n_seeds;
@@ -180,6 +193,7 @@ SK_HD bool chunk_estimate(const ChunkAcc& acc, uint32_t c, uint32_t k, uint32_t 
   if (putative > 0.950 && acc.tbcq > c * 4u && acc.rq1 - acc.rq0 < (FRAGMENT_LENGTH * 9u / 10u) &&
       (double)considered > 1.05 * (double)upper_lower) {             // :336-347
     considered = upper_lower;
+    if (filtered) *filtered = true;
   }
   double ml = (double)acc.total_anchors / (double)considered;
   if (ml > 1.0) ml = 1.0;                                            // f64::min(1., x) (:368-372)

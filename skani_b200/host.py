@@ -353,7 +353,8 @@ def _debug_dict(d):
                 chunk_first=arr(d.chunk_first, (d.n_chunks + 1,), np.uint32) if d.n_chunks else np.zeros(1, np.uint32),
                 chunk_nseeds=arr(d.chunk_nseeds, (d.n_chunks,), np.uint32),
                 intervals=arr(d.intervals, (d.n_intervals, 11), np.int64),
-                est=arr(d.est, (d.n_ests,), np.float64), weight=arr(d.weight, (d.n_ests,), np.uint64))
+                est=arr(d.est, (d.n_ests,), np.float64), weight=arr(d.weight, (d.n_ests,), np.uint64),
+                chunk_stats=arr(d.chunk_stats, (d.n_chunks, 9), np.uint32))
 
 
 def chain_pairs_debug(ctx, refs, queries, pairs, mp=None, keep=None):
@@ -375,6 +376,19 @@ def chain_pairs_debug(ctx, refs, queries, pairs, mp=None, keep=None):
 
 def chain_pair_debug(ctx, refs, queries, ref_id, query_id, mp=None):
     return chain_pairs_debug(ctx, refs, queries, [(ref_id << 32) | query_id], mp)[0]
+
+
+CHUNK_STAT_FIELDS = ("total_anchors", "rq0", "rq1", "tbcq", "n_int", "n_seeds", "num_in", "upper_lower", "filtered")
+
+
+def debug_chunk_estimate(ctx, inputs, c, k):
+    """sk_debug_chunk_estimate: the device's chunk_estimate over rows (total_anchors, rq0, rq1, tbcq, n_int, n_seeds, num_in,
+    upper_lower).  Returns (est f64, weight u32, valid u32: 0 no estimate, 1 estimate, 3 estimate with the filter applied)."""
+    x = np.ascontiguousarray(inputs, np.uint32).reshape(-1, 8)
+    n = len(x)
+    est = np.zeros(max(n, 1), np.float64); w = np.zeros(max(n, 1), np.uint32); v = np.zeros(max(n, 1), np.uint32)
+    ctx.check(ctx.L.sk_debug_chunk_estimate(ctx.h, n, x.ctypes.data, c, k, est.ctypes.data, w.ctypes.data, v.ctypes.data))
+    return est[:n], w[:n], v[:n]
 
 
 def triangle(ctx, bases, contig_off, genome_of_contig, n_genomes, sp=None, mp=None, as_array=False):

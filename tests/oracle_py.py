@@ -100,6 +100,9 @@ def lib():
     L.orc_debug_chunks.argtypes = [vp] * 3
     L.orc_debug_intervals.argtypes = [vp] * 2
     L.orc_debug_ests.argtypes = [vp] * 3
+    L.orc_debug_chunk_stats.argtypes = [vp] * 2
+    L.orc_chunk_estimate.restype = i32
+    L.orc_chunk_estimate.argtypes = [u64, vp, u32, u32, vp, vp, vp]
     L.orc_gbdt_predict.restype = C.c_float; L.orc_gbdt_predict.argtypes = [i32, vp]
     L.orc_final_estimate.restype = i32
     L.orc_final_estimate.argtypes = [vp, vp, u64, u32, u32, u64, u64, vp, vp, C.POINTER(OrcCmd), i32, C.POINTER(OrcResult)]
@@ -202,8 +205,10 @@ def chain_debug(ref, query, cp=None):
         L.orc_debug_intervals(d, iv.ctypes.data)
         est = np.zeros(ne, np.float64); w = np.zeros(ne, np.uint64)
         L.orc_debug_ests(d, est.ctypes.data, w.ctypes.data)
+        cs = np.zeros((nc, 9), np.uint32)
+        L.orc_debug_chunk_stats(d, cs.ctypes.data)
         return dict(result=res, switched=bool(L.orc_debug_switched(d)), anchors=a5, score=score, pointer=ptr,
-                    chunk_first=first, chunk_nseeds=nseeds, intervals=iv, est=est, weight=w)
+                    chunk_first=first, chunk_nseeds=nseeds, intervals=iv, est=est, weight=w, chunk_stats=cs)
     finally:
         L.orc_debug_free(d)
 
@@ -223,6 +228,16 @@ def final_estimate(est, weight, total_bases_covered, avg_chain_int_len, query_to
                              int(query_total_len), int(ref_total_len), qq.ctypes.data, qr.ctypes.data, C.byref(cp), model,
                              C.byref(r))
     return r
+
+
+def chunk_estimate(inputs, c, k):
+    """The oracle's chunk_estimate over rows (total_anchors, rq0, rq1, tbcq, n_int, n_seeds, num_in, upper_lower): (est f64,
+    weight u32, valid u32: 0 no estimate, 1 estimate, 3 estimate with the putative-ANI filter applied)."""
+    x = np.ascontiguousarray(inputs, np.uint32).reshape(-1, 8)
+    n = len(x)
+    est = np.zeros(max(n, 1), np.float64); w = np.zeros(max(n, 1), np.uint32); v = np.zeros(max(n, 1), np.uint32)
+    lib().orc_chunk_estimate(n, x.ctypes.data, c, k, est.ctypes.data, w.ctypes.data, v.ctypes.data)
+    return est[:n], w[:n], v[:n]
 
 
 def _results(out, n):
