@@ -14,6 +14,8 @@
 // that passed for some query exactly once, imports them to the device in one batch and chains every pair there.
 // --gpus N: dist and search split the references into contiguous blocks, one per GPU, and copy the query set to every GPU
 // (sk_screen_query_ref_multi / sk_chain_pairs_multi); the output is byte-identical to one GPU's.
+// triangle and dist take pre-sketched inputs as .sketch files and as consolidated databases (sketch_db.hpp: SketchInputs),
+// decoded and imported in groups of < 2^28 records so that host memory holds one decoded group at a time.
 #include <dirent.h>
 #include <fcntl.h>
 #include <sys/stat.h>
@@ -238,48 +240,100 @@ struct Flat {
   }
 };
 
-// inputs given as .sketch files (refs_are_sketch / queries_are_sketch, src/parse.rs:264-275): every file name contains
-// ".sketch" or "markers.bin"
-bool all_sketch_files(const std::vector<std::string>& files) {
+// inputs given as sketches (refs_are_sketch / queries_are_sketch, src/parse.rs:264-275): every file name contains
+// ".sketch" or "markers.bin", or is a consolidated sketch database (a directory with index.db and sketches.db).  A
+// database among FASTA inputs is refused.
+bool sketch_inputs_given(const std::vector<std::string>& files) {
   if (files.empty()) return false;
-  for (auto& f : files) if (f.find(".sketch") == std::string::npos && f.find("markers.bin") == std::string::npos) return false;
+  const std::string* db = nullptr;
+  bool all = true;
+  for (auto& f : files) {
+    if (skdb::is_sketch_db(f)) { if (!db) db = &f; }
+    else if (f.find(".sketch") == std::string::npos && f.find("markers.bin") == std::string::npos) all = false;
+  }
+  if (db && !all) { fprintf(stderr, "ERROR Sketch database %s cannot be mixed with FASTA/FASTQ inputs. Exiting.\n", db->c_str()); exit(1); }
+  return all;
+}
+
+// group bound of the sketch readers: < 2^28 seed records per sk_sketch_set_import_batch call.  SK_SKETCH_GROUP_RECORDS
+// lowers it (a test hook: many groups from a small input).
+uint64_t sketch_group_records() {
+  if (const char* e = getenv("SK_SKETCH_GROUP_RECORDS")) return (uint64_t)std::max(1ll, atoll(e));
+  return 1ull << 28;
+}
+
+Genome genome_of(const skdb::HostSketch& h) {
+  Genome g; g.file_name = h.file_name; g.contigs = h.contigs; g.contig_order = h.contig_order; g.total_len = h.total_len;
+  if (g.contigs.empty()) g.contigs.push_back("");   // a sketch without contig names still prints
+  return g;
+}
+
+// sketch inputs [a, b) read group by group: fn(set) gets each group imported as one device set on ctx and owns it;
+// meta[i - a] gets entry i's metadata.  The decoded group is freed before the next one is read.  false (after the reader's
+// ERROR line) when an entry cannot be loaded: the caller ends the run from the main thread.  One INFO line reports the time
+// spent reading + decoding and importing (fn included).
+template <class F>
+bool for_each_sketch_group(sk_ctx* ctx, const skdb::SketchInputs& si, size_t a, size_t b, int threads, const sk_sketch_params& sp, Genome* meta, F fn) {
+  using clk = std::chrono::steady_clock;
+  skdb::SketchGroupReader rd(si, a, b, threads, sketch_group_records());
+  std::vector<skdb::HostSketch> g;
+  double t_read = 0, t_import = 0;
+  size_t groups = 0;
+  for (auto t0 = clk::now(); rd.next(g); t0 = clk::now()) {
+    Flat f;
+    for (size_t i = 0; i < g.size(); i++) { f.add(g[i], true); meta[rd.first + i - a] = genome_of(g[i]); }
+    g.clear();
+    const auto t1 = clk::now();
+    fn(f.import(ctx, sp));
+    t_read += std::chrono::duration<double>(t1 - t0).count();
+    t_import += std::chrono::duration<double>(clk::now() - t1).count();
+    groups++;
+  }
+  if (rd.failed) return false;
+  fprintf(stderr, "INFO %zu sketches loaded in %zu group(s): read + decode %.2f s, import %.2f s.\n", b - a, groups, t_read, t_import);
   return true;
 }
 
-// file_io::sketches_from_sketch (src/file_io.rs:680-717): one (SketchParams, Sketch) blob per file, markers.bin skipped,
-// result sorted by file name; the sketches' parameters replace the command line's.  meta gets one Genome per sketch.
-void read_sketch_files(const std::vector<std::string>& files, skdb::DiskParams& dp, std::vector<Genome>& meta, std::vector<skdb::HostSketch>& hs) {
-  for (auto& f : files) {
-    if (f.find("markers.bin") != std::string::npos) continue;
-    std::vector<uint8_t> b;
-    if (!skdb::read_file(f, b)) { fprintf(stderr, "ERROR Problem reading sketch file %s. Perhaps your file path is wrong? Exiting.\n", f.c_str()); exit(1); }
-    try { hs.push_back(skdb::read_blob(b.data(), b.size(), &dp)); }
-    catch (const std::exception&) {
-      fprintf(stderr, "ERROR %s is not a valid .sketch file or is corrupted. Skani v0.3+ is not compatible with older sketch files.\n", f.c_str());
-    }
-  }
-  if (hs.empty()) return;
-  if (dp.use_aa) { fprintf(stderr, "ERROR amino-acid sketches are not supported\n"); exit(1); }
-  std::stable_sort(hs.begin(), hs.end(), [](const skdb::HostSketch& x, const skdb::HostSketch& y) { return x.file_name < y.file_name; });
-  for (auto& h : hs) {
-    Genome g; g.file_name = h.file_name; g.contigs = h.contigs; g.contig_order = h.contig_order; g.total_len = h.total_len;
-    if (g.contigs.empty()) g.contigs.push_back("");
-    meta.push_back(std::move(g));
-  }
+// sketch inputs [a, b) -> one device set on ctx, grown group by group with sk_sketch_set_append (which holds the old and the
+// merged set at once: about twice the set at its peak, see the estimate of sketch_bytes_estimate).  ok = false when an
+// entry cannot be loaded.
+sk_sketch_set* import_sketch_inputs(sk_ctx* ctx, const skdb::SketchInputs& si, size_t a, size_t b, int threads, const sk_sketch_params& sp, Genome* meta,
+                                    bool& ok) {
+  sk_sketch_set* set = nullptr;
+  ok = for_each_sketch_group(ctx, si, a, b, threads, sp, meta, [&](sk_sketch_set* s) {
+    if (!set) { set = s; return; }
+    CK(ctx, sk_sketch_set_append(set, s));
+    sk_sketch_set_free(s);
+  });
+  return set;
 }
 
-// host sketches [a, b) -> one device set on ctx
-sk_sketch_set* import_sketches(sk_ctx* ctx, const std::vector<skdb::HostSketch>& hs, size_t a, size_t b, const sk_sketch_params& sp) {
-  Flat f;
-  for (size_t i = a; i < b; i++) f.add(hs[i], true);
-  return f.import(ctx, sp);
+// sketch inputs -> a new host sketch store: each group's set is added and freed before the next group is read, so host
+// memory holds one decoded group besides the pinned store, and the device one imported group.  nullptr when an entry
+// cannot be loaded.
+sk_sketch_store* store_sketch_inputs(sk_ctx* ctx, const skdb::SketchInputs& si, int threads, const sk_sketch_params& sp, std::vector<Genome>& meta) {
+  sk_sketch_store* st = nullptr;
+  CK(ctx, sk_sketch_store_create(&sp, &st));
+  meta.resize(si.entries.size());
+  const bool ok = for_each_sketch_group(ctx, si, 0, si.entries.size(), threads, sp, meta.data(), [&](sk_sketch_set* s) {
+    CK(ctx, sk_sketch_store_add(st, s));
+    sk_sketch_set_free(s);
+  });
+  if (!ok) { sk_sketch_store_free(st); return nullptr; }
+  return st;
 }
 
-sk_sketch_set* load_sketch_files(sk_ctx* ctx, const std::vector<std::string>& files, skdb::DiskParams& dp, std::vector<Genome>& meta) {
-  std::vector<skdb::HostSketch> hs;
-  read_sketch_files(files, dp, meta, hs);
-  if (hs.empty()) return nullptr;
-  return import_sketches(ctx, hs, 0, hs.size(), sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c});
+// the parameters of sketch inputs, as sk_sketch_params
+sk_sketch_params params_of(const skdb::SketchInputs& si) {
+  return sk_sketch_params{(uint32_t)si.params.c, (uint32_t)si.params.k, (uint32_t)si.params.marker_c};
+}
+
+// the number of inputs as the reference counts query files, where a database counts once per sketch
+size_t n_inputs(const std::vector<std::string>& files, const skdb::SketchInputs& si) {
+  size_t n = files.size();
+  for (auto& e : si.entries) if (si.db_fd[e.input] >= 0) n++;
+  for (int fd : si.db_fd) if (fd >= 0) n--;
+  return n;
 }
 
 // --gpus N: contexts 1..n-1 next to ctx0, on (device + d) % device count.  With fewer devices than N the contexts share
@@ -340,13 +394,13 @@ size_t file_group_end(const std::vector<std::string>& files, size_t f0) {
 
 // triangle: whether the sketches are expected to exceed the device (the estimate of sk_triangle's memory guard: 56 B per
 // seed, 24 B per marker and 6 GB of workspace against 92 % of the device, from the file sizes, x 4 for .gz; .sketch files
-// about triple on the device) or SK_DEVICE_BUDGET_MB asks for the store path.  --gpus N with FASTA inputs keeps
-// sk_triangle_multi.
+// about triple on the device; a database counts the bytes of its sketches.db) or SK_DEVICE_BUDGET_MB asks for the store
+// path.  --gpus N with FASTA inputs keeps sk_triangle_multi; with sketch inputs it always takes the store path.
 double sketch_bytes_estimate(const Opts& op, const std::vector<std::string>& files, bool sketches) {
   uint64_t bytes = 0;
   for (auto& f : files) {
     struct stat st;
-    if (stat(f.c_str(), &st) != 0) continue;
+    if (stat(skdb::is_sketch_db(f) ? (f + "/sketches.db").c_str() : f.c_str(), &st) != 0) continue;
     const bool gz = f.size() > 3 && f.compare(f.size() - 3, 3, ".gz") == 0;
     bytes += (uint64_t)st.st_size * (gz ? 4 : 1);
   }
@@ -359,57 +413,40 @@ bool exceeds_device(const Opts& op, double need) {
   if (sk_device_memory(op.device, &free_b, &total_b) != 0) return false;
   return need > 0.92 * (double)total_b;
 }
-bool triangle_needs_store(const Opts& op, bool sketches, double* need_gb) {
+// Sketch inputs of more records than one import group are grown into one set by sk_sketch_set_append, which holds the old
+// and the merged set on the device at once: their estimate then counts twice.  records = the inputs' (or one context's
+// share of the) SketchEntry weights.
+double append_peak(uint64_t records) { return records >= sketch_group_records() ? 2.0 : 1.0; }
+uint64_t total_weight(const skdb::SketchInputs& si) {
+  uint64_t w = 0;
+  for (auto& e : si.entries) w += e.weight;
+  return w;
+}
+
+bool triangle_needs_store(const Opts& op, bool sketches, const skdb::SketchInputs& si, double* need_gb) {
   *need_gb = 0;
   if (op.gpus > 1 && !sketches) return false;
-  const double need = sketch_bytes_estimate(op, op.files, sketches) + 6.0e9;
+  const double need = sketch_bytes_estimate(op, op.files, sketches) * (sketches ? append_peak(total_weight(si)) : 1.0) + 6.0e9;
   *need_gb = need / 1e9;
-  return exceeds_device(op, need);
+  return (op.gpus > 1 && sketches) || exceeds_device(op, need);
 }
 
 // dist: the same estimate per context, where the references are split over --gpus contexts and every context holds the
 // whole query set
-bool dist_needs_store(const Opts& op, bool refs_sketch, bool queries_sketch, double* need_gb) {
-  const double need = sketch_bytes_estimate(op, op.refs, refs_sketch) / std::max(op.gpus, 1) + sketch_bytes_estimate(op, op.queries, queries_sketch) + 6.0e9;
+bool dist_needs_store(const Opts& op, bool refs_sketch, bool queries_sketch, const skdb::SketchInputs& rsi, const skdb::SketchInputs& qsi, double* need_gb) {
+  const int gpus = std::max(op.gpus, 1);
+  const double need = sketch_bytes_estimate(op, op.refs, refs_sketch) / gpus * (refs_sketch ? append_peak(total_weight(rsi) / gpus) : 1.0) +
+                      sketch_bytes_estimate(op, op.queries, queries_sketch) * (queries_sketch ? append_peak(total_weight(qsi)) : 1.0) + 6.0e9;
   *need_gb = need / 1e9;
   return exceeds_device(op, need);
 }
 
-// Host sketches (read_sketch_files' order) imported in groups of < 2^28 records, each group added to a new store and freed;
-// hs is emptied along the way.
-sk_sketch_store* store_from_sketches(sk_ctx* ctx, std::vector<skdb::HostSketch>& hs, const sk_sketch_params& sp) {
-  sk_sketch_store* st = nullptr;
-  CK(ctx, sk_sketch_store_create(&sp, &st));
-  for (size_t a = 0; a < hs.size();) {
-    size_t b = a;
-    uint64_t recs = 0;
-    while (b < hs.size() && (b == a || recs + hs[b].kmer.size() < (1ull << 28))) recs += hs[b++].kmer.size();
-    sk_sketch_set* set = import_sketches(ctx, hs, a, b, sp);
-    CK(ctx, sk_sketch_store_add(st, set));
-    sk_sketch_set_free(set);
-    for (size_t i = a; i < b; i++) hs[i] = skdb::HostSketch();
-    a = b;
-  }
-  return st;
-}
-
-// The store path of triangle and dist: files are sketched (or .sketch files imported) in groups, each group's set is added to a
-// host sketch store and freed, so device memory holds one group at a time and host memory one group of sequence plus the
-// sketches.  genomes gets the metadata of every genome in store order (= the order of the in-memory path).
-sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, const std::vector<std::string>& input_files, bool individual, bool sketches,
+// The store path of triangle and dist on FASTA inputs: files are sketched in groups, each group's set is added to a host
+// sketch store and freed, so device memory holds one group at a time and host memory one group of sequence plus the
+// sketches.  genomes gets the metadata of every genome in store order (= the order of the in-memory path).  Sketch inputs
+// fill their store through store_sketch_inputs.
+sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, const std::vector<std::string>& input_files, bool individual,
                             std::vector<Genome>& genomes, sk_sketch_params& sp) {
-  if (sketches) {
-    fprintf(stderr, "INFO Sketches detected.\n");
-    skdb::DiskParams dp;
-    std::vector<skdb::HostSketch> hs;
-    read_sketch_files(input_files, dp, genomes, hs);
-    if (hs.empty()) return nullptr;
-    if (dp.c != op.c || dp.marker_c != op.m)
-      fprintf(stderr, "WARN Input parameter c = %u, m = %u is not equal to the sketch parameter c = %llu,m = %llu. Using sketch parameters.\n", op.c, op.m,
-              (unsigned long long)dp.c, (unsigned long long)dp.marker_c);
-    sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
-    return store_from_sketches(ctx, hs, sp);
-  }
   sk_sketch_store* st = nullptr;
   CK(ctx, sk_sketch_store_create(&sp, &st));
   std::vector<std::string> files = input_files;
@@ -429,36 +466,70 @@ sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, const std::vector<std::
   return st;
 }
 
+// the contexts of the store paths: two on each of the --gpus devices ((device + d) % count, shared when fewer are visible),
+// ctx0 first.  One context gathers its next working set over PCIe while the other chains.
+std::vector<sk_ctx*> store_contexts(sk_ctx* ctx0, const Opts& op) {
+  const int ndev = std::max(sk_device_count(), 1), gpus = std::max(op.gpus, 1);
+  if (ndev < gpus) fprintf(stderr, "WARN --gpus %d but %d CUDA device(s) visible: contexts share devices.\n", gpus, ndev);
+  std::vector<sk_ctx*> ctxs(1, ctx0);
+  for (int d = 0; d < gpus; d++)
+    for (int k = d == 0; k < 2; k++) {
+      const int dev = (op.device + d) % ndev;
+      sk_ctx* c = nullptr;
+      if (sk_ctx_create(dev, &c) != 0) { fprintf(stderr, "ERROR cannot create a context on GPU %d\n", dev); exit(1); }
+      ctxs.push_back(c);
+    }
+  return ctxs;
+}
+
+// "WARN Input parameter ..." of triangle's sketch inputs (src/triangle.rs:16-24); the sketches' parameters are used
+void warn_sketch_params(const Opts& op, const skdb::SketchInputs& si) {
+  if (si.params.c != op.c || si.params.marker_c != op.m)
+    fprintf(stderr, "WARN Input parameter c = %u, m = %u is not equal to the sketch parameter c = %llu,m = %llu. Using sketch parameters.\n", op.c, op.m,
+            (unsigned long long)si.params.c, (unsigned long long)si.params.marker_c);
+}
+
 int run_triangle(Opts& op) {
   resolve_presets(op);
   if (op.files.empty()) { fprintf(stderr, "ERROR No reference inputs found.\n"); return 1; }
   Inputs in;
-  const bool refs_are_sketch = all_sketch_files(op.files);
+  const bool refs_are_sketch = sketch_inputs_given(op.files);
+  skdb::SketchInputs si;
+  if (refs_are_sketch) {      // .sketch files and databases (src/triangle.rs:16-24): opened here, decoded in groups below
+    fprintf(stderr, "INFO Sketches detected.\n");
+    if (!skdb::open_sketch_inputs(op.files, si)) return 1;   // file_io::sketches_from_sketch (src/file_io.rs:680-717)
+    if (si.entries.empty()) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }
+    warn_sketch_params(op, si);
+  }
   double need_gb = 0;
-  const bool use_store = triangle_needs_store(op, refs_are_sketch, &need_gb);
+  const bool use_store = triangle_needs_store(op, refs_are_sketch, si, &need_gb);
   if (!refs_are_sketch && !use_store) {
     load_inputs(op.files, op.individual, std::max(op.threads, 1), in);
     if (in.genomes.empty()) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }   // src/triangle.rs:46-49
   }
   sk_ctx* ctx = nullptr;
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
-  sk_sketch_params sp{op.c, op.k, op.m};
+  sk_sketch_params sp = refs_are_sketch ? params_of(si) : sk_sketch_params{op.c, op.k, op.m};
   sk_sketch_set* loaded = nullptr;
   sk_sketch_store* store = nullptr;
   if (use_store) {
-    fprintf(stderr, "INFO Store path: sketches (~%.1f GB estimated) are kept in a host sketch store and chained in working sets on GPU %d%s.\n", need_gb,
-            op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
-    store = fill_store(ctx, op, op.files, op.individual, refs_are_sketch, in.genomes, sp);
-    if (!store) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }
-  } else if (refs_are_sketch) {      // src/triangle.rs:16-24
-    fprintf(stderr, "INFO Sketches detected.\n");
-    skdb::DiskParams dp;
-    loaded = load_sketch_files(ctx, op.files, dp, in.genomes);
-    if (!loaded) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }
-    if (dp.c != op.c || dp.marker_c != op.m)
-      fprintf(stderr, "WARN Input parameter c = %u, m = %u is not equal to the sketch parameter c = %llu,m = %llu. Using sketch parameters.\n", op.c, op.m,
-              (unsigned long long)dp.c, (unsigned long long)dp.marker_c);
-    sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
+    if (op.gpus > 1)
+      fprintf(stderr, "INFO Store path: sketches (~%.1f GB estimated) are kept in a host sketch store and chained in working sets on %d GPU(s) from GPU %d%s.\n",
+              need_gb, op.gpus, op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
+    else
+      fprintf(stderr, "INFO Store path: sketches (~%.1f GB estimated) are kept in a host sketch store and chained in working sets on GPU %d%s.\n", need_gb,
+              op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
+    store = refs_are_sketch ? store_sketch_inputs(ctx, si, std::max(op.threads, 1), sp, in.genomes)
+                            : fill_store(ctx, op, op.files, op.individual, in.genomes, sp);
+    if (!store) {      // sketch inputs: an entry could not be loaded (reported)
+      if (!refs_are_sketch) fprintf(stderr, "ERROR No genomes/sketches found.\n");
+      return 1;
+    }
+  } else if (refs_are_sketch) {
+    in.genomes.resize(si.entries.size());
+    bool ok = true;
+    loaded = import_sketch_inputs(ctx, si, 0, si.entries.size(), std::max(op.threads, 1), sp, in.genomes.data(), ok);
+    if (!ok) return 1;
   }
   if (in.genomes.size() > 500 && !op.sparse) fprintf(stderr, "WARN > 500 genomes detected. The output matrix will be large. Consider using -E or --sparse for a tsv output instead.\n");
   sk_map_params mp{};
@@ -480,20 +551,27 @@ int run_triangle(Opts& op) {
   }
   std::vector<sk_ani_result> res;
   sk_sketch_set* set = nullptr;
+  // sketch inputs: one INFO line gives the time of the screen and the chaining (with the "sketches loaded" line, the split
+  // of a run from a database)
+  using clk = std::chrono::steady_clock;
+  double t_work = 0;
+  auto timed = [&](clk::time_point t0) { t_work += std::chrono::duration<double>(clk::now() - t0).count(); };
+  auto report_work = [&] { if (refs_are_sketch) fprintf(stderr, "INFO Screen + chain %.2f s.\n", t_work); };
   if (store) {
-    // two contexts on the device: one gathers its next working set over PCIe while the other chains; every row is written at
-    // the end (no intermediate "Writing results" flushes in sparse mode)
+    // two contexts on each of the --gpus devices (store_contexts); every row is written at the end (no intermediate
+    // "Writing results" flushes in sparse mode)
     CK(ctx, sk_sketch_store_set_name_ranks(store, ranks.data()));
-    sk_ctx* ctx2 = nullptr;
-    if (sk_ctx_create(op.device, &ctx2) != 0) { fprintf(stderr, "ERROR cannot create a second context on GPU %d\n", op.device); return 1; }
-    sk_ctx* ctxs[2] = {ctx, ctx2};
+    std::vector<sk_ctx*> sctx = store_contexts(ctx, op);
     uint64_t budget = 0;
     if (const char* e = getenv("SK_DEVICE_BUDGET_MB")) budget = (uint64_t)std::max(1ll, atoll(e)) << 20;
     sk_ani_result* r = nullptr; uint64_t nr = 0;
-    CK(ctx, sk_triangle_store(ctxs, 2, store, &mp, budget, &r, &nr, nullptr));
-    res.assign(r, r + nr);                  // sorted by (ref_id, query_id)
+    const auto t0 = clk::now();
+    CK(ctx, sk_triangle_store(sctx.data(), (uint32_t)sctx.size(), store, &mp, budget, &r, &nr, nullptr));
+    timed(t0);
+    res.assign(r, r + nr);
     sk_free(r);
-    sk_ctx_destroy(ctx2);
+    std::sort(res.begin(), res.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
+    for (size_t d = sctx.size(); d-- > 1;) sk_ctx_destroy(sctx[d]);
     sk_sketch_store_free(store);
   } else if (op.gpus > 1 && !loaded) {
     // --gpus N: one context per GPU, genome blocks + marker exchange + cross-block slices (sk_triangle_multi).  With fewer
@@ -510,7 +588,9 @@ int run_triangle(Opts& op) {
     set = loaded ? loaded : sketch(ctx, in, sp);
     sk_sketch_set_set_name_ranks(set, ranks.data());
     uint64_t* pairs = nullptr; uint64_t np = 0;
+    const auto t0 = clk::now();
     CK(ctx, sk_screen_triangle(ctx, set, &mp, &pairs, &np));
+    timed(t0);
     if (op.sparse) {
       // sparse output: rows are chained and APPENDED in blocks of INTERMEDIATE_WRITE_COUNT rows (src/triangle.rs:113-138),
       // so a long run leaves its finished rows on disk and holds at most one block of results in memory
@@ -524,7 +604,9 @@ int run_triangle(Opts& op) {
         uint64_t p1 = p0;
         while (p1 < np && (uint32_t)(pairs[p1] >> 32) < r0 + FL) p1++;      // pairs are sorted by (i, j)
         res.resize(p1 - p0);
+        const auto t1 = clk::now();
         CK(ctx, sk_chain_pairs(ctx, set, set, pairs + p0, p1 - p0, &mp, res.data()));
+        timed(t1);
         for (auto& r : res) if (r.ani > 0.1f) write_row(o, r, in.genomes[r.ref_id], in.genomes[r.query_id], op);
         fflush(o);
         if (r0 + FL < Nrows) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", FL);
@@ -532,14 +614,18 @@ int run_triangle(Opts& op) {
       }
       sk_free(pairs);
       if (o != stdout) fclose(o);
+      report_work();
       sk_sketch_set_free(set);
       sk_ctx_destroy(ctx);
       return 0;
     }
     res.resize(np);
+    const auto t1 = clk::now();
     CK(ctx, sk_chain_pairs(ctx, set, set, pairs, np, &mp, res.data()));
+    timed(t1);
     sk_free(pairs);
   }
+  report_work();
   const size_t N = in.genomes.size();
   FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
   if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
@@ -617,44 +703,50 @@ int run_dist(Opts& op) {
   resolve_presets(op);
   if (op.refs.empty() || op.queries.empty()) { fprintf(stderr, "ERROR No reference sketches/genomes or query sketches/genomes found.\n"); return 1; }
   Inputs rin, qin;
-  const bool refs_are_sketch = all_sketch_files(op.refs), queries_are_sketch = all_sketch_files(op.queries);
-  sk_ctx* ctx = nullptr;
-  if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
+  const bool refs_are_sketch = sketch_inputs_given(op.refs), queries_are_sketch = sketch_inputs_given(op.queries);
   sk_sketch_params sp{op.c, op.k, op.m};
-  // .sketch inputs carry their own parameters, which then also apply to FASTA inputs on the other side (src/dist.rs:17-50).
-  // They are read on the host here and imported once the contexts exist.
-  std::vector<skdb::HostSketch> rhs, qhs;
+  // sketch inputs (.sketch files, databases) carry their own parameters, which then also apply to FASTA inputs on the other
+  // side (src/dist.rs:17-50).  They are opened on the host here and decoded and imported in groups once the contexts exist.
+  skdb::SketchInputs rsi, qsi;
   if (refs_are_sketch) {
     fprintf(stderr, "INFO Sketches detected.\n");
-    skdb::DiskParams dp;
-    read_sketch_files(op.refs, dp, rin.genomes, rhs);
-    if (!rhs.empty()) {
+    if (!skdb::open_sketch_inputs(op.refs, rsi)) return 1;   // file_io::sketches_from_sketch (src/file_io.rs:680-717)
+    if (!rsi.entries.empty()) {
+      const sk_sketch_params dp = params_of(rsi);
       if (dp.c != sp.c || dp.k != sp.k || dp.marker_c != sp.marker_c)
         fprintf(stderr, "WARN Parameters from .sketch files not equal to the input parameters. Using parameters from .sketch files.\n");
-      sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
+      sp = dp;
     }
   }
   if (queries_are_sketch) {
-    skdb::DiskParams dp;
-    read_sketch_files(op.queries, dp, qin.genomes, qhs);
-    if (!qhs.empty() && (dp.c != sp.c || dp.k != sp.k || dp.marker_c != sp.marker_c)) {
+    if (!skdb::open_sketch_inputs(op.queries, qsi)) return 1;   // file_io::sketches_from_sketch (src/file_io.rs:680-717)
+    const sk_sketch_params dp = params_of(qsi);
+    if (!qsi.entries.empty() && (dp.c != sp.c || dp.k != sp.k || dp.marker_c != sp.marker_c)) {
       if (refs_are_sketch) { fprintf(stderr, "ERROR Query sketch parameters were not equal to reference sketch parameters. Exiting.\n"); return 1; }
       fprintf(stderr, "WARN Parameters from .sketch files not equal to the input parameters. Using parameters from .sketch files.\n");
-      sp = sk_sketch_params{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
+      sp = dp;
     }
   }
+  sk_ctx* ctx = nullptr;
+  if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
   // store path: both sides go into host sketch stores in groups and are chained in working sets (sk_query_ref_store)
   double need_gb = 0;
-  const bool use_store = dist_needs_store(op, refs_are_sketch, queries_are_sketch, &need_gb);
+  const bool use_store = dist_needs_store(op, refs_are_sketch, queries_are_sketch, rsi, qsi, &need_gb);
   sk_sketch_store *rstore = nullptr, *qstore = nullptr;
+  const int threads = std::max(op.threads, 1);
   if (use_store) {
     fprintf(stderr, "INFO Store path: sketches (~%.1f GB per context estimated) are kept in host sketch stores and chained in working sets on %d GPU(s) from GPU %d%s.\n",
             need_gb, std::max(op.gpus, 1), op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
-    rstore = refs_are_sketch ? store_from_sketches(ctx, rhs, sp) : fill_store(ctx, op, op.refs, op.ri, false, rin.genomes, sp);
-    qstore = queries_are_sketch ? store_from_sketches(ctx, qhs, sp) : fill_store(ctx, op, op.queries, op.qi, false, qin.genomes, sp);
+    rstore = refs_are_sketch ? store_sketch_inputs(ctx, rsi, threads, sp, rin.genomes) : fill_store(ctx, op, op.refs, op.ri, rin.genomes, sp);
+    if (refs_are_sketch && !rstore) return 1;      // an entry could not be loaded (reported)
+    qstore = queries_are_sketch ? store_sketch_inputs(ctx, qsi, threads, sp, qin.genomes) : fill_store(ctx, op, op.queries, op.qi, qin.genomes, sp);
+    if (queries_are_sketch && !qstore) return 1;
   } else {
-    if (!refs_are_sketch) load_inputs(op.refs, op.ri, std::max(op.threads, 1), rin);
-    if (!queries_are_sketch) load_inputs(op.queries, op.qi, std::max(op.threads, 1), qin);
+    // sketch inputs: names now (for the name ranks), the rest of the metadata when each side is imported below
+    if (!refs_are_sketch) load_inputs(op.refs, op.ri, threads, rin);
+    else for (auto& e : rsi.entries) { Genome g; g.file_name = e.file_name; rin.genomes.push_back(std::move(g)); }
+    if (!queries_are_sketch) load_inputs(op.queries, op.qi, threads, qin);
+    else for (auto& e : qsi.entries) { Genome g; g.file_name = e.file_name; qin.genomes.push_back(std::move(g)); }
   }
   if (rin.genomes.empty() || qin.genomes.empty()) { fprintf(stderr, "ERROR No reference sketches/genomes or query sketches/genomes found.\n"); return 1; }
   sk_map_params mp{};
@@ -665,7 +757,7 @@ int run_dist(Opts& op) {
   mp.rescue_small = !op.faster_small && !op.small_genomes;
   mp.learned_ani = !op.no_learned && op.c >= 70 && !op.qi && !op.ri && !op.median;
   if (mp.learned_ani) fprintf(stderr, "INFO Learned ANI mode detected. ANI may be adjusted according to a regression model trained on MAGs.\n");
-  const bool use_index = (op.queries.size() > 50 || op.qi) && !op.no_marker_index;   // FULL_INDEX_THRESH (src/parse.rs:750)
+  const bool use_index = (n_inputs(op.queries, qsi) > 50 || op.qi) && !op.no_marker_index;   // FULL_INDEX_THRESH (src/parse.rs:750)
   // file-name order for the switch_qr tie-break (src/chain.rs:19-21): rank all names together
   std::vector<uint64_t> rr(rin.genomes.size()), qr(qin.genomes.size());
   {
@@ -684,16 +776,7 @@ int run_dist(Opts& op) {
     // block of queries is written at the end, through the same writer as the in-memory path.
     CK(ctx, sk_sketch_store_set_name_ranks(rstore, rr.data()));
     CK(ctx, sk_sketch_store_set_name_ranks(qstore, qr.data()));
-    const int ndev = std::max(sk_device_count(), 1), gpus = std::max(op.gpus, 1);
-    if (ndev < gpus) fprintf(stderr, "WARN --gpus %d but %d CUDA device(s) visible: contexts share devices.\n", gpus, ndev);
-    std::vector<sk_ctx*> sctx(1, ctx);
-    for (int d = 0; d < gpus; d++)
-      for (int k = d == 0; k < 2; k++) {
-        const int dev = (op.device + d) % ndev;
-        sk_ctx* c = nullptr;
-        if (sk_ctx_create(dev, &c) != 0) { fprintf(stderr, "ERROR cannot create a context on GPU %d\n", dev); return 1; }
-        sctx.push_back(c);
-      }
+    std::vector<sk_ctx*> sctx = store_contexts(ctx, op);
     uint64_t budget = 0;
     if (const char* e = getenv("SK_DEVICE_BUDGET_MB")) budget = (uint64_t)std::max(1ll, atoll(e)) << 20;
     sk_ani_result* r = nullptr; uint64_t nr = 0;
@@ -713,19 +796,23 @@ int run_dist(Opts& op) {
     for (size_t d = sctx.size(); d-- > 0;) sk_ctx_destroy(sctx[d]);
     return rc;
   }
-  // --gpus N: the references in W contiguous blocks (genome order, balanced by bases, or by records for .sketch inputs), each
-  // sketched or imported on its own context; the queries once on context 0, then copied to the others
+  // --gpus N: the references in W contiguous blocks (genome order, balanced by bases, or by records for sketch inputs), each
+  // sketched or imported on its own context; the queries once on context 0, then copied to the others.  Sketch inputs are
+  // decoded and imported in groups (-t threads split over the contexts), so host memory holds one group per context.
   const size_t NR = rin.genomes.size(), W = std::min<size_t>(std::max(op.gpus, 1), NR);
   std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, W);
   std::vector<uint64_t> weight(NR);
-  for (size_t g = 0; g < NR; g++) weight[g] = refs_are_sketch ? rhs[g].kmer.size() : rin.genomes[g].total_len;
+  for (size_t g = 0; g < NR; g++) weight[g] = refs_are_sketch ? rsi.entries[g].weight : rin.genomes[g].total_len;
   const std::vector<size_t> gb = split_balanced(weight, W);
   std::vector<sk_sketch_set*> rsets(W, nullptr), qsets(W, nullptr);
   std::vector<uint32_t> ref_first(W);
   for (size_t d = 0; d < W; d++) ref_first[d] = (uint32_t)gb[d];
+  std::atomic<bool> load_failed{false};     // a sketch entry could not be loaded (reported); the run ends below
   per_context(W, [&](size_t d) {
     sk_ctx* c = ctxs[d];
-    if (refs_are_sketch) rsets[d] = import_sketches(c, rhs, gb[d], gb[d + 1], sp);
+    const int t_ctx = std::max(1, threads / (int)W + ((int)d < threads % (int)W ? 1 : 0));
+    bool ok = true;
+    if (refs_are_sketch) rsets[d] = import_sketch_inputs(c, rsi, gb[d], gb[d + 1], t_ctx, sp, rin.genomes.data() + gb[d], ok);
     else {
       const size_t c0 = std::lower_bound(rin.genome_of_contig.begin(), rin.genome_of_contig.end(), (uint32_t)gb[d]) - rin.genome_of_contig.begin();
       const size_t c1 = std::lower_bound(rin.genome_of_contig.begin(), rin.genome_of_contig.end(), (uint32_t)gb[d + 1]) - rin.genome_of_contig.begin();
@@ -733,12 +820,15 @@ int run_dist(Opts& op) {
       for (size_t i = c0; i < c1; i++) gl[i - c0] = rin.genome_of_contig[i] - (uint32_t)gb[d];
       CK(c, sk_sketch_batch(c, rin.bases.data(), rin.contig_off.data() + c0, (uint32_t)(c1 - c0), gl.data(), (uint32_t)(gb[d + 1] - gb[d]), &sp, &rsets[d]));
     }
+    if (!ok) { load_failed = true; return; }
     sk_sketch_set_set_name_ranks(rsets[d], rr.data() + gb[d]);
     if (d == 0) {
-      qsets[0] = queries_are_sketch ? import_sketches(c, qhs, 0, qhs.size(), sp) : sketch(c, qin, sp);
+      qsets[0] = queries_are_sketch ? import_sketch_inputs(c, qsi, 0, qsi.entries.size(), t_ctx, sp, qin.genomes.data(), ok) : sketch(c, qin, sp);
+      if (!ok) { load_failed = true; return; }
       sk_sketch_set_set_name_ranks(qsets[0], qr.data());
     }
   });
+  if (load_failed) return 1;
   for (size_t d = 1; d < W; d++) CK(ctxs[d], sk_sketch_set_copy(ctxs[d], qsets[0], &qsets[d]));
   uint64_t* pairs = nullptr; uint64_t np = 0;
   CK(ctx, sk_screen_query_ref_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), &mp, use_index ? 2 : 0, &pairs, &np));
@@ -848,13 +938,7 @@ int run_search(Opts& op) {
   const bool consolidated = path_exists(op.db_dir + "/sketches.db") && path_exists(op.db_dir + "/index.db");   // src/sketch_db.rs:142-146
   std::vector<skdb::IndexEntry> index;
   int db_fd = -1;
-  if (consolidated) {
-    try { skdb::read_index_db(op.db_dir + "/index.db", index); }
-    catch (const std::exception& e) { fprintf(stderr, "ERROR Failed to load consolidated database: %s\n", e.what()); return 1; }
-    if (index.size() != ref_mk.size()) { fprintf(stderr, "ERROR index.db and markers.bin disagree on the number of sketches\n"); return 1; }
-    db_fd = open((op.db_dir + "/sketches.db").c_str(), O_RDONLY);
-    if (db_fd < 0) { fprintf(stderr, "ERROR Failed to load consolidated database\n"); return 1; }
-  }
+  if (consolidated && !skdb::open_db(op.db_dir, index, db_fd)) return 1;   // the reader of triangle's and dist's database inputs
   sk_sketch_params sp{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
   sk_ctx* ctx = nullptr;
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
@@ -975,16 +1059,15 @@ int run_search(Opts& op) {
         for (int t = 0; t < T; t++) pool.emplace_back([&, t] {
           for (size_t i = h0 + t; i < h1; i += T) {
             const uint32_t r = hits[i];
-            std::vector<uint8_t> b;
             bool good;
             if (consolidated) {
-              b.resize(index[r].length);
-              good = pread(db_fd, b.data(), b.size(), (off_t)index[r].offset) == (ssize_t)b.size();
+              good = skdb::read_db_entry(db_fd, index[r], loaded[i - h0]);
             } else {                     // <dir>/<basename(file_name)>.sketch (src/search.rs:157-166)
+              std::vector<uint8_t> b;
               good = skdb::read_file(op.db_dir + "/" + base_name(ref_mk[r].file_name) + ".sketch", b);
+              try { if (good) loaded[i - h0] = skdb::read_blob(b.data(), b.size()); }
+              catch (const std::exception&) { good = false; }
             }
-            try { if (good) loaded[i - h0] = skdb::read_blob(b.data(), b.size()); }
-            catch (const std::exception&) { good = false; }
             if (!good) { ok[i - h0] = 0; fprintf(stderr, "ERROR Failed to load sketch %s\n", ref_mk[r].file_name.c_str()); }
           }
         });
@@ -1068,6 +1151,8 @@ void usage() {
           "skani-b200 (H100 CUDA implementation of skani v0.3.0's ANI hot path)\n"
           "  skani-b200 triangle [fasta ... | -l list] [-i] [-E|--sparse] [-o out] [--full-matrix] [--diagonal] [--distance]\n"
           "  skani-b200 dist [query] [refs ...] [-q ...] [-r ...] [--ql list] [--rl list] [--qi] [--ri] [-n N] [-o out]\n"
+          "      triangle and dist also take sketches: .sketch files and sketch databases (folders written by `sketch`, with\n"
+          "      index.db and sketches.db), mixed freely; a database stands for all of its sketches\n"
           "  skani-b200 sketch [fasta ... | -l list] -o new_folder [-i] [--separate-sketches]\n"
           "  skani-b200 search -d sketch_folder [query ... | -q ... | --ql list] [--qi] [-n N] [-o out]\n"
           "  common: -c C -m M -k K -s SCREEN%% --min-af P --both-min-af P --robust --median --no-learned-ani --faster-small\n"

@@ -5,6 +5,11 @@
 //                                                      markers.bin (records sorted by (kmer, contig, pos), markers ascending)
 //   skani-db-tool fastx <file>                      -> the CLI's FASTA/FASTQ(.gz) reader (fastx.hpp): "OK n" then one line per
 //                                                      record "<length> <fnv1a64 of the sequence> <id>", or "ERR"
+//   skani-db-tool groups <max_records> <threads> <input>...
+//                                                   -> the sketch inputs of triangle / dist (.sketch files and databases) as
+//                                                      the CLI opens and groups them: "PARAMS c k marker_c", "N entries", then
+//                                                      per group "G <first entry> <sketches> <records>" and per sketch
+//                                                      "S <records> <contig_order> <file name>"; ERROR and exit 1 on a refusal
 // Text form, one sketch = the lines
 //   S <contig_order> <total_len> <file name>
 //   C <contig header>            (one line per contig)
@@ -97,6 +102,21 @@ int main(int argc, char** argv) {
       for (auto& m : mk) print_sketch(m, "K");
       return 0;
     }
+    if (argc >= 5 && std::string(argv[1]) == "groups") {
+      SketchInputs si;
+      if (!open_sketch_inputs(std::vector<std::string>(argv + 4, argv + argc), si)) return 1;
+      printf("PARAMS %llu %llu %llu\nN %zu\n", (unsigned long long)si.params.c, (unsigned long long)si.params.k,
+             (unsigned long long)si.params.marker_c, si.entries.size());
+      SketchGroupReader rd(si, 0, si.entries.size(), atoi(argv[3]), strtoull(argv[2], nullptr, 10));
+      std::vector<HostSketch> g;
+      while (rd.next(g)) {
+        uint64_t recs = 0;
+        for (auto& h : g) recs += h.kmer.size();
+        printf("G %zu %zu %llu\n", rd.first, g.size(), (unsigned long long)recs);
+        for (auto& h : g) printf("S %zu %llu %s\n", h.kmer.size(), (unsigned long long)h.contig_order, h.file_name.c_str());
+      }
+      return rd.failed ? 1 : 0;
+    }
     if (argc >= 3 && std::string(argv[1]) == "fastx") {
       std::vector<fastx::Record> recs;
       if (!fastx::read_fastx(argv[2], recs, argc >= 4 ? std::max(1, atoi(argv[3])) : 1)) { printf("ERR\n"); return 0; }    // [threads]
@@ -112,6 +132,7 @@ int main(int argc, char** argv) {
     fprintf(stderr, "ERROR %s\n", e.what());
     return 1;
   }
-  fprintf(stderr, "usage: skani-db-tool write <dir> <c> <k> <marker_c> < text | skani-db-tool dump <dir>\n");
+  fprintf(stderr, "usage: skani-db-tool write <dir> <c> <k> <marker_c> < text | skani-db-tool dump <dir> | "
+                  "skani-db-tool groups <max_records> <threads> <input>...\n");
   return 2;
 }

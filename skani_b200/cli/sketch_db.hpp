@@ -12,11 +12,18 @@
 // ascending k-mers.  Map value (src/types.rs:207-244): bit 0 = 1 -> one position packed as
 // ((pos << 31 | contig_index_canonical) << 1) | 1; bit 0 = 0 -> (index into multi_position_storage) << 1.
 #pragma once
+#include <fcntl.h>
+#include <sys/stat.h>
+#include <unistd.h>
+
+#include <algorithm>
+#include <atomic>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <stdexcept>
 #include <string>
+#include <thread>
 #include <vector>
 
 namespace skdb {
@@ -290,5 +297,197 @@ inline HostSketch read_blob(const uint8_t* p, size_t n, DiskParams* params = nul
   if (params) *params = dp;
   return get_sketch(in, true);
 }
+
+// one entry of sketches.db (open as fd): pread of its slice, then read_blob.  false if it cannot be read or decoded.
+inline bool read_db_entry(int fd, const IndexEntry& e, HostSketch& out, DiskParams* params = nullptr) {
+  std::vector<uint8_t> b(e.length);
+  if (pread(fd, b.data(), b.size(), (off_t)e.offset) != (ssize_t)b.size()) return false;
+  try { out = read_blob(b.data(), b.size(), params); }
+  catch (const std::exception&) { return false; }
+  return true;
+}
+
+// the sketch count of markers.bin, read from its head only (the marker sketches themselves are not decoded)
+inline bool markers_bin_count(const std::string& path, uint64_t& n) {
+  FILE* f = fopen(path.c_str(), "rb");
+  if (!f) return false;
+  std::vector<uint8_t> b(4096);
+  b.resize(fread(b.data(), 1, b.size(), f));
+  fclose(f);
+  try { In in(b.data(), b.size()); get_params(in); n = in.u64(); }
+  catch (const std::exception&) { return false; }
+  return true;
+}
+
+// A consolidated database: index.db read, checked against markers.bin's sketch count when markers.bin exists, and
+// sketches.db opened read-only as fd.  false after an ERROR line (the messages of `search`).
+inline bool open_db(const std::string& dir, std::vector<IndexEntry>& index, int& fd) {
+  try { read_index_db(dir + "/index.db", index); }
+  catch (const std::exception& e) { fprintf(stderr, "ERROR Failed to load consolidated database: %s\n", e.what()); return false; }
+  uint64_t n_markers = 0;
+  struct stat st;
+  if (stat((dir + "/markers.bin").c_str(), &st) == 0 && (!markers_bin_count(dir + "/markers.bin", n_markers) || n_markers != index.size())) {
+    fprintf(stderr, "ERROR index.db and markers.bin disagree on the number of sketches\n");
+    return false;
+  }
+  fd = open((dir + "/sketches.db").c_str(), O_RDONLY);
+  if (fd < 0) { fprintf(stderr, "ERROR Failed to load consolidated database\n"); return false; }
+  return true;
+}
+
+// ---------------------------------------------------------------- sketch inputs of triangle / dist
+// A consolidated database (a directory holding index.db and sketches.db, src/sketch_db.rs:142-146) stands for all of its
+// sketches, exactly as if each entry were a .sketch file.  Opening the inputs reads index.db (and checks it against
+// markers.bin and the size of sketches.db) but decodes only a database's first entry; the sketches themselves are decoded
+// later, in groups (SketchGroupReader), so host memory holds one decoded group at a time.
+inline bool is_sketch_db(const std::string& p) {
+  struct stat st;
+  return stat(p.c_str(), &st) == 0 && S_ISDIR(st.st_mode) && stat((p + "/index.db").c_str(), &st) == 0 &&
+         stat((p + "/sketches.db").c_str(), &st) == 0;
+}
+
+struct SketchEntry {            // one sketch of the inputs
+  uint32_t input = 0;           // index into SketchInputs::paths
+  std::string file_name;        // sort key: the name in index.db, or the one stored in the .sketch file
+  uint64_t offset = 0, length = 0;   // slice of sketches.db (a .sketch file: the whole file)
+  uint64_t weight = 0;          // seed records (.sketch files, decoded when opened) or length / 12 (a database entry, not
+                                // yet decoded: a single-position record takes 12 bytes on disk)
+};
+
+struct SketchInputs {
+  std::vector<std::string> paths;    // .sketch files and database directories, in command-line order
+  std::vector<int> db_fd;            // sketches.db of paths[i], or -1 for a .sketch file
+  std::vector<SketchEntry> entries;  // every sketch, stably sorted by file name (src/file_io.rs:715)
+  DiskParams params;                 // of the first input (all inputs agree on c, k and marker_c)
+  SketchInputs() = default;
+  SketchInputs(const SketchInputs&) = delete;
+  SketchInputs& operator=(const SketchInputs&) = delete;
+  ~SketchInputs() { for (int fd : db_fd) if (fd >= 0) close(fd); }
+};
+
+// Opens the inputs (.sketch files, markers.bin names, which are skipped, and databases) into si.  Problems are reported
+// on stderr with an ERROR line; false means the run must stop.  A .sketch file that does not decode is skipped, as
+// file_io::sketches_from_sketch does (src/file_io.rs:680-717).
+inline bool open_sketch_inputs(const std::vector<std::string>& files, SketchInputs& si) {
+  std::string params_of;        // the input whose parameters si.params holds
+  auto take_params = [&](const DiskParams& p, const std::string& path, bool db) {
+    if (p.use_aa) { fprintf(stderr, db ? "ERROR amino-acid databases are not supported\n" : "ERROR amino-acid sketches are not supported\n"); return false; }
+    if (params_of.empty()) { si.params = p; params_of = path; return true; }
+    if (p.c == si.params.c && p.k == si.params.k && p.marker_c == si.params.marker_c) return true;
+    fprintf(stderr, "ERROR Sketch parameters of %s (c = %llu, k = %llu, m = %llu) differ from those of %s (c = %llu, k = %llu, m = %llu). Exiting.\n",
+            path.c_str(), (unsigned long long)p.c, (unsigned long long)p.k, (unsigned long long)p.marker_c, params_of.c_str(),
+            (unsigned long long)si.params.c, (unsigned long long)si.params.k, (unsigned long long)si.params.marker_c);
+    return false;
+  };
+  for (auto& f : files) {
+    const uint32_t input = (uint32_t)si.paths.size();
+    if (is_sketch_db(f)) {
+      std::vector<IndexEntry> index;
+      int fd = -1;
+      if (!open_db(f, index, fd)) return false;
+      si.paths.push_back(f);
+      si.db_fd.push_back(fd);
+      struct stat st;
+      if (fstat(fd, &st) != 0) { fprintf(stderr, "ERROR Failed to load consolidated database\n"); return false; }
+      for (auto& e : index)
+        if (e.offset > (uint64_t)st.st_size || e.length > (uint64_t)st.st_size - e.offset) {
+          fprintf(stderr, "ERROR Failed to load consolidated database: the entry of %s runs past the end of %s/sketches.db\n", e.file_name.c_str(), f.c_str());
+          return false;
+        }
+      if (index.empty()) continue;
+      HostSketch first;
+      DiskParams p;
+      if (!read_db_entry(fd, index[0], first, &p)) { fprintf(stderr, "ERROR Failed to load sketch %s\n", index[0].file_name.c_str()); return false; }
+      if (!take_params(p, f, true)) return false;
+      for (auto& e : index) si.entries.push_back(SketchEntry{input, e.file_name, e.offset, e.length, e.length / 12});
+    } else {
+      if (f.find("markers.bin") != std::string::npos) continue;
+      std::vector<uint8_t> b;
+      if (!read_file(f, b)) { fprintf(stderr, "ERROR Problem reading sketch file %s. Perhaps your file path is wrong? Exiting.\n", f.c_str()); return false; }
+      HostSketch h;
+      DiskParams p;
+      try { h = read_blob(b.data(), b.size(), &p); }
+      catch (const std::exception&) {
+        fprintf(stderr, "ERROR %s is not a valid .sketch file or is corrupted. Skani v0.3+ is not compatible with older sketch files.\n", f.c_str());
+        continue;
+      }
+      if (!take_params(p, f, false)) return false;
+      si.paths.push_back(f);
+      si.db_fd.push_back(-1);
+      si.entries.push_back(SketchEntry{input, h.file_name, 0, (uint64_t)b.size(), (uint64_t)h.kmer.size()});
+    }
+  }
+  std::stable_sort(si.entries.begin(), si.entries.end(), [](const SketchEntry& x, const SketchEntry& y) { return x.file_name < y.file_name; });
+  return true;
+}
+
+// Decodes the entries [begin, end) of si, in order, and hands them out in groups of < max_records seed records (a group
+// holds at least one sketch).  Entries are read and decoded in batches by `threads` threads; at most one batch waits
+// beyond the current group.  An entry that cannot be read or decoded, or whose name differs from its index entry, ends
+// the reading with an ERROR line: next() then returns false with failed set.
+class SketchGroupReader {
+ public:
+  SketchGroupReader(const SketchInputs& si, size_t begin, size_t end, int threads, uint64_t max_records)
+      : si_(si), next_(begin), end_(end), consumed_(begin), threads_(std::max(threads, 1)), max_records_(max_records) {}
+  bool failed = false;
+  size_t first = 0;             // entry index of g[0] after next()
+
+  bool next(std::vector<HostSketch>& g) {
+    g.clear();
+    first = consumed_;
+    uint64_t recs = 0;
+    for (;;) {
+      if (pending_pos_ == pending_.size() && !decode_batch()) break;
+      if (failed) return false;
+      HostSketch& h = pending_[pending_pos_];
+      if (!g.empty() && recs + h.kmer.size() >= max_records_) break;
+      recs += h.kmer.size();
+      g.push_back(std::move(h));
+      pending_pos_++;
+      consumed_++;
+    }
+    return !g.empty();
+  }
+
+ private:
+  bool decode_batch() {         // the next entries (at most 8 per thread and about 256 MiB on disk) into pending_
+    if (next_ >= end_) return false;
+    size_t b = next_;
+    uint64_t bytes = 0;
+    while (b < end_ && (b == next_ || (b - next_ < 8 * (size_t)threads_ && bytes < (256ull << 20)))) bytes += si_.entries[b++].length;
+    pending_.assign(b - next_, HostSketch());
+    pending_pos_ = 0;
+    std::atomic<size_t> at{0};
+    std::atomic<bool> bad{false};
+    auto worker = [&] {
+      for (size_t i; (i = at.fetch_add(1)) < pending_.size();) {
+        const SketchEntry& e = si_.entries[next_ + i];
+        const int fd = si_.db_fd[e.input];
+        bool good;
+        if (fd >= 0) good = read_db_entry(fd, IndexEntry{e.file_name, e.offset, e.length}, pending_[i]) && pending_[i].file_name == e.file_name;
+        else {
+          std::vector<uint8_t> buf;
+          good = read_file(si_.paths[e.input], buf);
+          try { if (good) pending_[i] = read_blob(buf.data(), buf.size()); }
+          catch (const std::exception&) { good = false; }
+        }
+        if (!good) { bad = true; fprintf(stderr, "ERROR Failed to load sketch %s\n", e.file_name.c_str()); }
+      }
+    };
+    std::vector<std::thread> pool;
+    for (int t = 1; t < threads_ && (size_t)t < pending_.size(); t++) pool.emplace_back(worker);
+    worker();
+    for (auto& t : pool) t.join();
+    next_ = b;
+    if (bad) { failed = true; pending_.clear(); }
+    return true;
+  }
+  const SketchInputs& si_;
+  size_t next_, end_, consumed_;
+  int threads_;
+  uint64_t max_records_;
+  std::vector<HostSketch> pending_;
+  size_t pending_pos_ = 0;
+};
 
 }  // namespace skdb
