@@ -245,41 +245,48 @@ __global__ void marker_keys_kernel(const uint64_t* __restrict__ seg_off, uint64_
   for (uint64_t i = b + (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; i < e; i += (uint64_t)blockDim.x * gridDim.y) mk[i] |= (uint64_t)g << (2 * MARKER_K);
 }
 
-// after the sort by k-mer: gather the k-mer view and flag group heads
+// The kernels below run one thread per SORTED record, in sorted order, and read the record's genome from its sort key
+// (key >> gshift, gshift = ibits + kbits).  Their gathers from and scatters to the position view (pv_pos / pv_cc / pv_mult
+// at the record's original index) then stay inside the few genomes whose records are in flight, which L2 holds (blocks
+// indexed by genome would keep every genome of the sub-batch in flight and send each gather to HBM).
+
+// after the sort by k-mer: gather the k-mer view and flag group heads (a genome's first record always differs from the
+// previous record in the genome bits of the key)
 __global__ void kview_gather_kernel(const uint64_t* __restrict__ seg_off, const uint64_t* __restrict__ skmer,
                                     const uint32_t* __restrict__ perm, const uint32_t* __restrict__ pv_pos,
                                     const uint32_t* __restrict__ pv_cc, uint32_t* __restrict__ kv_pos,
-                                    uint32_t* __restrict__ kv_cc, uint32_t* __restrict__ head, uint32_t ibits) {
-  uint32_t g = blockIdx.x;
-  uint64_t b = seg_off[g], e = seg_off[g + 1];
+                                    uint32_t* __restrict__ kv_cc, uint32_t* __restrict__ head, uint32_t ibits, uint32_t gshift,
+                                    uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
   const uint64_t imask = (1ull << ibits) - 1;
-  for (uint64_t i = b + (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; i < e; i += (uint64_t)blockDim.x * gridDim.y) {
-    const uint64_t k = skmer[i];
-    uint32_t r = ibits ? (uint32_t)(k & imask) : perm[i];
-    kv_pos[i] = pv_pos[b + r];
-    kv_cc[i] = pv_cc[b + r];
-    head[i] = (i == b || (k >> ibits) != (skmer[i - 1] >> ibits)) ? 1u : 0u;
-  }
+  const uint64_t k = skmer[i];
+  const uint64_t b = seg_off[k >> gshift];
+  const uint32_t r = ibits ? (uint32_t)(k & imask) : perm[i];
+  kv_pos[i] = pv_pos[b + r];
+  kv_cc[i] = pv_cc[b + r];
+  head[i] = (i == 0 || (k >> ibits) != (skmer[i - 1] >> ibits)) ? 1u : 0u;
 }
 
 // hscan = exclusive scan of head flags (global).  Group id of sorted element i = hscan[i] + head[i] - 1 (global);
-// writes distinct k-mers and local group starts (+ one sentinel per genome), then multiplicities per pv record.
+// writes distinct k-mers and local group starts; thread g < n_genomes also writes genome g's sentinel.
 __global__ void groups_kernel(const uint64_t* __restrict__ seg_off, const uint64_t* __restrict__ skmer, uint64_t kmask,
                               const uint32_t* __restrict__ head, const uint32_t* __restrict__ hscan,
-                              uint32_t n_genomes, uint32_t* __restrict__ ukmer, uint32_t* __restrict__ ustart, uint32_t ibits) {
-  uint32_t g = blockIdx.x;
-  uint64_t b = seg_off[g], e = seg_off[g + 1];
-  for (uint64_t i = b + (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; i < e; i += (uint64_t)blockDim.x * gridDim.y) {
-    if (head[i]) {
-      uint32_t gid = hscan[i];
-      ukmer[gid] = (uint32_t)((skmer[i] >> ibits) & kmask);
-      ustart[gid + g] = (uint32_t)(i - b);
-    }
+                              uint32_t n_genomes, uint32_t* __restrict__ ukmer, uint32_t* __restrict__ ustart, uint32_t ibits,
+                              uint32_t gshift, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && head[i]) {
+    const uint64_t k = skmer[i];
+    const uint32_t g = (uint32_t)(k >> gshift);
+    const uint32_t gid = hscan[i];
+    ukmer[gid] = (uint32_t)((k >> ibits) & kmask);
+    ustart[gid + g] = (uint32_t)(i - seg_off[g]);
   }
-  if (threadIdx.x == 0 && blockIdx.y == 0) {
+  if (i < n_genomes) {
     // sentinel of genome g sits right after its last group: global group index of next genome's first group
-    uint64_t total = seg_off[n_genomes];
-    uint32_t next_gid = (e < total) ? hscan[e] : hscan[total - 1] + head[total - 1];  // head[e] is always 1, so hscan[e] = #groups before e; past the end: all groups
+    const uint32_t g = i;
+    const uint64_t b = seg_off[g], e = seg_off[g + 1];
+    const uint32_t next_gid = (e < n) ? hscan[e] : hscan[n - 1] + head[n - 1];  // head[e] is always 1, so hscan[e] = #groups before e; past the end: all groups
     ustart[next_gid + g] = (uint32_t)(e - b);
   }
 }
@@ -287,16 +294,16 @@ __global__ void groups_kernel(const uint64_t* __restrict__ seg_off, const uint64
 __global__ void mult_kernel(const uint64_t* __restrict__ seg_off, const uint32_t* __restrict__ head,
                             const uint32_t* __restrict__ hscan, const uint32_t* __restrict__ perm,
                             const uint32_t* __restrict__ ustart, uint16_t* __restrict__ pv_mult,
-                            const uint64_t* __restrict__ skmer, uint32_t ibits) {
-  uint32_t g = blockIdx.x;
-  uint64_t b = seg_off[g], e = seg_off[g + 1];
+                            const uint64_t* __restrict__ skmer, uint32_t ibits, uint32_t gshift, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
   const uint64_t imask = (1ull << ibits) - 1;
-  for (uint64_t i = b + (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; i < e; i += (uint64_t)blockDim.x * gridDim.y) {
-    uint32_t gid = hscan[i] + head[i] - 1;
-    uint32_t cntv = ustart[gid + g + 1] - ustart[gid + g];
-    const uint32_t r = ibits ? (uint32_t)(skmer[i] & imask) : perm[i];
-    pv_mult[b + r] = (uint16_t)min(cntv, 65535u);
-  }
+  const uint64_t k = skmer[i];
+  const uint32_t g = (uint32_t)(k >> gshift);
+  const uint32_t gid = hscan[i] + head[i] - 1;
+  const uint32_t cntv = ustart[gid + g + 1] - ustart[gid + g];
+  const uint32_t r = ibits ? (uint32_t)(k & imask) : perm[i];
+  pv_mult[seg_off[g] + r] = (uint16_t)min(cntv, 65535u);
 }
 
 // bucket index over each genome's distinct k-mers: ubucket[g][b] = first index u with (ukmer[u] >> shift) >= b
@@ -383,11 +390,17 @@ void free_set_device(sk_sketch_set* s) {
 }
 
 // per-genome k-mer hash table for the probe kernel: one 8-byte entry holds key, group start and (saturated) group size,
-// so a probe costs ~1.2 divergent sector reads instead of a search + two ustart reads
+// so a probe costs ~1.2 divergent sector reads instead of a search + two ustart reads.
+// bpg consecutive blocks per genome (genome-major grid): the blocks in flight cover a few consecutive genomes, whose tables
+// (~1 MB each for 5 Mbp at c = 125) stay in L2 while their atomics land (with the genome as the fastest grid index, every
+// genome of the set would have blocks in flight and each atomic would go to HBM).
+static inline uint32_t hash_build_blocks(uint64_t max_uk) {
+  return (uint32_t)std::min<uint64_t>(64, std::max<uint64_t>(1, (max_uk + 255) / 256));
+}
 __global__ void hash_build_kernel(const uint64_t* __restrict__ uk_off, const uint64_t* __restrict__ ht_off,
                                   const uint32_t* __restrict__ ukmer, const uint32_t* __restrict__ ustart,
-                                  unsigned long long* __restrict__ htab, uint32_t g_base) {
-  const uint32_t g = g_base + blockIdx.x;
+                                  unsigned long long* __restrict__ htab, uint32_t g_base, uint32_t bpg) {
+  const uint32_t g = g_base + blockIdx.x / bpg, chunk = blockIdx.x % bpg;
   const uint64_t cap = ht_off[g + 1] - ht_off[g];
   if (cap == 0) return;
   const uint32_t nb = (uint32_t)(cap >> 2);                              // 4-entry (32-byte) buckets; cap is a power of two >= 16
@@ -397,7 +410,7 @@ __global__ void hash_build_kernel(const uint64_t* __restrict__ uk_off, const uin
   const uint32_t* us = ustart + uk_off[g] + g;
   unsigned long long* tab = htab + ht_off[g];
   const uint32_t n = (uint32_t)(uk_off[g + 1] - uk_off[g]);
-  for (uint32_t u = blockIdx.y * blockDim.x + threadIdx.x; u < n; u += blockDim.x * gridDim.y) {
+  for (uint32_t u = chunk * blockDim.x + threadIdx.x; u < n; u += blockDim.x * bpg) {
     const uint32_t key = uk[u], start = us[u], cntv = us[u + 1] - start;
     // key 0 with start 0 and count 0 cannot occur (count >= 1), so a stored entry is never 0 = "empty"
     const unsigned long long e = ((unsigned long long)key << 32) | ((unsigned long long)start << 12) | (cntv < 4095u ? cntv : 4095u);
@@ -446,7 +459,10 @@ int build_hash(sk_ctx* ctx, sk_sketch_set* set) {
   SK_CUDA(d_uk.alloc(G + 1, ctx)); SK_CUDA(d_ht.alloc(G + 1, ctx));
   SK_CUDA(h2d_small(ctx, d_uk.p, set->uk_off.data(), (G + 1) * 8));
   SK_CUDA(h2d_small(ctx, d_ht.p, set->ht_off.data(), (G + 1) * 8));
-  hash_build_kernel<<<dim3(G, 32), 256, 0, st>>>(d_uk.p, d_ht.p, set->ukmer, set->ustart, set->htab, 0); count_launch(ctx);
+  uint64_t max_uk = 0;
+  for (uint32_t g = 0; g < G; g++) max_uk = std::max<uint64_t>(max_uk, set->uk_off[g + 1] - set->uk_off[g]);
+  const uint32_t nb = hash_build_blocks(max_uk);
+  hash_build_kernel<<<G * nb, 256, 0, st>>>(d_uk.p, d_ht.p, set->ukmer, set->ustart, set->htab, 0, nb); count_launch(ctx);
   SK_CUDA(cudaStreamSynchronize(st));
   return SK_OK;
 }
@@ -486,7 +502,10 @@ int build_hash_range(sk_ctx* ctx, sk_sketch_set* set, uint32_t g_begin) {
   SK_CUDA(d_uk.alloc(G + 1, ctx)); SK_CUDA(d_ht.alloc(G + 1, ctx));
   SK_CUDA(h2d_small(ctx, d_uk.p, set->uk_off.data(), (G + 1) * 8));
   SK_CUDA(h2d_small(ctx, d_ht.p, set->ht_off.data(), (G + 1) * 8));
-  hash_build_kernel<<<dim3(G - g_begin, 32), 256, 0, st>>>(d_uk.p, d_ht.p, set->ukmer, set->ustart, set->htab, g_begin); count_launch(ctx);
+  uint64_t max_uk = 0;
+  for (uint32_t g = g_begin; g < G; g++) max_uk = std::max<uint64_t>(max_uk, set->uk_off[g + 1] - set->uk_off[g]);
+  const uint32_t nb = hash_build_blocks(max_uk);
+  hash_build_kernel<<<(G - g_begin) * nb, 256, 0, st>>>(d_uk.p, d_ht.p, set->ukmer, set->ustart, set->htab, g_begin, nb); count_launch(ctx);
   SK_CUDA(cudaStreamSynchronize(st));
   return SK_OK;
 }
@@ -537,8 +556,9 @@ int build_views(sk_ctx* ctx, sk_sketch_set* set, uint64_t* d_marker_raw, const u
       SK_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys.p, skmer.p, vals.p, perm.p, (int)S, 0, (int)(kbits + gbits), st));
     }
     count_launch(ctx);
-    kview_gather_kernel<<<dim3(G, 8), 256, 0, st>>>(d_seed_off.p, skmer.p, perm.p, set->pv_pos, set->pv_cc, set->kv_pos,
-                                           set->kv_cc, head.p, ibits); count_launch(ctx);
+    const uint32_t gshift = ibits + kbits;                                          // sort key >> gshift = genome
+    kview_gather_kernel<<<div_up(S, 256), 256, 0, st>>>(d_seed_off.p, skmer.p, perm.p, set->pv_pos, set->pv_cc, set->kv_pos,
+                                                        set->kv_cc, head.p, ibits, gshift, (uint32_t)S); count_launch(ctx);
     SK_TRY(scan_exclusive<uint32_t>(ctx, head.p, hscan.p, S));
     // per-genome group offsets (+ the total in the last slot) -> host, asynchronously
     DTmp<uint64_t> d_ukoff;
@@ -547,8 +567,10 @@ int build_views(sk_ctx* ctx, sk_sketch_set* set, uint64_t* d_marker_raw, const u
     SK_CUDA(cudaMemcpyAsync(h_ukoff, d_ukoff.p, (size_t)(G + 1) * 8, cudaMemcpyDeviceToHost, st));
     SK_CUDA(ctx->arena.alloc((void**)&set->ukmer, S * 4));                       // upper bound: distinct k-mers <= records
     SK_CUDA(ctx->arena.alloc((void**)&set->ustart, (size_t)(S + G + 1) * 4));
-    groups_kernel<<<dim3(G, 8), 256, 0, st>>>(d_seed_off.p, skmer.p, kmask, head.p, hscan.p, G, set->ukmer, set->ustart, ibits); count_launch(ctx);
-    mult_kernel<<<dim3(G, 8), 256, 0, st>>>(d_seed_off.p, head.p, hscan.p, perm.p, set->ustart, set->pv_mult, skmer.p, ibits); count_launch(ctx);
+    groups_kernel<<<div_up(std::max<uint64_t>(S, G), 256), 256, 0, st>>>(d_seed_off.p, skmer.p, kmask, head.p, hscan.p, G, set->ukmer,
+                                                                         set->ustart, ibits, gshift, (uint32_t)S); count_launch(ctx);
+    mult_kernel<<<div_up(S, 256), 256, 0, st>>>(d_seed_off.p, head.p, hscan.p, perm.p, set->ustart, set->pv_mult, skmer.p, ibits, gshift,
+                                                (uint32_t)S); count_launch(ctx);
   } else {
     set->U = 0;
     SK_CUDA(ctx->arena.alloc((void**)&set->ukmer, 4));
