@@ -241,6 +241,26 @@ void sk_chain_debug_free(sk_chain_debug* d);
  * 0 (no estimate), 1 (estimate) or 3 (estimate, the putative-ANI filter applied). */
 int sk_debug_chunk_estimate(sk_ctx* ctx, uint64_t n, const uint32_t* inputs, uint32_t c, uint32_t k, double* est,
                             uint32_t* weight, uint32_t* valid);
+/* (test use) the chain back end's DP and interval selection on given anchors (host arrays).  Pair p owns the chunks
+ * pair_chunk_off[p] .. pair_chunk_off[p + 1], chunk i the anchors chunk_anchor_off[i] .. chunk_anchor_off[i + 1] (both offset
+ * arrays start at 0), 5 x u32 per anchor as in sk_chain_debug.  A chunk holds at least one anchor, all of one query contig,
+ * sorted by (query_pos, ref_contig, ref_pos, reverse) as the chunking kernel emits them; ref contigs are < 2^30 and positions
+ * < 2^32 - 65536; anything else is refused (SK_ERR_PARAM with a message).  The workspace is filled as sk_chain_pairs' chunking
+ * leaves it (interval capacity floor(anchors / 3) per pair), and the DP instantiation sk_chain_pairs chooses for c (with the
+ * same SK_DP_* environment hooks) and the interval selection run on it.  out[p] receives anchors, chunk_first, score,
+ * pointer, the sorted intervals with kept flags and chunk_stats, whose first five fields are the selection's per-chunk sums
+ * (the seed counts are 0, result and ests are empty); pair_sums[2p] / [2p + 1] = the kept intervals' summed
+ * (q1 - q0) + 2c + k (wrapping) and their number.  switched[p] != 0: tbcq sums ref spans.  At most 65535 pairs. */
+int sk_debug_chain_anchors(sk_ctx* ctx, uint32_t c, uint32_t k, uint64_t n_pairs, const uint64_t* pair_chunk_off,
+                           const uint64_t* chunk_anchor_off, const uint32_t* anchors, const uint32_t* switched,
+                           sk_chain_debug* out /* n_pairs */, uint32_t* pair_sums /* 2 x n_pairs */);
+/* (test use) the interval selection alone on given intervals: pair p owns intervals pair_iv_off[p] .. pair_iv_off[p + 1]
+ * (10 x i64: score, num_anchors, q0, q1, r0, r1, ref_contig, query_contig, chunk, reverse; any order; q0 < q1, r0 < r1,
+ * chunk < pair_chunks[p], 0 <= score < 2^31, other fields u32) and pair_chunks[p] chunks; the interval capacity is the list's
+ * length.  Outputs as sk_debug_chain_anchors, without anchors. */
+int sk_debug_select_intervals(sk_ctx* ctx, uint32_t c, uint32_t k, uint64_t n_pairs, const uint64_t* pair_iv_off,
+                              const int64_t* intervals, const uint32_t* pair_chunks, const uint32_t* switched,
+                              sk_chain_debug* out /* n_pairs */, uint32_t* pair_sums /* 2 x n_pairs */);
 
 /* ---- whole triangle (src/triangle.rs:13-105: sketch -> screen -> chain -> keep ani > 0.1) from HOST sequence
  *      buffers; results malloc'd (sk_free).  Timing breakdown (seconds, device events) optional. -------------- */

@@ -280,6 +280,78 @@ void orc_debug_ests(void* dd, double* est, uint64_t* weight) {
   for (size_t i = 0; i < d.ani_ests.size(); i++) { est[i] = d.ani_ests[i].first; weight[i] = d.ani_ests[i].second; }
 }
 
+// ---- DP and interval selection on given lists ----------------------------------------------------------------------------
+// Shared tail of orc_chain_chunks / orc_select_intervals: the selection of chain.rs:1008-1099 over `good`, written out as
+// 11 x i64 per sorted interval (the orc_debug_intervals fields) plus 2 x u32 hits (ref, query: kept intervals overlapping
+// it), 5 x u32 per chunk (total_anchors, rq0, rq1, tbcq, n_int of the kept intervals, chain.rs:204-237) and the pair's
+// 2 x u32 (summed chain length, number of chains: avg_chain_int_len's terms, chain.rs:244-249).
+static void select_out(std::vector<ChainInterval>& good, uint64_t n_chunks, uint32_t c, uint32_t k, int switched,
+                       int64_t* iv_out, uint32_t* hits, uint32_t* chunk_acc, uint32_t* pair_sums) {
+  std::vector<uint8_t> kept;
+  std::vector<uint32_t> h;
+  auto per_chunk = get_nonoverlapping_chains(good, n_chunks, &kept, &h);
+  for (size_t i = 0; i < good.size(); i++) {
+    const ChainInterval& x = good[i];
+    int64_t* o = iv_out + 11 * i;
+    o[0] = (int64_t)x.score; o[1] = (int64_t)x.num_anchors; o[2] = x.q0; o[3] = x.q1; o[4] = x.r0; o[5] = x.r1;
+    o[6] = (int64_t)x.ref_contig; o[7] = (int64_t)x.query_contig; o[8] = (int64_t)x.chunk_id; o[9] = x.reverse_chain;
+    o[10] = kept[i];
+    hits[2 * i] = h[2 * i]; hits[2 * i + 1] = h[2 * i + 1];
+  }
+  for (uint64_t ch = 0; ch < n_chunks; ch++) {
+    const ChunkStats s = chunk_stats(per_chunk[ch], {}, c, k, MIN_LENGTH_COVER, switched != 0);
+    const uint32_t row[5] = {(uint32_t)s.total_anchors, s.rq0, s.rq1, s.tbcq, s.n_int};
+    memcpy(chunk_acc + 5 * ch, row, sizeof(row));
+  }
+  chain_len_sums(per_chunk, c, k, pair_sums, pair_sums + 1);
+}
+
+static MapParams unit_map_params(uint32_t c, uint32_t k) {
+  Sketch unit;
+  unit.c = c; unit.k = k;
+  return map_params_from_sketch(unit, CommandParams(), -1);
+}
+
+// One pair's chunks: chunk i holds anchors chunk_off[i] .. chunk_off[i + 1] of a5 (5 x u32 per anchor: query_contig,
+// query_pos, ref_contig, ref_pos, reverse), each chunk sorted as get_anchors leaves it.  Per anchor: score (i64) and
+// chunk-local pointer; the sorted intervals go to iv_out / hits (capacity: n_anchors / 3 intervals), *n_iv = their number;
+// the rest as select_out.
+int orc_chain_chunks(uint32_t c, uint32_t k, int switched, uint64_t n_chunks, const uint64_t* chunk_off, const uint32_t* a5,
+                     int64_t* score, uint32_t* pointer, int64_t* iv_out, uint32_t* hits, uint64_t* n_iv, uint32_t* chunk_acc,
+                     uint32_t* pair_sums) {
+  const MapParams mp = unit_map_params(c, k);
+  std::vector<std::vector<Anchor>> chunks(n_chunks);
+  for (uint64_t ch = 0; ch < n_chunks; ch++)
+    for (uint64_t i = chunk_off[ch]; i < chunk_off[ch + 1]; i++) {
+      const uint32_t* x = a5 + 5 * i;
+      chunks[ch].push_back(Anchor{x[0], x[1], x[2], x[3], x[4] != 0});
+    }
+  std::vector<double> sc;
+  std::vector<uint32_t> ptr;
+  std::vector<ChainInterval> good = chain_chunks(chunks, mp, &sc, &ptr);
+  for (size_t i = 0; i < sc.size(); i++) { score[i] = (int64_t)sc[i]; pointer[i] = ptr[i]; }
+  *n_iv = good.size();
+  select_out(good, n_chunks, c, k, switched, iv_out, hits, chunk_acc, pair_sums);
+  return 0;
+}
+
+// The selection alone on n given intervals, 10 x i64 each (the orc_debug_intervals fields without `kept`), chunk ids below
+// n_chunks; outputs as orc_chain_chunks (n intervals).
+int orc_select_intervals(uint32_t c, uint32_t k, int switched, uint64_t n_chunks, uint64_t n, const int64_t* iv_in,
+                         int64_t* iv_out, uint32_t* hits, uint32_t* chunk_acc, uint32_t* pair_sums) {
+  std::vector<ChainInterval> good(n);
+  for (uint64_t i = 0; i < n; i++) {
+    const int64_t* x = iv_in + 10 * i;
+    ChainInterval& v = good[i];
+    v.score = (double)x[0]; v.num_anchors = (size_t)x[1];
+    v.q0 = (uint32_t)x[2]; v.q1 = (uint32_t)x[3]; v.r0 = (uint32_t)x[4]; v.r1 = (uint32_t)x[5];
+    v.ref_contig = (size_t)x[6]; v.query_contig = (size_t)x[7]; v.chunk_id = (size_t)x[8]; v.reverse_chain = x[9] != 0;
+    v.overlap = 0;
+  }
+  select_out(good, n_chunks, c, k, switched, iv_out, hits, chunk_acc, pair_sums);
+  return 0;
+}
+
 float orc_gbdt_predict(int model, const float* x) { return gbdt_predict(model, x); }
 
 // final_estimate on a sorted (est, weight) list of n entries; quant_q / quant_r = {q10, q50, q90}; model -1 none, 0 C125,

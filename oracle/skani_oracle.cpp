@@ -791,11 +791,12 @@ static inline double score_anchors(const Anchor& cur, const Anchor& past, const 
   return mp.anchor_score - gap;
 }
 
-static std::vector<ChainingResult> chain_anchors_ani(const AnchorChunks& ac, const MapParams& mp) {  // chain.rs:838-896
+static std::vector<ChainingResult> chain_anchors_ani(const std::vector<std::vector<Anchor>>& chunks,
+                                                     const MapParams& mp) {  // chain.rs:838-896
   std::vector<ChainingResult> res;
   const double NEG = std::numeric_limits<double>::lowest();
   uint32_t past_chain_length = std::min<uint32_t>(mp.fragment_length / 2, mp.bp_chain_band);  // :842
-  for (const auto& chunk : ac.chunks) {
+  for (const auto& chunk : chunks) {
     ChainingResult cr;
     size_t n = chunk.size();
     cr.pointer_vec.assign(n, 0);
@@ -873,14 +874,15 @@ static inline int cmp_interval(const ChainInterval& x, const ChainInterval& y) {
   return 0;
 }
 
-static std::vector<std::vector<ChainInterval>> get_nonoverlapping_chains(std::vector<ChainInterval>& intervals,
-                                                                         size_t num_chunks, std::vector<uint8_t>* kept) {
+std::vector<std::vector<ChainInterval>> get_nonoverlapping_chains(std::vector<ChainInterval>& intervals, size_t num_chunks,
+                                                                  std::vector<uint8_t>* kept, std::vector<uint32_t>* hits_out) {
   // chain.rs:1008-1099.  bio IntervalTree (half-open overlap query) is restated as per-contig lists.
   std::stable_sort(intervals.begin(), intervals.end(),
                    [](const ChainInterval& a, const ChainInterval& b) { return cmp_interval(b, a) < 0; });  // :1012 descending
   std::unordered_map<size_t, std::vector<size_t>> tree_q, tree_r;
   std::vector<std::vector<ChainInterval>> good(num_chunks);
   if (kept) kept->assign(intervals.size(), 0);
+  if (hits_out) hits_out->assign(2 * intervals.size(), 0);
   for (size_t i = 0; i < intervals.size(); i++) {
     const ChainInterval& it = intervals[i];
     auto& tr = tree_r[it.ref_contig];
@@ -895,6 +897,7 @@ static std::vector<std::vector<ChainInterval>> get_nonoverlapping_chains(std::ve
         sum_r += std::min(it.r1 - ol.r0, ol.r1 - it.r0);  // :1034-1038
       }
     }
+    if (hits_out) (*hits_out)[2 * i] = (uint32_t)hits;
     if (hits == 0) no_overlap_ref = true;
     else no_overlap_ref = ((float)sum_r < (float)(it.r1 - it.r0) * OVERLAP_ORTHOLOGOUS_FRACTION);  // :1042
     hits = 0;
@@ -905,6 +908,7 @@ static std::vector<std::vector<ChainInterval>> get_nonoverlapping_chains(std::ve
         sum_q += std::min(it.q1 - ol.q0, ol.q1 - it.q0);  // :1064-1068
       }
     }
+    if (hits_out) (*hits_out)[2 * i + 1] = (uint32_t)hits;
     if (hits == 0) no_overlap_query = true;
     else no_overlap_query = ((float)sum_q < (float)(it.q1 - it.q0) * OVERLAP_ORTHOLOGOUS_FRACTION);  // :1072
     if (no_overlap_ref && no_overlap_query) {
@@ -1095,6 +1099,26 @@ ChunkStats chunk_stats(const std::vector<ChainInterval>& intervals, const std::v
   return s;
 }
 
+std::vector<ChainInterval> chain_chunks(const std::vector<std::vector<Anchor>>& chunks, const MapParams& mp,
+                                        std::vector<double>* score, std::vector<uint32_t>* pointer) {  // chain.rs:151-153
+  std::vector<ChainingResult> crs = chain_anchors_ani(chunks, mp);
+  std::vector<ChainInterval> good;
+  for (size_t i = 0; i < chunks.size(); i++) {
+    get_chain_intervals(good, crs[i], chunks[i], mp, i);
+    if (score) score->insert(score->end(), crs[i].score_vec.begin(), crs[i].score_vec.end());
+    if (pointer) for (size_t p : crs[i].pointer_vec) pointer->push_back((uint32_t)p);
+  }
+  return good;
+}
+
+void chain_len_sums(const std::vector<std::vector<ChainInterval>>& int_chunks, uint32_t c, size_t k, uint32_t* sum,
+                    uint32_t* n) {  // chain.rs:244-249
+  uint32_t s = 0, m = 0;
+  for (const auto& v : int_chunks)
+    for (const auto& in : v) { s += (in.q1 - in.q0) - in.overlap + 2 * c + (uint32_t)k; m += 1; }
+  *sum = s; *n = m;
+}
+
 static AniEstResult calculate_ani(const std::vector<std::vector<ChainInterval>>& int_chunks, const Sketch& ref_sketch,
                                   const Sketch& query_sketch, const AnchorChunks& ac, const MapParams& mp, bool switched,
                                   ChainDebug* dbg) {  // chain.rs:173-555
@@ -1104,13 +1128,9 @@ static AniEstResult calculate_ani(const std::vector<std::vector<ChainInterval>>&
   const bool sensitive_af = c < 200;
   uint32_t total_query_bases = 0, total_ref_range = 0;
   uint32_t avg_chain_int_len = 0, num_chains = 0;
+  chain_len_sums(int_chunks, c, k, &avg_chain_int_len, &num_chains);  // :249
+  if (sensitive_af) total_query_bases = total_ref_range = avg_chain_int_len;  // :244-247 add the same terms
   for (size_t i = 0; i < int_chunks.size(); i++) {
-    for (const auto& in : int_chunks[i]) {
-      uint32_t add = (in.q1 - in.q0) - in.overlap + 2 * c + (uint32_t)k;
-      if (sensitive_af) { total_query_bases += add; total_ref_range += add; }  // :244-247
-      avg_chain_int_len += add;  // :249
-      num_chains += 1;
-    }
     const ChunkStats cs = chunk_stats(int_chunks[i], ac.seeds_in_chunk[i], c, k, mp.min_length_cover, switched);
     if (dbg) {
       const uint32_t row[9] = {(uint32_t)cs.total_anchors, cs.rq0, cs.rq1, cs.tbcq, cs.n_int, (uint32_t)cs.n_seeds,
@@ -1149,9 +1169,7 @@ static AniEstResult calculate_ani(const std::vector<std::vector<ChainInterval>>&
 AniEstResult chain_seeds(const Sketch& ref, const Sketch& query, const MapParams& mp, ChainDebug* dbg) {  // chain.rs:144-171
   AnchorChunks ac;
   bool switched = get_anchors(ref, query, mp, ac, dbg ? &dbg->anchors : nullptr);
-  std::vector<ChainingResult> crs = chain_anchors_ani(ac, mp);
-  std::vector<ChainInterval> good;
-  for (size_t i = 0; i < ac.chunks.size(); i++) get_chain_intervals(good, crs[i], ac.chunks[i], mp, i);
+  std::vector<ChainInterval> good = chain_chunks(ac.chunks, mp, dbg ? &dbg->score : nullptr, dbg ? &dbg->pointer : nullptr);
   std::vector<uint8_t> kept;
   auto good_chunks = get_nonoverlapping_chains(good, ac.chunks.size(), dbg ? &kept : nullptr);
   if (dbg) {
@@ -1160,10 +1178,6 @@ AniEstResult chain_seeds(const Sketch& ref, const Sketch& query, const MapParams
     for (size_t i = 0; i < ac.chunks.size(); i++) {
       dbg->chunk_first.push_back(off);
       dbg->chunk_nseeds.push_back((uint32_t)ac.seeds_in_chunk[i].size());
-      for (size_t a = 0; a < ac.chunks[i].size(); a++) {
-        dbg->score.push_back(crs[i].score_vec[a]);
-        dbg->pointer.push_back((uint32_t)crs[i].pointer_vec[a]);
-      }
       off += (uint32_t)ac.chunks[i].size();
     }
     dbg->chunk_first.push_back(off);

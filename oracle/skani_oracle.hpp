@@ -213,6 +213,22 @@ void chunk_estimate(ChunkStats& s, uint32_t c, size_t k, uint32_t min_length_cov
 ChunkStats chunk_stats(const std::vector<ChainInterval>& intervals, const std::vector<uint32_t>& seeds, uint32_t c, size_t k,
                        uint32_t min_length_cover, bool switched);
 
+// chain_anchors_ani + get_chain_intervals (chain.rs:838-1007) on given chunks, each sorted as get_anchors leaves it
+// (chain.rs:721): the chain intervals of every chunk (chunk_id = its index) in emission order, and optionally the DP's score
+// and chunk-local pointer of every anchor, chunk after chunk
+std::vector<ChainInterval> chain_chunks(const std::vector<std::vector<Anchor>>& chunks, const MapParams& mp,
+                                        std::vector<double>* score = nullptr, std::vector<uint32_t>* pointer = nullptr);
+// get_nonoverlapping_chains (chain.rs:1008-1099): sorts `intervals` into the descending order of :1012 and returns the kept
+// ones per chunk.  Optionally per sorted interval: kept (0 / 1), and hits = 2 per interval, the number of kept intervals its
+// ref / query range overlaps (the IntervalTree::find counts of :1029, :1059)
+std::vector<std::vector<ChainInterval>> get_nonoverlapping_chains(std::vector<ChainInterval>& intervals, size_t num_chunks,
+                                                                  std::vector<uint8_t>* kept = nullptr,
+                                                                  std::vector<uint32_t>* hits = nullptr);
+// the kept intervals' summed (q1 - q0) - overlap + 2c + k (wrapping u32) and their number: avg_chain_int_len = sum / n
+// (chain.rs:244-249, :421)
+void chain_len_sums(const std::vector<std::vector<ChainInterval>>& int_chunks, uint32_t c, size_t k, uint32_t* sum,
+                    uint32_t* n);
+
 int get_model_id(uint64_t c, bool learned_ani);  // regression.rs:12-28
 MapParams map_params_from_sketch(const Sketch& ref, const CommandParams& cp, int model);  // chain.rs:88-142
 AniEstResult chain_seeds(const Sketch& ref, const Sketch& query, const MapParams& mp, ChainDebug* dbg = nullptr);  // chain.rs:144-171

@@ -86,6 +86,8 @@ SYMBOLS = [
     ("sk_chain_pairs_debug", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp]),
     ("sk_chain_debug_free", None, [PP(ChainDebug)]),
     ("sk_debug_chunk_estimate", i32, [vp, u64, vp, u32, u32, vp, vp, vp]),
+    ("sk_debug_chain_anchors", i32, [vp, u32, u32, u64, vp, vp, vp, vp, vp, vp]),
+    ("sk_debug_select_intervals", i32, [vp, u32, u32, u64, vp, vp, vp, vp, vp, vp]),
     ("sk_triangle", i32, [vp, vp, vp, u32, vp, u32, PP(SketchParams), PP(MapParams), PP(PP(AniResult)), PP(u64),
                           PP(TriangleStats)]),
     ("sk_triangle_local", i32, [vp, vp, vp, u32, vp, u32, PP(SketchParams), PP(MapParams), vp, PP(PP(AniResult)), PP(u64),

@@ -1488,6 +1488,49 @@ static int launch_dp_group(sk_ctx* ctx, uint32_t grid, uint64_t TC, const ChainP
   return SK_OK;
 }
 
+// The chain back end's DP and interval selection on the workspace as chunk_compact_kernel / init_chunk_acc_kernel leave it
+// (TC > 0 chunks of B pairs): the DP instantiation the band (and the SK_DP_* A/B hooks) choose, then select_kernel.  run_batch
+// and the test entries sk_debug_chain_anchors (dp) / sk_debug_select_intervals (!dp, intervals given) all launch through here.
+// taps: the DP also stores the per-anchor scores and pointers.
+static int launch_dp_select(sk_ctx* ctx, ChainScratch& S, uint32_t B, uint64_t TC, const ChainParams& prm, bool dp, bool taps) {
+  cudaStream_t st = ctx->stream;
+  Workspace& ws = S.ws;
+  if (dp) {
+    const uint32_t grid = (uint32_t)TC;
+    const uint32_t nb = prm.band / 32 + 2;   // register sets per lane: current block + ceil(band / 32) earlier ones
+#define DP_LAUNCH(NBV)                                                                                       \
+  if (taps) SK_LAUNCH(ctx, "dp_kernel", (dp_warp_kernel<NBV, true><<<grid, 32, 0, st>>>(TC, prm, ws)));       \
+  else SK_LAUNCH(ctx, "dp_kernel", (dp_warp_kernel<NBV, false><<<grid, 32, 0, st>>>(TC, prm, ws)));
+    if (prm.band <= 24 && getenv("SK_DP_WARP") == nullptr) {   // 4 chunks per warp, 8 lanes each
+      const int dp_gl = getenv("SK_DP_GL") ? atoi(getenv("SK_DP_GL")) : 4;   // lanes per chunk: 4 (default, faster in A/B runs) or 8
+      const int dp_minb = getenv("SK_DP_MINB") ? atoi(getenv("SK_DP_MINB")) : 25;   // register cap: 72 registers = 28 resident warps per SM (A/B: 1 = uncapped)
+      const uint32_t gw = dp_gl == 4 ? 8 : 4;
+      const uint32_t g4 = (uint32_t)((TC + gw - 1) / gw);
+      // group chunks of similar size: sort chunk ids by descending anchor count (cub radix sort, ~0.1 ms per batch)
+      SK_TRY(ensure(ctx, &ws.chunk_size, &S.c_chunk_size, TC)); SK_TRY(ensure(ctx, &ws.chunk_size_sorted, &S.c_chunk_size_sorted, TC));
+      SK_TRY(ensure(ctx, &ws.chunk_id, &S.c_chunk_id, TC)); SK_TRY(ensure(ctx, &ws.chunk_perm, &S.c_chunk_perm, TC));
+      chunk_size_kernel<<<(uint32_t)((TC + 255) / 256), 256, 0, st>>>(TC, ws); count_launch(ctx);
+      size_t tb = 0;
+      SK_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, (int)TC, 0, 32, st));
+      SK_TRY(ensure(ctx, &S.sort_tmp, &S.c_sort_tmp, tb));
+      SK_CUDA(cub::DeviceRadixSort::SortPairsDescending(S.sort_tmp, tb, ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, (int)TC, 0, 32, st));
+      // the debug taps run the instantiation production runs, with the score / pointer stores as the only difference
+#define DPG(GLV, NEV)                                                                                                   \
+  {                                                                                                                    \
+    if (taps) SK_TRY((launch_dp_group<true, GLV, NEV>(ctx, g4, TC, prm, ws, dp_minb)));                                \
+    else SK_TRY((launch_dp_group<false, GLV, NEV>(ctx, g4, TC, prm, ws, dp_minb)));                                   \
+  }
+      if (dp_gl == 4) { if (prm.band <= 20) DPG(4, 5) else DPG(4, 6) }
+      else { DPG(8, 3) }
+#undef DPG
+    } else if (nb <= 2) { DP_LAUNCH(2) } else if (nb <= 4) { DP_LAUNCH(4) } else if (nb <= 8) { DP_LAUNCH(8) }
+    else if (nb <= 16) { DP_LAUNCH(16) } else { ctx->err = "c too small: chain band > 479 anchors is not supported"; return SK_ERR_PARAM; }
+#undef DP_LAUNCH
+  }
+  SK_LAUNCH(ctx, "select_kernel", (select_kernel<<<B, CT, 0, st>>>(S.d_pairs, prm, ws)));
+  return SK_OK;
+}
+
 // Copies the intermediate products of every pair of the batch out of the batch arrays: pair i's anchors at pairAbase[i],
 // its chunks at pairCbase[i], its intervals at pairIbase[i] (pair_nint[i] of them, sorted order at iv_order + 4 ib + npow2,
 // kept flags at iv_kept + ib, both indexed by the pair-local interval index).  dbg[b0 + i] receives pair b0 + i.
@@ -1668,39 +1711,7 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
     SK_CUDA(h2d_small(ctx, ws.chunk_first + TC, &TA, 8));
     SK_LAUNCH(ctx, "chunk_compact_kernel", (chunk_compact_kernel<<<B, CT, 0, st>>>(S.d_pairs, ws)));
     init_chunk_acc_kernel<<<(uint32_t)((TC + 255) / 256), 256, 0, st>>>(TC, ws); count_launch(ctx);
-    {
-      const uint32_t grid = (uint32_t)TC;
-      const uint32_t nb = prm.band / 32 + 2;   // register sets per lane: current block + ceil(band / 32) earlier ones
-#define DP_LAUNCH(NBV)                                                                                       \
-  if (dbg) SK_LAUNCH(ctx, "dp_kernel", (dp_warp_kernel<NBV, true><<<grid, 32, 0, st>>>(TC, prm, ws)));       \
-  else SK_LAUNCH(ctx, "dp_kernel", (dp_warp_kernel<NBV, false><<<grid, 32, 0, st>>>(TC, prm, ws)));
-      if (prm.band <= 24 && getenv("SK_DP_WARP") == nullptr) {   // 4 chunks per warp, 8 lanes each
-        const int dp_gl = getenv("SK_DP_GL") ? atoi(getenv("SK_DP_GL")) : 4;   // lanes per chunk: 4 (default, faster in A/B runs) or 8
-        const int dp_minb = getenv("SK_DP_MINB") ? atoi(getenv("SK_DP_MINB")) : 25;   // register cap: 72 registers = 28 resident warps per SM (A/B: 1 = uncapped)
-        const uint32_t gw = dp_gl == 4 ? 8 : 4;
-        const uint32_t g4 = (uint32_t)((TC + gw - 1) / gw);
-        // group chunks of similar size: sort chunk ids by descending anchor count (cub radix sort, ~0.1 ms per batch)
-        SK_TRY(ensure(ctx, &ws.chunk_size, &S.c_chunk_size, TC)); SK_TRY(ensure(ctx, &ws.chunk_size_sorted, &S.c_chunk_size_sorted, TC));
-        SK_TRY(ensure(ctx, &ws.chunk_id, &S.c_chunk_id, TC)); SK_TRY(ensure(ctx, &ws.chunk_perm, &S.c_chunk_perm, TC));
-        chunk_size_kernel<<<(uint32_t)((TC + 255) / 256), 256, 0, st>>>(TC, ws); count_launch(ctx);
-        size_t tb = 0;
-        SK_CUDA(cub::DeviceRadixSort::SortPairsDescending(nullptr, tb, ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, (int)TC, 0, 32, st));
-        SK_TRY(ensure(ctx, &S.sort_tmp, &S.c_sort_tmp, tb));
-        SK_CUDA(cub::DeviceRadixSort::SortPairsDescending(S.sort_tmp, tb, ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, (int)TC, 0, 32, st));
-        // the debug taps run the instantiation production runs, with the score / pointer stores as the only difference
-#define DPG(GLV, NEV)                                                                                                   \
-  {                                                                                                                    \
-    if (dbg) SK_TRY((launch_dp_group<true, GLV, NEV>(ctx, g4, TC, prm, ws, dp_minb)));                                \
-    else SK_TRY((launch_dp_group<false, GLV, NEV>(ctx, g4, TC, prm, ws, dp_minb)));                                   \
-  }
-        if (dp_gl == 4) { if (prm.band <= 20) DPG(4, 5) else DPG(4, 6) }
-        else { DPG(8, 3) }
-#undef DPG
-      } else if (nb <= 2) { DP_LAUNCH(2) } else if (nb <= 4) { DP_LAUNCH(4) } else if (nb <= 8) { DP_LAUNCH(8) }
-      else if (nb <= 16) { DP_LAUNCH(16) } else { ctx->err = "c too small: chain band > 479 anchors is not supported"; return SK_ERR_PARAM; }
-#undef DP_LAUNCH
-    }
-    SK_LAUNCH(ctx, "select_kernel", (select_kernel<<<B, CT, 0, st>>>(S.d_pairs, prm, ws)));
+    SK_TRY(launch_dp_select(ctx, S, B, TC, prm, true, dbg != nullptr));
     SK_LAUNCH(ctx, "chunkstat_kernel", (chunkstat_kernel<<<(uint32_t)((TC + CS_WARPS * CS_PER_WARP - 1) / (CS_WARPS * CS_PER_WARP)), CS_WARPS * 32, 0, st>>>(TC, S.d_pairs, v0, v1, S.d_m0, S.d_m1, prm, ws, dbg_counts)));
   }
   // test hook: SK_FINAL_FORCE_REDO=1 takes the sequential bootstrap redo for every pair, as if some draw had been rejected
@@ -1713,6 +1724,90 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
 
   if (dbg) SK_TRY(copy_out_debug(ctx, ws, descs, b0, B, abase, cbase, ibase, dbg_counts, host_out, dbg));
   return SK_OK;
+}
+
+static ChainScratch& chain_scratch(sk_ctx* ctx) {
+  if (!ctx->chain_scratch) {
+    ctx->chain_scratch = new ChainScratch();
+    ctx->chain_scratch_free = [](void* p) { ((ChainScratch*)p)->free_all(); delete (ChainScratch*)p; };
+  }
+  return *(ChainScratch*)ctx->chain_scratch;   // grow-only device buffers, reused by every call on this context
+}
+
+// Test entries: the workspace of B pairs filled from host lists the way chunk_anchor_kernel / chunk_compact_kernel (anchors,
+// chunk descriptors, pair bases; h_anc non-empty) or the DP (intervals and their counts; h_iv non-empty) leave it, then
+// launch_dp_select and copy_out_debug as a debug run of run_batch.  cbase / abase / ibase: per-pair exclusive prefixes (B + 1).
+static int debug_dp_select(sk_ctx* ctx, uint32_t c, uint32_t k, const uint32_t* switched, const std::vector<uint64_t>& cbase,
+                           const std::vector<uint64_t>& abase, const std::vector<uint64_t>& ibase, const std::vector<AnchorRec>& h_anc,
+                           const std::vector<uint64_t>& h_first, const std::vector<uint32_t>& h_qctg,
+                           const std::vector<IntervalKey>& h_iv, const std::vector<uint32_t>& h_nint, bool dp, sk_chain_debug* out,
+                           uint32_t* pair_sums) {
+  SK_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const uint32_t B = (uint32_t)(cbase.size() - 1);
+  ChainParams prm{};
+  prm.c = c; prm.k = k; prm.band = BP_CHAIN_BAND / c; prm.model = -1;
+  if (prm.band / 32 + 2 > 16) { ctx->err = "c too small: chain band > 479 anchors is not supported"; return SK_ERR_PARAM; }
+  ChainScratch& S = chain_scratch(ctx);
+  Workspace& ws = S.ws;
+  const uint64_t TA = abase[B], TC = cbase[B], TI = ibase[B];
+  const size_t NA = std::max<uint64_t>(TA, 1), NCH = std::max<uint64_t>(TC, 1), NI = std::max<uint64_t>(TI, 1);
+#define ENS(field, capf, n) SK_TRY(ensure(ctx, &ws.field, &S.capf, n))
+  ENS(pairCbase, c_pairCbase, B + 1); ENS(pairIbase, c_pairIbase, B + 1); ENS(pair_nint, c_pair_nint, B);
+  ENS(pair_sumlen, c_pair_sumlen, B); ENS(pair_nchains, c_pair_nchains, B);
+  ENS(anc, c_anc, NA); ENS(score, c_score, NA); ENS(ptr, c_ptr, NA); ENS(rootkey, c_rootkey, NA); ENS(depth, c_depth, NA);
+  ENS(chunk_first, c_chunk_first, NCH + 1); ENS(chunk_pair, c_chunk_pair, NCH); ENS(chunk_qctg, c_chunk_qctg, NCH);
+  ENS(acc_total, c_acc_total, NCH); ENS(acc_rq0, c_acc_rq0, NCH); ENS(acc_rq1, c_acc_rq1, NCH); ENS(acc_tbcq, c_acc_tbcq, NCH);
+  ENS(acc_nint, c_acc_nint, NCH); ENS(chunk_head, c_chunk_head, NCH); ENS(chunk_est, c_chunk_est, NCH); ENS(chunk_w, c_chunk_w, NCH);
+  ENS(chunk_valid, c_chunk_valid, NCH); ENS(chunk_nseeds, c_chunk_nseeds, NCH);
+  ENS(iv, c_iv, NI); ENS(iv_keys, c_iv_keys, 2 * NI + 8); ENS(iv_order, c_iv_order, 4 * NI + 8); ENS(iv_kept, c_iv_kept, NI);
+  ENS(iv_next, c_iv_next, NI); ENS(acc_list, c_acc_list, NI);
+#undef ENS
+  SK_TRY(ensure(ctx, &S.dbg_counts, &S.c_dbg_counts, 3 * NCH));
+  SK_TRY(ensure(ctx, &S.d_pairs, &S.c_pairs, B));
+  std::vector<PairDesc> descs(B);
+  std::vector<uint32_t> h_pair(TC);
+  for (uint32_t p = 0; p < B; p++) {
+    PairDesc& d = descs[p];
+    memset(&d, 0, sizeof(d));
+    d.switched = switched[p] ? 1 : 0; d.valid = 1;
+    for (uint64_t i = cbase[p]; i < cbase[p + 1]; i++) h_pair[i] = p;
+  }
+  SK_CUDA(cudaMemcpyAsync(S.d_pairs, descs.data(), B * sizeof(PairDesc), cudaMemcpyHostToDevice, st));
+  SK_CUDA(cudaMemcpyAsync(ws.pairCbase, cbase.data(), (B + 1) * 8, cudaMemcpyHostToDevice, st));
+  SK_CUDA(cudaMemcpyAsync(ws.pairIbase, ibase.data(), (B + 1) * 8, cudaMemcpyHostToDevice, st));
+  SK_CUDA(cudaMemsetAsync(ws.pair_sumlen, 0, B * 4, st));
+  SK_CUDA(cudaMemsetAsync(ws.pair_nchains, 0, B * 4, st));
+  if (dp) SK_CUDA(cudaMemsetAsync(ws.pair_nint, 0, B * 4, st));
+  else SK_CUDA(cudaMemcpyAsync(ws.pair_nint, h_nint.data(), B * 4, cudaMemcpyHostToDevice, st));
+  if (TA) {
+    SK_CUDA(cudaMemcpyAsync(ws.anc, h_anc.data(), TA * sizeof(AnchorRec), cudaMemcpyHostToDevice, st));
+    SK_CUDA(cudaMemsetAsync(ws.score, 0, TA * 4, st));
+    SK_CUDA(cudaMemsetAsync(ws.ptr, 0, TA * 4, st));
+  }
+  SK_CUDA(cudaMemcpyAsync(ws.chunk_first, h_first.data(), (TC + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (TC) {
+    SK_CUDA(cudaMemcpyAsync(ws.chunk_pair, h_pair.data(), TC * 4, cudaMemcpyHostToDevice, st));
+    SK_CUDA(cudaMemcpyAsync(ws.chunk_qctg, h_qctg.data(), TC * 4, cudaMemcpyHostToDevice, st));
+    // no seeds here: chunkstat_kernel's outputs, which copy_out_debug also reads, are zero
+    SK_CUDA(cudaMemsetAsync(ws.chunk_nseeds, 0, TC * 4, st));
+    SK_CUDA(cudaMemsetAsync(ws.chunk_valid, 0, TC, st));
+    SK_CUDA(cudaMemsetAsync(S.dbg_counts, 0, TC * 12, st));
+  }
+  if (TI && !dp) SK_CUDA(cudaMemcpyAsync(ws.iv, h_iv.data(), TI * sizeof(IntervalKey), cudaMemcpyHostToDevice, st));
+  if (TC) {
+    init_chunk_acc_kernel<<<(uint32_t)((TC + 255) / 256), 256, 0, st>>>(TC, ws); count_launch(ctx);
+    SK_TRY(launch_dp_select(ctx, S, B, TC, prm, dp, true));
+  }
+  std::vector<sk_ani_result> res(B);
+  memset(res.data(), 0, B * sizeof(sk_ani_result));
+  std::vector<uint32_t> sl(B), nc(B);
+  SK_CUDA(cudaMemcpyAsync(sl.data(), ws.pair_sumlen, B * 4, cudaMemcpyDeviceToHost, st));
+  SK_CUDA(cudaMemcpyAsync(nc.data(), ws.pair_nchains, B * 4, cudaMemcpyDeviceToHost, st));
+  SK_CUDA(cudaStreamSynchronize(st));
+  SK_CUDA(cudaGetLastError());
+  for (uint32_t p = 0; p < B; p++) { pair_sums[2 * p] = sl[p]; pair_sums[2 * p + 1] = nc[p]; }
+  return copy_out_debug(ctx, ws, descs, 0, B, abase, cbase, ibase, S.dbg_counts, res.data(), out);
 }
 
 static int chain_impl(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* qs, const uint64_t* pairs, uint64_t n_pairs,
@@ -1738,11 +1833,7 @@ static int chain_impl(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_se
   // dp_warp_kernel holds at most 16 register sets of 32 anchors (band / 32 + 2 <= 16): refused before anything is launched
   if (prm.band / 32 + 2 > 16) { ctx->err = "c too small: chain band > 479 anchors is not supported"; return SK_ERR_PARAM; }
   const bool same = (refs == qs);
-  if (!ctx->chain_scratch) {
-    ctx->chain_scratch = new ChainScratch();
-    ctx->chain_scratch_free = [](void* p) { ((ChainScratch*)p)->free_all(); delete (ChainScratch*)p; };
-  }
-  ChainScratch& S = *(ChainScratch*)ctx->chain_scratch;   // grow-only device buffers, reused by every call on this context
+  ChainScratch& S = chain_scratch(ctx);
   std::vector<GenomeMeta> m0, m1;
   build_meta(refs, m0);
   build_meta(qs, m1);
@@ -1833,6 +1924,87 @@ int sk_debug_chunk_estimate(sk_ctx* ctx, uint64_t n, const uint32_t* inputs, uin
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) { ctx->err = cudaGetErrorString(e); rc = SK_ERR_CUDA; }
   cudaFree(d_in); cudaFree(d_e); cudaFree(d_w); cudaFree(d_v);
+  return rc;
+}
+
+int sk_debug_chain_anchors(sk_ctx* ctx, uint32_t c, uint32_t k, uint64_t n_pairs, const uint64_t* pair_chunk_off,
+                           const uint64_t* chunk_anchor_off, const uint32_t* anchors, const uint32_t* switched, sk_chain_debug* out,
+                           uint32_t* pair_sums) {
+  if (!ctx || c == 0 || (n_pairs && (!pair_chunk_off || !chunk_anchor_off || !switched || !out || !pair_sums))) return SK_ERR_PARAM;
+  if (n_pairs == 0) return SK_OK;
+  if (n_pairs > 65535) { ctx->err = "debug chain: at most 65535 pairs"; return SK_ERR_PARAM; }
+  memset(out, 0, n_pairs * sizeof(*out));
+  const uint64_t TC = pair_chunk_off[n_pairs], TA = chunk_anchor_off[TC];
+  if (pair_chunk_off[0] != 0 || chunk_anchor_off[0] != 0 || (TA && !anchors)) return SK_ERR_PARAM;
+  std::vector<uint64_t> cbase(n_pairs + 1), abase(n_pairs + 1, 0), ibase(n_pairs + 1, 0), first(TC + 1);
+  std::vector<uint32_t> qctg(TC);
+  std::vector<sk::AnchorRec> anc(TA);
+  for (uint64_t p = 0; p <= n_pairs; p++) {
+    cbase[p] = pair_chunk_off[p];
+    if (p && cbase[p] < cbase[p - 1]) { ctx->err = "debug chain: pair chunk offsets decrease"; return SK_ERR_PARAM; }
+  }
+  for (uint64_t p = 0; p < n_pairs; p++) {
+    for (uint64_t ch = cbase[p]; ch < cbase[p + 1]; ch++) {
+      const uint64_t a0 = chunk_anchor_off[ch], a1 = chunk_anchor_off[ch + 1];
+      if (a1 <= a0) { ctx->err = "debug chain: every chunk holds at least one anchor"; return SK_ERR_PARAM; }
+      first[ch] = a0;
+      qctg[ch] = anchors[5 * a0];
+      for (uint64_t i = a0; i < a1; i++) {
+        const uint32_t* x = anchors + 5 * i;
+        // types.rs:135-138 (contig index < 2^30: the DP's unfilled-set sentinels are no contig) and the sketch-time position bound
+        if (x[0] != qctg[ch]) { ctx->err = "debug chain: a chunk holds one query contig"; return SK_ERR_PARAM; }
+        if (x[2] >= (1u << 30) || x[4] > 1u) { ctx->err = "debug chain: ref contig >= 2^30 or reverse flag > 1"; return SK_ERR_PARAM; }
+        if (x[1] >= 0xFFFF0000u || x[3] >= 0xFFFF0000u) { ctx->err = "debug chain: position >= 2^32 - 65536"; return SK_ERR_PARAM; }
+        if (i > a0) {   // the order chunk_anchor_kernel emits: (query_pos, ref_contig, ref_pos, reverse)
+          const uint32_t* y = x - 5;
+          const bool sorted = y[1] != x[1] ? y[1] < x[1] : y[2] != x[2] ? y[2] < x[2] : y[3] != x[3] ? y[3] < x[3] : y[4] <= x[4];
+          if (!sorted) { ctx->err = "debug chain: the anchors of a chunk are not sorted by (qpos, rctg, rpos, rev)"; return SK_ERR_PARAM; }
+        }
+        anc[i].qpos = x[1]; anc[i].rpos = x[3]; anc[i].rc = (x[2] << 1) | x[4];
+      }
+    }
+    abase[p + 1] = chunk_anchor_off[cbase[p + 1]];
+    ibase[p + 1] = ibase[p] + (abase[p + 1] - abase[p]) / 3;   // run_batch's interval capacity
+  }
+  first[TC] = TA;
+  const int rc = sk::debug_dp_select(ctx, c, k, switched, cbase, abase, ibase, anc, first, qctg, {}, {}, true, out, pair_sums);
+  if (rc != SK_OK) for (uint64_t i = 0; i < n_pairs; i++) sk_chain_debug_free(out + i);
+  return rc;
+}
+
+int sk_debug_select_intervals(sk_ctx* ctx, uint32_t c, uint32_t k, uint64_t n_pairs, const uint64_t* pair_iv_off,
+                              const int64_t* intervals, const uint32_t* pair_chunks, const uint32_t* switched, sk_chain_debug* out,
+                              uint32_t* pair_sums) {
+  if (!ctx || c == 0 || (n_pairs && (!pair_iv_off || !pair_chunks || !switched || !out || !pair_sums))) return SK_ERR_PARAM;
+  if (n_pairs == 0) return SK_OK;
+  if (n_pairs > 65535) { ctx->err = "debug select: at most 65535 pairs"; return SK_ERR_PARAM; }
+  memset(out, 0, n_pairs * sizeof(*out));
+  const uint64_t TI = pair_iv_off[n_pairs];
+  if (pair_iv_off[0] != 0 || (TI && !intervals)) return SK_ERR_PARAM;
+  std::vector<uint64_t> cbase(n_pairs + 1, 0), abase(n_pairs + 1, 0), ibase(n_pairs + 1);
+  std::vector<uint32_t> nint(n_pairs);
+  std::vector<sk::IntervalKey> iv(TI);
+  for (uint64_t p = 0; p < n_pairs; p++) {
+    cbase[p + 1] = cbase[p] + pair_chunks[p];
+    ibase[p] = pair_iv_off[p];
+    if (pair_iv_off[p + 1] < pair_iv_off[p]) { ctx->err = "debug select: pair interval offsets decrease"; return SK_ERR_PARAM; }
+    nint[p] = (uint32_t)(pair_iv_off[p + 1] - pair_iv_off[p]);
+    for (uint64_t i = pair_iv_off[p]; i < pair_iv_off[p + 1]; i++) {
+      const int64_t* x = intervals + 10 * i;
+      bool ok = x[0] >= 0 && x[0] < (1ll << 31) && x[1] >= 0 && x[1] <= 0xFFFFFFFFll && x[8] >= 0 && x[8] < (int64_t)pair_chunks[p] &&
+                (x[9] == 0 || x[9] == 1);
+      for (int f = 2; f < 8; f++) ok = ok && x[f] >= 0 && x[f] <= 0xFFFFFFFFll;
+      if (!ok) { ctx->err = "debug select: interval field out of range"; return SK_ERR_PARAM; }
+      if (!(x[2] < x[3] && x[4] < x[5])) { ctx->err = "debug select: an interval needs q0 < q1 and r0 < r1"; return SK_ERR_PARAM; }
+      iv[i] = sk::make_interval((int32_t)x[0], (uint32_t)x[1], (uint32_t)x[2], (uint32_t)x[3], (uint32_t)x[4], (uint32_t)x[5],
+                                (uint32_t)x[6], (uint32_t)x[7], (uint32_t)x[8], (uint32_t)x[9]);
+    }
+  }
+  ibase[n_pairs] = TI;
+  std::vector<uint64_t> first(cbase[n_pairs] + 1, 0);
+  const int rc = sk::debug_dp_select(ctx, c, k, switched, cbase, abase, ibase, {}, first, std::vector<uint32_t>(cbase[n_pairs], 0),
+                                     iv, nint, false, out, pair_sums);
+  if (rc != SK_OK) for (uint64_t i = 0; i < n_pairs; i++) sk_chain_debug_free(out + i);
   return rc;
 }
 

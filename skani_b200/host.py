@@ -391,6 +391,46 @@ def debug_chunk_estimate(ctx, inputs, c, k):
     return est[:n], w[:n], v[:n]
 
 
+def _debug_pairs(ctx, fn, n, args, switched):
+    sw = np.ascontiguousarray(np.broadcast_to(np.asarray(switched, np.uint32), (n,)))
+    ds = (ChainDebug * max(n, 1))()
+    sums = np.zeros((max(n, 1), 2), np.uint32)
+    ctx.check(fn(*args, sw.ctypes.data, ds, sums.ctypes.data))
+    try:
+        out = []
+        for i in range(n):
+            d = _debug_dict(ds[i])
+            d["pair_sumlen"], d["pair_nchains"] = int(sums[i, 0]), int(sums[i, 1])
+            out.append(d)
+        return out
+    finally:
+        for i in range(n):
+            ctx.L.sk_chain_debug_free(C.byref(ds[i]))
+
+
+def debug_chain_anchors(ctx, c, k, pairs, switched=0):
+    """sk_debug_chain_anchors: the production DP and interval selection on given anchors.  pairs: one list of chunks per pair,
+    each chunk an (n, 5) array of (query_contig, query_pos, ref_contig, ref_pos, reverse).  Returns one chain_pairs_debug dict
+    per pair (chunk_stats columns 0-4 = the selection's per-chunk sums) plus pair_sumlen and pair_nchains."""
+    chunks = [np.asarray(ch, np.uint32).reshape(-1, 5) for p in pairs for ch in p]
+    pco = np.zeros(len(pairs) + 1, np.uint64); pco[1:] = np.cumsum([len(p) for p in pairs])
+    cao = np.zeros(len(chunks) + 1, np.uint64); cao[1:] = np.cumsum([len(ch) for ch in chunks])
+    a = np.ascontiguousarray(np.concatenate(chunks) if chunks else np.zeros((1, 5), np.uint32))
+    return _debug_pairs(ctx, ctx.L.sk_debug_chain_anchors, len(pairs),
+                        (ctx.h, c, k, len(pairs), pco.ctypes.data, cao.ctypes.data, a.ctypes.data), switched)
+
+
+def debug_select_intervals(ctx, c, k, pairs, n_chunks, switched=0):
+    """sk_debug_select_intervals: the interval selection alone.  pairs: one (n, 10) array per pair of (score, num_anchors, q0,
+    q1, r0, r1, ref_contig, query_contig, chunk, reverse); n_chunks: chunks per pair (scalar or per pair)."""
+    ivs = [np.asarray(p, np.int64).reshape(-1, 10) for p in pairs]
+    off = np.zeros(len(pairs) + 1, np.uint64); off[1:] = np.cumsum([len(x) for x in ivs])
+    x = np.ascontiguousarray(np.concatenate(ivs) if ivs else np.zeros((1, 10), np.int64))
+    nc = np.ascontiguousarray(np.broadcast_to(np.asarray(n_chunks, np.uint32), (len(pairs),)))
+    return _debug_pairs(ctx, ctx.L.sk_debug_select_intervals, len(pairs),
+                        (ctx.h, c, k, len(pairs), off.ctypes.data, x.ctypes.data, nc.ctypes.data), switched)
+
+
 def triangle(ctx, bases, contig_off, genome_of_contig, n_genomes, sp=None, mp=None, as_array=False):
     """Whole `skani triangle` hot path from host buffers (reference src/triangle.rs:13-105)."""
     sp = sp or sketch_params(); mp = mp or map_params()

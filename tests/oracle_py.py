@@ -103,6 +103,10 @@ def lib():
     L.orc_debug_chunk_stats.argtypes = [vp] * 2
     L.orc_chunk_estimate.restype = i32
     L.orc_chunk_estimate.argtypes = [u64, vp, u32, u32, vp, vp, vp]
+    L.orc_chain_chunks.restype = i32
+    L.orc_chain_chunks.argtypes = [u32, u32, i32, u64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.orc_select_intervals.restype = i32
+    L.orc_select_intervals.argtypes = [u32, u32, i32, u64, u64, vp, vp, vp, vp, vp]
     L.orc_gbdt_predict.restype = C.c_float; L.orc_gbdt_predict.argtypes = [i32, vp]
     L.orc_final_estimate.restype = i32
     L.orc_final_estimate.argtypes = [vp, vp, u64, u32, u32, u64, u64, vp, vp, C.POINTER(OrcCmd), i32, C.POINTER(OrcResult)]
@@ -238,6 +242,42 @@ def chunk_estimate(inputs, c, k):
     est = np.zeros(max(n, 1), np.float64); w = np.zeros(max(n, 1), np.uint32); v = np.zeros(max(n, 1), np.uint32)
     lib().orc_chunk_estimate(n, x.ctypes.data, c, k, est.ctypes.data, w.ctypes.data, v.ctypes.data)
     return est[:n], w[:n], v[:n]
+
+
+def _selection(iv, hits, acc, sums):
+    return dict(intervals=iv, hits=hits, chunk_acc=acc, pair_sumlen=int(sums[0]), pair_nchains=int(sums[1]))
+
+
+def chain_chunks(chunks, c, k, switched=False):
+    """chain_anchors_ani + get_chain_intervals + get_nonoverlapping_chains on given chunks of one pair (each an (n, 5) array
+    of (query_contig, query_pos, ref_contig, ref_pos, reverse), sorted as get_anchors sorts them).  Returns score (i64) and
+    chunk-local pointer per anchor, the sorted intervals (n, 11: the chain_debug fields with kept), hits (n, 2: kept
+    intervals overlapping each one on the ref / query axis), chunk_acc (per chunk: total_anchors, rq0, rq1, tbcq, n_int) and
+    the pair's pair_sumlen / pair_nchains (avg_chain_int_len = sumlen / nchains)."""
+    chunks = [np.asarray(ch, np.uint32).reshape(-1, 5) for ch in chunks]
+    off = np.zeros(len(chunks) + 1, np.uint64); off[1:] = np.cumsum([len(ch) for ch in chunks])
+    a = np.ascontiguousarray(np.concatenate(chunks) if chunks else np.zeros((1, 5), np.uint32))
+    na, nc = int(off[-1]), len(chunks)
+    cap = na // 3 + 1
+    score = np.zeros(max(na, 1), np.int64); ptr = np.zeros(max(na, 1), np.uint32)
+    iv = np.zeros((cap, 11), np.int64); hits = np.zeros((cap, 2), np.uint32)
+    acc = np.zeros((max(nc, 1), 5), np.uint32); sums = np.zeros(2, np.uint32); n_iv = C.c_uint64()
+    lib().orc_chain_chunks(c, k, int(switched), nc, off.ctypes.data, a.ctypes.data, score.ctypes.data, ptr.ctypes.data,
+                           iv.ctypes.data, hits.ctypes.data, C.byref(n_iv), acc.ctypes.data, sums.ctypes.data)
+    n = n_iv.value
+    return dict(score=score[:na], pointer=ptr[:na], **_selection(iv[:n], hits[:n], acc[:nc], sums))
+
+
+def select_intervals(intervals, n_chunks, c, k, switched=False):
+    """get_nonoverlapping_chains on given intervals ((n, 10): score, num_anchors, q0, q1, r0, r1, ref_contig, query_contig,
+    chunk, reverse) of one pair with n_chunks chunks; outputs as chain_chunks without score / pointer."""
+    x = np.ascontiguousarray(np.asarray(intervals, np.int64).reshape(-1, 10))
+    n = len(x)
+    iv = np.zeros((max(n, 1), 11), np.int64); hits = np.zeros((max(n, 1), 2), np.uint32)
+    acc = np.zeros((max(n_chunks, 1), 5), np.uint32); sums = np.zeros(2, np.uint32)
+    lib().orc_select_intervals(c, k, int(switched), n_chunks, n, x.ctypes.data, iv.ctypes.data, hits.ctypes.data,
+                               acc.ctypes.data, sums.ctypes.data)
+    return _selection(iv[:n], hits[:n], acc[:n_chunks], sums)
 
 
 def _results(out, n):
