@@ -683,7 +683,18 @@ dp_warp_kernel(uint64_t n_chunks, ChainParams prm, Workspace ws) {
 // per-step bookkeeping; 8-lane groups evaluate 3 candidates per lane and amortise the bookkeeping over 4 anchors.
 // Lane gl of a group owns the anchors congruent to gl mod 8; register set s holds the anchor of block (current - s).
 // Group-wide arg-max = two 3-step xor-butterflies (max score, then largest j among the maxima).
+//
+// Chain bookkeeping.  A chunk of at most DP_SMEM_ANCHORS anchors keeps it in its group's slab of shared memory: one word per
+// anchor, score << 16 | index << 8 | (depth - 1), which starts as the anchor's own (0, index, 0) and, at a root, ends as the
+// shared-memory atomicMax over the root's chained anchors -- the maximum is the largest index among the maximal scores, and
+// carries that end's depth.  A word whose index field is its own anchor is a singleton or not a root: no interval.  Longer
+// chunks keep the per-anchor rootkey / depth arrays in global memory.  Field widths: index and depth - 1 < 256, score <=
+// ANCHOR_SCORE * DP_SMEM_ANCHORS < 2^16.  224 covers every chunk of a `north` step (at most 215 anchors, DESIGN §3), and its
+// 7 KB slab per warp (8 groups) still lets the 28 warps per SM that 72 registers allow be resident (28 x (7 + 1 reserved) KB).
 // ------------------------------------------------------------------------------------------------------------
+constexpr uint32_t DP_SMEM_ANCHORS = 224;
+static_assert(DP_SMEM_ANCHORS <= 256 && (uint64_t)ANCHOR_SCORE * DP_SMEM_ANCHORS < (1u << 16), "dp_group_kernel's packed chain word");
+
 template <bool TAPS, int GL, int NE, bool FULLBAND, int MINB>
 __global__ void __launch_bounds__(32, MINB)
 dp_group_kernel(uint64_t n_chunks, ChainParams prm, Workspace ws) {
@@ -705,6 +716,9 @@ dp_group_kernel(uint64_t n_chunks, ChainParams prm, Workspace ws) {
   const AnchorRec* __restrict__ a = ws.anc + a0;
   unsigned long long* __restrict__ g_key = ws.rootkey + a0;
   uint32_t* __restrict__ g_depth = ws.depth + a0;
+  __shared__ uint32_t s_chain[GW][DP_SMEM_ANCHORS];
+  uint32_t* const s_word = s_chain[lane >> LG];
+  const bool onchip = n <= DP_SMEM_ANCHORS;
   const uint32_t band = prm.band;
   // longest chunk of the warp bounds the common loop
   uint32_t nmax = n;
@@ -723,7 +737,11 @@ dp_group_kernel(uint64_t n_chunks, ChainParams prm, Workspace ws) {
     const uint32_t idx = b0 + gl;
     {
       AnchorRec x; x.qpos = 0; x.rpos = 0; x.rc = 0xFFFFFFFEu;            // impossible contig: never matches
-      if (idx < n) { x = a[idx]; g_key[idx] = (unsigned long long)idx; }
+      if (idx < n) {
+        x = a[idx];
+        if (onchip) s_word[idx] = idx << 8;
+        else g_key[idx] = (unsigned long long)idx;
+      }
       // the ref position is held NEGATED for reverse-strand anchors: two anchors can only chain on the same contig and
       // strand, and then (r' of the current) - (r' of the candidate) is the reference's strand-corrected ref gap directly
       q[0] = x.qpos; r[0] = (x.rc & 1u) ? (0u - x.rpos) : x.rpos; rc[0] = x.rc; sc[0] = 0; rt[0] = idx; dpth[0] = 1;
@@ -783,8 +801,12 @@ dp_group_kernel(uint64_t n_chunks, ChainParams prm, Workspace ws) {
       my_ptr = mine ? jw : my_ptr;
     }
     if (idx < n) {
-      g_depth[idx] = dpth[0];
-      if (rt[0] != idx) atomicMax(&g_key[rt[0]], ((unsigned long long)(uint32_t)sc[0] << 32) | idx);
+      if (onchip) {
+        if (rt[0] != idx) atomicMax(&s_word[rt[0]], ((uint32_t)sc[0] << 16) | (idx << 8) | (dpth[0] - 1));
+      } else {
+        g_depth[idx] = dpth[0];
+        if (rt[0] != idx) atomicMax(&g_key[rt[0]], ((unsigned long long)(uint32_t)sc[0] << 32) | idx);
+      }
       if (TAPS) { ws.score[a0 + idx] = sc[0]; ws.ptr[a0 + idx] = my_ptr; }
     }
   }
@@ -795,11 +817,18 @@ dp_group_kernel(uint64_t n_chunks, ChainParams prm, Workspace ws) {
   const uint32_t qctg = ws.chunk_qctg[c];
   const uint32_t chunk_local_id = (uint32_t)(c - ws.pairCbase[p]);
   for (uint32_t i = gl; i < n; i += GL) {
-    if (((volatile uint32_t*)g_depth)[i] != 1) continue;            // not a root
-    const unsigned long long key = ((volatile unsigned long long*)g_key)[i];
-    const uint32_t b = (uint32_t)key, score = (uint32_t)(key >> 32);
-    if (b == i) continue;                                            // singleton
-    const uint32_t num_anchors = ((volatile uint32_t*)g_depth)[b];
+    uint32_t b, score, num_anchors;
+    if (onchip) {
+      const uint32_t w = ((volatile uint32_t*)s_word)[i];
+      b = (w >> 8) & 0xFFu; score = w >> 16; num_anchors = (w & 0xFFu) + 1;
+      if (b == i) continue;                                          // singleton or not a root
+    } else {
+      if (((volatile uint32_t*)g_depth)[i] != 1) continue;          // not a root
+      const unsigned long long key = ((volatile unsigned long long*)g_key)[i];
+      b = (uint32_t)key; score = (uint32_t)(key >> 32);
+      if (b == i) continue;                                          // singleton
+      num_anchors = ((volatile uint32_t*)g_depth)[b];
+    }
     if (num_anchors < MIN_ANCHORS || (int32_t)score < MIN_SCORE) continue;
     const AnchorRec f = a[i], l = a[b];
     uint32_t r0 = f.rpos < l.rpos ? f.rpos : l.rpos, r1 = f.rpos < l.rpos ? l.rpos : f.rpos;
