@@ -150,6 +150,17 @@ int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* params, uint
                                const uint32_t* kmer, const uint32_t* pos, const uint32_t* contig_canon,
                                const uint64_t* mk_off, const uint64_t* markers, const uint64_t* ctg_off,
                                const uint32_t* contig_lengths, const uint64_t* total_len, sk_sketch_set** out);
+/* Build a set of n_blobs genomes, in the order given, from skani v0.3 sketch blobs exactly as stored: a .sketch file's
+ * bytes or an index.db slice of sketches.db (blob g = bytes[blob_off[g], blob_off[g] + blob_len[g]), SketchParams
+ * included).  `bytes` is HOST memory (pinned or not).  The host walks each blob's framing; the k-mer map is expanded on
+ * the device, records in the same order as the host decoder's, so the set equals the one sk_sketch_set_import_batch builds
+ * from the decoded records (genome g: the blob's contig lengths and total_sequence_length).  Every blob's (c, k,
+ * marker_c) must equal *params; amino-acid blobs are refused.  On SK_ERR_PARAM, *bad_blob (may be NULL) names the blob
+ * that does not decode: the first one whose framing or parameters are refused, else the first one with a multi-position
+ * index past its lists; UINT32_MAX when the error is not a blob's.  Same limits as sk_sketch_set_import_batch
+ * (< 2^31 records, keys, markers and contigs per call). */
+int sk_sketch_set_import_blobs(sk_ctx* ctx, const sk_sketch_params* params, const uint8_t* bytes, const uint64_t* blob_off,
+                               const uint64_t* blob_len, uint32_t n_blobs, sk_sketch_set** out, uint32_t* bad_blob);
 
 /* ---- multi-GPU plumbing (the reference is single-process; SURVEY.md section 8e): a sketch set is flattened into ONE
  *      device buffer + a small host metadata vector so that ranks can exchange sketches with a single NCCL all-gather

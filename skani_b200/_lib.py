@@ -70,6 +70,7 @@ SYMBOLS = [
     ("sk_sketch_set_export", i32, [vp, u32, vp, vp, vp, vp, vp]),
     ("sk_sketch_set_import", i32, [vp, PP(SketchParams), vp, vp, vp, u64, vp, u64, vp, u32, PP(vp)]),
     ("sk_sketch_set_import_batch", i32, [vp, PP(SketchParams), u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, PP(vp)]),
+    ("sk_sketch_set_import_blobs", i32, [vp, PP(SketchParams), vp, vp, vp, u32, PP(vp), PP(u32)]),
     ("sk_sketch_set_blob_size", i32, [vp, PP(u64), PP(u64)]),
     ("sk_sketch_set_pack", i32, [vp, vp, vp]),
     ("sk_sketch_set_unpack", i32, [vp, u32, vp, vp, PP(vp)]),

@@ -15,7 +15,8 @@
 // --gpus N: dist and search split the references into contiguous blocks, one per GPU, and copy the query set to every GPU
 // (sk_screen_query_ref_multi / sk_chain_pairs_multi); the output is byte-identical to one GPU's.
 // triangle and dist take pre-sketched inputs as .sketch files and as consolidated databases (sketch_db.hpp: SketchInputs),
-// decoded and imported in groups of < 2^28 records so that host memory holds one decoded group at a time.
+// read as stored and imported in groups of < 2^28 records (sk_sketch_set_import_blobs expands them on the device), so that
+// host memory holds one group's bytes at a time.
 #include <dirent.h>
 #include <fcntl.h>
 #include <sys/stat.h>
@@ -255,36 +256,48 @@ bool sketch_inputs_given(const std::vector<std::string>& files) {
   return all;
 }
 
-// group bound of the sketch readers: < 2^28 seed records per sk_sketch_set_import_batch call.  SK_SKETCH_GROUP_RECORDS
+// group bound of the sketch readers: < 2^28 seed records per sk_sketch_set_import_blobs call.  SK_SKETCH_GROUP_RECORDS
 // lowers it (a test hook: many groups from a small input).
 uint64_t sketch_group_records() {
   if (const char* e = getenv("SK_SKETCH_GROUP_RECORDS")) return (uint64_t)std::max(1ll, atoll(e));
   return 1ull << 28;
 }
 
-Genome genome_of(const skdb::HostSketch& h) {
+Genome genome_of(const skdb::SketchScan& h) {
   Genome g; g.file_name = h.file_name; g.contigs = h.contigs; g.contig_order = h.contig_order; g.total_len = h.total_len;
   if (g.contigs.empty()) g.contigs.push_back("");   // a sketch without contig names still prints
   return g;
 }
 
+// a group of sketches as stored -> one device set (sk_sketch_set_import_blobs); nullptr after an ERROR line naming the
+// sketch (name_of(i) for blob i) when one does not decode on the device
+template <class N>
+sk_sketch_set* import_group(sk_ctx* ctx, const skdb::SketchGroup& g, const sk_sketch_params& sp, N name_of) {
+  sk_sketch_set* set = nullptr;
+  uint32_t bad = UINT32_MAX;
+  const int rc = sk_sketch_set_import_blobs(ctx, &sp, g.bytes.data(), g.off.data(), g.len.data(), (uint32_t)g.size(), &set, &bad);
+  if (rc != 0 && bad < g.size()) { fprintf(stderr, "ERROR Failed to load sketch %s\n", name_of(bad).c_str()); return nullptr; }
+  if (rc != 0) { fprintf(stderr, "ERROR sk_sketch_set_import_blobs failed (%d): %s\n", rc, sk_last_error(ctx)); exit(1); }
+  return set;
+}
+
 // sketch inputs [a, b) read group by group: fn(set) gets each group imported as one device set on ctx and owns it;
-// meta[i - a] gets entry i's metadata.  The decoded group is freed before the next one is read.  false (after the reader's
-// ERROR line) when an entry cannot be loaded: the caller ends the run from the main thread.  One INFO line reports the time
-// spent reading + decoding and importing (fn included).
+// meta[i - a] gets entry i's metadata.  A group's bytes are freed before the next one is read.  false (after an ERROR
+// line) when an entry cannot be loaded: the caller ends the run from the main thread.  One INFO line reports the time
+// spent reading + decoding (reading the entries as stored and walking their framing) and importing (fn included).
 template <class F>
 bool for_each_sketch_group(sk_ctx* ctx, const skdb::SketchInputs& si, size_t a, size_t b, int threads, const sk_sketch_params& sp, Genome* meta, F fn) {
   using clk = std::chrono::steady_clock;
   skdb::SketchGroupReader rd(si, a, b, threads, sketch_group_records());
-  std::vector<skdb::HostSketch> g;
+  skdb::SketchGroup g;
   double t_read = 0, t_import = 0;
   size_t groups = 0;
   for (auto t0 = clk::now(); rd.next(g); t0 = clk::now()) {
-    Flat f;
-    for (size_t i = 0; i < g.size(); i++) { f.add(g[i], true); meta[rd.first + i - a] = genome_of(g[i]); }
-    g.clear();
+    for (size_t i = 0; i < g.size(); i++) meta[rd.first + i - a] = genome_of(g.scan[i]);
     const auto t1 = clk::now();
-    fn(f.import(ctx, sp));
+    sk_sketch_set* s = import_group(ctx, g, sp, [&](size_t i) { return si.entries[rd.first + i].file_name; });
+    if (!s) return false;
+    fn(s);
     t_read += std::chrono::duration<double>(t1 - t0).count();
     t_import += std::chrono::duration<double>(clk::now() - t1).count();
     groups++;
@@ -309,7 +322,7 @@ sk_sketch_set* import_sketch_inputs(sk_ctx* ctx, const skdb::SketchInputs& si, s
 }
 
 // sketch inputs -> a new host sketch store: each group's set is added and freed before the next group is read, so host
-// memory holds one decoded group besides the pinned store, and the device one imported group.  nullptr when an entry
+// memory holds one group of stored sketches besides the pinned store, and the device one imported group.  nullptr when an entry
 // cannot be loaded.
 sk_sketch_store* store_sketch_inputs(sk_ctx* ctx, const skdb::SketchInputs& si, int threads, const sk_sketch_params& sp, std::vector<Genome>& meta) {
   sk_sketch_store* st = nullptr;
@@ -1043,52 +1056,65 @@ int run_search(Opts& op) {
   for (;;) {
     std::vector<size_t> lo(next), hi(next);                   // this round: context d imports hits [lo[d], hi[d])
     std::vector<sk_sketch_set*> rsets(W, nullptr);
-    std::atomic<bool> too_large{false};
+    std::atomic<bool> too_large{false}, load_failed{false};   // a reference that cannot be loaded ends the run (reported)
     per_context(W, [&](size_t d) {
       const size_t h0 = next[d], end = run[d + 1];
       if (h0 == end) return;
       size_t h1 = h0;
-      std::vector<skdb::HostSketch> loaded;
       uint64_t recs = 0;
       while (h1 < end && h1 - h0 < 60000 && recs < (1ull << 30)) h1++, recs += 45000;   // provisional bound, refined below
-      loaded.resize(h1 - h0);
-      std::vector<int> ok(h1 - h0, 1);
+      // the hits' sketches as stored, back to back in one buffer: the slices of sketches.db, or the .sketch files
+      // <dir>/<basename(file_name)>.sketch (src/search.rs:157-166)
+      skdb::SketchGroup g;
+      auto path_of = [&](uint32_t r) { return op.db_dir + "/" + base_name(ref_mk[r].file_name) + ".sketch"; };
+      uint64_t total = 0;
+      for (size_t i = h0; i < h1; i++) {
+        uint64_t n = 0;
+        struct stat st;
+        if (consolidated) n = index[hits[i]].length;
+        else if (stat(path_of(hits[i]).c_str(), &st) == 0) n = (uint64_t)st.st_size;
+        g.off.push_back(total); g.len.push_back(n);
+        total += n;
+      }
+      g.bytes.resize(total);
+      g.scan.resize(h1 - h0);
       {
         const int T = std::max(1, std::max(op.threads, 1) / (int)W + ((int)d < std::max(op.threads, 1) % (int)W ? 1 : 0));
         std::vector<std::thread> pool;
         for (int t = 0; t < T; t++) pool.emplace_back([&, t] {
           for (size_t i = h0 + t; i < h1; i += T) {
             const uint32_t r = hits[i];
+            uint8_t* dst = g.bytes.data() + g.off[i - h0];
+            const uint64_t n = g.len[i - h0];
             bool good;
-            if (consolidated) {
-              good = skdb::read_db_entry(db_fd, index[r], loaded[i - h0]);
-            } else {                     // <dir>/<basename(file_name)>.sketch (src/search.rs:157-166)
-              std::vector<uint8_t> b;
-              good = skdb::read_file(op.db_dir + "/" + base_name(ref_mk[r].file_name) + ".sketch", b);
-              try { if (good) loaded[i - h0] = skdb::read_blob(b.data(), b.size()); }
-              catch (const std::exception&) { good = false; }
+            if (consolidated) good = pread(db_fd, dst, n, (off_t)index[r].offset) == (ssize_t)n;
+            else {
+              FILE* f = fopen(path_of(r).c_str(), "rb");
+              good = f && fread(dst, 1, n, f) == n;
+              if (f) fclose(f);
             }
-            if (!good) { ok[i - h0] = 0; fprintf(stderr, "ERROR Failed to load sketch %s\n", ref_mk[r].file_name.c_str()); }
+            try { if (good) g.scan[i - h0] = skdb::scan_entry(dst, n); }
+            catch (const std::exception&) { good = false; }
+            if (!good) { load_failed = true; fprintf(stderr, "ERROR Failed to load sketch %s\n", ref_mk[r].file_name.c_str()); }
           }
         });
         for (auto& th : pool) th.join();
       }
+      if (load_failed) return;
       // keep the batch under 2^31 records: shrink it if the real sizes exceed the estimate (the rest goes to later rounds)
       uint64_t real = 0;
       size_t cut = h0;
-      while (cut < h1 && real + loaded[cut - h0].kmer.size() < (1ull << 31) - 1) real += loaded[cut - h0].kmer.size(), cut++;
+      while (cut < h1 && real + g.scan[cut - h0].n_records < (1ull << 31) - 1) real += g.scan[cut - h0].n_records, cut++;
       if (cut == h0) { too_large = true; return; }
-      Flat f;
+      g.off.resize(cut - h0); g.len.resize(cut - h0); g.scan.resize(cut - h0);
       std::vector<uint64_t> ranks;
-      for (size_t i = h0; i < cut; i++) {
-        if (!ok[i - h0]) loaded[i - h0] = skdb::HostSketch();     // unreadable reference: chains to "no anchors", dropped below
-        f.add(loaded[i - h0], true);
-        ranks.push_back(rrank[hits[i]]);
-      }
-      rsets[d] = f.import(ctxs[d], sp);
+      for (size_t i = h0; i < cut; i++) ranks.push_back(rrank[hits[i]]);
+      rsets[d] = import_group(ctxs[d], g, sp, [&](size_t i) { return ref_mk[hits[h0 + i]].file_name; });
+      if (!rsets[d]) { load_failed = true; return; }
       sk_sketch_set_set_name_ranks(rsets[d], ranks.data());
       hi[d] = next[d] = cut;
     });
+    if (load_failed) return 1;
     if (too_large) { fprintf(stderr, "ERROR reference sketch too large\n"); return 1; }
     // the round's refs are numbered run after run: context d's block starts at ref_first[d]
     std::vector<uint32_t> ref_first(W), round_hit;

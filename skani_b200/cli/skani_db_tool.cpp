@@ -108,12 +108,10 @@ int main(int argc, char** argv) {
       printf("PARAMS %llu %llu %llu\nN %zu\n", (unsigned long long)si.params.c, (unsigned long long)si.params.k,
              (unsigned long long)si.params.marker_c, si.entries.size());
       SketchGroupReader rd(si, 0, si.entries.size(), atoi(argv[3]), strtoull(argv[2], nullptr, 10));
-      std::vector<HostSketch> g;
+      SketchGroup g;
       while (rd.next(g)) {
-        uint64_t recs = 0;
-        for (auto& h : g) recs += h.kmer.size();
-        printf("G %zu %zu %llu\n", rd.first, g.size(), (unsigned long long)recs);
-        for (auto& h : g) printf("S %zu %llu %s\n", h.kmer.size(), (unsigned long long)h.contig_order, h.file_name.c_str());
+        printf("G %zu %zu %llu\n", rd.first, g.size(), (unsigned long long)g.records);
+        for (auto& h : g.scan) printf("S %llu %llu %s\n", (unsigned long long)h.n_records, (unsigned long long)h.contig_order, h.file_name.c_str());
       }
       return rd.failed ? 1 : 0;
     }

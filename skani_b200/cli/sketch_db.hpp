@@ -9,8 +9,8 @@
 //   (SketchParams, Vec<Sketch>)           `markers.bin`, sketches reduced by Sketch::get_markers_only
 //                                         (src/types.rs:322-340, src/sketch.rs:141-146)
 // The k-mer map is a Rust HashMap, so entry order in a file is arbitrary and carries no meaning; this writer emits
-// ascending k-mers.  Map value (src/types.rs:207-244): bit 0 = 1 -> one position packed as
-// ((pos << 31 | contig_index_canonical) << 1) | 1; bit 0 = 0 -> (index into multi_position_storage) << 1.
+// ascending k-mers.  Map value (src/types.rs:207-244): csrc/sketch_value.cuh, shared with the device expansion of
+// sk_sketch_set_import_blobs.
 #pragma once
 #include <fcntl.h>
 #include <sys/stat.h>
@@ -25,6 +25,8 @@
 #include <string>
 #include <thread>
 #include <vector>
+
+#include "../csrc/sketch_value.cuh"
 
 namespace skdb {
 
@@ -105,8 +107,8 @@ inline void put_sketch(Out& o, const HostSketch& s) {
       size_t j = i + 1;
       while (j < n && s.kmer[j] == s.kmer[i]) j++;
       o.u32(s.kmer[i]);
-      if (j - i == 1) o.u64(((((uint64_t)s.pos[i] << 31) | (uint64_t)s.cc[i]) << 1) | 1ull);
-      else o.u64((uint64_t)(storage++) << 1);
+      if (j - i == 1) o.u64(single_value(s.pos[i], s.cc[i]));
+      else o.u64(multi_value(storage++));
       i = j;
     }
     o.u64(n_multi);
@@ -161,55 +163,116 @@ inline DiskParams get_params(In& in) {
   return p;
 }
 
-// seeds = false skips materialising the records (markers.bin entries have none anyway)
-inline HostSketch get_sketch(In& in, bool seeds = true) {
-  HostSketch s;
+// The framing of one Sketch, walked without materialising its records or markers.  Byte offsets are relative to the
+// start of what was scanned (scan_entry: the blob).  The key block holds n_keys x {u32 k-mer, u64 value}
+// (sketch_value.cuh); multi-position list j holds multi_len[j] x {u32 pos, u32 contig_index_canonical} at multi_at[j].
+struct SketchScan {
+  DiskParams params;                 // scan_entry only
+  std::string file_name;
+  bool has_seeds = true;
+  uint64_t keys_at = 0, n_keys = 0;
+  std::vector<uint64_t> multi_at, multi_len;
+  std::vector<std::string> contigs;
+  uint64_t total_len = 0;
+  uint64_t ctg_len_at = 0, n_ctg_len = 0;      // u32 each
+  uint64_t repetitive_kmers = 0;
+  uint64_t markers_at = 0, n_markers = 0;      // u64 each
+  uint64_t marker_c = 125, c = 125, k = 15, contig_order = 0;
+  bool individual_contig = false, amino_acid = false;
+  // seed records: n_keys - n_multi + sum of the list lengths, exact when every list belongs to exactly one key (as
+  // skani writes them; the expansions count what the keys actually reference)
+  uint64_t n_records = 0;
+};
+
+inline uint32_t load_u32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
+inline uint64_t load_u64(const uint8_t* p) { uint64_t v; memcpy(&v, p, 8); return v; }
+
+// one Sketch at in.p (in is advanced past it); offsets relative to base.  Throws where the data cannot be a Sketch:
+// truncated, a length prefix longer than the bytes left, an Option tag > 1.  Whether the keys' multi-position indices
+// are in range is left to the expansion, which reads the values.
+inline SketchScan scan_sketch(In& in, const uint8_t* base) {
+  SketchScan s;
   s.file_name = in.str();
   const uint8_t tag = in.u8();
   if (tag > 1) throw std::runtime_error("corrupt Option tag (a pre-0.3 .sketch file?)");
   s.has_seeds = tag == 1;
-  std::vector<uint32_t> keys;
-  std::vector<uint64_t> vals;
   if (tag == 1) {
-    uint64_t n = in.len(12);
-    keys.resize(n); vals.resize(n);
-    for (uint64_t i = 0; i < n; i++) { keys[i] = in.u32(); vals[i] = in.u64(); }
+    s.n_keys = in.len(12);
+    s.keys_at = (uint64_t)(in.p - base);
+    in.p += s.n_keys * 12;
   }
   const uint64_t n_multi = in.len(8);
-  std::vector<const uint8_t*> multi_at(n_multi);
-  std::vector<uint64_t> multi_len(n_multi);
+  s.multi_at.resize(n_multi);
+  s.multi_len.resize(n_multi);
+  uint64_t listed = 0;
   for (uint64_t i = 0; i < n_multi; i++) {
-    multi_len[i] = in.len(8);
-    multi_at[i] = in.p;
-    in.p += multi_len[i] * 8;
+    s.multi_len[i] = in.len(8);
+    s.multi_at[i] = (uint64_t)(in.p - base);
+    in.p += s.multi_len[i] * 8;
+    listed += s.multi_len[i];
   }
-  if (seeds) {
-    for (size_t i = 0; i < keys.size(); i++) {
-      if (vals[i] & 1) {
-        const uint64_t packed = vals[i] >> 1;
-        s.kmer.push_back(keys[i]); s.pos.push_back((uint32_t)(packed >> 31)); s.cc.push_back((uint32_t)(packed & 0x7FFFFFFFull));
-      } else {
-        const uint64_t si = vals[i] >> 1;
-        if (si >= n_multi) throw std::runtime_error("multi-position index out of range");
-        for (uint64_t t = 0; t < multi_len[si]; t++) {
-          uint32_t a, b; memcpy(&a, multi_at[si] + 8 * t, 4); memcpy(&b, multi_at[si] + 8 * t + 4, 4);
-          s.kmer.push_back(keys[i]); s.pos.push_back(a); s.cc.push_back(b);
-        }
-      }
-    }
-  }
+  s.n_records = s.n_keys + listed >= n_multi ? s.n_keys + listed - n_multi : 0;
   uint64_t n = in.len(8);
   for (uint64_t i = 0; i < n; i++) s.contigs.push_back(in.str());
   s.total_len = in.u64();
-  n = in.len(4);
-  s.contig_lengths.resize(n);
-  for (uint64_t i = 0; i < n; i++) s.contig_lengths[i] = in.u32();
+  s.n_ctg_len = in.len(4);
+  s.ctg_len_at = (uint64_t)(in.p - base);
+  in.p += s.n_ctg_len * 4;
   s.repetitive_kmers = in.u64();
-  n = in.len(8);
-  s.markers.resize(n);
-  for (uint64_t i = 0; i < n; i++) s.markers[i] = in.u64();
+  s.n_markers = in.len(8);
+  s.markers_at = (uint64_t)(in.p - base);
+  in.p += s.n_markers * 8;
   s.marker_c = in.u64(); s.c = in.u64(); s.k = in.u64(); s.contig_order = in.u64();
   s.individual_contig = in.u8() != 0; s.amino_acid = in.u8() != 0;
+  return s;
+}
+
+// one (SketchParams, Sketch) blob: a `.sketch` file or a slice of sketches.db
+inline SketchScan scan_entry(const uint8_t* p, size_t n) {
+  In in(p, n);
+  const DiskParams dp = get_params(in);
+  SketchScan s = scan_sketch(in, p);
+  s.params = dp;
+  return s;
+}
+
+// the seed records of a scanned Sketch in file order (keys as stored, each multi-position list expanded in place), the
+// order the device expansion of sk_sketch_set_import_blobs writes too
+inline void expand_records(const uint8_t* base, const SketchScan& s, HostSketch& h) {
+  for (uint64_t i = 0; i < s.n_keys; i++) {
+    const uint8_t* e = base + s.keys_at + 12 * i;
+    const uint32_t key = load_u32(e);
+    const uint64_t v = load_u64(e + 4);
+    if (value_is_single(v)) {
+      h.kmer.push_back(key); h.pos.push_back(value_pos(v)); h.cc.push_back(value_cc(v));
+      continue;
+    }
+    const uint64_t si = value_multi_index(v);
+    if (si >= s.multi_at.size()) throw std::runtime_error("multi-position index out of range");
+    const uint8_t* l = base + s.multi_at[si];
+    for (uint64_t t = 0; t < s.multi_len[si]; t++) {
+      h.kmer.push_back(key); h.pos.push_back(load_u32(l + 8 * t)); h.cc.push_back(load_u32(l + 8 * t + 4));
+    }
+  }
+}
+
+// seeds = false skips materialising the records (markers.bin entries have none anyway)
+inline HostSketch get_sketch(In& in, bool seeds = true) {
+  const uint8_t* base = in.p;
+  const SketchScan sc = scan_sketch(in, base);
+  HostSketch s;
+  s.file_name = sc.file_name;
+  s.has_seeds = sc.has_seeds;
+  if (seeds) expand_records(base, sc, s);
+  s.contigs = sc.contigs;
+  s.total_len = sc.total_len;
+  s.contig_lengths.resize(sc.n_ctg_len);
+  for (uint64_t i = 0; i < sc.n_ctg_len; i++) s.contig_lengths[i] = load_u32(base + sc.ctg_len_at + 4 * i);
+  s.repetitive_kmers = sc.repetitive_kmers;
+  s.markers.resize(sc.n_markers);
+  for (uint64_t i = 0; i < sc.n_markers; i++) s.markers[i] = load_u64(base + sc.markers_at + 8 * i);
+  s.marker_c = sc.marker_c; s.c = sc.c; s.k = sc.k; s.contig_order = sc.contig_order;
+  s.individual_contig = sc.individual_contig; s.amino_acid = sc.amino_acid;
   return s;
 }
 
@@ -338,8 +401,8 @@ inline bool open_db(const std::string& dir, std::vector<IndexEntry>& index, int&
 // ---------------------------------------------------------------- sketch inputs of triangle / dist
 // A consolidated database (a directory holding index.db and sketches.db, src/sketch_db.rs:142-146) stands for all of its
 // sketches, exactly as if each entry were a .sketch file.  Opening the inputs reads index.db (and checks it against
-// markers.bin and the size of sketches.db) but decodes only a database's first entry; the sketches themselves are decoded
-// later, in groups (SketchGroupReader), so host memory holds one decoded group at a time.
+// markers.bin and the size of sketches.db) but decodes only a database's first entry; the sketches themselves are read
+// later, in groups and as stored (SketchGroupReader), so host memory holds one group's bytes at a time.
 inline bool is_sketch_db(const std::string& p) {
   struct stat st;
   return stat(p.c_str(), &st) == 0 && S_ISDIR(st.st_mode) && stat((p + "/index.db").c_str(), &st) == 0 &&
@@ -421,73 +484,118 @@ inline bool open_sketch_inputs(const std::vector<std::string>& files, SketchInpu
   return true;
 }
 
-// Decodes the entries [begin, end) of si, in order, and hands them out in groups of < max_records seed records (a group
-// holds at least one sketch).  Entries are read and decoded in batches by `threads` threads; at most one batch waits
-// beyond the current group.  An entry that cannot be read or decoded, or whose name differs from its index entry, ends
-// the reading with an ERROR line: next() then returns false with failed set.
+// bytes that are written before they are read: growing the buffer does not clear it
+template <class T>
+struct uninit_alloc : std::allocator<T> {
+  template <class U> struct rebind { using other = uninit_alloc<U>; };
+  template <class U> void construct(U* p) noexcept { ::new ((void*)p) U; }
+  template <class U, class... A> void construct(U* p, A&&... a) { ::new ((void*)p) U(std::forward<A>(a)...); }
+};
+
+// A group of sketch inputs as stored: blob i (a .sketch file or a sketches.db entry, SketchParams included) is
+// bytes[off[i], off[i] + len[i]), scan[i] its framing.  records = the sum of the scans' record counts.
+struct SketchGroup {
+  std::vector<uint8_t, uninit_alloc<uint8_t>> bytes;
+  std::vector<uint64_t> off, len;
+  std::vector<SketchScan> scan;
+  uint64_t records = 0;
+  size_t size() const { return scan.size(); }
+  void clear() { bytes.clear(); off.clear(); len.clear(); scan.clear(); records = 0; }
+};
+
+// Reads the entries [begin, end) of si, in order, and hands them out in groups of < max_records seed records (a group
+// holds at least one sketch), each group's blobs read into one buffer as stored and scanned (scan_entry), not decoded.
+// Entries are read and scanned in batches by `threads` threads; the entries of a batch that the current group cannot
+// take are carried into the next one.  An entry that cannot be read or scanned, or whose name differs from its index
+// entry, ends the reading with an ERROR line: next() then returns false with failed set.
 class SketchGroupReader {
  public:
   SketchGroupReader(const SketchInputs& si, size_t begin, size_t end, int threads, uint64_t max_records)
       : si_(si), next_(begin), end_(end), consumed_(begin), threads_(std::max(threads, 1)), max_records_(max_records) {}
   bool failed = false;
-  size_t first = 0;             // entry index of g[0] after next()
+  size_t first = 0;             // entry index of g's first blob after next()
 
-  bool next(std::vector<HostSketch>& g) {
-    g.clear();
+  bool next(SketchGroup& g) {
+    g = std::move(carry_);        // the previous group's buffer is freed here
+    carry_ = SketchGroup();
     first = consumed_;
+    size_t take = 0;            // g's blobs [0, take) fit the group
     uint64_t recs = 0;
     for (;;) {
-      if (pending_pos_ == pending_.size() && !decode_batch()) break;
-      if (failed) return false;
-      HostSketch& h = pending_[pending_pos_];
-      if (!g.empty() && recs + h.kmer.size() >= max_records_) break;
-      recs += h.kmer.size();
-      g.push_back(std::move(h));
-      pending_pos_++;
-      consumed_++;
+      while (take < g.size() && (take == 0 || recs + g.scan[take].n_records < max_records_)) recs += g.scan[take++].n_records;
+      if (take < g.size() || !read_batch(g)) break;
+      if (failed) { g.clear(); return false; }
     }
-    return !g.empty();
+    for (size_t i = take; i < g.size(); i++) {             // the rest of the last batch opens the next group
+      carry_.off.push_back(carry_.bytes.size());
+      carry_.bytes.insert(carry_.bytes.end(), g.bytes.begin() + g.off[i], g.bytes.begin() + g.off[i] + g.len[i]);
+      carry_.len.push_back(g.len[i]);
+      carry_.scan.push_back(std::move(g.scan[i]));
+      carry_.records += carry_.scan.back().n_records;
+    }
+    if (take < g.size()) {
+      g.bytes.resize(g.off[take]);
+      g.off.resize(take); g.len.resize(take); g.scan.resize(take);
+    }
+    g.records = recs;
+    consumed_ += g.size();
+    return g.size() != 0;
   }
 
  private:
-  bool decode_batch() {         // the next entries (at most 8 per thread and about 256 MiB on disk) into pending_
+  // the next entries (at most 8 per thread and about 256 MiB on disk) appended to g: read, then scanned
+  bool read_batch(SketchGroup& g) {
     if (next_ >= end_) return false;
     size_t b = next_;
     uint64_t bytes = 0;
     while (b < end_ && (b == next_ || (b - next_ < 8 * (size_t)threads_ && bytes < (256ull << 20)))) bytes += si_.entries[b++].length;
-    pending_.assign(b - next_, HostSketch());
-    pending_pos_ = 0;
+    const size_t n0 = g.size(), n = b - next_;
+    if (g.bytes.capacity() < g.bytes.size() + bytes) {   // room for the rest of the inputs, up to about a group's worth
+      uint64_t rest = 0;
+      for (size_t i = next_; i < end_ && rest < 16 * max_records_; i++) rest += si_.entries[i].length;
+      g.bytes.reserve(g.bytes.size() + std::max<uint64_t>(bytes, rest));
+    }
+    uint64_t end = g.bytes.size();
+    for (size_t i = 0; i < n; i++) {
+      g.off.push_back(end);
+      g.len.push_back(si_.entries[next_ + i].length);
+      end += g.len.back();
+    }
+    g.bytes.resize(end);
+    g.scan.resize(n0 + n);
     std::atomic<size_t> at{0};
     std::atomic<bool> bad{false};
     auto worker = [&] {
-      for (size_t i; (i = at.fetch_add(1)) < pending_.size();) {
+      for (size_t i; (i = at.fetch_add(1)) < n;) {
         const SketchEntry& e = si_.entries[next_ + i];
         const int fd = si_.db_fd[e.input];
+        uint8_t* dst = g.bytes.data() + g.off[n0 + i];
         bool good;
-        if (fd >= 0) good = read_db_entry(fd, IndexEntry{e.file_name, e.offset, e.length}, pending_[i]) && pending_[i].file_name == e.file_name;
-        else {
-          std::vector<uint8_t> buf;
-          good = read_file(si_.paths[e.input], buf);
-          try { if (good) pending_[i] = read_blob(buf.data(), buf.size()); }
-          catch (const std::exception&) { good = false; }
+        if (fd >= 0) good = pread(fd, dst, e.length, (off_t)e.offset) == (ssize_t)e.length;
+        else {                   // a .sketch file: its size when the inputs were opened
+          FILE* f = fopen(si_.paths[e.input].c_str(), "rb");
+          good = f && fread(dst, 1, e.length, f) == e.length;
+          if (f) fclose(f);
         }
+        try { if (good) g.scan[n0 + i] = scan_entry(dst, e.length); }
+        catch (const std::exception&) { good = false; }
+        if (good && fd >= 0) good = g.scan[n0 + i].file_name == e.file_name;
         if (!good) { bad = true; fprintf(stderr, "ERROR Failed to load sketch %s\n", e.file_name.c_str()); }
       }
     };
     std::vector<std::thread> pool;
-    for (int t = 1; t < threads_ && (size_t)t < pending_.size(); t++) pool.emplace_back(worker);
+    for (int t = 1; t < threads_ && (size_t)t < n; t++) pool.emplace_back(worker);
     worker();
     for (auto& t : pool) t.join();
     next_ = b;
-    if (bad) { failed = true; pending_.clear(); }
+    if (bad) failed = true;
     return true;
   }
   const SketchInputs& si_;
   size_t next_, end_, consumed_;
   int threads_;
   uint64_t max_records_;
-  std::vector<HostSketch> pending_;
-  size_t pending_pos_ = 0;
+  SketchGroup carry_;
 };
 
 }  // namespace skdb

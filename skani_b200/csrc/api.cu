@@ -12,9 +12,11 @@
 #include <functional>
 #include <thread>
 
+#include "../cli/sketch_db.hpp"
 #include "host_pack.hpp"
 #include "sk_core.cuh"
 #include "sk_internal.h"
+#include "sketch_value.cuh"
 
 using namespace sk;
 
@@ -178,6 +180,75 @@ __global__ void import_range_kernel(const T* __restrict__ v, uint64_t n, uint64_
   if (over) atomicOr(bad, flag);
 }
 
+// ---- sk_sketch_set_import_blobs: skani v0.3 sketch entries expanded on the device ---------------------------------------
+// Blob g of a call, as the host scan (skdb::scan_entry) found it; byte offsets into the uploaded bytes, indices into the
+// call's keys, multi-position lists and markers.
+struct BlobDesc {
+  uint64_t keys_at, key0, n_keys;      // n_keys x {u32 k-mer, u64 value}
+  uint64_t list0, n_lists;             // lists [list0, list0 + n_lists) of list_at / list_len
+  uint64_t markers_at, mk0, n_markers; // n_markers x u64
+};
+// Blobs start at arbitrary byte offsets (file-name lengths vary): loads join aligned 32-bit words with funnel shifts.
+// The upload is padded so that the word after a blob's last byte exists.
+__device__ __forceinline__ uint32_t load_u32_at(const uint8_t* b, uint64_t at) {
+  const uint32_t* w = (const uint32_t*)(b + (at & ~3ull));
+  return __funnelshift_r(w[0], w[1], (uint32_t)(at & 3) * 8);
+}
+__device__ __forceinline__ uint64_t load_u64_at(const uint8_t* b, uint64_t at) {
+  const uint32_t* w = (const uint32_t*)(b + (at & ~3ull));
+  const uint32_t sh = (uint32_t)(at & 3) * 8;
+  return (uint64_t)__funnelshift_r(w[0], w[1], sh) | ((uint64_t)__funnelshift_r(w[1], w[2], sh) << 32);
+}
+// records per key (1, or its list's length); a multi-position index past the blob's lists names the blob in bad_blob
+__global__ void blob_count_kernel(const uint8_t* __restrict__ buf, const BlobDesc* __restrict__ desc, const uint64_t* __restrict__ list_len,
+                                  uint64_t* __restrict__ cnt, uint32_t* __restrict__ bad_blob) {
+  const uint32_t g = blockIdx.x;
+  const BlobDesc d = desc[g];
+  for (uint64_t i = (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; i < d.n_keys; i += (uint64_t)blockDim.x * gridDim.y) {
+    const uint64_t v = load_u64_at(buf, d.keys_at + 12 * i + 4);
+    uint64_t c = 1;
+    if (!skdb::value_is_single(v)) {
+      const uint64_t li = skdb::value_multi_index(v);
+      if (li < d.n_lists) c = list_len[d.list0 + li];
+      else { c = 0; atomicMin(bad_blob, g); }
+    }
+    cnt[d.key0 + i] = c;
+  }
+}
+// first record of every blob (and the total): the exclusive scan of the counts at its first key
+__global__ void blob_rec_off_kernel(const BlobDesc* __restrict__ desc, uint32_t G, uint64_t n_keys, const uint64_t* __restrict__ key_rec,
+                                    uint64_t* __restrict__ rec_off) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g <= G) rec_off[g] = key_rec[g < G ? desc[g].key0 : n_keys];
+}
+// the records in the host decoder's order (skdb::expand_records): keys in file order, each multi-position list in place
+__global__ void blob_expand_kernel(const uint8_t* __restrict__ buf, const BlobDesc* __restrict__ desc, const uint64_t* __restrict__ list_at,
+                                   const uint64_t* __restrict__ list_len, const uint64_t* __restrict__ key_rec, uint32_t* __restrict__ kmer,
+                                   uint32_t* __restrict__ pos, uint32_t* __restrict__ cc) {
+  const uint32_t g = blockIdx.x;
+  const BlobDesc d = desc[g];
+  for (uint64_t i = (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; i < d.n_keys; i += (uint64_t)blockDim.x * gridDim.y) {
+    const uint64_t at = d.keys_at + 12 * i;
+    const uint32_t key = load_u32_at(buf, at);
+    const uint64_t v = load_u64_at(buf, at + 4);
+    const uint64_t r = key_rec[d.key0 + i];
+    if (skdb::value_is_single(v)) {
+      kmer[r] = key; pos[r] = skdb::value_pos(v); cc[r] = skdb::value_cc(v);
+      continue;
+    }
+    const uint64_t li = d.list0 + skdb::value_multi_index(v), n = list_len[li], a = list_at[li];
+    for (uint64_t t = 0; t < n; t++) {
+      kmer[r + t] = key; pos[r + t] = load_u32_at(buf, a + 8 * t); cc[r + t] = load_u32_at(buf, a + 8 * t + 4);
+    }
+  }
+}
+__global__ void blob_markers_kernel(const uint8_t* __restrict__ buf, const BlobDesc* __restrict__ desc, uint64_t* __restrict__ mraw) {
+  const uint32_t g = blockIdx.x;
+  const BlobDesc d = desc[g];
+  for (uint64_t i = (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; i < d.n_markers; i += (uint64_t)blockDim.x * gridDim.y)
+    mraw[d.mk0 + i] = load_u64_at(buf, d.markers_at + 8 * i);
+}
+
 __global__ void stage_copy_kernel(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src, size_t n_words) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_words) dst[i] = src[i];
@@ -252,10 +323,56 @@ int check_sketch_params(sk_ctx* ctx, const sk_sketch_params* sp) {
   return SK_OK;
 }
 
+// is the caller's buffer page-locked? then DMA straight from it; otherwise stage through our pinned buffers
+bool host_pinned(const void* p) {
+  if (!p) return false;
+  cudaPointerAttributes attr;
+  const bool pin = cudaPointerGetAttributes(&attr, p) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+  cudaGetLastError();
+  return pin;
+}
+
 void parallel_memcpy(sk_ctx* ctx, void* dst, const void* src, size_t n) {
   if (n < (8u << 20)) { memcpy(dst, src, n); return; }
   const size_t chunk = 4u << 20, nt = (n + chunk - 1) / chunk;
   ctx_pool(ctx)->run(nt, [&](size_t t) { const size_t b = t * chunk; memcpy((uint8_t*)dst + b, (const uint8_t*)src + b, std::min(chunk, n - b)); });
+}
+
+// host byte runs, back to back, -> dst on ctx->stream: straight from page-locked memory, otherwise staged through the
+// context's two pinned buffers (one filled by the worker pool while the other is in flight)
+int upload_runs(sk_ctx* ctx, uint8_t* dst, const std::vector<std::pair<const uint8_t*, uint64_t>>& runs, bool pinned) {
+  cudaStream_t st = ctx->stream;
+  if (pinned) {
+    for (auto& r : runs) { SK_CUDA(cudaMemcpyAsync(dst, r.first, r.second, cudaMemcpyHostToDevice, st)); dst += r.second; }
+    return SK_OK;
+  }
+  const size_t CHUNK = 64ull << 20;
+  if (ctx->pinned_bytes < CHUNK) {
+    for (int i = 0; i < 2; i++) {
+      if (ctx->pinned[i]) cudaFreeHost(ctx->pinned[i]);
+      ctx->pinned[i] = nullptr;
+      SK_CUDA(cudaHostAlloc((void**)&ctx->pinned[i], CHUNK, cudaHostAllocDefault));
+    }
+    ctx->pinned_bytes = CHUNK;
+  }
+  int b = 0;
+  size_t fill = 0;
+  auto flush = [&]() {
+    cudaError_t e = cudaMemcpyAsync(dst, ctx->pinned[b], fill, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaEventRecord(ctx->pinned_free[b], st);
+    dst += fill; fill = 0; b ^= 1;
+    return e;
+  };
+  for (auto& r : runs)
+    for (uint64_t done = 0; done < r.second;) {
+      if (fill == 0) SK_CUDA(cudaEventSynchronize(ctx->pinned_free[b]));     // the buffer's previous copy is done
+      const size_t n = (size_t)std::min<uint64_t>(ctx->pinned_bytes - fill, r.second - done);
+      parallel_memcpy(ctx, ctx->pinned[b] + fill, r.first + done, n);
+      fill += n; done += n;
+      if (fill == ctx->pinned_bytes) SK_CUDA(flush());
+    }
+  if (fill) SK_CUDA(flush());
+  return SK_OK;
 }
 
 // elements of blob array a in set s (ht_off is read for the table array only: a set growing in place extends it last)
@@ -301,6 +418,79 @@ int concat_sets(sk_ctx* ctx, const std::vector<const sk_sketch_set*>& parts, sk_
       dst += n * esz;
     }
   }
+  SK_CUDA(cudaStreamSynchronize(ctx->stream));
+  guard.s = nullptr;
+  *out = s;
+  return SK_OK;
+}
+
+// The end of sk_sketch_set_import_batch and sk_sketch_set_import_blobs.  s (owned from here on: freed on failure) holds the
+// host metadata: G, S, C, seed_off, ctg_off, ctg_len, total_len, name_rank.  rk / rp / rc hold the S records on the device,
+// genome g's at seed_off[g] in any order; mraw the markers, genome g's at raw_off[g].  Range checks, each genome's records
+// ordered by (contig, pos) ON THE DEVICE (one segmented radix sort over all genomes of the batch, so that a database of
+// tens of thousands of sketches imports at PCIe speed; src/search.rs deserialises and re-hashes per pair), the per-contig
+// first-record table with one sentinel per genome, then the views and hash tables.  rk / rp / rc are released before the
+// views are built.
+int import_finish(sk_ctx* ctx, sk_sketch_set* s, DTmp<uint32_t>& rk, DTmp<uint32_t>& rp, DTmp<uint32_t>& rc, DTmp<uint64_t>& mraw,
+                  const std::vector<uint64_t>& raw_off, sk_sketch_set** out) {
+  struct Guard { sk_sketch_set* s; ~Guard() { if (s) { free_set_device(s); delete s; } } } guard{s};
+  const uint32_t G = s->G;
+  const uint64_t n_records = s->S, n_contigs = s->C, n_markers = raw_off[G];
+  const sk_sketch_params* sp = &s->sp;
+  const size_t S1 = std::max<size_t>(n_records, 1);
+  SK_CUDA(ctx->arena.alloc((void**)&s->pv_kmer, S1 * 4)); SK_CUDA(ctx->arena.alloc((void**)&s->pv_pos, S1 * 4));
+  SK_CUDA(ctx->arena.alloc((void**)&s->pv_cc, S1 * 4));
+  SK_CUDA(ctx->arena.alloc((void**)&s->d_ctg_len, std::max<size_t>(n_contigs, 1) * 4));
+  SK_CUDA(ctx->arena.alloc((void**)&s->ctg_rec_off, (size_t)(n_contigs + G + 1) * 4));
+  cudaStream_t st = ctx->stream;
+  SK_CUDA(cudaStreamSynchronize(st));
+  if (n_contigs) SK_CUDA(cudaMemcpyAsync(s->d_ctg_len, s->ctg_len.data(), n_contigs * 4, cudaMemcpyHostToDevice, st));
+  {
+    DTmp<uint64_t> d_ro, d_co;
+    SK_CUDA(d_ro.alloc(G + 1, ctx)); SK_CUDA(d_co.alloc(G + 1, ctx));
+    SK_CUDA(h2d_small(ctx, d_ro.p, s->seed_off.data(), (G + 1) * 8));
+    SK_CUDA(h2d_small(ctx, d_co.p, s->ctg_off.data(), (G + 1) * 8));
+    DTmp<uint32_t> d_bad;
+    SK_CUDA(d_bad.alloc(1, ctx));
+    SK_CUDA(cudaMemsetAsync(d_bad.p, 0, 4, st));
+    enum { BAD_CONTIG = 1, BAD_MARKER = 2, BAD_KMER = 4 };
+    auto range_blocks = [](uint64_t n) { return (unsigned)std::min<uint64_t>((n + 255) / 256, 1024); };
+    if (n_markers) {
+      import_range_kernel<uint64_t><<<range_blocks(n_markers), 256, 0, st>>>(mraw.p, n_markers, 1ull << (2 * MARKER_K), d_bad.p, BAD_MARKER);
+      count_launch(ctx);
+    }
+    if (n_records) {
+      DTmp<uint32_t> vals, perm;
+      DTmp<uint64_t> keys, skeys;
+      SK_CUDA(vals.alloc(n_records, ctx)); SK_CUDA(perm.alloc(n_records, ctx)); SK_CUDA(keys.alloc(n_records, ctx)); SK_CUDA(skeys.alloc(n_records, ctx));
+      if (2 * sp->k < 32) {
+        import_range_kernel<uint32_t><<<range_blocks(n_records), 256, 0, st>>>(rk.p, n_records, 1ull << (2 * sp->k), d_bad.p, BAD_KMER);
+        count_launch(ctx);
+      }
+      import_keys_kernel<<<dim3(G, 8), 256, 0, st>>>(d_ro.p, rp.p, rc.p, keys.p, vals.p); count_launch(ctx);
+      size_t tb = 0;
+      SK_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb, keys.p, skeys.p, vals.p, perm.p, (int)n_records, (int)G, d_ro.p, d_ro.p + 1, 0, 62, st));
+      DTmp<uint8_t> tmp;
+      SK_CUDA(tmp.alloc(tb, ctx));
+      SK_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(tmp.p, tb, keys.p, skeys.p, vals.p, perm.p, (int)n_records, (int)G, d_ro.p, d_ro.p + 1, 0, 62, st));
+      count_launch(ctx);
+      import_gather_kernel<<<dim3(G, 8), 256, 0, st>>>(d_ro.p, perm.p, rk.p, rp.p, rc.p, s->pv_kmer, s->pv_pos, s->pv_cc); count_launch(ctx);
+      import_ctab_kernel<<<(unsigned)((n_contigs + G + 255) / 256), 256, 0, st>>>(d_ro.p, d_co.p, G, skeys.p, s->ctg_rec_off, d_bad.p); count_launch(ctx);
+      SK_CUDA(cudaStreamSynchronize(st));
+    } else {
+      SK_CUDA(cudaMemsetAsync(s->ctg_rec_off, 0, (size_t)(n_contigs + G + 1) * 4, st));
+    }
+    rk.release(); rp.release(); rc.release();
+    uint32_t bad = 0;
+    SK_CUDA(cudaMemcpyAsync(&bad, d_bad.p, 4, cudaMemcpyDeviceToHost, st));
+    SK_CUDA(cudaStreamSynchronize(st));
+    if (bad & BAD_MARKER) { ctx->err = "marker out of range (markers must be < 2^42)"; return SK_ERR_PARAM; }
+    if (bad & BAD_KMER) { ctx->err = "seed k-mer out of range (k-mers must be < 4^k)"; return SK_ERR_PARAM; }
+    if (bad & BAD_CONTIG) { ctx->err = "record contig index out of range"; return SK_ERR_PARAM; }
+  }
+  mbox_reset(ctx);                 // build_views takes pinned read-back space from the context's mailbox
+  SK_TRY(build_views(ctx, s, mraw.p, raw_off.data()));
+  SK_TRY(build_hash(ctx, s));
   SK_CUDA(cudaStreamSynchronize(ctx->stream));
   guard.s = nullptr;
   *out = s;
@@ -719,15 +909,7 @@ int sketch_batch_host(sk_ctx* ctx, const HostSeq& seq, const uint64_t* contig_of
   SK_TRY(check_sketch_params(ctx, sp));
   const bool prepacked = seq.units != nullptr;
   if (!prepacked && !seq.ascii && n_contigs && contig_off[n_contigs] > contig_off[0]) { ctx->err = "null sequence buffer"; return SK_ERR_PARAM; }
-  auto is_pinned = [](const void* p) {
-    if (!p) return false;
-    cudaPointerAttributes attr;
-    const bool pin = cudaPointerGetAttributes(&attr, p) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-    cudaGetLastError();
-    return pin;
-  };
-  // is the caller's buffer page-locked? then DMA straight from it; otherwise stage through our pinned buffers
-  const bool pinned_src = prepacked ? (is_pinned(seq.units) && (!seq.nmask || is_pinned(seq.nmask))) : is_pinned(seq.ascii);
+  const bool pinned_src = prepacked ? (host_pinned(seq.units) && (!seq.nmask || host_pinned(seq.nmask))) : host_pinned(seq.ascii);
   // sub-batch plan (whole genomes) + unit offset of every contig in the caller's packed layout
   struct Part { uint32_t c0, c1, g_begin, g_end; uint64_t b0, b1, units; };
   std::vector<Part> plan;
@@ -1152,10 +1334,6 @@ int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* sp, uint32_t
   sk_sketch_set* s = new sk_sketch_set();
   s->ctx = ctx; s->sp = *sp; s->G = G;
   struct Guard { sk_sketch_set* s; ~Guard() { if (s) { free_set_device(s); delete s; } } } guard{s};
-  // position view = each genome's records ordered by (contig, pos); per-contig first-record table with one sentinel per
-  // genome.  The records arrive in arbitrary (hash-map) order: they are sorted ON THE DEVICE (one segmented radix sort over
-  // all genomes of the batch), so that a database of tens of thousands of sketches imports at PCIe speed (src/search.rs
-  // deserialises and re-hashes per pair; here the host only concatenates)
   s->S = n_records; s->C = n_contigs;
   s->seed_off.resize(G + 1); s->ctg_off.resize(G + 1);
   for (uint32_t g = 0; g <= G; g++) { s->seed_off[g] = rec_off[g] - r0; s->ctg_off[g] = ctg_off[g] - c0; }
@@ -1169,72 +1347,126 @@ int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* sp, uint32_t
     s->total_len[g] = tl;
     s->name_rank[g] = g;
   }
-  const size_t S1 = std::max<size_t>(n_records, 1);
-  SK_CUDA(ctx->arena.alloc((void**)&s->pv_kmer, S1 * 4)); SK_CUDA(ctx->arena.alloc((void**)&s->pv_pos, S1 * 4));
-  SK_CUDA(ctx->arena.alloc((void**)&s->pv_cc, S1 * 4));
-  SK_CUDA(ctx->arena.alloc((void**)&s->d_ctg_len, std::max<size_t>(n_contigs, 1) * 4));
-  SK_CUDA(ctx->arena.alloc((void**)&s->ctg_rec_off, (size_t)(n_contigs + G + 1) * 4));
-  cudaStream_t st = ctx->stream;
-  SK_CUDA(cudaStreamSynchronize(st));
-  if (n_contigs) SK_CUDA(cudaMemcpyAsync(s->d_ctg_len, contig_lengths + c0, n_contigs * 4, cudaMemcpyHostToDevice, st));
-  DTmp<uint64_t> mraw;
-  {
-    DTmp<uint64_t> d_ro, d_co;
-    SK_CUDA(d_ro.alloc(G + 1, ctx)); SK_CUDA(d_co.alloc(G + 1, ctx));
-    SK_CUDA(h2d_small(ctx, d_ro.p, s->seed_off.data(), (G + 1) * 8));
-    SK_CUDA(h2d_small(ctx, d_co.p, s->ctg_off.data(), (G + 1) * 8));
-    DTmp<uint32_t> d_bad;
-    SK_CUDA(d_bad.alloc(1, ctx));
-    SK_CUDA(cudaMemsetAsync(d_bad.p, 0, 4, st));
-    enum { BAD_CONTIG = 1, BAD_MARKER = 2, BAD_KMER = 4 };
-    auto range_blocks = [](uint64_t n) { return (unsigned)std::min<uint64_t>((n + 255) / 256, 1024); };
-    SK_CUDA(mraw.alloc(n_markers, ctx));
-    if (n_markers) {
-      SK_CUDA(cudaMemcpyAsync(mraw.p, markers + m0, n_markers * 8, cudaMemcpyHostToDevice, st));
-      import_range_kernel<uint64_t><<<range_blocks(n_markers), 256, 0, st>>>(mraw.p, n_markers, 1ull << (2 * MARKER_K), d_bad.p, BAD_MARKER);
-      count_launch(ctx);
-    }
-    if (n_records) {
-      DTmp<uint32_t> rk, rp, rc, vals, perm;
-      DTmp<uint64_t> keys, skeys;
-      SK_CUDA(rk.alloc(n_records, ctx)); SK_CUDA(rp.alloc(n_records, ctx)); SK_CUDA(rc.alloc(n_records, ctx));
-      SK_CUDA(vals.alloc(n_records, ctx)); SK_CUDA(perm.alloc(n_records, ctx)); SK_CUDA(keys.alloc(n_records, ctx)); SK_CUDA(skeys.alloc(n_records, ctx));
-      SK_CUDA(cudaMemcpyAsync(rk.p, kmer + r0, n_records * 4, cudaMemcpyHostToDevice, st));
-      SK_CUDA(cudaMemcpyAsync(rp.p, pos + r0, n_records * 4, cudaMemcpyHostToDevice, st));
-      SK_CUDA(cudaMemcpyAsync(rc.p, cc + r0, n_records * 4, cudaMemcpyHostToDevice, st));
-      if (2 * sp->k < 32) {
-        import_range_kernel<uint32_t><<<range_blocks(n_records), 256, 0, st>>>(rk.p, n_records, 1ull << (2 * sp->k), d_bad.p, BAD_KMER);
-        count_launch(ctx);
-      }
-      import_keys_kernel<<<dim3(G, 8), 256, 0, st>>>(d_ro.p, rp.p, rc.p, keys.p, vals.p); count_launch(ctx);
-      size_t tb = 0;
-      SK_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb, keys.p, skeys.p, vals.p, perm.p, (int)n_records, (int)G, d_ro.p, d_ro.p + 1, 0, 62, st));
-      DTmp<uint8_t> tmp;
-      SK_CUDA(tmp.alloc(tb, ctx));
-      SK_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(tmp.p, tb, keys.p, skeys.p, vals.p, perm.p, (int)n_records, (int)G, d_ro.p, d_ro.p + 1, 0, 62, st));
-      count_launch(ctx);
-      import_gather_kernel<<<dim3(G, 8), 256, 0, st>>>(d_ro.p, perm.p, rk.p, rp.p, rc.p, s->pv_kmer, s->pv_pos, s->pv_cc); count_launch(ctx);
-      import_ctab_kernel<<<(unsigned)((n_contigs + G + 255) / 256), 256, 0, st>>>(d_ro.p, d_co.p, G, skeys.p, s->ctg_rec_off, d_bad.p); count_launch(ctx);
-      SK_CUDA(cudaStreamSynchronize(st));
-    } else {
-      SK_CUDA(cudaMemsetAsync(s->ctg_rec_off, 0, (size_t)(n_contigs + G + 1) * 4, st));
-    }
-    uint32_t bad = 0;
-    SK_CUDA(cudaMemcpyAsync(&bad, d_bad.p, 4, cudaMemcpyDeviceToHost, st));
-    SK_CUDA(cudaStreamSynchronize(st));
-    if (bad & BAD_MARKER) { ctx->err = "marker out of range (markers must be < 2^42)"; return SK_ERR_PARAM; }
-    if (bad & BAD_KMER) { ctx->err = "seed k-mer out of range (k-mers must be < 4^k)"; return SK_ERR_PARAM; }
-    if (bad & BAD_CONTIG) { ctx->err = "record contig index out of range"; return SK_ERR_PARAM; }
-  }
   std::vector<uint64_t> raw_off(G + 1);
   for (uint32_t g = 0; g <= G; g++) raw_off[g] = mk_off[g] - m0;
-  mbox_reset(ctx);                 // build_views takes pinned read-back space from the context's mailbox
-  SK_TRY(build_views(ctx, s, mraw.p, raw_off.data()));
-  SK_TRY(build_hash(ctx, s));
-  SK_CUDA(cudaStreamSynchronize(ctx->stream));
+  cudaStream_t st = ctx->stream;
+  DTmp<uint64_t> mraw;
+  DTmp<uint32_t> rk, rp, rc;
+  SK_CUDA(mraw.alloc(n_markers, ctx));
+  if (n_markers) SK_CUDA(cudaMemcpyAsync(mraw.p, markers + m0, n_markers * 8, cudaMemcpyHostToDevice, st));
+  if (n_records) {
+    SK_CUDA(rk.alloc(n_records, ctx)); SK_CUDA(rp.alloc(n_records, ctx)); SK_CUDA(rc.alloc(n_records, ctx));
+    SK_CUDA(cudaMemcpyAsync(rk.p, kmer + r0, n_records * 4, cudaMemcpyHostToDevice, st));
+    SK_CUDA(cudaMemcpyAsync(rp.p, pos + r0, n_records * 4, cudaMemcpyHostToDevice, st));
+    SK_CUDA(cudaMemcpyAsync(rc.p, cc + r0, n_records * 4, cudaMemcpyHostToDevice, st));
+  }
   guard.s = nullptr;
-  *out = s;
-  return SK_OK;
+  return import_finish(ctx, s, rk, rp, rc, mraw, raw_off, out);
+}
+
+int sk_sketch_set_import_blobs(sk_ctx* ctx, const sk_sketch_params* sp, const uint8_t* bytes, const uint64_t* blob_off,
+                               const uint64_t* blob_len, uint32_t n_blobs, sk_sketch_set** out, uint32_t* bad_blob) {
+  if (bad_blob) *bad_blob = UINT32_MAX;
+  if (!ctx || !out || n_blobs == 0 || !bytes || !blob_off || !blob_len) return SK_ERR_PARAM;
+  SK_CUDA(cudaSetDevice(ctx->device));
+  SK_TRY(check_sketch_params(ctx, sp));
+  const uint32_t G = n_blobs;
+  auto refuse = [&](uint32_t g, const std::string& why) {
+    ctx->err = "sketch blob " + std::to_string(g) + ": " + why;
+    if (bad_blob) *bad_blob = g;
+    return SK_ERR_PARAM;
+  };
+  // ---- host: the framing of every blob (skdb::scan_entry), on the worker pool
+  std::vector<skdb::SketchScan> sc(G);
+  std::vector<std::string> why(G);
+  ctx_pool(ctx)->run(G, [&](size_t g) {
+    try {
+      sc[g] = skdb::scan_entry(bytes + blob_off[g], blob_len[g]);
+      const skdb::DiskParams& p = sc[g].params;
+      if (p.use_aa) why[g] = "amino-acid sketches are not supported";
+      else if (p.c != sp->c || p.k != sp->k || p.marker_c != sp->marker_c) why[g] = "sketch parameters differ from the call's";
+    } catch (const std::exception& e) { why[g] = e.what(); }
+  });
+  for (uint32_t g = 0; g < G; g++) if (!why[g].empty()) return refuse(g, why[g]);
+  // ---- descriptors (blob g's bytes land at dev_at in the device copy, the blobs back to back) and host metadata
+  sk_sketch_set* s = new sk_sketch_set();
+  s->ctx = ctx; s->sp = *sp; s->G = G;
+  struct Guard { sk_sketch_set* s; ~Guard() { if (s) { free_set_device(s); delete s; } } } guard{s};
+  std::vector<BlobDesc> desc(G);
+  std::vector<uint64_t> list_at, list_len, raw_off(G + 1, 0);
+  std::vector<std::pair<const uint8_t*, uint64_t>> runs;
+  s->ctg_off.assign(1, 0);
+  uint64_t K = 0, M = 0, dev_at = 0;
+  for (uint32_t g = 0; g < G; g++) {
+    const skdb::SketchScan& x = sc[g];
+    const uint8_t* p = bytes + blob_off[g];
+    desc[g] = BlobDesc{dev_at + x.keys_at, K, x.n_keys, list_at.size(), x.multi_at.size(), dev_at + x.markers_at, M, x.n_markers};
+    for (size_t j = 0; j < x.multi_at.size(); j++) { list_at.push_back(dev_at + x.multi_at[j]); list_len.push_back(x.multi_len[j]); }
+    for (uint64_t c = 0; c < x.n_ctg_len; c++) s->ctg_len.push_back(skdb::load_u32(p + x.ctg_len_at + 4 * c));
+    s->ctg_off.push_back(s->ctg_len.size());
+    s->total_len.push_back(x.total_len);
+    s->name_rank.push_back(g);
+    K += x.n_keys; M += x.n_markers;
+    raw_off[g + 1] = M;
+    if (!runs.empty() && runs.back().first + runs.back().second == p) runs.back().second += blob_len[g];   // adjacent in memory
+    else runs.push_back({p, blob_len[g]});
+    dev_at += blob_len[g];
+  }
+  s->C = s->ctg_len.size();
+  if (K + 1 >= (1ull << 31) || M >= (1ull << 31) || s->C >= (1ull << 31)) {
+    ctx->err = "import batch too large (>= 2^31 keys, markers or contigs): import in several batches and sk_sketch_set_append";
+    return SK_ERR_PARAM;
+  }
+  // ---- device: the bytes as stored, the count of every key's records, their exclusive scan, then the expansion.  The
+  //      bytes are released before import_finish takes its sort temporaries: the peak stays below sk_sketch_set_import_batch's
+  //      for the same records (bytes ~ 12 per record + 8 per marker, against 32 per record of sort temporaries there)
+  cudaStream_t st = ctx->stream;
+  DTmp<uint8_t> dbuf;
+  DTmp<BlobDesc> d_desc;
+  DTmp<uint64_t> d_list_at, d_list_len, key_rec, d_ro;
+  DTmp<uint32_t> d_bad;
+  SK_CUDA(dbuf.alloc(dev_at + 16, ctx));
+  SK_CUDA(d_desc.alloc(G, ctx)); SK_CUDA(d_list_at.alloc(list_at.size(), ctx)); SK_CUDA(d_list_len.alloc(list_len.size(), ctx));
+  SK_CUDA(key_rec.alloc(K + 1, ctx)); SK_CUDA(d_ro.alloc(G + 1, ctx)); SK_CUDA(d_bad.alloc(1, ctx));
+  SK_CUDA(cudaMemsetAsync(dbuf.p + dev_at, 0, 16, st));
+  SK_TRY(upload_runs(ctx, dbuf.p, runs, host_pinned(bytes)));
+  SK_CUDA(cudaMemcpyAsync(d_desc.p, desc.data(), G * sizeof(BlobDesc), cudaMemcpyHostToDevice, st));
+  if (!list_at.empty()) {
+    SK_CUDA(cudaMemcpyAsync(d_list_at.p, list_at.data(), list_at.size() * 8, cudaMemcpyHostToDevice, st));
+    SK_CUDA(cudaMemcpyAsync(d_list_len.p, list_len.data(), list_len.size() * 8, cudaMemcpyHostToDevice, st));
+  }
+  SK_CUDA(cudaMemsetAsync(d_bad.p, 0xFF, 4, st));
+  SK_CUDA(cudaMemsetAsync(key_rec.p + K, 0, 8, st));
+  if (K) { blob_count_kernel<<<dim3(G, 8), 256, 0, st>>>(dbuf.p, d_desc.p, d_list_len.p, key_rec.p, d_bad.p); count_launch(ctx); }
+  {
+    size_t tb = 0;
+    SK_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, key_rec.p, key_rec.p, (int)(K + 1), st));
+    DTmp<uint8_t> tmp;
+    SK_CUDA(tmp.alloc(tb, ctx));
+    SK_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, key_rec.p, key_rec.p, (int)(K + 1), st));
+    count_launch(ctx);
+  }
+  blob_rec_off_kernel<<<(G + 256) / 256, 256, 0, st>>>(d_desc.p, G, K, key_rec.p, d_ro.p); count_launch(ctx);
+  s->seed_off.resize(G + 1);
+  uint32_t bad = UINT32_MAX;
+  SK_CUDA(cudaMemcpyAsync(s->seed_off.data(), d_ro.p, (G + 1) * 8, cudaMemcpyDeviceToHost, st));
+  SK_CUDA(cudaMemcpyAsync(&bad, d_bad.p, 4, cudaMemcpyDeviceToHost, st));
+  SK_CUDA(cudaStreamSynchronize(st));
+  if (bad != UINT32_MAX) return refuse(bad, "multi-position index out of range");
+  s->S = s->seed_off[G];
+  if (s->S >= (1ull << 31)) { ctx->err = "import batch too large (>= 2^31 records): import in several batches and sk_sketch_set_append"; return SK_ERR_PARAM; }
+  DTmp<uint32_t> rk, rp, rc;
+  DTmp<uint64_t> mraw;
+  SK_CUDA(rk.alloc(s->S, ctx)); SK_CUDA(rp.alloc(s->S, ctx)); SK_CUDA(rc.alloc(s->S, ctx)); SK_CUDA(mraw.alloc(M, ctx));
+  if (s->S) {
+    blob_expand_kernel<<<dim3(G, 8), 256, 0, st>>>(dbuf.p, d_desc.p, d_list_at.p, d_list_len.p, key_rec.p, rk.p, rp.p, rc.p);
+    count_launch(ctx);
+  }
+  if (M) { blob_markers_kernel<<<dim3(G, 8), 256, 0, st>>>(dbuf.p, d_desc.p, mraw.p); count_launch(ctx); }
+  SK_CUDA(cudaGetLastError());
+  dbuf.release(); key_rec.release(); d_list_at.release(); d_list_len.release(); d_desc.release();
+  guard.s = nullptr;
+  return import_finish(ctx, s, rk, rp, rc, mraw, raw_off, out);
 }
 
 int sk_sketch_set_import(sk_ctx* ctx, const sk_sketch_params* sp, const uint32_t* kmer, const uint32_t* pos,

@@ -260,6 +260,31 @@ def import_sketches(ctx, sketches, sp=None, seeds=True):
     return SketchSet(ctx, h)
 
 
+class BlobError(SkaniError):
+    """sk_sketch_set_import_blobs refused a blob: .blob is its index (None when the error is not a blob's)."""
+    def __init__(self, msg, blob):
+        super().__init__(msg)
+        self.blob = blob
+
+
+def import_blobs(ctx, data, offsets, lengths, sp=None):
+    """Device sketch set from skani v0.3 sketch blobs as stored (.sketch file bytes or sketches.db slices located by
+    index.db): blob g = data[offsets[g]:offsets[g] + lengths[g]], expanded on the device.  data: bytes or a uint8 array
+    (pinned or pageable host memory).  Raises BlobError naming the first blob that does not decode."""
+    sp = sp or sketch_params()
+    buf = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8)
+    off = np.ascontiguousarray(offsets, np.uint64)
+    ln = np.ascontiguousarray(lengths, np.uint64)
+    if len(off) != len(ln) or (len(off) and int((off + ln).max()) > len(buf)):
+        raise ValueError("blob offsets / lengths outside the data")
+    h, bad = C.c_void_p(), C.c_uint32()
+    rc = ctx.L.sk_sketch_set_import_blobs(ctx.h, C.byref(sp), buf.ctypes.data if len(buf) else None, off.ctypes.data, ln.ctypes.data,
+                                          len(off), C.byref(h), C.byref(bad))
+    if rc != 0:
+        raise BlobError("rc=%d: %s" % (rc, ctx.L.sk_last_error(ctx.h).decode()), None if bad.value == 0xFFFFFFFF else bad.value)
+    return SketchSet(ctx, h)
+
+
 def _pairs_out(ctx, fn, *args):
     pp = C.POINTER(C.c_uint64)(); n = C.c_uint64()
     ctx.check(fn(*args, C.byref(pp), C.byref(n)))
