@@ -162,6 +162,35 @@ int sk_sketch_set_import_batch(sk_ctx* ctx, const sk_sketch_params* params, uint
 int sk_sketch_set_import_blobs(sk_ctx* ctx, const sk_sketch_params* params, const uint8_t* bytes, const uint64_t* blob_off,
                                const uint64_t* blob_len, uint32_t n_blobs, sk_sketch_set** out, uint32_t* bad_blob);
 
+/* Genomes [g0, g0 + n) of a set encoded on the device as skani v0.3 entries, byte for byte what the host writer
+ * (skani_b200/cli/sketch_db.hpp: put_params + put_sketch) writes for the same sketch:
+ *   SK_ENTRY_FULL     (SketchParams, Sketch): one sketches.db entry, or a whole .sketch file
+ *   SK_ENTRY_MARKERS  Sketch::get_markers_only, without params: one element of markers.bin's Vec<Sketch>
+ * k-mers ascend, each with its records in (contig, pos) order.  The set gives c, k, marker_c (SketchParams; the Sketch's
+ * marker_c field holds c, src/types.rs:347), total_sequence_length, contig lengths, records and markers;
+ * repetitive_kmers is 0 and both flags false.  The caller gives what the set does not hold, in sk_entry_meta (entry i is
+ * genome g0 + i):
+ *   file_name        names[name_off[i], name_off[i + 1])
+ *   contigs          contig names j in [contig_first[i], contig_first[i + 1]), name j = contig_names[contig_name_off[j],
+ *                    contig_name_off[j + 1]) (written as given, independently of the set's contig lengths)
+ *   contig_order     contig_order[i]
+ * sk_sketch_set_encode_sizes: entry_len[i] = the length of entry i (one count pass on the device for the full form).
+ * sk_sketch_set_encode: the entries back to back from out[0] (host memory, pinned or not; entry_len may be NULL).
+ * g0 + n past the set, an unknown form, missing or decreasing metadata, or out_cap below the entries' total give
+ * SK_ERR_PARAM.  n = 0 writes nothing.  At most 2^31 - 2 k-mers per call. */
+typedef enum { SK_ENTRY_FULL = 0, SK_ENTRY_MARKERS = 1 } sk_entry_form;
+typedef struct {
+  const char* names;
+  const uint64_t* name_off;          /* [n + 1] */
+  const char* contig_names;
+  const uint64_t* contig_name_off;   /* [contig_first[n] + 1] */
+  const uint64_t* contig_first;      /* [n + 1] */
+  const uint64_t* contig_order;      /* [n] */
+} sk_entry_meta;
+int sk_sketch_set_encode_sizes(const sk_sketch_set* set, uint32_t g0, uint32_t n, int form, const sk_entry_meta* meta, uint64_t* entry_len);
+int sk_sketch_set_encode(const sk_sketch_set* set, uint32_t g0, uint32_t n, int form, const sk_entry_meta* meta, uint8_t* out,
+                         uint64_t out_cap, uint64_t* entry_len);
+
 /* ---- multi-GPU plumbing (the reference is single-process; SURVEY.md section 8e): a sketch set is flattened into ONE
  *      device buffer + a small host metadata vector so that ranks can exchange sketches with a single NCCL all-gather
  *      over NVLink, then rebuilt (rank-major genome order) on every GPU.

@@ -11,6 +11,10 @@ class SketchParams(C.Structure):
     _fields_ = [("c", C.c_uint32), ("k", C.c_uint32), ("marker_c", C.c_uint32)]
 
 
+class EntryMeta(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("names", "name_off", "contig_names", "contig_name_off", "contig_first", "contig_order")]
+
+
 class MapParams(C.Structure):
     _fields_ = [("screen_val", C.c_double), ("min_aligned_frac", C.c_double), ("both_min_aligned_frac", C.c_double),
                 ("robust", C.c_int32), ("median", C.c_int32), ("learned_ani", C.c_int32), ("rescue_small", C.c_int32)]
@@ -71,6 +75,8 @@ SYMBOLS = [
     ("sk_sketch_set_import", i32, [vp, PP(SketchParams), vp, vp, vp, u64, vp, u64, vp, u32, PP(vp)]),
     ("sk_sketch_set_import_batch", i32, [vp, PP(SketchParams), u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, PP(vp)]),
     ("sk_sketch_set_import_blobs", i32, [vp, PP(SketchParams), vp, vp, vp, u32, PP(vp), PP(u32)]),
+    ("sk_sketch_set_encode_sizes", i32, [vp, u32, u32, i32, PP(EntryMeta), vp]),
+    ("sk_sketch_set_encode", i32, [vp, u32, u32, i32, PP(EntryMeta), vp, u64, vp]),
     ("sk_sketch_set_blob_size", i32, [vp, PP(u64), PP(u64)]),
     ("sk_sketch_set_pack", i32, [vp, vp, vp]),
     ("sk_sketch_set_unpack", i32, [vp, u32, vp, vp, PP(vp)]),

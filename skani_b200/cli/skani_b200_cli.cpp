@@ -14,6 +14,8 @@
 // that passed for some query exactly once, imports them to the device in one batch and chains every pair there.
 // --gpus N: dist and search split the references into contiguous blocks, one per GPU, and copy the query set to every GPU
 // (sk_screen_query_ref_multi / sk_chain_pairs_multi); the output is byte-identical to one GPU's.
+// sketch encodes the database entries on the GPU (sk_sketch_set_encode) and, with --gpus N, sketches each group of files
+// in N contiguous runs, one per GPU; the database is byte-identical for every N.
 // triangle and dist take pre-sketched inputs as .sketch files and as consolidated databases (sketch_db.hpp: SketchInputs),
 // read as stored and imported in groups of < 2^28 records (sk_sketch_set_import_blobs expands them on the device), so that
 // host memory holds one group's bytes at a time.
@@ -393,11 +395,16 @@ std::vector<size_t> split_balanced(const std::vector<uint64_t>& w, size_t W) {
 }
 
 // sorted files [f0, end) form the next group that goes through the GPU at once: at most 4096 files and about 8 GiB of
-// sequence (file sizes x 4, as gz inflates ~4x), at least one file
+// sequence (file sizes x 4, as gz inflates ~4x), at least one file.  SK_SKETCH_GROUP_FILES lowers the file bound (a test
+// hook: many groups from a few files).
 size_t file_group_end(const std::vector<std::string>& files, size_t f0) {
+  static const size_t max_files = [] {
+    const char* e = getenv("SK_SKETCH_GROUP_FILES");
+    return e ? (size_t)std::max(1ll, std::min(4096ll, atoll(e))) : (size_t)4096;
+  }();
   size_t f1 = f0;
   uint64_t bytes = 0;
-  while (f1 < files.size() && (f1 == f0 || (f1 - f0 < 4096 && bytes < (8ull << 30)))) {
+  while (f1 < files.size() && (f1 == f0 || (f1 - f0 < max_files && bytes < (8ull << 30)))) {
     struct stat st;
     bytes += stat(files[f1].c_str(), &st) == 0 ? (uint64_t)st.st_size * 4 : 0;
     f1++;
@@ -870,19 +877,54 @@ void make_dirs(const std::string& p) {
     if (i == p.size() || p[i] == '/') mkdir(p.substr(0, i).c_str(), 0777);
 }
 
-// device sketch g -> the host form the database writer takes (records grouped by k-mer, src/types.rs:253-277)
-skdb::HostSketch export_sketch(sk_ctx* ctx, const sk_sketch_set* set, uint32_t g, const Genome& meta, const sk_sketch_params& sp) {
-  uint64_t nr = 0, nk = 0, nm = 0, nc = 0, tl = 0;
-  CK(ctx, sk_sketch_set_genome_info(set, g, &nr, &nk, &nm, &nc, &tl));
-  skdb::HostSketch h;
-  h.file_name = meta.file_name; h.contigs = meta.contigs; h.contig_order = meta.contig_order; h.total_len = tl;
-  h.kmer.resize(nr); h.pos.resize(nr); h.cc.resize(nr); h.markers.resize(nm); h.contig_lengths.resize(nc);
-  CK(ctx, sk_sketch_set_export(set, g, h.kmer.data(), h.pos.data(), h.cc.data(), h.markers.data(), h.contig_lengths.data()));
-  h.c = sp.c; h.k = sp.k; h.marker_c = sp.c;     // the sketch's marker_c field holds c (Sketch::new, src/types.rs:347)
-  return h;
+// genomes [a, b) of a group as sk_entry_meta (the arrays it points into)
+struct EntryMetaArrays {
+  std::string names, contig_names;
+  std::vector<uint64_t> name_off{0}, contig_name_off{0}, contig_first{0}, contig_order;
+  EntryMetaArrays(const std::vector<Genome>& gs, size_t a, size_t b) {
+    for (size_t g = a; g < b; g++) {
+      names += gs[g].file_name;
+      name_off.push_back(names.size());
+      for (auto& c : gs[g].contigs) { contig_names += c; contig_name_off.push_back(contig_names.size()); }
+      contig_first.push_back(contig_name_off.size() - 1);
+      contig_order.push_back(gs[g].contig_order);
+    }
+  }
+  sk_entry_meta meta() const {
+    return sk_entry_meta{names.data(), name_off.data(), contig_names.data(), contig_name_off.data(), contig_first.data(), contig_order.data()};
+  }
+};
+
+// one context's run of a group encoded on the device (sk_sketch_set_encode): full entries and markers-only entries, each
+// form back to back
+struct EncodedRun {
+  std::vector<uint8_t, skdb::uninit_alloc<uint8_t>> full, mk;
+  std::vector<uint64_t> full_len, mk_len;
+};
+
+void encode_run(sk_ctx* ctx, const sk_sketch_set* set, const EntryMetaArrays& ma, EncodedRun& out) {
+  const uint32_t n = sk_sketch_set_n_genomes(set);
+  const sk_entry_meta m = ma.meta();
+  auto encode = [&](int form, std::vector<uint8_t, skdb::uninit_alloc<uint8_t>>& bytes, std::vector<uint64_t>& len) {
+    len.resize(n);
+    CK(ctx, sk_sketch_set_encode_sizes(set, 0, n, form, &m, len.data()));
+    uint64_t total = 0;
+    for (uint64_t l : len) total += l;
+    bytes.resize(total);
+    CK(ctx, sk_sketch_set_encode(set, 0, n, form, &m, bytes.data(), total, nullptr));
+  };
+  encode(SK_ENTRY_FULL, out.full, out.full_len);
+  encode(SK_ENTRY_MARKERS, out.mk, out.mk_len);
 }
 
+// `sketch`: the files go through the GPU in groups (file_group_end), three stages deep.  While the contexts sketch and encode
+// group n, a reader thread loads group n + 1 and a writer thread appends group n - 1's entries in database order,
+// (file_name, contig_order).  A group's genomes are cut into --gpus contiguous runs balanced by bases, one per context, and
+// the runs are written in order, so the output does not depend on --gpus.  Encoding waits for the previous group's writer:
+// host memory holds at most two groups of sequence (the one sketched, the one read) and one group's encoded entries.
 int run_sketch(Opts& op) {
+  using clk = std::chrono::steady_clock;
+  auto secs = [](clk::time_point t0) { return std::chrono::duration<double>(clk::now() - t0).count(); };
   resolve_presets(op);
   if (op.files.empty()) { fprintf(stderr, "ERROR No reference inputs found.\n"); return 1; }
   if (op.out.empty()) { fprintf(stderr, "ERROR an output folder is required (-o)\n"); return 1; }
@@ -892,48 +934,99 @@ int run_sketch(Opts& op) {
     fprintf(stderr, "WARN --separate-sketches combined with -i (individual contigs) is NOT compatible with `skani search`.\n");
   sk_ctx* ctx = nullptr;
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
+  const size_t W = (size_t)std::max(op.gpus, 1);
+  std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, W);
   sk_sketch_params sp{op.c, op.k, op.m};
   skdb::DiskParams dp;
   dp.c = op.c; dp.k = op.k; dp.marker_c = op.m;
   skdb::DbWriter w;
-  std::vector<skdb::HostSketch> sep_markers;
-  if (!op.separate_sketches && !w.open(op.out, dp)) { fprintf(stderr, "ERROR Failed to create consolidated database writer\n"); return 1; }
+  if (!w.open(op.out, dp, op.separate_sketches)) { fprintf(stderr, "ERROR Failed to create the sketch database writer in %s\n", op.out.c_str()); return 1; }
   std::vector<std::string> files = op.files;
   std::sort(files.begin(), files.end());
+  std::vector<size_t> fb{0};
+  while (fb.back() < files.size()) fb.push_back(file_group_end(files, fb.back()));
+  const size_t n_groups = fb.size() - 1;
+  double t_read = 0, t_sketch = 0, t_encode = 0, t_write = 0;
+  auto load = [&](size_t k, Inputs* in) {
+    const auto t0 = clk::now();
+    load_inputs(std::vector<std::string>(files.begin() + fb[k], files.begin() + fb[k + 1]), op.individual, std::max(op.threads, 1), *in);
+    t_read += secs(t0);
+  };
+  // the writer's group: its genomes, its runs' first genomes and their encoded entries
+  std::vector<Genome> wr_genomes;
+  std::vector<size_t> wr_bounds;
+  std::vector<EncodedRun> wr_enc;
+  std::atomic<bool> write_failed{false};
   size_t total = 0;
-  // files go through the GPU in groups (bounds the host copy of the sequences); database order = (file_name, contig_order)
-  for (size_t f0 = 0; f0 < files.size();) {
-    const size_t f1 = file_group_end(files, f0);
-    Inputs in;
-    load_inputs(std::vector<std::string>(files.begin() + f0, files.begin() + f1), op.individual, std::max(op.threads, 1), in);
-    f0 = f1;
-    if (in.genomes.empty()) continue;
-    sk_sketch_set* set = sketch(ctx, in, sp);
+  auto write_group = [&] {
+    const auto t0 = clk::now();
     size_t j_in_file = 0;
-    for (size_t g = 0; g < in.genomes.size(); g++) {
-      skdb::HostSketch h = export_sketch(ctx, set, (uint32_t)g, in.genomes[g], sp);
-      j_in_file = (g && in.genomes[g].file_name == in.genomes[g - 1].file_name) ? j_in_file + 1 : 0;
-      if (op.separate_sketches) {      // src/sketch.rs:38-101: <basename>.sketch, or <j>_<basename>.sketch with -i
-        std::string name = op.out + "/" + (op.individual ? std::to_string(j_in_file) + "_" : std::string()) + base_name(h.file_name) + ".sketch";
-        skdb::Out o;
-        skdb::put_params(o, dp);
-        skdb::put_sketch(o, h);
-        if (!skdb::write_file(name, o.b)) { fprintf(stderr, "ERROR cannot write %s\n", name.c_str()); return 1; }
-        sep_markers.push_back(skdb::markers_only(h));
-      } else if (!w.add(h)) { fprintf(stderr, "ERROR Failed to add sketch to database\n"); return 1; }
-      if (++total % 100 == 0) fprintf(stderr, "INFO %zu sequences sketched.\n", total);
+    for (size_t d = 0; d + 1 < wr_bounds.size() && !write_failed; d++) {
+      const EncodedRun& e = wr_enc[d];
+      uint64_t fo = 0, mo = 0;
+      for (size_t i = 0; i < wr_bounds[d + 1] - wr_bounds[d]; i++) {
+        const size_t g = wr_bounds[d] + i;
+        const Genome& ge = wr_genomes[g];
+        j_in_file = (g && ge.file_name == wr_genomes[g - 1].file_name) ? j_in_file + 1 : 0;
+        std::string path;        // src/sketch.rs:38-101: <basename>.sketch, or <j>_<basename>.sketch with -i
+        if (op.separate_sketches) path = op.out + "/" + (op.individual ? std::to_string(j_in_file) + "_" : std::string()) + base_name(ge.file_name) + ".sketch";
+        if (!w.add(ge.file_name, path, e.full.data() + fo, e.full_len[i], e.mk.data() + mo, e.mk_len[i])) {
+          if (op.separate_sketches) fprintf(stderr, "ERROR cannot write %s\n", path.c_str());
+          else fprintf(stderr, "ERROR Failed to add sketch to database\n");
+          write_failed = true;
+          break;
+        }
+        fo += e.full_len[i]; mo += e.mk_len[i];
+        if (++total % 100 == 0) fprintf(stderr, "INFO %zu sequences sketched.\n", total);
+      }
     }
-    sk_sketch_set_free(set);
+    wr_enc.clear();
+    t_write += secs(t0);
+  };
+  Inputs cur, next;
+  std::thread reader, writer;
+  if (n_groups) load(0, &cur);
+  for (size_t k = 0; k < n_groups; k++) {
+    if (k + 1 < n_groups) reader = std::thread(load, k + 1, &next);
+    const size_t G = cur.genomes.size(), R = std::min(W, G);
+    std::vector<uint64_t> weight(G);
+    for (size_t g = 0; g < G; g++) weight[g] = cur.genomes[g].total_len;
+    const std::vector<size_t> gb = R ? split_balanced(weight, R) : std::vector<size_t>{0};
+    std::vector<sk_sketch_set*> sets(R, nullptr);
+    auto t0 = clk::now();
+    per_context(R, [&](size_t d) {
+      const size_t c0 = std::lower_bound(cur.genome_of_contig.begin(), cur.genome_of_contig.end(), (uint32_t)gb[d]) - cur.genome_of_contig.begin();
+      const size_t c1 = std::lower_bound(cur.genome_of_contig.begin(), cur.genome_of_contig.end(), (uint32_t)gb[d + 1]) - cur.genome_of_contig.begin();
+      std::vector<uint32_t> gl(c1 - c0);
+      for (size_t i = c0; i < c1; i++) gl[i - c0] = cur.genome_of_contig[i] - (uint32_t)gb[d];
+      CK(ctxs[d], sk_sketch_batch(ctxs[d], cur.bases.data(), cur.contig_off.data() + c0, (uint32_t)(c1 - c0), gl.data(), (uint32_t)(gb[d + 1] - gb[d]),
+                                  &sp, &sets[d]));
+    });
+    t_sketch += secs(t0);
+    std::vector<Genome> genomes = std::move(cur.genomes);
+    cur = Inputs();                                           // the group's sequence is no longer needed
+    if (writer.joinable()) writer.join();
+    if (write_failed) { if (reader.joinable()) reader.join(); return 1; }
+    std::vector<EncodedRun> enc(R);
+    t0 = clk::now();
+    per_context(R, [&](size_t d) {
+      encode_run(ctxs[d], sets[d], EntryMetaArrays(genomes, gb[d], gb[d + 1]), enc[d]);
+      sk_sketch_set_free(sets[d]);
+    });
+    t_encode += secs(t0);
+    wr_genomes = std::move(genomes); wr_bounds = gb; wr_enc = std::move(enc);
+    writer = std::thread(write_group);
+    if (reader.joinable()) reader.join();
+    cur = std::move(next);
+    next = Inputs();
   }
-  if (op.separate_sketches) {
-    skdb::Out mk;
-    skdb::put_params(mk, dp);
-    mk.u64(sep_markers.size());
-    for (auto& m : sep_markers) skdb::put_sketch(mk, m);
-    if (!skdb::write_file(op.out + "/markers.bin", mk.b)) { fprintf(stderr, "ERROR cannot write markers.bin\n"); return 1; }
-  } else if (!w.finalize()) { fprintf(stderr, "ERROR Failed to finalize consolidated database\n"); return 1; }
+  if (writer.joinable()) writer.join();
+  if (write_failed) return 1;
+  if (!w.finalize()) { fprintf(stderr, op.separate_sketches ? "ERROR cannot write markers.bin\n" : "ERROR Failed to finalize consolidated database\n"); return 1; }
+  fprintf(stderr, "INFO %zu sketches written in %zu group(s): read %.2f s, sketch %.2f s, encode %.2f s, write %.2f s.\n", total, n_groups, t_read,
+          t_sketch, t_encode, t_write);
   fprintf(stderr, "INFO Successfully wrote %zu sketches to %s\n", total, op.out.c_str());
-  sk_ctx_destroy(ctx);
+  for (size_t d = ctxs.size(); d-- > 0;) sk_ctx_destroy(ctxs[d]);
   return 0;
 }
 
@@ -1183,7 +1276,7 @@ void usage() {
           "  skani-b200 search -d sketch_folder [query ... | -q ... | --ql list] [--qi] [-n N] [-o out]\n"
           "  common: -c C -m M -k K -s SCREEN%% --min-af P --both-min-af P --robust --median --no-learned-ani --faster-small\n"
           "          --small-genomes --fast --medium --slow --ci --detailed --short-header --no-marker-index -t THREADS --device D\n"
-          "          --gpus N (triangle, dist, search: one context per GPU, devices D, D+1, ...)\n");
+          "          --gpus N (triangle, dist, search, sketch: one context per GPU, devices D, D+1, ...)\n");
 }
 
 }  // namespace

@@ -74,7 +74,7 @@ int main(int argc, char** argv) {
           case 'L': { size_t n; is >> n; s.contig_lengths.resize(n); for (auto& x : s.contig_lengths) is >> x; break; }
           case 'R': { size_t n; is >> n; s.kmer.resize(n); s.pos.resize(n); s.cc.resize(n); for (size_t i = 0; i < n; i++) is >> s.kmer[i] >> s.pos[i] >> s.cc[i]; break; }
           case 'M': { size_t n; is >> n; s.markers.resize(n); for (auto& x : s.markers) is >> x; break; }
-          case 'E': if (!w.add(s)) { fprintf(stderr, "write failed\n"); return 1; } break;
+          case 'E': if (!w.add(s, dp)) { fprintf(stderr, "write failed\n"); return 1; } break;
           default: break;
         }
       }

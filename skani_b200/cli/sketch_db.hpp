@@ -295,41 +295,66 @@ inline bool write_file(const std::string& path, const std::vector<uint8_t>& b) {
   return fclose(f) == 0 && w == b.size();
 }
 
-// consolidated database writer (SketchDbWriter, src/sketch_db.rs:17-84 + markers.bin, src/sketch.rs:141-146)
+// Database writer over encoded entries (SketchDbWriter, src/sketch_db.rs:17-84, + markers.bin, src/sketch.rs:141-146).
+// add() takes one full entry, (SketchParams, Sketch) as put_params + put_sketch or sk_sketch_set_encode write it, and the
+// same sketch's markers-only Sketch (put_sketch(markers_only(s))).  Consolidated, the entry is appended to sketches.db and
+// listed in index.db; with separate sketches it becomes the file sketch_path.  markers.bin is appended entry by entry and
+// its count filled in by finalize(), so the writer holds no sketches.
 struct DbWriter {
   std::string dir;
-  DiskParams params;
+  bool separate = false;
   FILE* concat = nullptr;
+  FILE* markers = nullptr;
+  long count_at = 0;                 // markers.bin: where the Vec<Sketch> length goes
   std::vector<IndexEntry> index;
-  std::vector<HostSketch> marker_sketches;
-  uint64_t offset = 0;
-  bool open(const std::string& d, const DiskParams& p) {
-    dir = d; params = p;
-    concat = fopen((dir + "/sketches.db").c_str(), "wb");
-    return concat != nullptr;
+  uint64_t offset = 0, n_markers = 0;
+  bool open(const std::string& d, const DiskParams& p, bool separate_sketches = false) {
+    dir = d; separate = separate_sketches;
+    if (!separate && !(concat = fopen((dir + "/sketches.db").c_str(), "wb"))) return false;
+    if (!(markers = fopen((dir + "/markers.bin").c_str(), "wb"))) return false;
+    Out head;
+    put_params(head, p);
+    count_at = (long)head.b.size();
+    head.u64(0);
+    return fwrite(head.b.data(), 1, head.b.size(), markers) == head.b.size();
   }
-  bool add(const HostSketch& s) {
-    Out o;
-    put_params(o, params);
+  bool add(const std::string& file_name, const std::string& sketch_path, const uint8_t* entry, uint64_t len, const uint8_t* marker_entry,
+           uint64_t marker_len) {
+    if (separate) {
+      FILE* f = fopen(sketch_path.c_str(), "wb");
+      if (!f) return false;
+      const bool ok = fwrite(entry, 1, len, f) == len;
+      if (fclose(f) != 0 || !ok) return false;
+    } else {
+      if (fwrite(entry, 1, len, concat) != len) return false;
+      index.push_back(IndexEntry{file_name, offset, len});
+      offset += len;
+    }
+    n_markers++;
+    return fwrite(marker_entry, 1, marker_len, markers) == marker_len;
+  }
+  bool add(const HostSketch& s, const DiskParams& p, const std::string& sketch_path = std::string()) {   // the host encoder
+    Out o, m;
+    put_params(o, p);
     put_sketch(o, s);
-    if (fwrite(o.b.data(), 1, o.b.size(), concat) != o.b.size()) return false;
-    index.push_back(IndexEntry{s.file_name, offset, (uint64_t)o.b.size()});
-    offset += o.b.size();
-    marker_sketches.push_back(markers_only(s));
-    return true;
+    put_sketch(m, markers_only(s));
+    return add(s.file_name, sketch_path, o.b.data(), o.b.size(), m.b.data(), m.b.size());
   }
   bool finalize() {
-    if (fclose(concat) != 0) return false;
-    concat = nullptr;
-    Out ix;
-    ix.u64(index.size());
-    for (auto& e : index) { ix.str(e.file_name); ix.u64(e.offset); ix.u64(e.length); }
-    if (!write_file(dir + "/index.db", ix.b)) return false;
-    Out mk;
-    put_params(mk, params);
-    mk.u64(marker_sketches.size());
-    for (auto& m : marker_sketches) put_sketch(mk, m);
-    return write_file(dir + "/markers.bin", mk.b);
+    if (concat) {
+      if (fclose(concat) != 0) return false;
+      concat = nullptr;
+      Out ix;
+      ix.u64(index.size());
+      for (auto& e : index) { ix.str(e.file_name); ix.u64(e.offset); ix.u64(e.length); }
+      if (!write_file(dir + "/index.db", ix.b)) return false;
+    }
+    Out n;
+    n.u64(n_markers);
+    const bool ok = fseek(markers, count_at, SEEK_SET) == 0 && fwrite(n.b.data(), 1, 8, markers) == 8;
+    const bool closed = fclose(markers) == 0;
+    markers = nullptr;
+    return ok && closed;
   }
 };
 

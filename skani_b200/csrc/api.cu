@@ -13,6 +13,7 @@
 #include <thread>
 
 #include "../cli/sketch_db.hpp"
+#include "entry_layout.cuh"
 #include "host_pack.hpp"
 #include "sk_core.cuh"
 #include "sk_internal.h"
@@ -249,6 +250,70 @@ __global__ void blob_markers_kernel(const uint8_t* __restrict__ buf, const BlobD
     mraw[d.mk0 + i] = load_u64_at(buf, d.markers_at + 8 * i);
 }
 
+// ---- sk_sketch_set_encode: skani v0.3 sketch entries written on the device (the inverse of the expansion above) ----------
+// Entry i of a chunk, laid out by skdb::entry_layout; offsets are absolute in the chunk's device buffer.  The host writes
+// the sections it owns (params, names, contig names and lengths, counts, tail) into host[host_at ...) as head | mid | tail.
+struct EncDesc {
+  uint64_t at, keys_at, multi_at, markers_at, mid_at, tail_at;   // entry start; first key; n_multi; first marker; mid; tail
+  uint64_t host_at, head_len, mid_len, tail_len;
+  uint64_t uk0, us0, rec0, mk0, f0;   // first ukmer, its ustart slot, first kv record, first marker, first key of the call
+  uint64_t nu, nm, n_multi;
+};
+// Entries start at any byte offset (names have any length): a store is one aligned word where it can be, bytes otherwise.
+__device__ __forceinline__ void store_u32_at(uint8_t* b, uint64_t at, uint32_t v) {
+  if ((at & 3) == 0) { *(uint32_t*)(b + at) = v; return; }
+  for (int i = 0; i < 4; i++) b[at + i] = (uint8_t)(v >> (8 * i));
+}
+__device__ __forceinline__ void store_u64_at(uint8_t* b, uint64_t at, uint64_t v) {
+  if ((at & 7) == 0) { *(uint64_t*)(b + at) = v; return; }
+  store_u32_at(b, at, (uint32_t)v);
+  store_u32_at(b, at + 4, (uint32_t)(v >> 32));
+}
+// multi[f0 + u] = 1 when unique k-mer u of the entry has two or more records
+__global__ void enc_count_kernel(const EncDesc* __restrict__ desc, const uint32_t* __restrict__ ustart, uint32_t* __restrict__ multi) {
+  const EncDesc d = desc[blockIdx.x];
+  for (uint64_t u = (uint64_t)blockIdx.y * blockDim.x + threadIdx.x; u < d.nu; u += (uint64_t)blockDim.x * gridDim.y)
+    multi[d.f0 + u] = ustart[d.us0 + u + 1] - ustart[d.us0 + u] > 1;
+}
+// n_multi of every entry from the exclusive scan of the flags
+__global__ void enc_n_multi_kernel(const EncDesc* __restrict__ desc, uint32_t n, const uint32_t* __restrict__ scan, uint64_t* __restrict__ n_multi) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) n_multi[i] = scan[desc[i].f0 + desc[i].nu] - scan[desc[i].f0];
+}
+// Key u with records kv [s, e): {k-mer, value}; a multi key's storage index is its rank r among the entry's multi keys (the
+// writer's storage++ order), and its list follows the r lists before it, which hold s - u + r records.
+__global__ void enc_write_kernel(const EncDesc* __restrict__ desc, const uint32_t* __restrict__ ukmer, const uint32_t* __restrict__ ustart,
+                                 const uint32_t* __restrict__ kv_pos, const uint32_t* __restrict__ kv_cc, const uint64_t* __restrict__ markers,
+                                 const uint32_t* __restrict__ scan, const uint8_t* __restrict__ host, uint8_t* __restrict__ out) {
+  const EncDesc d = desc[blockIdx.x];
+  const uint64_t t0 = (uint64_t)blockIdx.y * blockDim.x + threadIdx.x, step = (uint64_t)blockDim.x * gridDim.y;
+  if (d.nu) {
+    const uint32_t r0 = scan[d.f0];
+    for (uint64_t u = t0; u < d.nu; u += step) {
+      const uint64_t s = ustart[d.us0 + u], e = ustart[d.us0 + u + 1], at = d.keys_at + 12 * u;
+      store_u32_at(out, at, ukmer[d.uk0 + u]);
+      if (e - s == 1) {
+        store_u64_at(out, at + 4, skdb::single_value(kv_pos[d.rec0 + s], kv_cc[d.rec0 + s]));
+        continue;
+      }
+      const uint64_t r = scan[d.f0 + u] - r0, l = d.multi_at + 8 + 8 * r + 8 * (s - u + r);
+      store_u64_at(out, at + 4, skdb::multi_value(r));
+      store_u64_at(out, l, e - s);
+      for (uint64_t i = s; i < e; i++) {
+        store_u32_at(out, l + 8 + 8 * (i - s), kv_pos[d.rec0 + i]);
+        store_u32_at(out, l + 12 + 8 * (i - s), kv_cc[d.rec0 + i]);
+      }
+    }
+  }
+  if (scan && t0 == 0) store_u64_at(out, d.multi_at, d.n_multi);
+  for (uint64_t i = t0; i < d.nm; i += step) store_u64_at(out, d.markers_at + 8 * i, markers[d.mk0 + i]);
+  const uint64_t nh = d.head_len + d.mid_len + d.tail_len;
+  for (uint64_t i = t0; i < nh; i += step) {
+    const uint64_t dst = i < d.head_len ? d.at + i : i < d.head_len + d.mid_len ? d.mid_at + (i - d.head_len) : d.tail_at + (i - d.head_len - d.mid_len);
+    out[dst] = host[d.host_at + i];
+  }
+}
+
 __global__ void stage_copy_kernel(uint32_t* __restrict__ dst, const uint32_t* __restrict__ src, size_t n_words) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_words) dst[i] = src[i];
@@ -340,12 +405,8 @@ void parallel_memcpy(sk_ctx* ctx, void* dst, const void* src, size_t n) {
 
 // host byte runs, back to back, -> dst on ctx->stream: straight from page-locked memory, otherwise staged through the
 // context's two pinned buffers (one filled by the worker pool while the other is in flight)
-int upload_runs(sk_ctx* ctx, uint8_t* dst, const std::vector<std::pair<const uint8_t*, uint64_t>>& runs, bool pinned) {
-  cudaStream_t st = ctx->stream;
-  if (pinned) {
-    for (auto& r : runs) { SK_CUDA(cudaMemcpyAsync(dst, r.first, r.second, cudaMemcpyHostToDevice, st)); dst += r.second; }
-    return SK_OK;
-  }
+// the context's two pinned staging buffers, at least 64 MiB each
+int ensure_pinned_staging(sk_ctx* ctx) {
   const size_t CHUNK = 64ull << 20;
   if (ctx->pinned_bytes < CHUNK) {
     for (int i = 0; i < 2; i++) {
@@ -355,6 +416,16 @@ int upload_runs(sk_ctx* ctx, uint8_t* dst, const std::vector<std::pair<const uin
     }
     ctx->pinned_bytes = CHUNK;
   }
+  return SK_OK;
+}
+
+int upload_runs(sk_ctx* ctx, uint8_t* dst, const std::vector<std::pair<const uint8_t*, uint64_t>>& runs, bool pinned) {
+  cudaStream_t st = ctx->stream;
+  if (pinned) {
+    for (auto& r : runs) { SK_CUDA(cudaMemcpyAsync(dst, r.first, r.second, cudaMemcpyHostToDevice, st)); dst += r.second; }
+    return SK_OK;
+  }
+  SK_TRY(ensure_pinned_staging(ctx));
   int b = 0;
   size_t fill = 0;
   auto flush = [&]() {
@@ -373,6 +444,160 @@ int upload_runs(sk_ctx* ctx, uint8_t* dst, const std::vector<std::pair<const uin
     }
   if (fill) SK_CUDA(flush());
   return SK_OK;
+}
+
+// device bytes [src, src + n) -> host dst, synchronously: straight into page-locked memory, otherwise through the context's
+// two pinned buffers (the next piece in flight while the worker pool copies this one out)
+int download_bytes(sk_ctx* ctx, uint8_t* dst, const uint8_t* src, uint64_t n, bool pinned) {
+  cudaStream_t st = ctx->stream;
+  if (pinned) {
+    if (n) SK_CUDA(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, st));
+    SK_CUDA(cudaStreamSynchronize(st));
+    return SK_OK;
+  }
+  SK_TRY(ensure_pinned_staging(ctx));
+  const uint64_t P = ctx->pinned_bytes, pieces = (n + P - 1) / P;
+  auto issue = [&](uint64_t k) {
+    const int b = (int)(k & 1);
+    cudaError_t e = cudaMemcpyAsync(ctx->pinned[b], src + k * P, std::min(P, n - k * P), cudaMemcpyDeviceToHost, st);
+    return e == cudaSuccess ? cudaEventRecord(ctx->pinned_free[b], st) : e;
+  };
+  if (pieces) SK_CUDA(issue(0));
+  for (uint64_t k = 0; k < pieces; k++) {
+    if (k + 1 < pieces) SK_CUDA(issue(k + 1));     // its buffer was copied out in iteration k - 1
+    SK_CUDA(cudaEventSynchronize(ctx->pinned_free[k & 1]));
+    parallel_memcpy(ctx, dst + k * P, ctx->pinned[k & 1], (size_t)std::min(P, n - k * P));
+  }
+  SK_CUDA(cudaStreamSynchronize(st));
+  return SK_OK;
+}
+
+// ---- sk_sketch_set_encode: host side.  Genomes [g0, g0 + n) of s with the caller's metadata; n_multi is filled by
+// count_multi (full form) before layout() is called.
+struct EncodeJob {
+  const sk_sketch_set* s;
+  uint32_t g0, n;
+  bool full;
+  const sk_entry_meta* meta;
+  std::vector<EncDesc> desc;        // per entry: the set's indices; layout() adds the offsets (relative to the first entry)
+  std::vector<skdb::EntryLayout> lay;
+};
+
+int check_encode_args(sk_ctx* ctx, const sk_sketch_set* s, uint32_t g0, uint32_t n, int form, const sk_entry_meta* m) {
+  if (form != SK_ENTRY_FULL && form != SK_ENTRY_MARKERS) { ctx->err = "encode: unknown entry form"; return SK_ERR_PARAM; }
+  if ((uint64_t)g0 + n > s->G) { ctx->err = "encode: genomes [g0, g0 + n) outside the set"; return SK_ERR_PARAM; }
+  if (n == 0) return SK_OK;
+  if (!m || !m->names || !m->name_off || !m->contig_first || !m->contig_order || (m->contig_first[n] > m->contig_first[0] && (!m->contig_names || !m->contig_name_off))) {
+    ctx->err = "encode: metadata arrays missing"; return SK_ERR_PARAM;
+  }
+  for (uint32_t i = 0; i < n; i++)
+    if (m->name_off[i + 1] < m->name_off[i] || m->contig_first[i + 1] < m->contig_first[i]) { ctx->err = "encode: metadata offsets decrease"; return SK_ERR_PARAM; }
+  for (uint64_t j = m->contig_first[0]; j < m->contig_first[n]; j++)
+    if (m->contig_name_off[j + 1] < m->contig_name_off[j]) { ctx->err = "encode: contig name offsets decrease"; return SK_ERR_PARAM; }
+  return SK_OK;
+}
+
+void encode_job_init(EncodeJob& j) {
+  const sk_sketch_set* s = j.s;
+  j.desc.assign(j.n, EncDesc{});
+  uint64_t f = 0;
+  for (uint32_t i = 0; i < j.n; i++) {
+    const uint32_t g = j.g0 + i;
+    EncDesc& d = j.desc[i];
+    d.uk0 = s->uk_off[g]; d.us0 = s->uk_off[g] + g; d.rec0 = s->seed_off[g]; d.mk0 = s->mk_off[g]; d.f0 = f;
+    d.nu = j.full ? s->uk_off[g + 1] - s->uk_off[g] : 0;
+    d.nm = s->mk_off[g + 1] - s->mk_off[g];
+    f += d.nu;
+  }
+}
+
+// the n_multi of every entry (one count pass, a scan, one copy-back); scan keeps the exclusive sum of the multi flags
+int count_multi(sk_ctx* ctx, EncodeJob& j, DTmp<EncDesc>& d_desc, DTmp<uint32_t>& scan) {
+  cudaStream_t st = ctx->stream;
+  const uint64_t U = j.desc.back().f0 + j.desc.back().nu;
+  if (U + 1 >= (1ull << 31)) { ctx->err = "encode: >= 2^31 k-mers in one call: encode fewer genomes at a time"; return SK_ERR_PARAM; }
+  DTmp<uint64_t> d_nm;
+  SK_CUDA(d_desc.alloc(j.n, ctx)); SK_CUDA(scan.alloc(U + 1, ctx)); SK_CUDA(d_nm.alloc(j.n, ctx));
+  SK_CUDA(cudaMemcpyAsync(d_desc.p, j.desc.data(), j.n * sizeof(EncDesc), cudaMemcpyHostToDevice, st));
+  SK_CUDA(cudaMemsetAsync(scan.p + U, 0, 4, st));
+  if (U) { enc_count_kernel<<<dim3(j.n, 8), 256, 0, st>>>(d_desc.p, j.s->ustart, scan.p); count_launch(ctx); }
+  size_t tb = 0;
+  SK_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, scan.p, scan.p, (int)(U + 1), st));
+  {
+    DTmp<uint8_t> tmp;
+    SK_CUDA(tmp.alloc(tb, ctx));
+    SK_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, scan.p, scan.p, (int)(U + 1), st));
+    count_launch(ctx);
+  }
+  enc_n_multi_kernel<<<(j.n + 255) / 256, 256, 0, st>>>(d_desc.p, j.n, scan.p, d_nm.p); count_launch(ctx);
+  std::vector<uint64_t> nm(j.n);
+  SK_CUDA(cudaMemcpyAsync(nm.data(), d_nm.p, j.n * 8, cudaMemcpyDeviceToHost, st));
+  SK_CUDA(cudaStreamSynchronize(st));
+  for (uint32_t i = 0; i < j.n; i++) j.desc[i].n_multi = nm[i];
+  return SK_OK;
+}
+
+// every entry's layout and its offset from the first entry's first byte; returns the total length
+uint64_t encode_layout(EncodeJob& j) {
+  const sk_sketch_set* s = j.s;
+  const sk_entry_meta* m = j.meta;
+  j.lay.resize(j.n);
+  uint64_t at = 0;
+  for (uint32_t i = 0; i < j.n; i++) {
+    const uint32_t g = j.g0 + i;
+    EncDesc& d = j.desc[i];
+    skdb::EntryCounts c;
+    c.params = c.seeds = j.full;
+    c.name_len = m->name_off[i + 1] - m->name_off[i];
+    c.n_keys = d.nu; c.n_multi = d.n_multi;
+    c.n_records = j.full ? s->seed_off[g + 1] - s->seed_off[g] : 0;
+    c.n_contigs = m->contig_first[i + 1] - m->contig_first[i];
+    c.contig_name_bytes = c.n_contigs ? m->contig_name_off[m->contig_first[i + 1]] - m->contig_name_off[m->contig_first[i]] : 0;
+    c.n_contig_lengths = j.full ? s->ctg_off[g + 1] - s->ctg_off[g] : 0;
+    c.n_markers = d.nm;
+    const skdb::EntryLayout l = skdb::entry_layout(c);
+    j.lay[i] = l;
+    d.at = at;
+    d.keys_at = at + l.keys_at + 8; d.multi_at = at + l.multi_at; d.markers_at = at + l.markers_at + 8;
+    d.mid_at = at + l.contigs_at; d.tail_at = at + l.tail_at;
+    d.head_len = j.full ? l.keys_at + 8 : l.contigs_at;
+    d.mid_len = l.markers_at + 8 - l.contigs_at;
+    d.tail_len = skdb::TAIL_BYTES;
+    at += l.length;
+  }
+  return at;
+}
+
+// the host sections of entry i (head | mid | tail, as put_params + put_sketch write them) appended to o
+void encode_host_sections(const EncodeJob& j, uint32_t i, skdb::Out& o) {
+  const sk_sketch_set* s = j.s;
+  const sk_entry_meta* m = j.meta;
+  const uint32_t g = j.g0 + i;
+  const EncDesc& d = j.desc[i];
+  auto str = [&](const char* p, uint64_t n) { o.u64(n); o.b.insert(o.b.end(), p, p + n); };
+  if (j.full) {
+    skdb::DiskParams dp;
+    dp.c = s->sp.c; dp.k = s->sp.k; dp.marker_c = s->sp.marker_c;
+    skdb::put_params(o, dp);
+  }
+  str(m->names + m->name_off[i], m->name_off[i + 1] - m->name_off[i]);
+  o.u8(j.full ? 1 : 0);
+  o.u64(d.nu);                                   // n_keys (full) or multi_position_storage's empty length (markers-only)
+  o.u64(m->contig_first[i + 1] - m->contig_first[i]);
+  for (uint64_t c = m->contig_first[i]; c < m->contig_first[i + 1]; c++)
+    str(m->contig_names + m->contig_name_off[c], m->contig_name_off[c + 1] - m->contig_name_off[c]);
+  o.u64(s->total_len[g]);
+  if (j.full) {
+    o.u64(s->ctg_off[g + 1] - s->ctg_off[g]);
+    for (uint64_t c = s->ctg_off[g]; c < s->ctg_off[g + 1]; c++) o.u32(s->ctg_len[c]);
+  } else {
+    o.u64(0);
+  }
+  o.u64(0);                                      // repetitive_kmers
+  o.u64(d.nm);
+  o.u64(s->sp.c); o.u64(s->sp.c); o.u64(s->sp.k);   // marker_c field = c (src/types.rs:347)
+  o.u64(m->contig_order[i]);
+  o.u8(0); o.u8(0);                              // individual_contig, amino_acid
 }
 
 // elements of blob array a in set s (ht_off is read for the table array only: a set growing in place extends it last)
@@ -1474,6 +1699,70 @@ int sk_sketch_set_import(sk_ctx* ctx, const sk_sketch_params* sp, const uint32_t
                          const uint32_t* contig_lengths, uint32_t n_contigs, sk_sketch_set** out) {
   const uint64_t ro[2] = {0, n_records}, mo[2] = {0, n_markers}, co[2] = {0, n_contigs};
   return sk_sketch_set_import_batch(ctx, sp, 1, ro, kmer, pos, cc, mo, markers, co, contig_lengths, nullptr, out);
+}
+
+int sk_sketch_set_encode_sizes(const sk_sketch_set* s, uint32_t g0, uint32_t n, int form, const sk_entry_meta* meta, uint64_t* entry_len) {
+  if (!s) return SK_ERR_PARAM;
+  sk_ctx* ctx = s->ctx;
+  SK_TRY(check_encode_args(ctx, s, g0, n, form, meta));
+  if (n == 0) return SK_OK;
+  if (!entry_len) { ctx->err = "encode: entry_len is required"; return SK_ERR_PARAM; }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  EncodeJob j{s, g0, n, form == SK_ENTRY_FULL, meta, {}, {}};
+  encode_job_init(j);
+  DTmp<EncDesc> d_desc;
+  DTmp<uint32_t> scan;
+  if (j.full) SK_TRY(count_multi(ctx, j, d_desc, scan));
+  encode_layout(j);
+  for (uint32_t i = 0; i < n; i++) entry_len[i] = j.lay[i].length;
+  return SK_OK;
+}
+
+int sk_sketch_set_encode(const sk_sketch_set* s, uint32_t g0, uint32_t n, int form, const sk_entry_meta* meta, uint8_t* out, uint64_t out_cap,
+                         uint64_t* entry_len) {
+  if (!s) return SK_ERR_PARAM;
+  sk_ctx* ctx = s->ctx;
+  SK_TRY(check_encode_args(ctx, s, g0, n, form, meta));
+  if (n == 0) return SK_OK;
+  SK_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  EncodeJob j{s, g0, n, form == SK_ENTRY_FULL, meta, {}, {}};
+  encode_job_init(j);
+  DTmp<EncDesc> d_all;
+  DTmp<uint32_t> scan;
+  if (j.full) SK_TRY(count_multi(ctx, j, d_all, scan));
+  const uint64_t total = encode_layout(j);
+  if (!out || out_cap < total) { ctx->err = "encode: the output buffer holds " + std::to_string(out_cap) + " bytes, the entries take " + std::to_string(total); return SK_ERR_PARAM; }
+  if (entry_len) for (uint32_t i = 0; i < n; i++) entry_len[i] = j.lay[i].length;
+  const bool pinned = host_pinned(out);
+  // entries in chunks of about CHUNK bytes (at least one entry), each written into one device buffer and copied out
+  const uint64_t CHUNK = 1ull << 30;
+  for (uint32_t a = 0; a < n;) {
+    uint32_t b = a + 1;
+    while (b < n && j.desc[b].at + j.lay[b].length - j.desc[a].at <= CHUNK) b++;
+    const uint64_t base = j.desc[a].at, bytes = j.desc[b - 1].at + j.lay[b - 1].length - base;
+    std::vector<EncDesc> cd(j.desc.begin() + a, j.desc.begin() + b);
+    skdb::Out host;
+    for (uint32_t i = a; i < b; i++) {
+      EncDesc& d = cd[i - a];
+      d.at -= base; d.keys_at -= base; d.multi_at -= base; d.markers_at -= base; d.mid_at -= base; d.tail_at -= base;
+      d.host_at = host.b.size();
+      encode_host_sections(j, i, host);
+      if (host.b.size() - d.host_at != d.head_len + d.mid_len + d.tail_len) { ctx->err = "encode: host sections disagree with the entry layout"; return SK_ERR_STATE; }
+    }
+    DTmp<uint8_t> dbuf, dhost;
+    DTmp<EncDesc> d_desc;
+    SK_CUDA(dbuf.alloc(bytes, ctx)); SK_CUDA(dhost.alloc(host.b.size(), ctx)); SK_CUDA(d_desc.alloc(b - a, ctx));
+    SK_CUDA(cudaMemcpyAsync(d_desc.p, cd.data(), cd.size() * sizeof(EncDesc), cudaMemcpyHostToDevice, st));
+    SK_CUDA(cudaMemcpyAsync(dhost.p, host.b.data(), host.b.size(), cudaMemcpyHostToDevice, st));
+    enc_write_kernel<<<dim3(b - a, 8), 256, 0, st>>>(d_desc.p, s->ukmer, s->ustart, s->kv_pos, s->kv_cc, s->markers, j.full ? scan.p : nullptr,
+                                                     dhost.p, dbuf.p);
+    count_launch(ctx);
+    SK_CUDA(cudaGetLastError());
+    SK_TRY(download_bytes(ctx, out + base, dbuf.p, bytes, pinned));
+    a = b;
+  }
+  return SK_OK;
 }
 
 }  // extern "C"

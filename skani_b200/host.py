@@ -105,6 +105,46 @@ class SketchSet:
                                                        mk.ctypes.data, cl.ctypes.data))
         return dict(kmer=kmer, pos=pos, cc=cc, markers=mk, contig_lengths=cl)
 
+    def _entry_meta(self, g0, n, names, contigs, contig_order):
+        """sk_entry_meta of genomes [g0, g0 + n): names[i] (str or bytes), contigs[i] (list of names), contig_order[i]"""
+        enc = lambda s: s.encode() if isinstance(s, str) else bytes(s)          # noqa: E731
+        nm = [enc(x) for x in names]
+        cn = [[enc(x) for x in c] for c in contigs]
+        if not (len(nm) == len(cn) == len(contig_order) == n):
+            raise ValueError("names, contigs and contig_order need one entry per genome")
+        keep = dict(
+            names=np.frombuffer(b"".join(nm) + b"\0", np.uint8),
+            name_off=np.cumsum([0] + [len(x) for x in nm], dtype=np.uint64),
+            contig_names=np.frombuffer(b"".join(b"".join(c) for c in cn) + b"\0", np.uint8),
+            contig_name_off=np.cumsum([0] + [len(x) for c in cn for x in c], dtype=np.uint64),
+            contig_first=np.cumsum([0] + [len(c) for c in cn], dtype=np.uint64),
+            contig_order=np.ascontiguousarray(list(contig_order) + [0], np.uint64))
+        meta = _lib.EntryMeta(*[keep[f].ctypes.data for f, _ in _lib.EntryMeta._fields_])
+        return meta, keep
+
+    def encode_sizes(self, names, contigs, contig_order, g0=0, n=None, markers_only=False):
+        """Lengths of the skani v0.3 entries encode writes for genomes [g0, g0 + n)."""
+        n = len(self) - g0 if n is None else n
+        meta, _keep = self._entry_meta(g0, n, names, contigs, contig_order)
+        ln = np.zeros(max(n, 1), np.uint64)
+        self.ctx.check(self.ctx.L.sk_sketch_set_encode_sizes(self.h, g0, n, int(markers_only), C.byref(meta), ln.ctypes.data))
+        return ln[:n]
+
+    def encode(self, names, contigs, contig_order, g0=0, n=None, markers_only=False, out=None):
+        """Genomes [g0, g0 + n) as skani v0.3 entries, encoded on the device (sk_sketch_set_encode): (SketchParams, Sketch)
+        each (a sketches.db entry or .sketch file), or Sketch::get_markers_only (an element of markers.bin) with
+        markers_only.  names[i], contigs[i] and contig_order[i] are genome g0 + i's file name, contig names and
+        contig_order.  out: optional uint8 array (pinned or pageable) to write into.  Returns (bytes, entry lengths)."""
+        n = len(self) - g0 if n is None else n
+        meta, _keep = self._entry_meta(g0, n, names, contigs, contig_order)
+        if out is None:
+            out = np.empty(int(self.encode_sizes(names, contigs, contig_order, g0, n, markers_only).sum()), np.uint8)
+        ln = np.zeros(max(n, 1), np.uint64)
+        buf = out if len(out) else np.zeros(1, np.uint8)
+        self.ctx.check(self.ctx.L.sk_sketch_set_encode(self.h, g0, n, int(markers_only), C.byref(meta), buf.ctypes.data, len(out),
+                                                       ln.ctypes.data))
+        return out[:int(ln[:n].sum())], ln[:n]
+
     def set_name_ranks(self, ranks):
         """Order of the sketches' FILE names (equal names -> equal ranks): the tie-break of switch_qr
         (reference src/chain.rs:19-21) compares file names, and with -i / --qi / --ri all records of one file share a name."""
