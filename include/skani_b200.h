@@ -428,6 +428,36 @@ int sk_query_ref_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_stor
                        const sk_map_params* mp, int mode, uint64_t device_budget, sk_ani_result** out, uint64_t* n_out,
                        sk_store_stats* stats);
 
+/* ---- clustering of a triangle's results (what the reference leaves to scripts/clustermap_triangle.py or a host loop over
+ *      `triangle` output): genomes 0..n_genomes-1, results as sk_triangle / sk_triangle_store / sk_triangle_multi return them.
+ * Edges: the rows with ani > 0.1 (the rows `triangle -E` prints) and ani >= min_ani (a float comparison: ani == min_ani is an
+ * edge; NaN and -1 never are) join ref_id and query_id; the graph is undirected.  rank[g] is a permutation of 0..n-1, rank 0
+ * the first choice as a representative.
+ *   greedy (single_linkage = 0): genomes are visited in rank order and become representatives unless they have an edge to a
+ *     representative already chosen; every other genome is assigned to its representative neighbour of highest ANI, ties to
+ *     the smaller rank (that neighbour may rank after it).
+ *   single linkage: clusters are the connected components; a component's representative is its member of smallest rank.
+ * rep[g] = g's representative (g itself for a representative); cluster[g] = its cluster id, representatives numbered 0..C-1
+ * in rank order; edge[g] = the index in results of the row joining g to rep[g], UINT64_MAX for representatives and for
+ * single-linkage members not adjacent to their representative.  The outputs are a function of (edges, rank, method) alone.
+ * An id >= n_genomes, a self pair, a pair listed twice among the edges, a rank that is not a permutation, a NaN min_ani or
+ * NULL outputs give SK_ERR_PARAM with a message; edges that do not fit the device, or more than 2^30 - 1 of them, give
+ * SK_ERR_NOMEM.  n_genomes = 0 and inputs without edges are valid.  results is HOST memory (pinned or not), uploaded in
+ * chunks.
+ * stats (may be NULL): edges, clusters, rounds (greedy decision rounds or single-linkage hook passes) and t_device, the
+ * seconds from the first upload to the last read-back. */
+typedef struct {
+  float min_ani;           /* as a fraction, e.g. 0.95 */
+  int32_t single_linkage;  /* 0 = greedy representatives */
+} sk_cluster_params;
+typedef struct {
+  uint64_t n_edges;
+  uint32_t n_clusters, rounds;
+  double t_device;
+} sk_cluster_stats;
+int sk_cluster(sk_ctx* ctx, uint32_t n_genomes, const sk_ani_result* results, uint64_t n_results, const uint32_t* rank,
+               const sk_cluster_params* cp, uint32_t* rep, uint32_t* cluster, uint64_t* edge, sk_cluster_stats* stats /* may be NULL */);
+
 #ifdef __cplusplus
 }
 #endif

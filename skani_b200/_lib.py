@@ -47,6 +47,14 @@ class StoreStats(C.Structure):
                 ("max_working_set_bytes", C.c_uint64), ("t_screen", C.c_double), ("t_gather", C.c_double), ("t_chain", C.c_double)]
 
 
+class ClusterParams(C.Structure):
+    _fields_ = [("min_ani", C.c_float), ("single_linkage", C.c_int32)]
+
+
+class ClusterStats(C.Structure):
+    _fields_ = [("n_edges", C.c_uint64), ("n_clusters", C.c_uint32), ("rounds", C.c_uint32), ("t_device", C.c_double)]
+
+
 # every symbol include/skani_b200.h declares: (name, restype, argtypes)
 vp, u64, u32, i32 = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int
 PP = C.POINTER
@@ -115,6 +123,7 @@ SYMBOLS = [
     ("sk_sketch_store_free", i32, [vp]),
     ("sk_triangle_store", i32, [vp, u32, vp, PP(MapParams), u64, PP(PP(AniResult)), PP(u64), PP(StoreStats)]),
     ("sk_query_ref_store", i32, [vp, u32, vp, vp, PP(MapParams), i32, u64, PP(PP(AniResult)), PP(u64), PP(StoreStats)]),
+    ("sk_cluster", i32, [vp, u32, vp, u64, vp, PP(ClusterParams), vp, vp, vp, PP(ClusterStats)]),
 ]
 
 _lib = None

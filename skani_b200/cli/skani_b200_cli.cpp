@@ -1,4 +1,4 @@
-// skani_b200_cli.cpp -- `skani-b200 triangle|dist|sketch|search`: host driver over the C ABI (include/skani_b200.h).
+// skani_b200_cli.cpp -- `skani-b200 triangle|dist|sketch|search|cluster`: host driver over the C ABI (include/skani_b200.h).
 //
 // Mirrors the reference's command drivers:
 //   triangle  src/triangle.rs:13-169  (flags src/cli.rs:236-330, defaults src/parse.rs:790-921)
@@ -33,6 +33,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <string>
 #include <thread>
@@ -165,6 +166,8 @@ struct Opts {
   int threads = 3, device = 0, gpus = 1;
   std::string db_dir;               // search -d
   bool separate_sketches = false;   // sketch --separate-sketches
+  double cluster_ani = 95.0;        // cluster --ani (percent)
+  bool single_linkage = false;      // cluster --single-linkage
 };
 
 void write_header(FILE* o, bool ci, bool detailed) {   // src/file_io.rs:15-23
@@ -509,10 +512,18 @@ void warn_sketch_params(const Opts& op, const skdb::SketchInputs& si) {
             (unsigned long long)si.params.c, (unsigned long long)si.params.marker_c);
 }
 
-int run_triangle(Opts& op) {
+// One block of chained rows of the in-memory triangle; more = further blocks follow.  false ends the run (after an ERROR line).
+using BlockWriter = std::function<bool(const std::vector<sk_ani_result>& rows, bool more)>;
+
+// The triangle up to its writers, on every path (in memory, --gpus N through sk_triangle_multi, the host sketch store, sketch
+// inputs): in.genomes gets the genomes in genome-index order ((file_name, contig_order)), res the result of every screened pair
+// in the order the writers print them (they keep ani > 0.1), ctx the context on --device, which the caller destroys.  With
+// `stream`, the in-memory path chains and hands over the rows in blocks of INTERMEDIATE_WRITE_COUNT rows instead
+// (src/triangle.rs:113-138), so a long run leaves its finished rows on disk and holds at most one block of results in memory.
+// Returns 0, or the exit code after an ERROR line.
+int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_result>& res, const BlockWriter* stream) {
   resolve_presets(op);
   if (op.files.empty()) { fprintf(stderr, "ERROR No reference inputs found.\n"); return 1; }
-  Inputs in;
   const bool refs_are_sketch = sketch_inputs_given(op.files);
   skdb::SketchInputs si;
   if (refs_are_sketch) {      // .sketch files and databases (src/triangle.rs:16-24): opened here, decoded in groups below
@@ -527,7 +538,6 @@ int run_triangle(Opts& op) {
     load_inputs(op.files, op.individual, std::max(op.threads, 1), in);
     if (in.genomes.empty()) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }   // src/triangle.rs:46-49
   }
-  sk_ctx* ctx = nullptr;
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
   sk_sketch_params sp = refs_are_sketch ? params_of(si) : sk_sketch_params{op.c, op.k, op.m};
   sk_sketch_set* loaded = nullptr;
@@ -551,7 +561,7 @@ int run_triangle(Opts& op) {
     loaded = import_sketch_inputs(ctx, si, 0, si.entries.size(), std::max(op.threads, 1), sp, in.genomes.data(), ok);
     if (!ok) return 1;
   }
-  if (in.genomes.size() > 500 && !op.sparse) fprintf(stderr, "WARN > 500 genomes detected. The output matrix will be large. Consider using -E or --sparse for a tsv output instead.\n");
+  if (op.cmd == "triangle" && in.genomes.size() > 500 && !op.sparse) fprintf(stderr, "WARN > 500 genomes detected. The output matrix will be large. Consider using -E or --sparse for a tsv output instead.\n");
   sk_map_params mp{};
   mp.screen_val = op.s / 100.0;
   mp.min_aligned_frac = (op.min_af > -1e8 ? op.min_af : 15.0) / 100.0;
@@ -569,7 +579,6 @@ int run_triangle(Opts& op) {
       ranks[i] = rank;
     }
   }
-  std::vector<sk_ani_result> res;
   sk_sketch_set* set = nullptr;
   // sketch inputs: one INFO line gives the time of the screen and the chaining (with the "sketches loaded" line, the split
   // of a run from a database)
@@ -611,32 +620,25 @@ int run_triangle(Opts& op) {
     const auto t0 = clk::now();
     CK(ctx, sk_screen_triangle(ctx, set, &mp, &pairs, &np));
     timed(t0);
-    if (op.sparse) {
-      // sparse output: rows are chained and APPENDED in blocks of INTERMEDIATE_WRITE_COUNT rows (src/triangle.rs:113-138),
-      // so a long run leaves its finished rows on disk and holds at most one block of results in memory
-      FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
-      if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
-      write_header(o, op.ci, op.detailed);
-      if (op.diagonal) for (auto& g : in.genomes) write_perfect(o, g, op);
+    if (stream) {
       const size_t FL = intermediate_write_count(), Nrows = in.genomes.size();
       uint64_t p0 = 0;
-      for (size_t r0 = 0; r0 < Nrows; r0 += FL) {
+      bool ok = true;
+      for (size_t r0 = 0; r0 < Nrows && ok; r0 += FL) {
         uint64_t p1 = p0;
         while (p1 < np && (uint32_t)(pairs[p1] >> 32) < r0 + FL) p1++;      // pairs are sorted by (i, j)
         res.resize(p1 - p0);
         const auto t1 = clk::now();
         CK(ctx, sk_chain_pairs(ctx, set, set, pairs + p0, p1 - p0, &mp, res.data()));
         timed(t1);
-        for (auto& r : res) if (r.ani > 0.1f) write_row(o, r, in.genomes[r.ref_id], in.genomes[r.query_id], op);
-        fflush(o);
-        if (r0 + FL < Nrows) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", FL);
+        ok = (*stream)(res, r0 + FL < Nrows);
         p0 = p1;
       }
+      res.clear();
       sk_free(pairs);
-      if (o != stdout) fclose(o);
-      report_work();
       sk_sketch_set_free(set);
-      sk_ctx_destroy(ctx);
+      if (!ok) return 1;
+      report_work();
       return 0;
     }
     res.resize(np);
@@ -644,8 +646,35 @@ int run_triangle(Opts& op) {
     CK(ctx, sk_chain_pairs(ctx, set, set, pairs, np, &mp, res.data()));
     timed(t1);
     sk_free(pairs);
+    sk_sketch_set_free(set);
   }
   report_work();
+  return 0;
+}
+
+int run_triangle(Opts& op) {
+  Inputs in;
+  sk_ctx* ctx = nullptr;
+  std::vector<sk_ani_result> res;
+  FILE* so = nullptr;   // the sparse output, opened with the first streamed block
+  const BlockWriter stream = [&](const std::vector<sk_ani_result>& rows, bool more) {
+    if (!so) {
+      so = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
+      if (!so) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return false; }
+      write_header(so, op.ci, op.detailed);
+      if (op.diagonal) for (auto& g : in.genomes) write_perfect(so, g, op);
+    }
+    for (auto& r : rows) if (r.ani > 0.1f) write_row(so, r, in.genomes[r.ref_id], in.genomes[r.query_id], op);
+    fflush(so);
+    if (more) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", intermediate_write_count());
+    return true;
+  };
+  if (const int rc = triangle_results(op, in, ctx, res, op.sparse ? &stream : nullptr)) return rc;
+  if (so) {             // written block by block
+    if (so != stdout) fclose(so);
+    sk_ctx_destroy(ctx);
+    return 0;
+  }
   const size_t N = in.genomes.size();
   FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
   if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
@@ -688,7 +717,53 @@ int run_triangle(Opts& op) {
     fprintf(stderr, "INFO Aligned fraction matrix written to %s\n", af_name.c_str());
   }
   if (o != stdout) fclose(o);
-  if (set) sk_sketch_set_free(set);
+  sk_ctx_destroy(ctx);
+  return 0;
+}
+
+// cluster: the triangle's results (the rows `triangle -E` prints) clustered on the GPU by sk_cluster at ANI >= --ani, greedy
+// representatives or --single-linkage, genomes ranked by total sequence length (longest first, ties by genome index).  One TSV
+// row per genome in genome-index order: its representative, cluster, and the ANI / aligned fractions of the row joining them.
+int run_cluster(Opts& op) {
+  if (op.sparse || op.full_matrix || op.diagonal || op.distance || op.ci || op.detailed) {
+    fprintf(stderr, "ERROR -E/--sparse, --full-matrix, --diagonal, --distance, --ci and --detailed are triangle output options; cluster does not take them.\n");
+    return 2;
+  }
+  Inputs in;
+  sk_ctx* ctx = nullptr;
+  std::vector<sk_ani_result> all;
+  if (const int rc = triangle_results(op, in, ctx, all, nullptr)) return rc;
+  std::vector<sk_ani_result> res;
+  for (auto& r : all) if (r.ani > 0.1f) res.push_back(r);
+  all = std::vector<sk_ani_result>();
+  const uint32_t N = (uint32_t)in.genomes.size();
+  std::vector<uint32_t> order(N), rank(N), rep(N), cluster(N);
+  std::vector<uint64_t> edge(N);
+  for (uint32_t g = 0; g < N; g++) order[g] = g;
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return in.genomes[a].total_len > in.genomes[b].total_len; });
+  for (uint32_t i = 0; i < N; i++) rank[order[i]] = i;
+  const sk_cluster_params cp{(float)(op.cluster_ani / 100.0), op.single_linkage ? 1 : 0};
+  sk_cluster_stats st{};
+  CK(ctx, sk_cluster(ctx, N, res.data(), res.size(), rank.data(), &cp, rep.data(), cluster.data(), edge.data(), &st));
+  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
+  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
+  fprintf(o, "Genome_file\tRepresentative_file\tCluster\tANI\tAlign_fraction_genome\tAlign_fraction_representative\tGenome_name\tRepresentative_name\n");
+  for (uint32_t g = 0; g < N; g++) {
+    const Genome &gg = in.genomes[g], &rg = in.genomes[rep[g]];
+    fprintf(o, "%s\t%s\t%u\t", gg.file_name.c_str(), rg.file_name.c_str(), cluster[g]);
+    if (rep[g] == g) fputs("100.00\t100.00\t100.00", o);
+    else if (edge[g] == UINT64_MAX) fputs("NA\tNA\tNA", o);
+    else {
+      const sk_ani_result& r = res[edge[g]];
+      const bool is_ref = r.ref_id == g;
+      fprintf(o, "%.2f\t%.2f\t%.2f", (double)(r.ani * 100.f), (double)((is_ref ? r.af_ref : r.af_query) * 100.f),
+              (double)((is_ref ? r.af_query : r.af_ref) * 100.f));
+    }
+    fprintf(o, "\t%s\t%s\n", short_name(gg.contigs[0], op.short_header).c_str(), short_name(rg.contigs[0], op.short_header).c_str());
+  }
+  if (o != stdout) fclose(o);
+  fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (%s), clustering %.1f ms\n", N, st.n_clusters, op.cluster_ani,
+          op.single_linkage ? "single linkage" : "greedy", st.t_device * 1e3);
   sk_ctx_destroy(ctx);
   return 0;
 }
@@ -1274,9 +1349,12 @@ void usage() {
           "      index.db and sketches.db), mixed freely; a database stands for all of its sketches\n"
           "  skani-b200 sketch [fasta ... | -l list] -o new_folder [-i] [--separate-sketches]\n"
           "  skani-b200 search -d sketch_folder [query ... | -q ... | --ql list] [--qi] [-n N] [-o out]\n"
+          "  skani-b200 cluster [fasta | sketch ... | -l list] [-i] [--ani T] [--single-linkage] [-o out]\n"
+          "      the triangle's genomes clustered at ANI >= T %% (default 95, 10 < T <= 100): greedy representatives, longest\n"
+          "      genomes first, or --single-linkage components; one TSV row per genome with its representative and cluster\n"
           "  common: -c C -m M -k K -s SCREEN%% --min-af P --both-min-af P --robust --median --no-learned-ani --faster-small\n"
           "          --small-genomes --fast --medium --slow --ci --detailed --short-header --no-marker-index -t THREADS --device D\n"
-          "          --gpus N (triangle, dist, search, sketch: one context per GPU, devices D, D+1, ...)\n");
+          "          --gpus N (triangle, dist, search, sketch, cluster: one context per GPU, devices D, D+1, ...)\n");
 }
 
 }  // namespace
@@ -1285,7 +1363,7 @@ int main(int argc, char** argv) {
   if (argc < 2) { usage(); return 2; }
   Opts op;
   op.cmd = argv[1];
-  if (op.cmd != "triangle" && op.cmd != "dist" && op.cmd != "sketch" && op.cmd != "search" && op.cmd != "ingest") { usage(); return 2; }
+  if (op.cmd != "triangle" && op.cmd != "dist" && op.cmd != "sketch" && op.cmd != "search" && op.cmd != "ingest" && op.cmd != "cluster") { usage(); return 2; }
   std::vector<std::string> positional;
   enum { NONE, QS, RS } multi = NONE;
   for (int i = 2; i < argc; i++) {
@@ -1333,13 +1411,23 @@ int main(int argc, char** argv) {
     else if (a == "--device") op.device = atoi(val().c_str());
     else if (a == "-d") op.db_dir = val();
     else if (a == "--separate-sketches") op.separate_sketches = true;
+    else if (a == "--ani" && op.cmd == "cluster") {
+      const std::string v = val();
+      char* end = nullptr;
+      op.cluster_ani = strtod(v.c_str(), &end);
+      if (v.empty() || *end || !(op.cluster_ani > 10.0 && op.cluster_ani <= 100.0)) {
+        fprintf(stderr, "ERROR --ani %s: the threshold is a percentage in (10, 100] (rows with ANI <= 10 %% are never reported).\n", v.c_str());
+        return 2;
+      }
+    }
+    else if (a == "--single-linkage" && op.cmd == "cluster") op.single_linkage = true;
     else if (a == "--keep-refs") {}   // search already loads every passing reference exactly once
     else if (a == "-v" || a == "--debug" || a == "--trace") {}
     else { fprintf(stderr, "ERROR unknown option %s\n", a.c_str()); usage(); return 2; }
   }
-  if (op.cmd == "triangle" || op.cmd == "sketch" || op.cmd == "ingest") {
+  if (op.cmd == "triangle" || op.cmd == "sketch" || op.cmd == "ingest" || op.cmd == "cluster") {
     op.files.insert(op.files.end(), positional.begin(), positional.end());
-    return op.cmd == "triangle" ? run_triangle(op) : op.cmd == "sketch" ? run_sketch(op) : run_ingest(op);
+    return op.cmd == "triangle" ? run_triangle(op) : op.cmd == "sketch" ? run_sketch(op) : op.cmd == "cluster" ? run_cluster(op) : run_ingest(op);
   }
   if (op.cmd == "search") {
     op.queries.insert(op.queries.end(), positional.begin(), positional.end());

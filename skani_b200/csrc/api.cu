@@ -388,6 +388,9 @@ int check_sketch_params(sk_ctx* ctx, const sk_sketch_params* sp) {
   return SK_OK;
 }
 
+}  // namespace
+
+namespace sk {
 // is the caller's buffer page-locked? then DMA straight from it; otherwise stage through our pinned buffers
 bool host_pinned(const void* p) {
   if (!p) return false;
@@ -445,6 +448,9 @@ int upload_runs(sk_ctx* ctx, uint8_t* dst, const std::vector<std::pair<const uin
   if (fill) SK_CUDA(flush());
   return SK_OK;
 }
+}  // namespace sk
+
+namespace {
 
 // device bytes [src, src + n) -> host dst, synchronously: straight into page-locked memory, otherwise through the context's
 // two pinned buffers (the next piece in flight while the worker pool copies this one out)

@@ -253,4 +253,8 @@ cudaError_t zero_absent_arrays(sk_ctx* ctx, uint8_t* blob, const BlobLayout& b, 
 // screen.cu / chain.cu
 uint64_t count_launch(sk_ctx* ctx, uint64_t n = 1);
 cudaError_t h2d_small(sk_ctx* ctx, void* dst, const void* src, size_t bytes);  // api.cu
+bool host_pinned(const void* p);   // api.cu: is a host buffer page-locked?
+// host byte runs, back to back, -> device dst on ctx->stream: straight from page-locked memory (pinned), otherwise staged
+// through the context's two pinned buffers (api.cu)
+int upload_runs(sk_ctx* ctx, uint8_t* dst, const std::vector<std::pair<const uint8_t*, uint64_t>>& runs, bool pinned);
 }  // namespace sk

@@ -4,7 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import AniResult, ChainDebug, MapParams, SketchParams, StoreStats, TriangleStats
+from ._lib import AniResult, ChainDebug, ClusterParams, ClusterStats, MapParams, SketchParams, StoreStats, TriangleStats
 
 # numpy view of sk_ani_result (include/skani_b200.h): lets callers take 10^5..10^6 results without per-row Python objects
 RESULT_DTYPE = np.dtype([(n, np.float32) for n in ("ani", "af_query", "af_ref", "ci_lower", "ci_upper", "std", "q90_q", "q90_r", "q50_q",
@@ -651,3 +651,26 @@ def query_ref_store(ctxs, ref_store, query_store, mp=None, mode=0, device_budget
     c0.check(c0.L.sk_query_ref_store(hs, len(ctxs), None if ref_store is None else ref_store.h, None if query_store is None else query_store.h,
                                      C.byref(mp), int(mode), int(device_budget), C.byref(out), C.byref(n), C.byref(st)))
     return _take_results(c0, out, n, as_array), st
+
+
+NO_EDGE = np.uint64(0xFFFFFFFFFFFFFFFF)   # edge[g] of a representative (sk_cluster)
+
+
+def cluster(ctx, n_genomes, results, rank, min_ani=0.95, single_linkage=False):
+    """sk_cluster: ANI clustering of triangle results (a RESULT_DTYPE array, as as_array=True returns).  Edges are the rows with
+    ani > 0.1 and ani >= min_ani; rank[g] is a permutation, rank 0 the first choice as a representative.  Greedy
+    representatives by default, connected components with single_linkage.  Returns (rep, cluster, edge, stats): rep[g] and
+    cluster[g] (representatives numbered in rank order), edge[g] = the index in results of the row joining g to rep[g] or
+    NO_EDGE, and the ClusterStats."""
+    res = np.ascontiguousarray(results)
+    if res.dtype != RESULT_DTYPE:
+        raise TypeError("results must be a RESULT_DTYPE array")
+    rk = np.ascontiguousarray(rank, np.uint32)
+    if len(rk) != n_genomes:
+        raise ValueError("rank needs one entry per genome")
+    n = max(int(n_genomes), 1)
+    rep = np.zeros(n, np.uint32); cl = np.zeros(n, np.uint32); edge = np.zeros(n, np.uint64)
+    cp = ClusterParams(float(min_ani), int(bool(single_linkage))); st = ClusterStats()
+    ctx.check(ctx.L.sk_cluster(ctx.h, int(n_genomes), res.ctypes.data if len(res) else None, len(res), rk.ctypes.data if len(rk) else None,
+                               C.byref(cp), rep.ctypes.data, cl.ctypes.data, edge.ctypes.data, C.byref(st)))
+    return rep[:n_genomes], cl[:n_genomes], edge[:n_genomes], st
