@@ -11,7 +11,8 @@
 // All heavy work happens on the GPU through libskani_b200.so.  search keeps the reference's structure but not its memory
 // model: instead of deserialising a reference sketch from the mmap'd database for every passing pair
 // (src/search.rs:142-166) it screens ALL queries against ALL marker sketches in one GPU pass, loads each reference sketch
-// that passed for some query exactly once, imports them to the device in one batch and chains every pair there.
+// that passed for some query exactly once (per block of queries), imports them to the device in groups through the same
+// reader as triangle's and dist's sketch inputs, and chains every pair there.
 // --gpus N: dist and search split the references into contiguous blocks, one per GPU, and copy the query set to every GPU
 // (sk_screen_query_ref_multi / sk_chain_pairs_multi); the output is byte-identical to one GPU's.
 // sketch encodes the database entries on the GPU (sk_sketch_set_encode) and, with --gpus N, sketches each group of files
@@ -20,12 +21,11 @@
 // read as stored and imported in groups of < 2^28 records (sk_sketch_set_import_blobs expands them on the device), so that
 // host memory holds one group's bytes at a time.
 #include <dirent.h>
-#include <fcntl.h>
 #include <sys/stat.h>
-#include <unistd.h>
 #include <zlib.h>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <atomic>
 #include <cmath>
@@ -35,6 +35,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <numeric>
 #include <string>
 #include <thread>
 #include <vector>
@@ -201,12 +202,18 @@ void write_perfect(FILE* o, const Genome& g, const Opts& op) {   // write_ani_re
 
 #define CK(ctx, call) do { int rc__ = (call); if (rc__ != 0) { fprintf(stderr, "ERROR %s failed (%d): %s\n", #call, rc__, sk_last_error(ctx)); exit(1); } } while (0)
 
-sk_sketch_set* sketch(sk_ctx* ctx, const Inputs& in, const sk_sketch_params& sp) {
+// the genomes [g0, g1) of in sketched on ctx (genome g becomes the set's genome g - g0)
+sk_sketch_set* sketch(sk_ctx* ctx, const Inputs& in, const sk_sketch_params& sp, size_t g0, size_t g1) {
+  const auto& goc = in.genome_of_contig;
+  const size_t c0 = std::lower_bound(goc.begin(), goc.end(), (uint32_t)g0) - goc.begin();
+  const size_t c1 = std::lower_bound(goc.begin(), goc.end(), (uint32_t)g1) - goc.begin();
+  std::vector<uint32_t> gl(c1 - c0);
+  for (size_t i = c0; i < c1; i++) gl[i - c0] = goc[i] - (uint32_t)g0;
   sk_sketch_set* set = nullptr;
-  CK(ctx, sk_sketch_batch(ctx, in.bases.data(), in.contig_off.data(), (uint32_t)in.genome_of_contig.size(), in.genome_of_contig.data(),
-                          (uint32_t)in.genomes.size(), &sp, &set));
+  CK(ctx, sk_sketch_batch(ctx, in.bases.data(), in.contig_off.data() + c0, (uint32_t)(c1 - c0), gl.data(), (uint32_t)(g1 - g0), &sp, &set));
   return set;
 }
+sk_sketch_set* sketch(sk_ctx* ctx, const Inputs& in, const sk_sketch_params& sp) { return sketch(ctx, in, sp, 0, in.genomes.size()); }
 
 // INTERMEDIATE_WRITE_COUNT (src/params.rs:9): results are appended to the output every this many processed rows / queries
 // (src/triangle.rs:113-138, src/dist.rs:151-175, src/search.rs:255-279).  SK_INTERMEDIATE_WRITE_COUNT overrides it (tests).
@@ -261,14 +268,16 @@ bool sketch_inputs_given(const std::vector<std::string>& files) {
   return all;
 }
 
-// group bound of the sketch readers: < 2^28 seed records per sk_sketch_set_import_blobs call.  SK_SKETCH_GROUP_RECORDS
-// lowers it (a test hook: many groups from a small input).
-uint64_t sketch_group_records() {
+// group bound of the sketch readers: < `bound` seed records per sk_sketch_set_import_blobs call (2^28 for triangle and
+// dist).  SK_SKETCH_GROUP_RECORDS lowers it (a test hook: many groups from a small input).
+uint64_t sketch_group_records(uint64_t bound = 1ull << 28) {
   if (const char* e = getenv("SK_SKETCH_GROUP_RECORDS")) return (uint64_t)std::max(1ll, atoll(e));
-  return 1ull << 28;
+  return bound;
 }
 
-Genome genome_of(const skdb::SketchScan& h) {
+// the metadata of a scanned (skdb::SketchScan) or decoded (skdb::HostSketch) sketch
+template <class S>
+Genome genome_of(const S& h) {
   Genome g; g.file_name = h.file_name; g.contigs = h.contigs; g.contig_order = h.contig_order; g.total_len = h.total_len;
   if (g.contigs.empty()) g.contigs.push_back("");   // a sketch without contig names still prints
   return g;
@@ -293,14 +302,16 @@ sk_sketch_set* import_group(sk_ctx* ctx, const skdb::SketchGroup& g, const sk_sk
 template <class F>
 bool for_each_sketch_group(sk_ctx* ctx, const skdb::SketchInputs& si, size_t a, size_t b, int threads, const sk_sketch_params& sp, Genome* meta, F fn) {
   using clk = std::chrono::steady_clock;
-  skdb::SketchGroupReader rd(si, a, b, threads, sketch_group_records());
+  std::vector<size_t> list(b - a);
+  std::iota(list.begin(), list.end(), a);
+  skdb::SketchGroupReader rd(si, std::move(list), threads, sketch_group_records());
   skdb::SketchGroup g;
   double t_read = 0, t_import = 0;
   size_t groups = 0;
   for (auto t0 = clk::now(); rd.next(g); t0 = clk::now()) {
-    for (size_t i = 0; i < g.size(); i++) meta[rd.first + i - a] = genome_of(g.scan[i]);
+    for (size_t i = 0; i < g.size(); i++) meta[rd.first + i] = genome_of(g.scan[i]);
     const auto t1 = clk::now();
-    sk_sketch_set* s = import_group(ctx, g, sp, [&](size_t i) { return si.entries[rd.first + i].file_name; });
+    sk_sketch_set* s = import_group(ctx, g, sp, [&](size_t i) { return si.entries[a + rd.first + i].file_name; });
     if (!s) return false;
     fn(s);
     t_read += std::chrono::duration<double>(t1 - t0).count();
@@ -354,20 +365,26 @@ size_t n_inputs(const std::vector<std::string>& files, const skdb::SketchInputs&
   return n;
 }
 
-// --gpus N: contexts 1..n-1 next to ctx0, on (device + d) % device count.  With fewer devices than N the contexts share
-// devices (same code path; copies between them stay on the device).
-std::vector<sk_ctx*> make_contexts(sk_ctx* ctx0, const Opts& op, size_t n) {
-  std::vector<sk_ctx*> ctxs(1, ctx0);
-  if (op.gpus <= 1) return ctxs;
-  const int ndev = sk_device_count();
+// --gpus N: per_device contexts on each of n devices, device d being (device + d) % device count, ctx0 (on --device) first.
+// With fewer devices than N the contexts share devices (same code path; copies between them stay on the device).
+std::vector<sk_ctx*> make_contexts(sk_ctx* ctx0, const Opts& op, size_t n, int per_device = 1) {
+  const int ndev = std::max(sk_device_count(), 1);
   if (ndev < op.gpus) fprintf(stderr, "WARN --gpus %d but %d CUDA device(s) visible: contexts share devices.\n", op.gpus, ndev);
-  for (size_t d = 1; d < n; d++) {
-    const int dev = (op.device + (int)d) % std::max(ndev, 1);
-    sk_ctx* c = nullptr;
-    if (sk_ctx_create(dev, &c) != 0) { fprintf(stderr, "ERROR cannot create a context on GPU %d\n", dev); exit(1); }
-    ctxs.push_back(c);
-  }
+  std::vector<sk_ctx*> ctxs(1, ctx0);
+  for (size_t d = 0; d < n; d++)
+    for (int k = d == 0; k < per_device; k++) {
+      const int dev = (op.device + (int)d) % ndev;
+      sk_ctx* c = nullptr;
+      if (sk_ctx_create(dev, &c) != 0) { fprintf(stderr, "ERROR cannot create a context on GPU %d\n", dev); exit(1); }
+      ctxs.push_back(c);
+    }
   return ctxs;
+}
+
+// the share of -t threads of context d of n
+int context_threads(const Opts& op, size_t d, size_t n) {
+  const int t = std::max(op.threads, 1);
+  return std::max(1, t / (int)n + ((int)d < t % (int)n ? 1 : 0));
 }
 
 // fn(d) for d < n, one host thread per context
@@ -429,9 +446,15 @@ double sketch_bytes_estimate(const Opts& op, const std::vector<std::string>& fil
   }
   return sketches ? 3.0 * bytes : (double)bytes / op.c * 56.0 + (double)bytes / op.m * 24.0;
 }
+// SK_DEVICE_BUDGET_MB: the device bytes the store paths' working sets may take, and a request for the store path (a test
+// hook: the store path on small inputs); 0 when unset (the working sets are then sized from the free device memory)
+uint64_t device_budget() {
+  const char* e = getenv("SK_DEVICE_BUDGET_MB");
+  return e ? (uint64_t)std::max(1ll, atoll(e)) << 20 : 0;
+}
 // need bytes against 92 % of the device, or SK_DEVICE_BUDGET_MB asks for the store path
 bool exceeds_device(const Opts& op, double need) {
-  if (getenv("SK_DEVICE_BUDGET_MB")) return true;
+  if (device_budget()) return true;
   uint64_t free_b = 0, total_b = 0;
   if (sk_device_memory(op.device, &free_b, &total_b) != 0) return false;
   return need > 0.92 * (double)total_b;
@@ -464,6 +487,15 @@ bool dist_needs_store(const Opts& op, bool refs_sketch, bool queries_sketch, con
   return exceeds_device(op, need);
 }
 
+// the INFO line of the store paths (dist: the estimate per context, one store per side)
+void info_store_path(const Opts& op, double need_gb, bool dist) {
+  char on[64];
+  if (dist || op.gpus > 1) snprintf(on, sizeof(on), "%d GPU(s) from GPU %d", op.gpus, op.device);
+  else snprintf(on, sizeof(on), "GPU %d", op.device);
+  fprintf(stderr, "INFO Store path: sketches (~%.1f GB%s estimated) are kept in %s and chained in working sets on %s%s.\n", need_gb,
+          dist ? " per context" : "", dist ? "host sketch stores" : "a host sketch store", on, device_budget() ? " (SK_DEVICE_BUDGET_MB set)" : "");
+}
+
 // The store path of triangle and dist on FASTA inputs: files are sketched in groups, each group's set is added to a host
 // sketch store and freed, so device memory holds one group at a time and host memory one group of sequence plus the
 // sketches.  genomes gets the metadata of every genome in store order (= the order of the in-memory path).  Sketch inputs
@@ -489,27 +521,41 @@ sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, const std::vector<std::
   return st;
 }
 
-// the contexts of the store paths: two on each of the --gpus devices ((device + d) % count, shared when fewer are visible),
-// ctx0 first.  One context gathers its next working set over PCIe while the other chains.
-std::vector<sk_ctx*> store_contexts(sk_ctx* ctx0, const Opts& op) {
-  const int ndev = std::max(sk_device_count(), 1), gpus = std::max(op.gpus, 1);
-  if (ndev < gpus) fprintf(stderr, "WARN --gpus %d but %d CUDA device(s) visible: contexts share devices.\n", gpus, ndev);
-  std::vector<sk_ctx*> ctxs(1, ctx0);
-  for (int d = 0; d < gpus; d++)
-    for (int k = d == 0; k < 2; k++) {
-      const int dev = (op.device + d) % ndev;
-      sk_ctx* c = nullptr;
-      if (sk_ctx_create(dev, &c) != 0) { fprintf(stderr, "ERROR cannot create a context on GPU %d\n", dev); exit(1); }
-      ctxs.push_back(c);
-    }
-  return ctxs;
-}
-
 // "WARN Input parameter ..." of triangle's sketch inputs (src/triangle.rs:16-24); the sketches' parameters are used
 void warn_sketch_params(const Opts& op, const skdb::SketchInputs& si) {
   if (si.params.c != op.c || si.params.marker_c != op.m)
     fprintf(stderr, "WARN Input parameter c = %u, m = %u is not equal to the sketch parameter c = %llu,m = %llu. Using sketch parameters.\n", op.c, op.m,
             (unsigned long long)si.params.c, (unsigned long long)si.params.marker_c);
+}
+
+// the map parameters of triangle and dist (search sets its own); learned_ani = regression::use_learned_ani
+// (src/regression.rs:8-10) as the command decides it
+sk_map_params map_params(const Opts& op, bool learned_ani) {
+  sk_map_params mp{};
+  mp.screen_val = op.s / 100.0;
+  mp.min_aligned_frac = (op.min_af > -1e8 ? op.min_af : 15.0) / 100.0;
+  mp.both_min_aligned_frac = op.both_min_af / 100.0;
+  mp.robust = op.robust; mp.median = op.median;
+  mp.rescue_small = !op.faster_small && !op.small_genomes;
+  mp.learned_ani = learned_ani;
+  if (mp.learned_ani) fprintf(stderr, "INFO Learned ANI mode detected. ANI may be adjusted according to a regression model trained on MAGs.\n");
+  return mp;
+}
+
+// file-name order for the switch_qr tie-break (src/chain.rs:19-21): the names of a and b ranked together, equal names
+// sharing a rank (with -i all records of a file share its name); [0] holds a's ranks, [1] b's
+std::array<std::vector<uint64_t>, 2> name_ranks(const std::vector<Genome>& a, const std::vector<Genome>& b = {}) {
+  std::vector<std::pair<const std::string*, uint64_t*>> names;
+  std::array<std::vector<uint64_t>, 2> ranks{std::vector<uint64_t>(a.size()), std::vector<uint64_t>(b.size())};
+  for (size_t i = 0; i < a.size(); i++) names.push_back({&a[i].file_name, &ranks[0][i]});
+  for (size_t i = 0; i < b.size(); i++) names.push_back({&b[i].file_name, &ranks[1][i]});
+  std::sort(names.begin(), names.end(), [](auto& x, auto& y) { return *x.first < *y.first; });
+  uint64_t rank = 0;
+  for (size_t i = 0; i < names.size(); i++) {
+    if (i && *names[i].first != *names[i - 1].first) rank++;
+    *names[i].second = rank;
+  }
+  return ranks;
 }
 
 // One block of chained rows of the in-memory triangle; more = further blocks follow.  false ends the run (after an ERROR line).
@@ -543,12 +589,7 @@ int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_resu
   sk_sketch_set* loaded = nullptr;
   sk_sketch_store* store = nullptr;
   if (use_store) {
-    if (op.gpus > 1)
-      fprintf(stderr, "INFO Store path: sketches (~%.1f GB estimated) are kept in a host sketch store and chained in working sets on %d GPU(s) from GPU %d%s.\n",
-              need_gb, op.gpus, op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
-    else
-      fprintf(stderr, "INFO Store path: sketches (~%.1f GB estimated) are kept in a host sketch store and chained in working sets on GPU %d%s.\n", need_gb,
-              op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
+    info_store_path(op, need_gb, false);
     store = refs_are_sketch ? store_sketch_inputs(ctx, si, std::max(op.threads, 1), sp, in.genomes)
                             : fill_store(ctx, op, op.files, op.individual, in.genomes, sp);
     if (!store) {      // sketch inputs: an entry could not be loaded (reported)
@@ -562,40 +603,21 @@ int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_resu
     if (!ok) return 1;
   }
   if (op.cmd == "triangle" && in.genomes.size() > 500 && !op.sparse) fprintf(stderr, "WARN > 500 genomes detected. The output matrix will be large. Consider using -E or --sparse for a tsv output instead.\n");
-  sk_map_params mp{};
-  mp.screen_val = op.s / 100.0;
-  mp.min_aligned_frac = (op.min_af > -1e8 ? op.min_af : 15.0) / 100.0;
-  mp.both_min_aligned_frac = op.both_min_af / 100.0;
-  mp.robust = op.robust; mp.median = op.median;
-  mp.rescue_small = !op.faster_small && !op.small_genomes;
-  mp.learned_ani = !op.no_learned && op.c >= 70 && !op.individual && !op.median;   // regression::use_learned_ani (src/regression.rs:8-10)
-  if (mp.learned_ani) fprintf(stderr, "INFO Learned ANI mode detected. ANI may be adjusted according to a regression model trained on MAGs.\n");
-  // file-name order for the switch_qr tie-break (src/chain.rs:19-21): with -i all records of a file share its name
-  std::vector<uint64_t> ranks(in.genomes.size());
-  {
-    uint64_t rank = 0;
-    for (size_t i = 0; i < in.genomes.size(); i++) {
-      if (i && in.genomes[i].file_name != in.genomes[i - 1].file_name) rank++;
-      ranks[i] = rank;
-    }
-  }
-  sk_sketch_set* set = nullptr;
+  const sk_map_params mp = map_params(op, !op.no_learned && op.c >= 70 && !op.individual && !op.median);
+  const std::vector<uint64_t> ranks = name_ranks(in.genomes)[0];
   // sketch inputs: one INFO line gives the time of the screen and the chaining (with the "sketches loaded" line, the split
   // of a run from a database)
   using clk = std::chrono::steady_clock;
   double t_work = 0;
   auto timed = [&](clk::time_point t0) { t_work += std::chrono::duration<double>(clk::now() - t0).count(); };
-  auto report_work = [&] { if (refs_are_sketch) fprintf(stderr, "INFO Screen + chain %.2f s.\n", t_work); };
   if (store) {
-    // two contexts on each of the --gpus devices (store_contexts); every row is written at the end (no intermediate
-    // "Writing results" flushes in sparse mode)
+    // two contexts on each of the --gpus devices: one gathers its next working set over PCIe while the other chains.  Every
+    // row is written at the end (no intermediate "Writing results" flushes in sparse mode).
     CK(ctx, sk_sketch_store_set_name_ranks(store, ranks.data()));
-    std::vector<sk_ctx*> sctx = store_contexts(ctx, op);
-    uint64_t budget = 0;
-    if (const char* e = getenv("SK_DEVICE_BUDGET_MB")) budget = (uint64_t)std::max(1ll, atoll(e)) << 20;
+    std::vector<sk_ctx*> sctx = make_contexts(ctx, op, op.gpus, 2);
     sk_ani_result* r = nullptr; uint64_t nr = 0;
     const auto t0 = clk::now();
-    CK(ctx, sk_triangle_store(sctx.data(), (uint32_t)sctx.size(), store, &mp, budget, &r, &nr, nullptr));
+    CK(ctx, sk_triangle_store(sctx.data(), (uint32_t)sctx.size(), store, &mp, device_budget(), &r, &nr, nullptr));
     timed(t0);
     res.assign(r, r + nr);
     sk_free(r);
@@ -614,41 +636,32 @@ int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_resu
     std::sort(res.begin(), res.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
     for (size_t d = 1; d < ctxs.size(); d++) sk_ctx_destroy(ctxs[d]);
   } else {
-    set = loaded ? loaded : sketch(ctx, in, sp);
+    sk_sketch_set* set = loaded ? loaded : sketch(ctx, in, sp);
     sk_sketch_set_set_name_ranks(set, ranks.data());
     uint64_t* pairs = nullptr; uint64_t np = 0;
     const auto t0 = clk::now();
     CK(ctx, sk_screen_triangle(ctx, set, &mp, &pairs, &np));
     timed(t0);
-    if (stream) {
-      const size_t FL = intermediate_write_count(), Nrows = in.genomes.size();
-      uint64_t p0 = 0;
-      bool ok = true;
-      for (size_t r0 = 0; r0 < Nrows && ok; r0 += FL) {
-        uint64_t p1 = p0;
-        while (p1 < np && (uint32_t)(pairs[p1] >> 32) < r0 + FL) p1++;      // pairs are sorted by (i, j)
-        res.resize(p1 - p0);
-        const auto t1 = clk::now();
-        CK(ctx, sk_chain_pairs(ctx, set, set, pairs + p0, p1 - p0, &mp, res.data()));
-        timed(t1);
-        ok = (*stream)(res, r0 + FL < Nrows);
-        p0 = p1;
-      }
-      res.clear();
-      sk_free(pairs);
-      sk_sketch_set_free(set);
-      if (!ok) return 1;
-      report_work();
-      return 0;
+    // rows in blocks of FL: with `stream` each block is handed over and replaced by the next, without it the one block of
+    // all rows stays in res
+    const size_t N = in.genomes.size(), FL = stream ? intermediate_write_count() : N;
+    uint64_t p0 = 0;
+    bool ok = true;
+    for (size_t r0 = 0; r0 < N && ok; r0 += FL) {
+      uint64_t p1 = p0;
+      while (p1 < np && (uint32_t)(pairs[p1] >> 32) < r0 + FL) p1++;      // pairs are sorted by (i, j)
+      res.resize(p1 - p0);
+      const auto t1 = clk::now();
+      CK(ctx, sk_chain_pairs(ctx, set, set, pairs + p0, p1 - p0, &mp, res.data()));
+      timed(t1);
+      if (stream) ok = (*stream)(res, r0 + FL < N);
+      p0 = p1;
     }
-    res.resize(np);
-    const auto t1 = clk::now();
-    CK(ctx, sk_chain_pairs(ctx, set, set, pairs, np, &mp, res.data()));
-    timed(t1);
     sk_free(pairs);
     sk_sketch_set_free(set);
+    if (!ok) return 1;
   }
-  report_work();
+  if (refs_are_sketch) fprintf(stderr, "INFO Screen + chain %.2f s.\n", t_work);
   return 0;
 }
 
@@ -656,7 +669,7 @@ int run_triangle(Opts& op) {
   Inputs in;
   sk_ctx* ctx = nullptr;
   std::vector<sk_ani_result> res;
-  FILE* so = nullptr;   // the sparse output, opened with the first streamed block
+  FILE* so = nullptr;   // the sparse output, opened with the first block
   const BlockWriter stream = [&](const std::vector<sk_ani_result>& rows, bool more) {
     if (!so) {
       so = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
@@ -670,19 +683,14 @@ int run_triangle(Opts& op) {
     return true;
   };
   if (const int rc = triangle_results(op, in, ctx, res, op.sparse ? &stream : nullptr)) return rc;
-  if (so) {             // written block by block
-    if (so != stdout) fclose(so);
-    sk_ctx_destroy(ctx);
-    return 0;
-  }
-  const size_t N = in.genomes.size();
-  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
-  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
-  if (op.sparse) {   // write_sparse_matrix (src/file_io.rs:541-606); rows emitted in (i, j) order (the reference's order is arbitrary)
-    write_header(o, op.ci, op.detailed);
-    if (op.diagonal) for (auto& g : in.genomes) write_perfect(o, g, op);
-    for (auto& r : res) if (r.ani > 0.1f) write_row(o, r, in.genomes[r.ref_id], in.genomes[r.query_id], op);
-  } else {           // write_phyllip_matrix (src/file_io.rs:364-539)
+  // write_sparse_matrix (src/file_io.rs:541-606): rows in (i, j) order (the reference's order is arbitrary), written block by
+  // block on the in-memory path and here at once on the store and --gpus N paths
+  if (op.sparse && !so && !stream(res, false)) return 1;
+  FILE* o = so;
+  if (!op.sparse) {           // write_phyllip_matrix (src/file_io.rs:364-539)
+    const size_t N = in.genomes.size();
+    o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
+    if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
     std::map<std::pair<uint32_t, uint32_t>, const sk_ani_result*> m;
     for (auto& r : res) if (r.ani > 0.1f) m[{r.ref_id, r.query_id}] = &r;
     const double perfect = op.distance ? 0. : 100., none = 100. - perfect;
@@ -768,9 +776,11 @@ int run_cluster(Opts& op) {
   return 0;
 }
 
-// write_query_ref_list (src/file_io.rs:608-678) of dist: queries in blocks of INTERMEDIATE_WRITE_COUNT (src/dist.rs:151-175).
-// block(q0, q1, res) fills res with the results of the queries [q0, q1) in (query, ref) order; each block is grouped by the
-// query's first contig name, each group sorted by ANI (descending, stable) and its top n written, then flushed.
+// write_query_ref_list (src/file_io.rs:608-678) of dist and search: queries in blocks of INTERMEDIATE_WRITE_COUNT
+// (src/dist.rs:151-175, src/search.rs:255-279).  block(q0, q1, res) fills res with the results of the queries [q0, q1), rows
+// of equal ANI in the order they print, or returns false (after an ERROR line) to end the run with exit code 1.  Each block
+// is grouped by the query's first contig name, each group sorted by ANI (descending, stable) and its top n written, then
+// flushed.
 template <class F>
 int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vector<Genome>& queries, F block) {
   FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
@@ -778,8 +788,9 @@ int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vecto
   write_header(o, op.ci, op.detailed);
   const size_t FL = intermediate_write_count(), NQ = queries.size();
   std::vector<sk_ani_result> res;
+  int rc = 0;
   for (size_t q0 = 0; q0 < NQ; q0 += FL) {
-    block(q0, std::min(q0 + FL, NQ), res);
+    if (!block(q0, std::min(q0 + FL, NQ), res)) { rc = 1; break; }
     std::map<std::string, std::vector<const sk_ani_result*>> groups;
     for (auto& r : res) if (r.ani > 0.1f) groups[queries[r.query_id].contigs[0]].push_back(&r);
     for (auto& kv : groups) {
@@ -791,7 +802,7 @@ int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vecto
     if (q0 + FL < NQ) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", FL);
   }
   if (o != stdout) fclose(o);
-  return 0;
+  return rc;
 }
 
 int run_dist(Opts& op) {
@@ -830,8 +841,7 @@ int run_dist(Opts& op) {
   sk_sketch_store *rstore = nullptr, *qstore = nullptr;
   const int threads = std::max(op.threads, 1);
   if (use_store) {
-    fprintf(stderr, "INFO Store path: sketches (~%.1f GB per context estimated) are kept in host sketch stores and chained in working sets on %d GPU(s) from GPU %d%s.\n",
-            need_gb, std::max(op.gpus, 1), op.device, getenv("SK_DEVICE_BUDGET_MB") ? " (SK_DEVICE_BUDGET_MB set)" : "");
+    info_store_path(op, need_gb, true);
     rstore = refs_are_sketch ? store_sketch_inputs(ctx, rsi, threads, sp, rin.genomes) : fill_store(ctx, op, op.refs, op.ri, rin.genomes, sp);
     if (refs_are_sketch && !rstore) return 1;      // an entry could not be loaded (reported)
     qstore = queries_are_sketch ? store_sketch_inputs(ctx, qsi, threads, sp, qin.genomes) : fill_store(ctx, op, op.queries, op.qi, qin.genomes, sp);
@@ -844,38 +854,18 @@ int run_dist(Opts& op) {
     else for (auto& e : qsi.entries) { Genome g; g.file_name = e.file_name; qin.genomes.push_back(std::move(g)); }
   }
   if (rin.genomes.empty() || qin.genomes.empty()) { fprintf(stderr, "ERROR No reference sketches/genomes or query sketches/genomes found.\n"); return 1; }
-  sk_map_params mp{};
-  mp.screen_val = op.s / 100.0;
-  mp.min_aligned_frac = (op.min_af > -1e8 ? op.min_af : 15.0) / 100.0;
-  mp.both_min_aligned_frac = op.both_min_af / 100.0;
-  mp.robust = op.robust; mp.median = op.median;
-  mp.rescue_small = !op.faster_small && !op.small_genomes;
-  mp.learned_ani = !op.no_learned && op.c >= 70 && !op.qi && !op.ri && !op.median;
-  if (mp.learned_ani) fprintf(stderr, "INFO Learned ANI mode detected. ANI may be adjusted according to a regression model trained on MAGs.\n");
+  const sk_map_params mp = map_params(op, !op.no_learned && op.c >= 70 && !op.qi && !op.ri && !op.median);
   const bool use_index = (n_inputs(op.queries, qsi) > 50 || op.qi) && !op.no_marker_index;   // FULL_INDEX_THRESH (src/parse.rs:750)
-  // file-name order for the switch_qr tie-break (src/chain.rs:19-21): rank all names together
-  std::vector<uint64_t> rr(rin.genomes.size()), qr(qin.genomes.size());
-  {
-    std::vector<std::pair<std::string, std::pair<int, size_t>>> names;
-    for (size_t i = 0; i < rin.genomes.size(); i++) names.push_back({rin.genomes[i].file_name, {0, i}});
-    for (size_t i = 0; i < qin.genomes.size(); i++) names.push_back({qin.genomes[i].file_name, {1, i}});
-    std::sort(names.begin(), names.end(), [](auto& a, auto& b) { return a.first < b.first; });
-    uint64_t rank = 0;
-    for (size_t i = 0; i < names.size(); i++) {
-      if (i && names[i].first != names[i - 1].first) rank++;
-      (names[i].second.first ? qr : rr)[names[i].second.second] = rank;
-    }
-  }
+  const auto ranks = name_ranks(rin.genomes, qin.genomes);
+  const std::vector<uint64_t> &rr = ranks[0], &qr = ranks[1];
   if (use_store) {
     // two contexts on each of the --gpus devices: one gathers its next working set over PCIe while the other chains.  Every
     // block of queries is written at the end, through the same writer as the in-memory path.
     CK(ctx, sk_sketch_store_set_name_ranks(rstore, rr.data()));
     CK(ctx, sk_sketch_store_set_name_ranks(qstore, qr.data()));
-    std::vector<sk_ctx*> sctx = store_contexts(ctx, op);
-    uint64_t budget = 0;
-    if (const char* e = getenv("SK_DEVICE_BUDGET_MB")) budget = (uint64_t)std::max(1ll, atoll(e)) << 20;
+    std::vector<sk_ctx*> sctx = make_contexts(ctx, op, op.gpus, 2);
     sk_ani_result* r = nullptr; uint64_t nr = 0;
-    CK(ctx, sk_query_ref_store(sctx.data(), (uint32_t)sctx.size(), rstore, qstore, &mp, use_index ? 2 : 0, budget, &r, &nr, nullptr));
+    CK(ctx, sk_query_ref_store(sctx.data(), (uint32_t)sctx.size(), rstore, qstore, &mp, use_index ? 2 : 0, device_budget(), &r, &nr, nullptr));
     std::vector<sk_ani_result> all(r, r + nr);
     sk_free(r);
     std::sort(all.begin(), all.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.query_id != b.query_id ? a.query_id < b.query_id : a.ref_id < b.ref_id; });
@@ -885,6 +875,7 @@ int run_dist(Opts& op) {
       while (p1 < all.size() && all[p1].query_id < q1) p1++;
       res.assign(all.begin() + p0, all.begin() + p1);
       p0 = p1;
+      return true;
     });
     sk_sketch_store_free(rstore);
     sk_sketch_store_free(qstore);
@@ -905,16 +896,10 @@ int run_dist(Opts& op) {
   std::atomic<bool> load_failed{false};     // a sketch entry could not be loaded (reported); the run ends below
   per_context(W, [&](size_t d) {
     sk_ctx* c = ctxs[d];
-    const int t_ctx = std::max(1, threads / (int)W + ((int)d < threads % (int)W ? 1 : 0));
+    const int t_ctx = context_threads(op, d, W);
     bool ok = true;
     if (refs_are_sketch) rsets[d] = import_sketch_inputs(c, rsi, gb[d], gb[d + 1], t_ctx, sp, rin.genomes.data() + gb[d], ok);
-    else {
-      const size_t c0 = std::lower_bound(rin.genome_of_contig.begin(), rin.genome_of_contig.end(), (uint32_t)gb[d]) - rin.genome_of_contig.begin();
-      const size_t c1 = std::lower_bound(rin.genome_of_contig.begin(), rin.genome_of_contig.end(), (uint32_t)gb[d + 1]) - rin.genome_of_contig.begin();
-      std::vector<uint32_t> gl(c1 - c0);
-      for (size_t i = c0; i < c1; i++) gl[i - c0] = rin.genome_of_contig[i] - (uint32_t)gb[d];
-      CK(c, sk_sketch_batch(c, rin.bases.data(), rin.contig_off.data() + c0, (uint32_t)(c1 - c0), gl.data(), (uint32_t)(gb[d + 1] - gb[d]), &sp, &rsets[d]));
-    }
+    else rsets[d] = sketch(c, rin, sp, gb[d], gb[d + 1]);
     if (!ok) { load_failed = true; return; }
     sk_sketch_set_set_name_ranks(rsets[d], rr.data() + gb[d]);
     if (d == 0) {
@@ -938,6 +923,7 @@ int run_dist(Opts& op) {
     res.resize(p1 - p0);
     CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), byq.data() + p0, p1 - p0, &mp, res.data()));
     p0 = p1;
+    return true;
   });
   for (size_t d = 0; d < W; d++) { sk_sketch_set_free(rsets[d]); sk_sketch_set_free(qsets[d]); }
   for (size_t d = W; d-- > 0;) sk_ctx_destroy(ctxs[d]);
@@ -1069,14 +1055,7 @@ int run_sketch(Opts& op) {
     const std::vector<size_t> gb = R ? split_balanced(weight, R) : std::vector<size_t>{0};
     std::vector<sk_sketch_set*> sets(R, nullptr);
     auto t0 = clk::now();
-    per_context(R, [&](size_t d) {
-      const size_t c0 = std::lower_bound(cur.genome_of_contig.begin(), cur.genome_of_contig.end(), (uint32_t)gb[d]) - cur.genome_of_contig.begin();
-      const size_t c1 = std::lower_bound(cur.genome_of_contig.begin(), cur.genome_of_contig.end(), (uint32_t)gb[d + 1]) - cur.genome_of_contig.begin();
-      std::vector<uint32_t> gl(c1 - c0);
-      for (size_t i = c0; i < c1; i++) gl[i - c0] = cur.genome_of_contig[i] - (uint32_t)gb[d];
-      CK(ctxs[d], sk_sketch_batch(ctxs[d], cur.bases.data(), cur.contig_off.data() + c0, (uint32_t)(c1 - c0), gl.data(), (uint32_t)(gb[d + 1] - gb[d]),
-                                  &sp, &sets[d]));
-    });
+    per_context(R, [&](size_t d) { sets[d] = sketch(ctxs[d], cur, sp, gb[d], gb[d + 1]); });
     t_sketch += secs(t0);
     std::vector<Genome> genomes = std::move(cur.genomes);
     cur = Inputs();                                           // the group's sequence is no longer needed
@@ -1116,10 +1095,27 @@ int run_search(Opts& op) {
   catch (const std::exception& e) { fprintf(stderr, "ERROR Problem reading %s. Exiting. (%s)\n", marker_file.c_str(), e.what()); return 1; }
   if (dp.use_aa) { fprintf(stderr, "ERROR amino-acid databases are not supported\n"); return 1; }
   if (ref_mk.empty()) { fprintf(stderr, "ERROR No valid reference fastas or sketches found.\n"); return 1; }
+  std::vector<Genome> refs;
+  for (auto& h : ref_mk) refs.push_back(genome_of(h));
+  // the references' sketches as stored, entry r = reference r of markers.bin: the entries of index.db in index order, or the
+  // .sketch files <dir>/<basename(file_name)>.sketch (src/search.rs:157-166), whose sizes are read when a block of queries
+  // first needs them
   const bool consolidated = path_exists(op.db_dir + "/sketches.db") && path_exists(op.db_dir + "/index.db");   // src/sketch_db.rs:142-146
-  std::vector<skdb::IndexEntry> index;
-  int db_fd = -1;
-  if (consolidated && !skdb::open_db(op.db_dir, index, db_fd)) return 1;   // the reader of triangle's and dist's database inputs
+  skdb::SketchInputs rsi;
+  if (consolidated) {
+    std::vector<skdb::IndexEntry> index;
+    int fd = -1;
+    if (!skdb::open_db(op.db_dir, index, fd)) return 1;   // the reader of triangle's and dist's database inputs
+    rsi.paths.push_back(op.db_dir);
+    rsi.db_fd.push_back(fd);
+    for (auto& e : index) rsi.entries.push_back(skdb::SketchEntry{0, e.file_name, e.offset, e.length, e.length / 12});
+  } else {
+    for (size_t r = 0; r < refs.size(); r++) {
+      rsi.paths.push_back(op.db_dir + "/" + base_name(refs[r].file_name) + ".sketch");
+      rsi.db_fd.push_back(-1);
+      rsi.entries.push_back(skdb::SketchEntry{(uint32_t)r, refs[r].file_name, 0, 0, 0});
+    }
+  }
   sk_sketch_params sp{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
   sk_ctx* ctx = nullptr;
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
@@ -1142,12 +1138,7 @@ int run_search(Opts& op) {
     std::stable_sort(qs.begin(), qs.end(), [](const skdb::HostSketch& a, const skdb::HostSketch& b) { return a.file_name < b.file_name; });   // src/file_io.rs:715
     if (qs.empty()) { fprintf(stderr, "ERROR No query sketches found.\n"); return 1; }
     Flat f;
-    for (auto& h : qs) {
-      f.add(h, true);
-      Genome g; g.file_name = h.file_name; g.contigs = h.contigs; g.contig_order = h.contig_order; g.total_len = h.total_len;
-      if (g.contigs.empty()) g.contigs.push_back("");   // a .sketch without contig names still prints (as load_sketch_files does)
-      qmeta.push_back(std::move(g));
-    }
+    for (auto& h : qs) { f.add(h, true); qmeta.push_back(genome_of(h)); }
     qset = f.import(ctx, sp);
   } else {
     Inputs qin;
@@ -1177,151 +1168,79 @@ int run_search(Opts& op) {
   uint64_t* pairs = nullptr; uint64_t np = 0;
   CK(ctx, sk_screen_query_ref(ctx, rmk, qset, &mp, use_index ? 3 : 1, &pairs, &np));
   sk_sketch_set_free(rmk);
-  // file-name order for the switch_qr tie-break (src/chain.rs:19-21): rank all names together
-  std::vector<uint64_t> rrank(ref_mk.size()), qrank(qmeta.size());
-  {
-    std::vector<std::pair<const std::string*, std::pair<int, size_t>>> names;
-    for (size_t i = 0; i < ref_mk.size(); i++) names.push_back({&ref_mk[i].file_name, {0, i}});
-    for (size_t i = 0; i < qmeta.size(); i++) names.push_back({&qmeta[i].file_name, {1, i}});
-    std::sort(names.begin(), names.end(), [](auto& a, auto& b) { return *a.first < *b.first; });
-    uint64_t rank = 0;
-    for (size_t i = 0; i < names.size(); i++) {
-      if (i && *names[i].first != *names[i - 1].first) rank++;
-      (names[i].second.first ? qrank : rrank)[names[i].second.second] = rank;
-    }
-    sk_sketch_set_set_name_ranks(qset, qrank.data());
-  }
+  const auto ranks = name_ranks(refs, qmeta);
+  sk_sketch_set_set_name_ranks(qset, ranks[1].data());
   // --gpus N: the query set is copied to every context once; each query block's references are spread over them below
-  const size_t W = std::max(op.gpus, 1);
+  const size_t W = op.gpus;
   std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, W);
   std::vector<sk_sketch_set*> qsets(W, qset);
   for (size_t d = 1; d < W; d++) CK(ctxs[d], sk_sketch_set_copy(ctxs[d], qset, &qsets[d]));
   // ---- queries are processed, and their results appended, in blocks of INTERMEDIATE_WRITE_COUNT (src/search.rs:255-279).
   //      Inside a block: the references that passed for at least one of its queries ("hits") are loaded ONCE each and their
   //      pairs chained (the reference deserialises a sketch per passing PAIR, src/search.rs:142-166).  The hits are cut into
-  //      W contiguous runs balanced by estimated records (marker counts), one per context.  Every round, each context loads
-  //      the next part of its run (-t threads split over the contexts) and imports it, then one sk_chain_pairs_multi call
-  //      chains the round's pairs on all contexts.
-  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
-  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
-  write_header(o, op.ci, op.detailed);
+  //      W contiguous runs balanced by estimated records (marker counts), one per context, and each context reads its run in
+  //      groups of < 2^31 - 1 records.  Every round, each context imports its next group (-t threads split over the contexts
+  //      read it), then one sk_chain_pairs_multi call chains the round's pairs on all contexts.
   std::vector<uint64_t> all_pairs(pairs, pairs + np);
   sk_free(pairs);
-  const size_t FL = intermediate_write_count(), NQ = qmeta.size();
-  for (size_t q0 = 0; q0 < NQ; q0 += FL) {
-  std::vector<uint64_t> blockp;
-  for (uint64_t x : all_pairs) if ((uint32_t)x >= q0 && (uint32_t)x < q0 + FL) blockp.push_back(x);   // stays sorted by (ref, query)
-  std::vector<uint32_t> hits;
-  std::vector<size_t> hit_pairs;          // pairs of hits[h]: blockp[hit_pairs[h], hit_pairs[h + 1])
-  for (size_t i = 0; i < blockp.size(); i++)
-    if (hits.empty() || hits.back() != (uint32_t)(blockp[i] >> 32)) { hits.push_back((uint32_t)(blockp[i] >> 32)); hit_pairs.push_back(i); }
-  hit_pairs.push_back(blockp.size());
-  std::vector<uint64_t> est(hits.size());
-  for (size_t h = 0; h < hits.size(); h++) est[h] = ref_mk[hits[h]].markers.size() + 1;
-  const std::vector<size_t> run = split_balanced(est, W);     // context d: hits [run[d], run[d + 1])
-  std::vector<size_t> next(run.begin(), run.end() - 1);
-  std::vector<sk_ani_result> kept;
-  for (;;) {
-    std::vector<size_t> lo(next), hi(next);                   // this round: context d imports hits [lo[d], hi[d])
-    std::vector<sk_sketch_set*> rsets(W, nullptr);
-    std::atomic<bool> too_large{false}, load_failed{false};   // a reference that cannot be loaded ends the run (reported)
-    per_context(W, [&](size_t d) {
-      const size_t h0 = next[d], end = run[d + 1];
-      if (h0 == end) return;
-      size_t h1 = h0;
-      uint64_t recs = 0;
-      while (h1 < end && h1 - h0 < 60000 && recs < (1ull << 30)) h1++, recs += 45000;   // provisional bound, refined below
-      // the hits' sketches as stored, back to back in one buffer: the slices of sketches.db, or the .sketch files
-      // <dir>/<basename(file_name)>.sketch (src/search.rs:157-166)
-      skdb::SketchGroup g;
-      auto path_of = [&](uint32_t r) { return op.db_dir + "/" + base_name(ref_mk[r].file_name) + ".sketch"; };
-      uint64_t total = 0;
-      for (size_t i = h0; i < h1; i++) {
-        uint64_t n = 0;
-        struct stat st;
-        if (consolidated) n = index[hits[i]].length;
-        else if (stat(path_of(hits[i]).c_str(), &st) == 0) n = (uint64_t)st.st_size;
-        g.off.push_back(total); g.len.push_back(n);
-        total += n;
+  const uint64_t group_records = sketch_group_records((1ull << 31) - 1);
+  const int rc = write_dist(op, refs, qmeta, [&](size_t q0, size_t q1, std::vector<sk_ani_result>& res) {
+    std::vector<uint64_t> blockp;
+    for (uint64_t x : all_pairs) if ((uint32_t)x >= q0 && (uint32_t)x < q1) blockp.push_back(x);   // stays sorted by (ref, query)
+    std::vector<uint32_t> hits;
+    std::vector<size_t> hit_pairs;          // pairs of hits[h]: blockp[hit_pairs[h], hit_pairs[h + 1])
+    for (size_t i = 0; i < blockp.size(); i++)
+      if (hits.empty() || hits.back() != (uint32_t)(blockp[i] >> 32)) { hits.push_back((uint32_t)(blockp[i] >> 32)); hit_pairs.push_back(i); }
+    hit_pairs.push_back(blockp.size());
+    std::vector<uint64_t> est(hits.size());
+    for (size_t h = 0; h < hits.size(); h++) est[h] = ref_mk[hits[h]].markers.size() + 1;
+    const std::vector<size_t> run = split_balanced(est, W);     // context d: hits [run[d], run[d + 1])
+    if (!consolidated)
+      for (uint32_t r : hits) { struct stat st; rsi.entries[r].length = stat(rsi.paths[r].c_str(), &st) == 0 ? (uint64_t)st.st_size : 0; }
+    std::vector<skdb::SketchGroupReader> rd;
+    rd.reserve(W);
+    for (size_t d = 0; d < W; d++)
+      rd.emplace_back(rsi, std::vector<size_t>(hits.begin() + run[d], hits.begin() + run[d + 1]), context_threads(op, d, W), group_records);
+    res.clear();
+    for (;;) {
+      std::vector<size_t> lo(W, 0), hi(W, 0);                   // this round: context d imports hits [lo[d], hi[d])
+      std::vector<sk_sketch_set*> rsets(W, nullptr);
+      std::atomic<bool> load_failed{false};                     // a reference that cannot be loaded ends the run (reported)
+      per_context(W, [&](size_t d) {
+        skdb::SketchGroup g;
+        if (!rd[d].next(g)) { if (rd[d].failed) load_failed = true; return; }
+        lo[d] = run[d] + rd[d].first;
+        hi[d] = lo[d] + g.size();
+        std::vector<uint64_t> rk(g.size());
+        for (size_t i = 0; i < g.size(); i++) rk[i] = ranks[0][hits[lo[d] + i]];
+        rsets[d] = import_group(ctxs[d], g, sp, [&](size_t i) { return rsi.entries[hits[lo[d] + i]].file_name; });
+        if (!rsets[d]) { load_failed = true; return; }
+        sk_sketch_set_set_name_ranks(rsets[d], rk.data());
+      });
+      if (load_failed) return false;
+      // the round's refs are numbered run after run: context d's block starts at ref_first[d]
+      std::vector<uint32_t> ref_first(W), round_hit;
+      std::vector<uint64_t> local;
+      for (size_t d = 0; d < W; d++) {
+        ref_first[d] = (uint32_t)round_hit.size();
+        for (size_t h = lo[d]; h < hi[d]; h++) {
+          for (size_t i = hit_pairs[h]; i < hit_pairs[h + 1]; i++) local.push_back(((uint64_t)round_hit.size() << 32) | (uint32_t)blockp[i]);
+          round_hit.push_back((uint32_t)h);
+        }
       }
-      g.bytes.resize(total);
-      g.scan.resize(h1 - h0);
-      {
-        const int T = std::max(1, std::max(op.threads, 1) / (int)W + ((int)d < std::max(op.threads, 1) % (int)W ? 1 : 0));
-        std::vector<std::thread> pool;
-        for (int t = 0; t < T; t++) pool.emplace_back([&, t] {
-          for (size_t i = h0 + t; i < h1; i += T) {
-            const uint32_t r = hits[i];
-            uint8_t* dst = g.bytes.data() + g.off[i - h0];
-            const uint64_t n = g.len[i - h0];
-            bool good;
-            if (consolidated) good = pread(db_fd, dst, n, (off_t)index[r].offset) == (ssize_t)n;
-            else {
-              FILE* f = fopen(path_of(r).c_str(), "rb");
-              good = f && fread(dst, 1, n, f) == n;
-              if (f) fclose(f);
-            }
-            try { if (good) g.scan[i - h0] = skdb::scan_entry(dst, n); }
-            catch (const std::exception&) { good = false; }
-            if (!good) { load_failed = true; fprintf(stderr, "ERROR Failed to load sketch %s\n", ref_mk[r].file_name.c_str()); }
-          }
-        });
-        for (auto& th : pool) th.join();
-      }
-      if (load_failed) return;
-      // keep the batch under 2^31 records: shrink it if the real sizes exceed the estimate (the rest goes to later rounds)
-      uint64_t real = 0;
-      size_t cut = h0;
-      while (cut < h1 && real + g.scan[cut - h0].n_records < (1ull << 31) - 1) real += g.scan[cut - h0].n_records, cut++;
-      if (cut == h0) { too_large = true; return; }
-      g.off.resize(cut - h0); g.len.resize(cut - h0); g.scan.resize(cut - h0);
-      std::vector<uint64_t> ranks;
-      for (size_t i = h0; i < cut; i++) ranks.push_back(rrank[hits[i]]);
-      rsets[d] = import_group(ctxs[d], g, sp, [&](size_t i) { return ref_mk[hits[h0 + i]].file_name; });
-      if (!rsets[d]) { load_failed = true; return; }
-      sk_sketch_set_set_name_ranks(rsets[d], ranks.data());
-      hi[d] = next[d] = cut;
-    });
-    if (load_failed) return 1;
-    if (too_large) { fprintf(stderr, "ERROR reference sketch too large\n"); return 1; }
-    // the round's refs are numbered run after run: context d's block starts at ref_first[d]
-    std::vector<uint32_t> ref_first(W), round_hit;
-    std::vector<uint64_t> local;
-    for (size_t d = 0; d < W; d++) {
-      ref_first[d] = (uint32_t)round_hit.size();
-      for (size_t h = lo[d]; h < hi[d]; h++) {
-        for (size_t i = hit_pairs[h]; i < hit_pairs[h + 1]; i++) local.push_back(((uint64_t)round_hit.size() << 32) | (uint32_t)blockp[i]);
-        round_hit.push_back((uint32_t)h);
-      }
+      if (round_hit.empty()) break;
+      std::vector<sk_ani_result> round(local.size());
+      CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(), &mp, round.data()));
+      for (auto& r : round) if (r.ani > 0.5f) { r.ref_id = hits[round_hit[r.ref_id]]; res.push_back(r); }   // src/search.rs:174
+      for (auto* s : rsets) sk_sketch_set_free(s);
     }
-    if (round_hit.empty()) break;
-    std::vector<sk_ani_result> res(local.size());
-    CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(), &mp, res.data()));
-    for (auto& r : res) if (r.ani > 0.5f) { r.ref_id = hits[round_hit[r.ref_id]]; kept.push_back(r); }   // src/search.rs:174
-    for (auto* s : rsets) sk_sketch_set_free(s);
-  }
-  // the writer's input order: pairs sorted by (ref, query), as one context chaining the hits in order produces them
-  std::sort(kept.begin(), kept.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
-  // write_query_ref_list (src/file_io.rs:608-678): group by the query's first contig name, ANI descending, top n
-  std::map<std::string, std::vector<const sk_ani_result*>> groups;
-  for (auto& r : kept) groups[qmeta[r.query_id].contigs[0]].push_back(&r);
-  for (auto& kv : groups) {
-    auto v = kv.second;
-    std::stable_sort(v.begin(), v.end(), [](const sk_ani_result* a, const sk_ani_result* b) { return a->ani > b->ani; });
-    for (size_t i = 0; i < v.size() && i < op.n; i++) {
-      Genome ref; ref.file_name = ref_mk[v[i]->ref_id].file_name; ref.contigs = ref_mk[v[i]->ref_id].contigs;
-      if (ref.contigs.empty()) ref.contigs.push_back("");
-      write_row(o, *v[i], ref, qmeta[v[i]->query_id], op);
-    }
-  }
-  fflush(o);
-  if (q0 + FL < NQ) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", FL);
-  }
-  if (db_fd >= 0) close(db_fd);
-  if (o != stdout) fclose(o);
+    // rows of equal ANI print in (ref, query) order, as one context chaining the hits in order produces them
+    std::sort(res.begin(), res.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
+    return true;
+  });
   for (auto* s : qsets) sk_sketch_set_free(s);
   for (size_t d = W; d-- > 0;) sk_ctx_destroy(ctxs[d]);
-  return 0;
+  return rc;
 }
 
 // `skani-b200 ingest [-t T] files...`: parse the inputs exactly as triangle / dist / sketch do (no GPU work) and report the

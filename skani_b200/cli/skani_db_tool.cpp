@@ -107,7 +107,9 @@ int main(int argc, char** argv) {
       if (!open_sketch_inputs(std::vector<std::string>(argv + 4, argv + argc), si)) return 1;
       printf("PARAMS %llu %llu %llu\nN %zu\n", (unsigned long long)si.params.c, (unsigned long long)si.params.k,
              (unsigned long long)si.params.marker_c, si.entries.size());
-      SketchGroupReader rd(si, 0, si.entries.size(), atoi(argv[3]), strtoull(argv[2], nullptr, 10));
+      std::vector<size_t> all(si.entries.size());
+      std::iota(all.begin(), all.end(), 0);
+      SketchGroupReader rd(si, std::move(all), atoi(argv[3]), strtoull(argv[2], nullptr, 10));
       SketchGroup g;
       while (rd.next(g)) {
         printf("G %zu %zu %llu\n", rd.first, g.size(), (unsigned long long)g.records);

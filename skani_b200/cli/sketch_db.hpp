@@ -423,7 +423,7 @@ inline bool open_db(const std::string& dir, std::vector<IndexEntry>& index, int&
   return true;
 }
 
-// ---------------------------------------------------------------- sketch inputs of triangle / dist
+// ---------------------------------------------------------------- sketch inputs of triangle / dist / search
 // A consolidated database (a directory holding index.db and sketches.db, src/sketch_db.rs:142-146) stands for all of its
 // sketches, exactly as if each entry were a .sketch file.  Opening the inputs reads index.db (and checks it against
 // markers.bin and the size of sketches.db) but decodes only a database's first entry; the sketches themselves are read
@@ -443,9 +443,9 @@ struct SketchEntry {            // one sketch of the inputs
 };
 
 struct SketchInputs {
-  std::vector<std::string> paths;    // .sketch files and database directories, in command-line order
+  std::vector<std::string> paths;    // .sketch files and database directories (open_sketch_inputs: in command-line order)
   std::vector<int> db_fd;            // sketches.db of paths[i], or -1 for a .sketch file
-  std::vector<SketchEntry> entries;  // every sketch, stably sorted by file name (src/file_io.rs:715)
+  std::vector<SketchEntry> entries;  // every sketch (open_sketch_inputs: stably sorted by file name, src/file_io.rs:715)
   DiskParams params;                 // of the first input (all inputs agree on c, k and marker_c)
   SketchInputs() = default;
   SketchInputs(const SketchInputs&) = delete;
@@ -528,17 +528,17 @@ struct SketchGroup {
   void clear() { bytes.clear(); off.clear(); len.clear(); scan.clear(); records = 0; }
 };
 
-// Reads the entries [begin, end) of si, in order, and hands them out in groups of < max_records seed records (a group
-// holds at least one sketch), each group's blobs read into one buffer as stored and scanned (scan_entry), not decoded.
-// Entries are read and scanned in batches by `threads` threads; the entries of a batch that the current group cannot
-// take are carried into the next one.  An entry that cannot be read or scanned, or whose name differs from its index
-// entry, ends the reading with an ERROR line: next() then returns false with failed set.
+// Reads the entries of si listed in `list` (entry indices), in list order, and hands them out in groups of < max_records
+// seed records (a group holds at least one sketch), each group's blobs read into one buffer as stored and scanned
+// (scan_entry), not decoded.  Entries are read and scanned in batches by `threads` threads; the entries of a batch that
+// the current group cannot take are carried into the next one.  An entry that cannot be read or scanned, or whose name
+// differs from its index entry, ends the reading with an ERROR line: next() then returns false with failed set.
 class SketchGroupReader {
  public:
-  SketchGroupReader(const SketchInputs& si, size_t begin, size_t end, int threads, uint64_t max_records)
-      : si_(si), next_(begin), end_(end), consumed_(begin), threads_(std::max(threads, 1)), max_records_(max_records) {}
+  SketchGroupReader(const SketchInputs& si, std::vector<size_t> list, int threads, uint64_t max_records)
+      : si_(si), list_(std::move(list)), threads_(std::max(threads, 1)), max_records_(max_records) {}
   bool failed = false;
-  size_t first = 0;             // entry index of g's first blob after next()
+  size_t first = 0;             // position in the list of g's first blob after next()
 
   bool next(SketchGroup& g) {
     g = std::move(carry_);        // the previous group's buffer is freed here
@@ -570,20 +570,21 @@ class SketchGroupReader {
  private:
   // the next entries (at most 8 per thread and about 256 MiB on disk) appended to g: read, then scanned
   bool read_batch(SketchGroup& g) {
-    if (next_ >= end_) return false;
+    const size_t listed = list_.size();
+    if (next_ >= listed) return false;
     size_t b = next_;
     uint64_t bytes = 0;
-    while (b < end_ && (b == next_ || (b - next_ < 8 * (size_t)threads_ && bytes < (256ull << 20)))) bytes += si_.entries[b++].length;
+    while (b < listed && (b == next_ || (b - next_ < 8 * (size_t)threads_ && bytes < (256ull << 20)))) bytes += si_.entries[list_[b++]].length;
     const size_t n0 = g.size(), n = b - next_;
     if (g.bytes.capacity() < g.bytes.size() + bytes) {   // room for the rest of the inputs, up to about a group's worth
       uint64_t rest = 0;
-      for (size_t i = next_; i < end_ && rest < 16 * max_records_; i++) rest += si_.entries[i].length;
+      for (size_t i = next_; i < listed && rest < 16 * max_records_; i++) rest += si_.entries[list_[i]].length;
       g.bytes.reserve(g.bytes.size() + std::max<uint64_t>(bytes, rest));
     }
     uint64_t end = g.bytes.size();
     for (size_t i = 0; i < n; i++) {
       g.off.push_back(end);
-      g.len.push_back(si_.entries[next_ + i].length);
+      g.len.push_back(si_.entries[list_[next_ + i]].length);
       end += g.len.back();
     }
     g.bytes.resize(end);
@@ -592,12 +593,12 @@ class SketchGroupReader {
     std::atomic<bool> bad{false};
     auto worker = [&] {
       for (size_t i; (i = at.fetch_add(1)) < n;) {
-        const SketchEntry& e = si_.entries[next_ + i];
+        const SketchEntry& e = si_.entries[list_[next_ + i]];
         const int fd = si_.db_fd[e.input];
         uint8_t* dst = g.bytes.data() + g.off[n0 + i];
         bool good;
         if (fd >= 0) good = pread(fd, dst, e.length, (off_t)e.offset) == (ssize_t)e.length;
-        else {                   // a .sketch file: its size when the inputs were opened
+        else {                   // a .sketch file: the size its entry records
           FILE* f = fopen(si_.paths[e.input].c_str(), "rb");
           good = f && fread(dst, 1, e.length, f) == e.length;
           if (f) fclose(f);
@@ -617,7 +618,8 @@ class SketchGroupReader {
     return true;
   }
   const SketchInputs& si_;
-  size_t next_, end_, consumed_;
+  std::vector<size_t> list_;
+  size_t next_ = 0, consumed_ = 0;   // positions in list_: the next entry to read, the first not yet handed out
   int threads_;
   uint64_t max_records_;
   SketchGroup carry_;

@@ -13,8 +13,8 @@ EC, K12, VIR, O157 = (os.path.join(GOLD, f) for f in ("e.coli-EC590.fasta.gz", "
 FILES = [K12, VIR, EC]
 
 
-def run(args, write_count=None):
-    env = dict(os.environ)
+def run(args, write_count=None, env=None):
+    env = dict(os.environ, **(env or {}))
     if write_count:
         env["SK_INTERMEDIATE_WRITE_COUNT"] = str(write_count)
     p = subprocess.run([BIN] + args, capture_output=True, text=True, timeout=900, env=env)
@@ -66,3 +66,7 @@ def test_search(dbs, layout):
     same_with_gpus(["search", "-d", db, VIR, "--qi"], write_count=1, min_rows=0)
     same_with_gpus(["search", "-d", db, O157, "--qi", "-n", "1"], write_count=100, min_rows=0)
     same_with_gpus(["search", "-d", db] + dbs[2], min_rows=3)                 # .sketch queries
+    # one reference per import group: every context imports and chains its hits over several rounds
+    one = run(["search", "-d", db] + FILES)
+    for gpus in ("1", "2"):
+        assert run(["search", "-d", db] + FILES + ["--gpus", gpus], env={"SK_SKETCH_GROUP_RECORDS": "1"}) == one
