@@ -71,9 +71,12 @@ struct ChainParams {
 
 // per-batch workspace (device pointers)
 struct Workspace {
-  // per record of the query-role genome
-  uint16_t* rec_nh;       // bits 0..14 = number of anchors, bit 15 = "counted" (enters seeds_in_chunk)
-  uint32_t* rec_rs;       // hit records only: start of the matching group in the ref-role k-mer view
+  // per record slot of the query-role genome (PairDesc::rec_off slices): probe tile j of a pair writes its hit records, in
+  // record order, to slots [j * TILE, j * TILE + tile_hits[j]) of the pair's slice
+  uint2* hit;             // .x = start of the matching group in the ref-role k-mer view, .y = record's index in its tile | nh << 10
+  // per probe tile (tile_off indexing)
+  uint32_t* tile_hits;    // hit records of the tile; chunk_anchor_kernel turns a pair's counts into pair-local exclusive offsets
+  uint32_t* rec_cnt;      // TILE / 32 words per tile: bit i of word w = record 32 w + i is "counted" (enters seeds_in_chunk)
   // per pair
   uint32_t* tile_off;                    // exclusive prefix of the pairs' probe tiles (probe_kernel block -> pair), B + 1 entries
   uint32_t *pairA, *pairC;               // anchors, chunks
@@ -139,13 +142,16 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, uint32_t pari
 }
 constexpr uint32_t PROBE_STAGE_ENTRIES = 2048;   // 16 KB: fits the (otherwise unused) bucket-index array of the block
 
-constexpr uint32_t TILE = CT * ITEMS;            // query records per probe_kernel block / per chunk_anchor_kernel step
+constexpr uint32_t TILE = CT * ITEMS;            // query records per probe_kernel block / hit records per chunk_anchor_kernel step
+static_assert(TILE / 32 == 32, "probe_kernel offsets a tile's 32 (item, warp) hit groups with one warp scan");
 constexpr int PROBE_MINB = 4;                    // resident blocks per SM (register caps through __launch_bounds__)
 constexpr int CHUNK_ANCHOR_MINB = 3;
 
 // One block per TILE-record tile of the batch (PairDesc::rec_off slices, tile_off = tiles per pair): the tiles of a pair are
-// independent, so there are no scans and nothing is carried between tiles.  Per query record: rec_nh, and rec_rs for hit
-// records; the tile's anchor count goes to pairA with one atomic (integer sum: order-free).
+// independent, so nothing is carried between tiles.  The tile writes its hit records compacted in record order (warp ballots,
+// per-warp counts in shared memory) with their count in tile_hits, and the "counted" bit of every record to rec_cnt (one
+// ballot word per warp and item: 32 consecutive records).  The tile's anchor count goes to pairA with one atomic (integer
+// sum: order-free).
 // STAGED = the batch is dominated by small ref-role genomes: their tables are bulk-copied to shared memory (generic loads);
 // otherwise every probe is a read-only global load.
 template <bool STAGED, int MINB>
@@ -155,6 +161,7 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
   __shared__ __align__(16) uint32_t s_bucket[UBUCKETS + 4];
   __shared__ __align__(8) unsigned long long s_bar;
   __shared__ uint32_t s_warp_sum[CT / 32];
+  __shared__ uint32_t s_group_hits[ITEMS * CT / 32];
   // the tile's pair: the last p with tile_off[p] <= blockIdx.x (pairs without records own no tiles)
   uint32_t plo = 0, phi = n_pairs;
   while (phi - plo > 1) {
@@ -192,10 +199,8 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
     for (uint32_t b = threadIdx.x; b <= UBUCKETS; b += CT) s_bucket[b] = gb[b];
     __syncthreads();
   }
-  uint16_t* __restrict__ nhv = ws.rec_nh + pd.rec_off;
-  uint32_t* __restrict__ rsv = ws.rec_rs + pd.rec_off;
-  uint32_t sum = 0;
-  // record t = t0 + it * CT + threadIdx.x: every load and store of the tile is coalesced
+  uint32_t hn[ITEMS], hr[ITEMS], hc[ITEMS];   // per record: anchors (nh), ref group start, counted
+  // record t = t0 + it * CT + threadIdx.x: every load of the tile is coalesced
   if (use_hash) {
     // one 32-byte BUCKET (4 entries = one memory sector) per record: a probe almost never needs a second access, so the
     // lanes of a warp finish together (with one entry per step the warp waited for its longest probe chain).  The ITEMS probes of a thread are independent.
@@ -222,7 +227,6 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
       }
 #pragma unroll
     for (int it = 0; it < ITEMS; it++) {
-      const uint32_t t = t0 + it * CT + threadIdx.x;
       uint32_t nh = 0, rst = 0, counted = 0;
       if (live[it]) {
         unsigned long long e = 0ull;
@@ -244,11 +248,7 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
           counted = 1;                                       // no hit: position still counts (:684-687)
         }
       }
-      if (t < qm.n_rec) {
-        nhv[t] = (uint16_t)(nh | (counted << 15));
-        if (nh) rsv[t] = rst;
-      }
-      sum += nh;
+      hn[it] = nh; hr[it] = rst; hc[it] = counted;
     }
   } else {
     uint32_t kmer[ITEMS], lo[ITEMS], hi[ITEMS], bend[ITEMS];
@@ -282,7 +282,6 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
     }
 #pragma unroll
     for (int it = 0; it < ITEMS; it++) {
-      const uint32_t t = t0 + it * CT + threadIdx.x;
       uint32_t nh = 0, rst = 0, counted = 0;
       if (live[it]) {
         if (lo[it] < bend[it] && lo[it] < nuk && ruk[lo[it]] == kmer[it]) {
@@ -292,17 +291,45 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
           counted = 1;                                 // no hit: position still counts (:684-687)
         }
       }
-      if (t < qm.n_rec) {
-        nhv[t] = (uint16_t)(nh | (counted << 15));
-        if (nh) rsv[t] = rst;
-      }
-      sum += nh;
+      hn[it] = nh; hr[it] = rst; hc[it] = counted;
     }
   }
-  sum = __reduce_add_sync(0xFFFFFFFFu, sum);
-  if ((threadIdx.x & 31u) == 0) s_warp_sum[threadIdx.x >> 5] = sum;
+  // The lanes of warp w for item it hold the 32 consecutive records it * CT + 32 w + lane of the tile: one ballot word
+  // each for rec_cnt and for the hit mask.  Group (it, w) precedes group (it', w') in record order iff it * 8 + w is smaller.
+  const unsigned FULL = 0xFFFFFFFFu;
+  const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+  uint32_t hm[ITEMS], sum = 0;
+#pragma unroll
+  for (int it = 0; it < ITEMS; it++) {
+    hm[it] = __ballot_sync(FULL, hn[it] != 0);
+    const uint32_t cm = __ballot_sync(FULL, hc[it] != 0);
+    if (lane == 0) {
+      ws.rec_cnt[(size_t)blockIdx.x * (TILE / 32) + it * (CT / 32) + w] = cm;
+      s_group_hits[it * (CT / 32) + w] = __popc(hm[it]);
+    }
+    sum += hn[it];
+  }
+  sum = __reduce_add_sync(FULL, sum);
+  if (lane == 0) s_warp_sum[w] = sum;
   __syncthreads();
+  // every warp scans the 32 group counts itself: exclusive offset of each group among the tile's hits
+  const uint32_t gv = s_group_hits[lane];
+  uint32_t ginc = gv;
+#pragma unroll
+  for (uint32_t o = 1; o < 32; o <<= 1) {
+    const uint32_t x = __shfl_up_sync(FULL, ginc, o);
+    if (lane >= o) ginc += x;
+  }
+  uint2* __restrict__ hv = ws.hit + pd.rec_off + t0;
+  const uint32_t lt = (1u << lane) - 1u;
+#pragma unroll
+  for (int it = 0; it < ITEMS; it++) {
+    const uint32_t gbase = __shfl_sync(FULL, ginc - gv, it * (CT / 32) + w);
+    if (hn[it]) hv[gbase + __popc(hm[it] & lt)] = make_uint2(hr[it], (it * CT + threadIdx.x) | (hn[it] << 10));
+  }
+  const uint32_t tile_total = __shfl_sync(FULL, ginc, 31);
   if (threadIdx.x == 0) {
+    ws.tile_hits[blockIdx.x] = tile_total;
     uint32_t total = 0;
 #pragma unroll
     for (int w = 0; w < CT / 32; w++) total += s_warp_sum[w];
@@ -311,14 +338,15 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// K2: chunk assignment + anchors + chunk descriptors, block per pair, streaming the query-role genome's records in tiles.
-// Per hit record, with in-tile block scans carried across tiles: the pair-local offset of its first anchor (sum of nh),
+// K2: chunk assignment + anchors + chunk descriptors, block per pair, streaming the query-role genome's hit records (the
+// probe's compacted per-tile lists) in steps of TILE hits.  Records without hits enter every scan as its identity, so only
+// hit records are scanned.  Per hit record, with in-step block scans carried across steps: the pair-local offset of its first anchor (sum of nh),
 // P0 / A0 of its contig (position / anchor offset of the contig's first hit, segmented "first" scan), need, and the
 // contig-local chunk of its first and last anchor (segmented prefix min, the closed form in chain_core.cuh); then the
 // chunk-start flags and chunk ids (sum).  Descriptors go to the pair's staging slice; chunk_compact_kernel packs them.
 //
-// Few memory round trips lie in series inside a tile: the records of tile i + 1 are copied to shared memory (cp.async)
-// while tile i scans and emits, and the tile's anchors are emitted anchor-parallel, one thread per anchor, so that the
+// Few memory round trips lie in series inside a step: the hits of step i + 1 are staged in shared memory (cp.async) while
+// step i scans and emits, and the step's anchors are emitted anchor-parallel, one thread per anchor, so that the
 // gathers of a round are independent of each other and of the round's stores.  What remains is mostly the instruction
 // work of the four block scans (hence the branch-free FirstOp / MinOp).
 // ------------------------------------------------------------------------------------------------------------
@@ -330,15 +358,15 @@ __device__ __forceinline__ void cp_async4(void* dst_smem, const void* src_gmem) 
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all_but_newest() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
 
-static_assert(TILE == 1024, "ChunkAnchorSmem::arec packs the record's index in the tile into 10 bits");
-struct __align__(16) RecTile {       // one tile of query-role records
-  uint32_t pos[TILE], cc[TILE];
-  uint32_t rs[TILE];                 // stale for records without hits: never used for them
-  uint32_t nhw[TILE / 2 + 1];        // the aligned 4-byte words holding the tile's rec_nh: record i is halfword i + nh_odd
+static_assert(TILE == 1024, "ChunkAnchorSmem::arec and Workspace::hit pack an index in the step / tile into 10 bits");
+struct __align__(16) RecTile {       // one step of hit records of the query-role genome
+  uint32_t pos[TILE], cc[TILE];      // not copied for the padding slots after the pair's last hit
+  uint32_t rs[TILE];
+  uint32_t nh[TILE];                 // 0 for the padding slots
 };
 struct ChunkAnchorSmem {
-  RecTile tile[2];                   // double buffer: tile i + 1 is in flight while tile i scans and emits
-  // per hit record of the current tile (index in the tile), read by the threads that emit its anchors
+  RecTile tile[2];                   // double buffer: step i + 1 is in flight while step i scans and emits
+  // per hit record of the current step (index in the step), read by the threads that emit its anchors
   uint32_t clf[TILE];                // contig-local chunk of the record's first anchor
   uint32_t need[TILE];               // need | (the first anchor starts a chunk) << 31
   uint32_t cid[TILE];                // pair-local chunk id of the first anchor
@@ -346,25 +374,37 @@ struct ChunkAnchorSmem {
   uint32_t arec[TILE];               // anchor of the current round -> its record | its index in the record << 10
 };
 
-// Issue the copies of records [t0, min(t0 + TILE, n_rec)) into b.  rec_nh slices start at any halfword (nh_odd = the
-// slice's start is not 4-byte aligned), so whole aligned words are copied: one halfword before and one after the tile's
-// may come along; both lie inside the allocation (the one after is at most index n_rec of the slice, and ensure()
-// over-allocates).
-__device__ __forceinline__ void stage_rec_tile(RecTile& b, uint32_t t0, uint32_t n_rec, const uint16_t* nhv, uint32_t nh_odd,
-                                               const uint32_t* rsv, const uint32_t* qpv, const uint32_t* qcv) {
-  const uint32_t n = min(TILE, n_rec - t0);
+// Stage the pair's hits [h0, min(h0 + TILE, H)) into b.  Hit h lies in probe tile j, the last tile with hoff[j] <= h (a
+// tile without hits shares its offset with the next tile, so the search passes over it); its entry is read at once, and
+// its record's pos / cc are copied asynchronously (increasing addresses inside the tile's window of TILE records).
+// hoff: the pair's n_t tile offsets, written by this block (plain loads, not the read-only path).
+__device__ __forceinline__ void stage_hit_step(RecTile& b, uint32_t h0, uint32_t H, const uint32_t* hoff, uint32_t n_t,
+                                               const uint2* hv, const uint32_t* qpv, const uint32_t* qcv) {
+  uint32_t h[ITEMS], j[ITEMS];
+#pragma unroll
+  for (int it = 0; it < ITEMS; it++) { h[it] = h0 + it * CT + threadIdx.x; j[it] = 0; }
+  for (uint32_t len = n_t; len > 1;) {             // the ITEMS searches in lock-step: their loads overlap
+    const uint32_t half = len >> 1;
+#pragma unroll
+    for (int it = 0; it < ITEMS; it++)
+      if (hoff[j[it] + half] <= h[it]) j[it] += half;
+    len -= half;
+  }
 #pragma unroll
   for (int it = 0; it < ITEMS; it++) {
     const uint32_t i = it * CT + threadIdx.x;
-    if (i < n) {
-      cp_async4(&b.pos[i], qpv + t0 + i);
-      cp_async4(&b.cc[i], qcv + t0 + i);
-      cp_async4(&b.rs[i], rsv + t0 + i);
+    uint32_t nh = 0;
+    if (h[it] < H) {
+      const uint32_t r0 = j[it] * TILE;                // the tile's first record = its first hit slot
+      const uint2 e = hv[r0 + (h[it] - hoff[j[it]])];
+      const uint32_t r = r0 + (e.y & (TILE - 1));
+      cp_async4(&b.pos[i], qpv + r);
+      cp_async4(&b.cc[i], qcv + r);
+      b.rs[i] = e.x;
+      nh = e.y >> 10;
     }
+    b.nh[i] = nh;
   }
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(nhv + t0 - nh_odd);
-  const uint32_t nw = (n + nh_odd + 1) >> 1;
-  for (uint32_t i = threadIdx.x; i < nw; i += CT) cp_async4(&b.nhw[i], w + i);
 }
 
 template <int MINB>
@@ -389,8 +429,7 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
   }
   const GenomeMeta qm = (pd.qset ? m1 : m0)[pd.qg];
   const GenomeMeta rm = (pd.rset ? m1 : m0)[pd.rg];
-  const uint16_t* __restrict__ nhv = ws.rec_nh + pd.rec_off;
-  const uint32_t* __restrict__ rsv = ws.rec_rs + pd.rec_off;
+  const uint2* __restrict__ hv = ws.hit + pd.rec_off;
   // the fields are selected one by one (see probe_kernel)
   const uint32_t* __restrict__ qpv = (pd.qset ? s1.pv_pos : s0.pv_pos) + qm.seed_off;
   const uint32_t* __restrict__ qcv = (pd.qset ? s1.pv_cc : s0.pv_cc) + qm.seed_off;
@@ -399,19 +438,38 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
   const uint64_t abase = ws.pairAbase[p], sbase = pd.chunk_off;
   AnchorRec* __restrict__ anc = ws.anc + abase;
   const uint32_t cmax = pd.max_chunks;
-  const uint32_t nh_odd = (uint32_t)(reinterpret_cast<uintptr_t>(nhv) >> 1) & 1u;
+  // the probe's per-tile hit counts -> pair-local exclusive offsets (in place), H = the pair's hit records
+  const uint32_t tb = ws.tile_off[p], n_t = ws.tile_off[p + 1] - tb;
+  uint32_t* hoff = ws.tile_hits + tb;
+  uint32_t H = 0;
+  for (uint32_t j0 = 0; j0 < n_t; j0 += TILE) {
+    uint32_t x[ITEMS], ex[ITEMS], agg;
+#pragma unroll
+    for (int it = 0; it < ITEMS; it++) {
+      const uint32_t j = j0 + threadIdx.x * ITEMS + it;
+      x[it] = j < n_t ? hoff[j] : 0u;
+    }
+    ScanU(tmp_a).ExclusiveSum(x, ex, agg);
+#pragma unroll
+    for (int it = 0; it < ITEMS; it++) {
+      const uint32_t j = j0 + threadIdx.x * ITEMS + it;
+      if (j < n_t) hoff[j] = H + ex[it];
+    }
+    H += agg;
+    __syncthreads();                                // tmp_a is reused; the offsets are visible to the whole block
+  }
   FirstState carryF; carryF.valid = 0; carryF.ctg = 0; carryF.p0 = 0; carryF.a0 = 0;
   MinState carryM; carryM.valid = 0; carryM.ctg = 0; carryM.v = 0;
   MinState identM; identM.valid = 0; identM.ctg = 0; identM.v = 0;
   uint32_t carryA = 0, carryC = 0;                  // anchors / chunk starts so far
   __shared__ uint32_t s_last_q, s_last_c;          // the pair's last hit record: its position, the chunk of its last anchor
-  stage_rec_tile(S.tile[0], 0, qm.n_rec, nhv, nh_odd, rsv, qpv, qcv);
+  stage_hit_step(S.tile[0], 0, H, hoff, n_t, hv, qpv, qcv);
   cp_async_commit();
   uint32_t buf = 0;
-  for (uint32_t t0 = 0; t0 < qm.n_rec; t0 += TILE, buf ^= 1u) {
-    // the other buffer was last read before the previous tile's final barrier
-    if (t0 + TILE < qm.n_rec) stage_rec_tile(S.tile[buf ^ 1u], t0 + TILE, qm.n_rec, nhv, nh_odd, rsv, qpv, qcv);
-    cp_async_commit();                              // possibly empty: the group before it is always this tile's
+  for (uint32_t h0 = 0; h0 < H; h0 += TILE, buf ^= 1u) {
+    // the other buffer was last read before the previous step's final barrier
+    if (h0 + TILE < H) stage_hit_step(S.tile[buf ^ 1u], h0 + TILE, H, hoff, n_t, hv, qpv, qcv);
+    cp_async_commit();                              // possibly empty: the group before it is always this step's
     cp_async_wait_all_but_newest();
     __syncthreads();
     const RecTile& T = S.tile[buf];
@@ -419,15 +477,13 @@ chunk_anchor_kernel(const PairDesc* __restrict__ pairs, SetView s0, SetView s1, 
     {
       const uint4 p4 = *reinterpret_cast<const uint4*>(&T.pos[threadIdx.x * ITEMS]);
       const uint4 c4 = *reinterpret_cast<const uint4*>(&T.cc[threadIdx.x * ITEMS]);
+      const uint4 n4 = *reinterpret_cast<const uint4*>(&T.nh[threadIdx.x * ITEMS]);
       pos[0] = p4.x; pos[1] = p4.y; pos[2] = p4.z; pos[3] = p4.w;
       cc[0] = c4.x; cc[1] = c4.y; cc[2] = c4.z; cc[3] = c4.w;
-      const uint16_t* nh16 = reinterpret_cast<const uint16_t*>(T.nhw) + nh_odd;
+      nh[0] = n4.x; nh[1] = n4.y; nh[2] = n4.z; nh[3] = n4.w;
 #pragma unroll
-      for (int it = 0; it < ITEMS; it++) {
-        const uint32_t i = threadIdx.x * ITEMS + it;
-        nh[it] = (t0 + i < qm.n_rec) ? nh16[i] & 0x7FFFu : 0u;
-        if (!nh[it]) pos[it] = cc[it] = 0;
-      }
+      for (int it = 0; it < ITEMS; it++)
+        if (!nh[it]) pos[it] = cc[it] = 0;          // padding slots: never copied
     }
     uint32_t aoff[ITEMS], aggA;
     ScanU(tmp_a).ExclusiveSum(nh, aoff, aggA);
@@ -1108,7 +1164,7 @@ chunkstat_kernel(uint64_t n_chunks, const PairDesc* __restrict__ pairs, SetView 
     uint32_t cap = min(r1, first + 1024u);
     if (cap < r1 && (int64_t)pos[cap - 1] <= hi) cap = r1;
     const uint32_t last = warp_first_greater(pos, first, cap, hi, lane);   // [first, last)
-    const uint16_t* nhv = ws.rec_nh + pd.rec_off;
+    const uint32_t* cnt = ws.rec_cnt + (size_t)ws.tile_off[p] * (TILE / 32);   // the pair's "counted" bits
     const uint64_t ib = ws.pairIbase[p];
     const bool has_int = n_int > 0;
     // the chunk's kept intervals, padded by c on both sides (src/chain.rs:239-240), staged by lane 0
@@ -1133,7 +1189,7 @@ chunkstat_kernel(uint64_t n_chunks, const PairDesc* __restrict__ pairs, SetView 
     }
     uint32_t n_seeds = 0, num_in = 0, upper_lower = 0;
     for (uint32_t t = first + lane; t < last; t += 32) {
-      if (!(nhv[t] & 0x8000u)) continue;
+      if (!((cnt[t >> 5] >> (t & 31u)) & 1u)) continue;
       n_seeds++;
       if (!has_int) continue;
       const uint32_t ps = pos[t];
@@ -1479,7 +1535,7 @@ static int ensure(sk_ctx* ctx, T** p, size_t* cap, size_t need) {
 struct ChainScratch {
   Workspace ws{};
   size_t cap_rec = 0, cap_pair = 0, cap_anc = 0, cap_chunk = 0, cap_iv = 0;
-  size_t c_rec_nh = 0, c_rec_rs = 0, c_tile_off = 0;
+  size_t c_hit = 0, c_tile_hits = 0, c_rec_cnt = 0, c_tile_off = 0;
   size_t c_stg_first = 0, c_stg_qctg = 0, c_stg_lo = 0, c_stg_hi = 0;
   size_t c_pairA = 0, c_pairC = 0, c_pairAbase = 0, c_pairCbase = 0, c_pairIbase = 0, c_pair_nint = 0, c_pair_sumlen = 0,
          c_pair_nchains = 0, c_pair_tqb = 0;
@@ -1495,7 +1551,7 @@ struct ChainScratch {
   GenomeMeta *d_m0 = nullptr, *d_m1 = nullptr;
   size_t c_m0 = 0, c_m1 = 0;
   void free_all() {
-    void* ptrs[] = {ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, sort_tmp, dbg_counts, ws.rec_nh, ws.rec_rs, ws.tile_off, ws.stg_first, ws.stg_qctg, ws.stg_lo, ws.stg_hi,
+    void* ptrs[] = {ws.chunk_size, ws.chunk_size_sorted, ws.chunk_id, ws.chunk_perm, sort_tmp, dbg_counts, ws.hit, ws.tile_hits, ws.rec_cnt, ws.tile_off, ws.stg_first, ws.stg_qctg, ws.stg_lo, ws.stg_hi,
                     ws.pairA, ws.pairC, ws.pairAbase, ws.pairCbase, ws.pairIbase, ws.pair_nint, ws.pair_sumlen, ws.pair_nchains, ws.pair_tqb_ns, ws.anc,
                     ws.score, ws.ptr, ws.rootkey, ws.depth, ws.chunk_first, ws.chunk_pair, ws.chunk_qctg, ws.chunk_lo, ws.chunk_hi,
                     ws.acc_total, ws.acc_rq0, ws.acc_rq1, ws.acc_tbcq, ws.acc_nint, ws.chunk_head, ws.chunk_est, ws.chunk_w, ws.chunk_valid,
@@ -1670,7 +1726,8 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
   const size_t NR = std::max<uint64_t>(total_rec, 1);
 #define ENS(field, capf, n) SK_TRY(ensure(ctx, &ws.field, &S.capf, n))
   const size_t NS = std::max<uint64_t>(total_chunks, 1);
-  ENS(rec_nh, c_rec_nh, NR); ENS(rec_rs, c_rec_rs, NR); ENS(tile_off, c_tile_off, B + 1);
+  const size_t NT = std::max<uint32_t>(tile_off[B], 1);
+  ENS(hit, c_hit, NR); ENS(tile_hits, c_tile_hits, NT); ENS(rec_cnt, c_rec_cnt, NT * (TILE / 32)); ENS(tile_off, c_tile_off, B + 1);
   ENS(stg_first, c_stg_first, NS); ENS(stg_qctg, c_stg_qctg, NS); ENS(stg_lo, c_stg_lo, NS); ENS(stg_hi, c_stg_hi, NS);
   ENS(pairA, c_pairA, B); ENS(pairC, c_pairC, B); ENS(pairAbase, c_pairAbase, B + 1); ENS(pairCbase, c_pairCbase, B + 1);
   ENS(pairIbase, c_pairIbase, B + 1); ENS(pair_nint, c_pair_nint, B); ENS(pair_sumlen, c_pair_sumlen, B); ENS(pair_nchains, c_pair_nchains, B);

@@ -1,12 +1,13 @@
 #!/usr/bin/env python3
-"""Anchor and chunk counts of one step of bench.py's `value` leg, and the distribution of anchors per chunk that the chain
-back end's DP sees (the sizes that decide dp_group_kernel's on-chip bound).
+"""Record, hit-record, anchor and chunk counts of one step of bench.py's `value` leg, and the distribution of anchors per
+chunk that the chain back end's DP sees (the sizes that decide dp_group_kernel's on-chip bound).  Records are the
+query-role genomes' records the probe reads; hit records are those with anchors (the records chunk_anchor_kernel scans).
 
   python tools/count_chain_shapes.py [--config north|c2|dense|c5] [--genomes N] [--batch P]
 
 Sketches and screens the same synthetic genomes as tools/profile_value_leg.py, then re-chains the screened pairs with
 sk_chain_pairs_debug, P pairs per call (the same batching and kernels as chain_pairs), keeping only each pair's chunk
-boundaries.  Prints the totals and a histogram of anchors per chunk."""
+boundaries and its distinct anchor query positions.  Prints the totals and a histogram of anchors per chunk."""
 import argparse
 import os
 import sys
@@ -52,8 +53,18 @@ def main():
     sizes = []
     n_anchors = 0
     n_iv = 0
+    n_rec = 0
+    n_hit = 0
+    n_rec_of = {}
     for b in range(0, n_pairs, a.batch):
-        for d in sk.chain_pairs_debug(ctx, gs, gs, pairs[b:b + a.batch], mp):
+        for pid, d in zip(pairs[b:b + a.batch], sk.chain_pairs_debug(ctx, gs, gs, pairs[b:b + a.batch], mp)):
+            g = int(pid) >> 32 if d["switched"] else int(pid) & 0xFFFFFFFF      # the query-role (iterated) genome
+            if g not in n_rec_of:
+                n_rec_of[g] = gs.info(g)["n_records"]
+            n_rec += n_rec_of[g]
+            an = d["anchors"]
+            if len(an):                                       # one hit record = one (query contig, query position)
+                n_hit += len(np.unique(an[:, 0].astype(np.uint64) << np.uint64(32) | an[:, 1].astype(np.uint64)))
             cf = d["chunk_first"].astype(np.int64)
             sizes.append(np.diff(cf))
             n_anchors += int(d["anchors"].shape[0])
@@ -61,6 +72,8 @@ def main():
     sizes = np.concatenate(sizes) if sizes else np.zeros(0, np.int64)
     print("card: %s" % card())
     print("config %s: %d genomes x %d bp, cluster %d, c=%d: %d pairs chained" % (a.config, N, L, G, cfg["c"], n_pairs))
+    print("query-role records %d, hit records %d (%.1f %% of records), anchors %d (%.3f per hit record)"
+          % (n_rec, n_hit, 100.0 * n_hit / max(n_rec, 1), n_anchors, n_anchors / max(n_hit, 1)))
     print("anchors %d, chunks %d (%d with anchors), DP intervals %d" % (n_anchors, len(sizes), int((sizes > 0).sum()), n_iv))
     nz = sizes[sizes > 0]
     if len(nz):
