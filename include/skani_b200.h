@@ -458,6 +458,45 @@ typedef struct {
 int sk_cluster(sk_ctx* ctx, uint32_t n_genomes, const sk_ani_result* results, uint64_t n_results, const uint32_t* rank,
                const sk_cluster_params* cp, uint32_t* rep, uint32_t* cluster, uint64_t* edge, sk_cluster_stats* stats /* may be NULL */);
 
+/* ---- average (UPGMA) and complete linkage of a triangle's results (what the reference's scripts/clustermap_triangle.py
+ *      does with scipy on the dense 100 - ANI matrix), from the edge list alone.  Inputs as for sk_cluster.
+ * Edges: every row with ani > 0.1 (the rows `triangle -E` prints; NaN and -1 never are); min_ani does NOT filter them, it
+ * is only the cut.  A pair of genomes without an edge has similarity 0.  q = ani * 2^27 is an exact integer for every
+ * float in (0.1, 2); a row with ani >= 2 (or +inf) is refused, and so is min_ani outside (0.1, 1].
+ * Value of a cluster pair (A, B), P = |A| |B|: average S / (P 2^27) with S = sum of q over the edges between A and B;
+ * complete min q / 2^27 when all P member pairs are edges, otherwise 0.  Values are compared exactly (128-bit
+ * cross-multiplication).  A cluster's id is its smallest member rank; its best partner has the largest value, ties to the
+ * smaller partner id.
+ * Rounds: every active cluster finds its best partner; every pair that are each other's best partner and whose value is
+ * >= q(min_ani) (in dendrogram mode: > 0) merges; clusters with no partner that could still qualify are deactivated; the
+ * rounds end when none is left.  For inputs without ties the merges are those of sequential HAC (scipy's); with ties this
+ * round procedure is the definition, and it is deterministic.
+ * Flat clusters are the merges with value >= the cut, whatever the mode: rep[g] = the member of smallest rank, cluster[g]
+ * = clusters numbered in rank order of their representatives, edge[g] = the index of the row joining g and rep[g],
+ * UINT64_MAX for none.
+ * Dendrogram (dendrogram != 0; merges has n_genomes - 1 rows, may be NULL otherwise): a scipy linkage matrix.  Genomes are
+ * 0..n-1 in genome-index order, row j's cluster is n + j, a < b.  Rows are sorted by (value descending, round, id);
+ * height = 1 - S / ldexp(P, 27) (average) or 1 - ldexp(min q, -27) (complete), rounded to nearest; the clusters left at
+ * the end (no pair with value > 0 between them) are joined at height exactly 1.0 in id order, ((r0 r1) r2) ...
+ * stats (may be NULL): edges, flat clusters, rounds (the rounds that merged something) and t_device.
+ * Refusals as for sk_cluster, plus ani >= 2, min_ani out of range or NaN, a method other than 0 / 1 and NULL merges in
+ * dendrogram mode (SK_ERR_PARAM); more than n rounds give SK_ERR_STATE. */
+typedef struct {
+  float min_ani;       /* the cut, as a fraction in (0.1, 1] */
+  int32_t method;      /* SK_LINKAGE_AVERAGE or SK_LINKAGE_COMPLETE */
+  int32_t dendrogram;  /* 1 = every merge with value > 0, written to merges */
+} sk_linkage_params;
+#define SK_LINKAGE_AVERAGE 0
+#define SK_LINKAGE_COMPLETE 1
+typedef struct {
+  uint32_t a, b;   /* the joined clusters: genome index < n_genomes, or n_genomes + row */
+  double height;   /* 1 - similarity */
+  uint64_t size;   /* genomes in the new cluster */
+} sk_merge;
+int sk_cluster_linkage(sk_ctx* ctx, uint32_t n_genomes, const sk_ani_result* results, uint64_t n_results, const uint32_t* rank,
+                       const sk_linkage_params* lp, uint32_t* rep, uint32_t* cluster, uint64_t* edge, sk_merge* merges,
+                       sk_cluster_stats* stats /* may be NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -169,6 +169,8 @@ struct Opts {
   bool separate_sketches = false;   // sketch --separate-sketches
   double cluster_ani = 95.0;        // cluster --ani (percent)
   bool single_linkage = false;      // cluster --single-linkage
+  std::string linkage;              // cluster --linkage average|complete
+  std::string dendrogram;           // cluster --dendrogram FILE
 };
 
 void write_header(FILE* o, bool ci, bool detailed) {   // src/file_io.rs:15-23
@@ -730,13 +732,21 @@ int run_triangle(Opts& op) {
 }
 
 // cluster: the triangle's results (the rows `triangle -E` prints) clustered on the GPU by sk_cluster at ANI >= --ani, greedy
-// representatives or --single-linkage, genomes ranked by total sequence length (longest first, ties by genome index).  One TSV
-// row per genome in genome-index order: its representative, cluster, and the ANI / aligned fractions of the row joining them.
+// representatives or --single-linkage, or by sk_cluster_linkage (--linkage average|complete: every printed row is a
+// similarity, --ani the cut; --dendrogram FILE writes the scipy linkage matrix), genomes ranked by total sequence length
+// (longest first, ties by genome index).  One TSV row per genome in genome-index order: its representative, cluster, and the
+// ANI / aligned fractions of the row joining them.
 int run_cluster(Opts& op) {
   if (op.sparse || op.full_matrix || op.diagonal || op.distance || op.ci || op.detailed) {
     fprintf(stderr, "ERROR -E/--sparse, --full-matrix, --diagonal, --distance, --ci and --detailed are triangle output options; cluster does not take them.\n");
     return 2;
   }
+  if (!op.linkage.empty() && op.linkage != "average" && op.linkage != "complete") {
+    fprintf(stderr, "ERROR --linkage %s: the methods are average and complete.\n", op.linkage.c_str());
+    return 2;
+  }
+  if (!op.linkage.empty() && op.single_linkage) { fprintf(stderr, "ERROR --linkage and --single-linkage exclude each other.\n"); return 2; }
+  if (!op.dendrogram.empty() && op.linkage.empty()) { fprintf(stderr, "ERROR --dendrogram needs --linkage average|complete.\n"); return 2; }
   Inputs in;
   sk_ctx* ctx = nullptr;
   std::vector<sk_ani_result> all;
@@ -750,9 +760,24 @@ int run_cluster(Opts& op) {
   for (uint32_t g = 0; g < N; g++) order[g] = g;
   std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return in.genomes[a].total_len > in.genomes[b].total_len; });
   for (uint32_t i = 0; i < N; i++) rank[order[i]] = i;
-  const sk_cluster_params cp{(float)(op.cluster_ani / 100.0), op.single_linkage ? 1 : 0};
   sk_cluster_stats st{};
-  CK(ctx, sk_cluster(ctx, N, res.data(), res.size(), rank.data(), &cp, rep.data(), cluster.data(), edge.data(), &st));
+  std::vector<sk_merge> merges;
+  if (op.linkage.empty()) {
+    const sk_cluster_params cp{(float)(op.cluster_ani / 100.0), op.single_linkage ? 1 : 0};
+    CK(ctx, sk_cluster(ctx, N, res.data(), res.size(), rank.data(), &cp, rep.data(), cluster.data(), edge.data(), &st));
+  } else {
+    const sk_linkage_params lp{(float)(op.cluster_ani / 100.0), op.linkage == "complete" ? SK_LINKAGE_COMPLETE : SK_LINKAGE_AVERAGE,
+                               op.dendrogram.empty() ? 0 : 1};
+    if (!op.dendrogram.empty()) merges.resize(N ? N - 1 : 0);
+    CK(ctx, sk_cluster_linkage(ctx, N, res.data(), res.size(), rank.data(), &lp, rep.data(), cluster.data(), edge.data(),
+                               merges.empty() ? nullptr : merges.data(), &st));
+  }
+  if (!op.dendrogram.empty()) {   // scipy linkage matrix, heights in percent distance as `triangle --distance` prints them
+    FILE* z = fopen(op.dendrogram.c_str(), "w");
+    if (!z) { fprintf(stderr, "ERROR cannot open %s\n", op.dendrogram.c_str()); return 1; }
+    for (const sk_merge& m : merges) fprintf(z, "%u\t%u\t%.6f\t%llu\n", m.a, m.b, 100.0 * m.height, (unsigned long long)m.size);
+    fclose(z);
+  }
   FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
   if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
   fprintf(o, "Genome_file\tRepresentative_file\tCluster\tANI\tAlign_fraction_genome\tAlign_fraction_representative\tGenome_name\tRepresentative_name\n");
@@ -770,8 +795,12 @@ int run_cluster(Opts& op) {
     fprintf(o, "\t%s\t%s\n", short_name(gg.contigs[0], op.short_header).c_str(), short_name(rg.contigs[0], op.short_header).c_str());
   }
   if (o != stdout) fclose(o);
-  fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (%s), clustering %.1f ms\n", N, st.n_clusters, op.cluster_ani,
-          op.single_linkage ? "single linkage" : "greedy", st.t_device * 1e3);
+  if (op.linkage.empty())
+    fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (%s), clustering %.1f ms\n", N, st.n_clusters, op.cluster_ani,
+            op.single_linkage ? "single linkage" : "greedy", st.t_device * 1e3);
+  else
+    fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (%s linkage, %u rounds), clustering %.1f ms\n", N, st.n_clusters,
+            op.cluster_ani, op.linkage.c_str(), st.rounds, st.t_device * 1e3);
   sk_ctx_destroy(ctx);
   return 0;
 }
@@ -1268,9 +1297,12 @@ void usage() {
           "      index.db and sketches.db), mixed freely; a database stands for all of its sketches\n"
           "  skani-b200 sketch [fasta ... | -l list] -o new_folder [-i] [--separate-sketches]\n"
           "  skani-b200 search -d sketch_folder [query ... | -q ... | --ql list] [--qi] [-n N] [-o out]\n"
-          "  skani-b200 cluster [fasta | sketch ... | -l list] [-i] [--ani T] [--single-linkage] [-o out]\n"
+          "  skani-b200 cluster [fasta | sketch ... | -l list] [-i] [--ani T] [--single-linkage | --linkage average|complete]\n"
+          "                    [--dendrogram Z.tsv] [-o out]\n"
           "      the triangle's genomes clustered at ANI >= T %% (default 95, 10 < T <= 100): greedy representatives, longest\n"
-          "      genomes first, or --single-linkage components; one TSV row per genome with its representative and cluster\n"
+          "      genomes first, --single-linkage components, or --linkage average / complete (UPGMA / complete linkage of\n"
+          "      100 - ANI, 100 for pairs not printed, cut at 100 - T); one TSV row per genome with its representative and\n"
+          "      cluster; --dendrogram writes the linkage matrix (a b height size, heights in percent) that scipy takes\n"
           "  common: -c C -m M -k K -s SCREEN%% --min-af P --both-min-af P --robust --median --no-learned-ani --faster-small\n"
           "          --small-genomes --fast --medium --slow --ci --detailed --short-header --no-marker-index -t THREADS --device D\n"
           "          --gpus N (triangle, dist, search, sketch, cluster: one context per GPU, devices D, D+1, ...)\n");
@@ -1340,6 +1372,8 @@ int main(int argc, char** argv) {
       }
     }
     else if (a == "--single-linkage" && op.cmd == "cluster") op.single_linkage = true;
+    else if (a == "--linkage" && op.cmd == "cluster") op.linkage = val();
+    else if (a == "--dendrogram" && op.cmd == "cluster") op.dendrogram = val();
     else if (a == "--keep-refs") {}   // search already loads every passing reference exactly once
     else if (a == "-v" || a == "--debug" || a == "--trace") {}
     else { fprintf(stderr, "ERROR unknown option %s\n", a.c_str()); usage(); return 2; }

@@ -4,7 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import AniResult, ChainDebug, ClusterParams, ClusterStats, MapParams, SketchParams, StoreStats, TriangleStats
+from ._lib import AniResult, ChainDebug, ClusterParams, ClusterStats, LinkageParams, MapParams, SketchParams, StoreStats, TriangleStats
 
 # numpy view of sk_ani_result (include/skani_b200.h): lets callers take 10^5..10^6 results without per-row Python objects
 RESULT_DTYPE = np.dtype([(n, np.float32) for n in ("ani", "af_query", "af_ref", "ci_lower", "ci_upper", "std", "q90_q", "q90_r", "q50_q",
@@ -674,3 +674,34 @@ def cluster(ctx, n_genomes, results, rank, min_ani=0.95, single_linkage=False):
     ctx.check(ctx.L.sk_cluster(ctx.h, int(n_genomes), res.ctypes.data if len(res) else None, len(res), rk.ctypes.data if len(rk) else None,
                                C.byref(cp), rep.ctypes.data, cl.ctypes.data, edge.ctypes.data, C.byref(st)))
     return rep[:n_genomes], cl[:n_genomes], edge[:n_genomes], st
+
+
+MERGE_DTYPE = np.dtype([("a", np.uint32), ("b", np.uint32), ("height", np.float64), ("size", np.uint64)])   # sk_merge
+LINKAGE_METHODS = {"average": 0, "complete": 1}
+
+
+def cluster_linkage(ctx, n_genomes, results, rank, method="average", min_ani=0.95, dendrogram=False):
+    """sk_cluster_linkage: average (UPGMA) or complete linkage of triangle results (a RESULT_DTYPE array) over the rows with
+    ani > 0.1, similarity 0 for pairs without a row; flat clusters at min_ani in (0.1, 1].  Returns (rep, cluster, edge, Z,
+    stats) with rep / cluster / edge as cluster() defines them and Z, when dendrogram is set, the (n - 1, 4) float64 scipy
+    linkage matrix (a, b, 1 - similarity, size) over genome indices; None otherwise."""
+    if method not in LINKAGE_METHODS:
+        raise ValueError("method must be 'average' or 'complete'")
+    res = np.ascontiguousarray(results)
+    if res.dtype != RESULT_DTYPE:
+        raise TypeError("results must be a RESULT_DTYPE array")
+    rk = np.ascontiguousarray(rank, np.uint32)
+    if len(rk) != n_genomes:
+        raise ValueError("rank needs one entry per genome")
+    n = max(int(n_genomes), 1)
+    rep = np.zeros(n, np.uint32); cl = np.zeros(n, np.uint32); edge = np.zeros(n, np.uint64)
+    merges = np.zeros(max(n - 1, 1), MERGE_DTYPE) if dendrogram else None
+    lp = LinkageParams(float(min_ani), LINKAGE_METHODS[method], int(bool(dendrogram))); st = ClusterStats()
+    ctx.check(ctx.L.sk_cluster_linkage(ctx.h, int(n_genomes), res.ctypes.data if len(res) else None, len(res),
+                                       rk.ctypes.data if len(rk) else None, C.byref(lp), rep.ctypes.data, cl.ctypes.data,
+                                       edge.ctypes.data, None if merges is None else merges.ctypes.data, C.byref(st)))
+    Z = None
+    if dendrogram:
+        m = merges[:max(int(n_genomes) - 1, 0)]
+        Z = np.stack([m["a"].astype(np.float64), m["b"].astype(np.float64), m["height"], m["size"].astype(np.float64)], 1).reshape(-1, 4)
+    return rep[:n_genomes], cl[:n_genomes], edge[:n_genomes], Z, st
