@@ -497,6 +497,34 @@ int sk_cluster_linkage(sk_ctx* ctx, uint32_t n_genomes, const sk_ani_result* res
                        const sk_linkage_params* lp, uint32_t* rep, uint32_t* cluster, uint64_t* edge, sk_merge* merges,
                        sk_cluster_stats* stats /* may be NULL */);
 
+/* ---- neighbour-joining tree of a triangle's results (what users otherwise get by printing `--full-matrix --distance` and
+ *      running quicktree or rapidnj on it).  Inputs and refusals as for sk_cluster_linkage, plus: a row with ani > 1 gives
+ *      SK_ERR_PARAM (its distance would be negative).  results is HOST memory.
+ * Distances: d(i,j) = 1 - (double)ani for every row with ani > 0.1 (exact: such a float is a multiple of 2^-27), 1.0 for a
+ * pair without one, d(i,i) = 0; R_i = sum_j d(i,j) (exact for n < 2^26).  A node's id is the smallest genome index among
+ * its leaves; live nodes are ordered by id.  While m > 2 nodes are live, in float64 with every operation rounded on its own:
+ *   Q = ((m-2) d_ij - R_i) - R_j over live pairs i < j; the join is the smallest Q, ties to the smallest (i, j);
+ *   delta_i = 0.5 d_ij + (R_i - R_j) / (2.0 (m-2)), delta_j = d_ij - delta_i;
+ *   for every other live k: d_uk = 0.5 ((d_ik + d_jk) - d_ij), R_k = ((R_k - d_ik) - d_jk) + d_uk;
+ *   R_u = 0.5 ((R_i + R_j) - m d_ij); the new node u takes i's id and j leaves.
+ * joins (n_genomes - 1 rows; may be NULL for n < 2): row t = (a, b, delta_i, delta_j), nodes numbered the scipy way (leaves
+ * 0..n-1, row t creates n + t), a the node of smaller id.  Row n - 2 joins the last two nodes with len_a = len_b = d / 2: a
+ * binary tree rooted at the midpoint of the last edge.  Branch lengths may be negative; they are returned as computed.
+ * The device holds the n x n float64 matrix plus a compacted copy (at most 8 n^2 (1 + 9/16) bytes); more than fits gives
+ * SK_ERR_NOMEM with the bytes needed.
+ * stats (may be NULL): edges, joins written, compactions of the matrix and t_device. */
+typedef struct {
+  uint32_t a, b;        /* the joined nodes: genome index < n_genomes, or n_genomes + row */
+  double len_a, len_b;  /* branch lengths from the new node to a and to b (distance, 1 - ANI scale) */
+} sk_nj_join;
+typedef struct {
+  uint64_t n_edges;
+  uint32_t joins, compactions;
+  double t_device;
+} sk_nj_stats;
+int sk_neighbor_joining(sk_ctx* ctx, uint32_t n_genomes, const sk_ani_result* results, uint64_t n_results, sk_nj_join* joins,
+                        sk_nj_stats* stats /* may be NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -63,6 +63,10 @@ class Merge(C.Structure):
     _fields_ = [("a", C.c_uint32), ("b", C.c_uint32), ("height", C.c_double), ("size", C.c_uint64)]
 
 
+class NjStats(C.Structure):
+    _fields_ = [("n_edges", C.c_uint64), ("joins", C.c_uint32), ("compactions", C.c_uint32), ("t_device", C.c_double)]
+
+
 # every symbol include/skani_b200.h declares: (name, restype, argtypes)
 vp, u64, u32, i32 = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int
 PP = C.POINTER
@@ -133,6 +137,7 @@ SYMBOLS = [
     ("sk_query_ref_store", i32, [vp, u32, vp, vp, PP(MapParams), i32, u64, PP(PP(AniResult)), PP(u64), PP(StoreStats)]),
     ("sk_cluster", i32, [vp, u32, vp, u64, vp, PP(ClusterParams), vp, vp, vp, PP(ClusterStats)]),
     ("sk_cluster_linkage", i32, [vp, u32, vp, u64, vp, PP(LinkageParams), vp, vp, vp, vp, PP(ClusterStats)]),
+    ("sk_neighbor_joining", i32, [vp, u32, vp, u64, vp, PP(NjStats)]),
 ]
 
 _lib = None

@@ -171,6 +171,7 @@ struct Opts {
   bool single_linkage = false;      // cluster --single-linkage
   std::string linkage;              // cluster --linkage average|complete
   std::string dendrogram;           // cluster --dendrogram FILE
+  std::string tree_method = "nj";   // tree --method nj|average|complete
 };
 
 void write_header(FILE* o, bool ci, bool detailed) {   // src/file_io.rs:15-23
@@ -731,6 +732,16 @@ int run_triangle(Opts& op) {
   return 0;
 }
 
+// genomes ranked by total sequence length, longest first, ties by genome index (cluster's choice of representatives)
+std::vector<uint32_t> length_rank(const Inputs& in) {
+  const uint32_t N = (uint32_t)in.genomes.size();
+  std::vector<uint32_t> order(N), rank(N);
+  for (uint32_t g = 0; g < N; g++) order[g] = g;
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return in.genomes[a].total_len > in.genomes[b].total_len; });
+  for (uint32_t i = 0; i < N; i++) rank[order[i]] = i;
+  return rank;
+}
+
 // cluster: the triangle's results (the rows `triangle -E` prints) clustered on the GPU by sk_cluster at ANI >= --ani, greedy
 // representatives or --single-linkage, or by sk_cluster_linkage (--linkage average|complete: every printed row is a
 // similarity, --ani the cut; --dendrogram FILE writes the scipy linkage matrix), genomes ranked by total sequence length
@@ -755,11 +766,9 @@ int run_cluster(Opts& op) {
   for (auto& r : all) if (r.ani > 0.1f) res.push_back(r);
   all = std::vector<sk_ani_result>();
   const uint32_t N = (uint32_t)in.genomes.size();
-  std::vector<uint32_t> order(N), rank(N), rep(N), cluster(N);
+  const std::vector<uint32_t> rank = length_rank(in);
+  std::vector<uint32_t> rep(N), cluster(N);
   std::vector<uint64_t> edge(N);
-  for (uint32_t g = 0; g < N; g++) order[g] = g;
-  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return in.genomes[a].total_len > in.genomes[b].total_len; });
-  for (uint32_t i = 0; i < N; i++) rank[order[i]] = i;
   sk_cluster_stats st{};
   std::vector<sk_merge> merges;
   if (op.linkage.empty()) {
@@ -801,6 +810,113 @@ int run_cluster(Opts& op) {
   else
     fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (%s linkage, %u rounds), clustering %.1f ms\n", N, st.n_clusters,
             op.cluster_ani, op.linkage.c_str(), st.rounds, st.t_device * 1e3);
+  sk_ctx_destroy(ctx);
+  return 0;
+}
+
+// a Newick label: as is, or single-quoted with every ' doubled when it holds whitespace or any of ()[]':;,
+std::string newick_label(const std::string& s) {
+  if (!s.empty() && s.find_first_of(" \t\r\n()[]':;,") == std::string::npos) return s;
+  std::string q = "'";
+  for (char c : s) q += c == '\'' ? std::string("''") : std::string(1, c);
+  return q + "'";
+}
+
+// Newick text of a tree whose internal nodes list their (child, branch length) pairs: nodes < n_leaves are leaves, `root`
+// is written without a length.  An explicit stack, not recursion: a caterpillar of 50 000 leaves nests 50 000 deep.
+std::string newick(uint32_t n_leaves, const std::vector<std::string>& labels,
+                   const std::vector<std::vector<std::pair<uint32_t, double>>>& kids, uint32_t root) {
+  if (root < n_leaves) return labels[root] + ";\n";
+  std::string out = "(";
+  char len[64];
+  struct Frame { uint32_t v; size_t next; double len; };
+  std::vector<Frame> st{{root, 0, 0.0}};
+  while (!st.empty()) {
+    Frame& f = st.back();
+    if (f.next < kids[f.v].size()) {
+      if (f.next) out += ',';
+      const std::pair<uint32_t, double> c = kids[f.v][f.next++];
+      if (c.first < n_leaves) {
+        snprintf(len, sizeof(len), ":%.6f", 100.0 * c.second);
+        out += labels[c.first];
+        out += len;
+      } else {
+        out += '(';
+        st.push_back({c.first, 0, c.second});
+      }
+      continue;
+    }
+    out += ')';
+    if (st.size() > 1) { snprintf(len, sizeof(len), ":%.6f", 100.0 * f.len); out += len; }
+    st.pop_back();
+  }
+  return out + ";\n";
+}
+
+// tree: the triangle's genomes (every row `triangle -E` prints) as a Newick tree, branch lengths in percent distance.
+// --method nj (default): sk_neighbor_joining, written unrooted with the basal trifurcation (X, Y, K): X and Y the children
+// of the last internal node, K the other last node at the full last-edge length.  --method average | complete:
+// sk_cluster_linkage's dendrogram (genomes ranked as cluster ranks them), rooted, a child at (h_parent - h_child) / 2 below
+// its parent, so that patristic distances are the cophenetic ones.  Labels as triangle's matrix names its rows.
+int run_tree(Opts& op) {
+  if (op.sparse || op.full_matrix || op.diagonal || op.distance || op.ci || op.detailed) {
+    fprintf(stderr, "ERROR -E/--sparse, --full-matrix, --diagonal, --distance, --ci and --detailed are triangle output options; tree does not take them.\n");
+    return 2;
+  }
+  if (op.tree_method != "nj" && op.tree_method != "average" && op.tree_method != "complete") {
+    fprintf(stderr, "ERROR --method %s: the methods are nj, average and complete.\n", op.tree_method.c_str());
+    return 2;
+  }
+  Inputs in;
+  sk_ctx* ctx = nullptr;
+  std::vector<sk_ani_result> all;
+  if (const int rc = triangle_results(op, in, ctx, all, nullptr)) return rc;
+  std::vector<sk_ani_result> res;
+  for (auto& r : all) if (r.ani > 0.1f) res.push_back(r);
+  all = std::vector<sk_ani_result>();
+  const uint32_t N = (uint32_t)in.genomes.size();
+  std::vector<std::string> labels(N);
+  for (uint32_t g = 0; g < N; g++) labels[g] = newick_label(op.individual ? in.genomes[g].contigs[0] : in.genomes[g].file_name);
+  std::vector<std::vector<std::pair<uint32_t, double>>> kids(N ? 2 * N : 0);   // node 2N - 1: the NJ trifurcation
+  uint32_t root = N ? 2 * N - 2 : 0, steps = 0;
+  double t_device = 0;
+  if (op.tree_method == "nj") {
+    std::vector<sk_nj_join> joins(N > 1 ? N - 1 : 0);
+    sk_nj_stats st{};
+    CK(ctx, sk_neighbor_joining(ctx, N, res.data(), res.size(), joins.empty() ? nullptr : joins.data(), &st));
+    for (uint32_t t = 0; t < joins.size(); t++) kids[N + t] = {{joins[t].a, joins[t].len_a}, {joins[t].b, joins[t].len_b}};
+    if (N >= 3) {   // unroot: the last internal node's children and the other last node, at the whole last edge
+      const sk_nj_join& l = joins[N - 2];
+      const uint32_t last = 2 * N - 3, other = l.a == last ? l.b : l.a;
+      root = 2 * N - 1;
+      kids[root] = kids[last];
+      kids[root].push_back({other, l.len_a + l.len_b});
+    }
+    steps = st.compactions;
+    t_device = st.t_device;
+  } else {
+    std::vector<uint32_t> rep(N), cluster(N);
+    std::vector<uint64_t> edge(N);
+    std::vector<sk_merge> merges(N > 1 ? N - 1 : 0);
+    const std::vector<uint32_t> rank = length_rank(in);
+    const sk_linkage_params lp{(float)(op.cluster_ani / 100.0), op.tree_method == "complete" ? SK_LINKAGE_COMPLETE : SK_LINKAGE_AVERAGE, 1};
+    sk_cluster_stats st{};
+    CK(ctx, sk_cluster_linkage(ctx, N, res.data(), res.size(), rank.data(), &lp, rep.data(), cluster.data(), edge.data(),
+                               merges.empty() ? nullptr : merges.data(), &st));
+    const auto height = [&](uint32_t v) { return v < N ? 0.0 : merges[v - N].height; };
+    for (uint32_t j = 0; j < merges.size(); j++) {
+      const double h = merges[j].height;
+      kids[N + j] = {{merges[j].a, (h - height(merges[j].a)) / 2}, {merges[j].b, (h - height(merges[j].b)) / 2}};
+    }
+    steps = st.rounds;
+    t_device = st.t_device;
+  }
+  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
+  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
+  if (N) fputs(newick(N, labels, kids, root).c_str(), o);
+  if (o != stdout) fclose(o);
+  fprintf(stderr, "INFO %u genomes, tree by %s (%u %s), %.1f ms on the device\n", N, op.tree_method.c_str(), steps,
+          op.tree_method == "nj" ? "compactions" : "rounds", t_device * 1e3);
   sk_ctx_destroy(ctx);
   return 0;
 }
@@ -1303,9 +1419,13 @@ void usage() {
           "      genomes first, --single-linkage components, or --linkage average / complete (UPGMA / complete linkage of\n"
           "      100 - ANI, 100 for pairs not printed, cut at 100 - T); one TSV row per genome with its representative and\n"
           "      cluster; --dendrogram writes the linkage matrix (a b height size, heights in percent) that scipy takes\n"
+          "  skani-b200 tree [fasta | sketch ... | -l list] [-i] [--method nj|average|complete] [-o tree.nwk]\n"
+          "      the triangle's genomes as a Newick tree of 100 - ANI (100 for pairs not printed), branch lengths in percent:\n"
+          "      neighbour joining (default; unrooted, basal trifurcation) or the average / complete linkage dendrogram\n"
+          "      (rooted, a node at half its merge height)\n"
           "  common: -c C -m M -k K -s SCREEN%% --min-af P --both-min-af P --robust --median --no-learned-ani --faster-small\n"
           "          --small-genomes --fast --medium --slow --ci --detailed --short-header --no-marker-index -t THREADS --device D\n"
-          "          --gpus N (triangle, dist, search, sketch, cluster: one context per GPU, devices D, D+1, ...)\n");
+          "          --gpus N (triangle, dist, search, sketch, cluster, tree: one context per GPU, devices D, D+1, ...)\n");
 }
 
 }  // namespace
@@ -1314,7 +1434,8 @@ int main(int argc, char** argv) {
   if (argc < 2) { usage(); return 2; }
   Opts op;
   op.cmd = argv[1];
-  if (op.cmd != "triangle" && op.cmd != "dist" && op.cmd != "sketch" && op.cmd != "search" && op.cmd != "ingest" && op.cmd != "cluster") { usage(); return 2; }
+  if (op.cmd != "triangle" && op.cmd != "dist" && op.cmd != "sketch" && op.cmd != "search" && op.cmd != "ingest" && op.cmd != "cluster" &&
+      op.cmd != "tree") { usage(); return 2; }
   std::vector<std::string> positional;
   enum { NONE, QS, RS } multi = NONE;
   for (int i = 2; i < argc; i++) {
@@ -1374,13 +1495,15 @@ int main(int argc, char** argv) {
     else if (a == "--single-linkage" && op.cmd == "cluster") op.single_linkage = true;
     else if (a == "--linkage" && op.cmd == "cluster") op.linkage = val();
     else if (a == "--dendrogram" && op.cmd == "cluster") op.dendrogram = val();
+    else if (a == "--method" && op.cmd == "tree") op.tree_method = val();
     else if (a == "--keep-refs") {}   // search already loads every passing reference exactly once
     else if (a == "-v" || a == "--debug" || a == "--trace") {}
     else { fprintf(stderr, "ERROR unknown option %s\n", a.c_str()); usage(); return 2; }
   }
-  if (op.cmd == "triangle" || op.cmd == "sketch" || op.cmd == "ingest" || op.cmd == "cluster") {
+  if (op.cmd == "triangle" || op.cmd == "sketch" || op.cmd == "ingest" || op.cmd == "cluster" || op.cmd == "tree") {
     op.files.insert(op.files.end(), positional.begin(), positional.end());
-    return op.cmd == "triangle" ? run_triangle(op) : op.cmd == "sketch" ? run_sketch(op) : op.cmd == "cluster" ? run_cluster(op) : run_ingest(op);
+    return op.cmd == "triangle" ? run_triangle(op) : op.cmd == "sketch" ? run_sketch(op) : op.cmd == "cluster" ? run_cluster(op)
+         : op.cmd == "tree" ? run_tree(op) : run_ingest(op);
   }
   if (op.cmd == "search") {
     op.queries.insert(op.queries.end(), positional.begin(), positional.end());

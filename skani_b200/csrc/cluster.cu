@@ -298,32 +298,9 @@ __global__ void lk_relabel_kernel(uint64_t* __restrict__ key, uint32_t m, const 
   key[i] = a == LK_NONE || b == LK_NONE || a == b ? sent : (uint64_t)a << 32 | b;
 }
 
-// device temporaries of sk_cluster and sk_cluster_linkage (`who`): a failed allocation is SK_ERR_NOMEM
-template <typename T>
-int cl_alloc(sk_ctx* ctx, DTmp<T>& t, uint64_t count, const char* what, const char* who = "sk_cluster") {
-  if (t.alloc(count, ctx) != cudaSuccess) {
-    cudaGetLastError();
-    ctx->err = std::string(who) + ": out of device memory (" + what + ", " + std::to_string(count * sizeof(T)) + " bytes)";
-    return SK_ERR_NOMEM;
-  }
-  return SK_OK;
-}
+}  // namespace
 
-std::string row_text(const sk_ani_result* results, uint64_t row) {
-  return "row " + std::to_string(row) + " (" + std::to_string(results[row].ref_id) + ", " + std::to_string(results[row].query_id) + ")";
-}
-
-// the edges of a triangle's results and their symmetric CSR (adj: keys a << 32 | b ascending, adj_e: edge index)
-struct Graph {
-  DTmp<uint64_t> ekey, erow, key[2], off;
-  DTmp<float> eani;
-  DTmp<uint32_t> val[2];
-  uint64_t E = 0;
-  const uint64_t* adj = nullptr;
-  const uint32_t* adj_e = nullptr;
-};
-
-int build_graph(sk_ctx* ctx, const char* who, uint32_t n, const sk_ani_result* results, uint64_t n_results, float min_ani, Graph& g) {
+int sk::build_graph(sk_ctx* ctx, const char* who, uint32_t n, const sk_ani_result* results, uint64_t n_results, float min_ani, Graph& g) {
   cudaStream_t st = ctx->stream;
   const auto launched = [&](unsigned k = 1) { count_launch(ctx, k); return cudaGetLastError(); };
   DTmp<uint8_t> chunk;
@@ -391,6 +368,8 @@ int build_graph(sk_ctx* ctx, const char* who, uint32_t n, const sk_ani_result* r
   }
   return SK_OK;
 }
+
+namespace {
 
 // representatives (flag[rank[v]] = 1) numbered in rank order, then rep / cluster / edge read back
 int number_and_read_back(sk_ctx* ctx, const char* who, uint32_t n, const uint32_t* d_rank, const uint32_t* d_rep, const uint64_t* d_edge,

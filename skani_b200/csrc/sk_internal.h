@@ -257,4 +257,30 @@ bool host_pinned(const void* p);   // api.cu: is a host buffer page-locked?
 // host byte runs, back to back, -> device dst on ctx->stream: straight from page-locked memory (pinned), otherwise staged
 // through the context's two pinned buffers (api.cu)
 int upload_runs(sk_ctx* ctx, uint8_t* dst, const std::vector<std::pair<const uint8_t*, uint64_t>>& runs, bool pinned);
+
+// cluster.cu / nj.cu: device temporaries of the calls on a triangle's results (`who`): a failed allocation is SK_ERR_NOMEM
+template <typename T>
+int cl_alloc(sk_ctx* ctx, DTmp<T>& t, uint64_t count, const char* what, const char* who = "sk_cluster") {
+  if (t.alloc(count, ctx) != cudaSuccess) {
+    cudaGetLastError();
+    ctx->err = std::string(who) + ": out of device memory (" + what + ", " + std::to_string(count * sizeof(T)) + " bytes)";
+    return SK_ERR_NOMEM;
+  }
+  return SK_OK;
+}
+inline std::string row_text(const sk_ani_result* results, uint64_t row) {
+  return "row " + std::to_string(row) + " (" + std::to_string(results[row].ref_id) + ", " + std::to_string(results[row].query_id) + ")";
+}
+// the edges of a triangle's results (rows with ani > 0.1 and ani >= min_ani: ekey = min id << 32 | max id, eani, erow = the
+// result row) and their symmetric CSR (adj: keys a << 32 | b ascending, adj_e: edge index).  build_graph refuses an id >=
+// n, a self pair and a pair listed twice among the edges (SK_ERR_PARAM, with `who` in the message).
+struct Graph {
+  DTmp<uint64_t> ekey, erow, key[2], off;
+  DTmp<float> eani;
+  DTmp<uint32_t> val[2];
+  uint64_t E = 0;
+  const uint64_t* adj = nullptr;
+  const uint32_t* adj_e = nullptr;
+};
+int build_graph(sk_ctx* ctx, const char* who, uint32_t n, const sk_ani_result* results, uint64_t n_results, float min_ani, Graph& g);
 }  // namespace sk

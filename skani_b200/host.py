@@ -4,7 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import AniResult, ChainDebug, ClusterParams, ClusterStats, LinkageParams, MapParams, SketchParams, StoreStats, TriangleStats
+from ._lib import AniResult, ChainDebug, ClusterParams, ClusterStats, LinkageParams, MapParams, NjStats, SketchParams, StoreStats, TriangleStats
 
 # numpy view of sk_ani_result (include/skani_b200.h): lets callers take 10^5..10^6 results without per-row Python objects
 RESULT_DTYPE = np.dtype([(n, np.float32) for n in ("ani", "af_query", "af_ref", "ci_lower", "ci_upper", "std", "q90_q", "q90_r", "q50_q",
@@ -705,3 +705,21 @@ def cluster_linkage(ctx, n_genomes, results, rank, method="average", min_ani=0.9
         m = merges[:max(int(n_genomes) - 1, 0)]
         Z = np.stack([m["a"].astype(np.float64), m["b"].astype(np.float64), m["height"], m["size"].astype(np.float64)], 1).reshape(-1, 4)
     return rep[:n_genomes], cl[:n_genomes], edge[:n_genomes], Z, st
+
+
+NJ_JOIN_DTYPE = np.dtype([("a", np.uint32), ("b", np.uint32), ("len_a", np.float64), ("len_b", np.float64)])   # sk_nj_join
+
+
+def neighbor_joining(ctx, n_genomes, results):
+    """sk_neighbor_joining: the neighbour-joining tree of triangle results (a RESULT_DTYPE array) over the rows with ani > 0.1,
+    distance 1 - ani, 1.0 for pairs without a row.  Returns (joins, stats): joins an NJ_JOIN_DTYPE array of n - 1 rows (a, b,
+    len_a, len_b), nodes numbered the scipy way (leaves 0..n-1, row t creates n + t), the last row joining the final two nodes
+    at half their distance each; stats the sk_nj_stats struct."""
+    res = np.ascontiguousarray(results)
+    if res.dtype != RESULT_DTYPE:
+        raise TypeError("results must be a RESULT_DTYPE array")
+    n = int(n_genomes)
+    joins = np.zeros(max(n - 1, 1), NJ_JOIN_DTYPE)
+    st = NjStats()
+    ctx.check(ctx.L.sk_neighbor_joining(ctx.h, n, res.ctypes.data if len(res) else None, len(res), joins.ctypes.data, C.byref(st)))
+    return joins[:max(n - 1, 0)], st
