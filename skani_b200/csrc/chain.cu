@@ -195,8 +195,9 @@ probe_kernel(const PairDesc* __restrict__ pairs, uint32_t n_pairs, SetView s0, S
   }
   const uint32_t ht_shift = use_hash ? (32u - (uint32_t)__ffs((int)(rm.ht_cap >> 2)) + 1u) : 32u;   // 32 - log2(buckets); capacity >= 16 entries
   if (!use_hash) {  // fallback (genomes with >= 2^20 records): bucket index (16 KB) staged in shared memory
+    // a genome without seed k-mers has neither a table nor a bucket index (the set may have none at all): every probe misses
     const uint32_t* gb = (pd.rset ? s1.ubucket : s0.ubucket) + (size_t)rm.g * (UBUCKETS + 1);
-    for (uint32_t b = threadIdx.x; b <= UBUCKETS; b += CT) s_bucket[b] = gb[b];
+    for (uint32_t b = threadIdx.x; b <= UBUCKETS; b += CT) s_bucket[b] = nuk ? gb[b] : 0u;
     __syncthreads();
   }
   uint32_t hn[ITEMS], hr[ITEMS], hc[ITEMS];   // per record: anchors (nh), ref group start, counted
