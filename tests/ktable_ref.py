@@ -10,10 +10,12 @@ key's group start in the genome's k-mer view (records sorted by k-mer) and count
 bucket whose last slot is empty."""
 import numpy as np
 
+import seed_ref
+from seed_ref import MARKER_K, is_seed, mm_hash64  # noqa: F401  (the GPU table tests use them through this module)
+
 GOLDEN = 0x9E3779B1
 COUNT_MAX = 4095                  # 12-bit count field
 START_BITS = 20                   # 20-bit start field: genomes of >= 2^20 records get no table
-MARKER_K = 21                     # seeding windows are 21-mers (the marker k)
 U64 = np.uint64
 
 
@@ -145,52 +147,20 @@ def build_table(keys, starts, counts, cap, order=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# seeding (for planting chosen k-mers): the 4-lane FracMinHash seeder's semantics, numpy-vectorised over rows
+# seeding (for planting chosen k-mers): seed_ref's restatement of the 4-lane FracMinHash seeder
 # ---------------------------------------------------------------------------------------------------------------------
-_CODE = np.zeros(256, np.uint64)
-_CODE[np.frombuffer(b"ACGT", np.uint8)] = np.arange(4, dtype=np.uint64)
-_CODE[np.frombuffer(b"acgt", np.uint8)] = np.arange(4, dtype=np.uint64)
-
-
-def mm_hash64(x):
-    with np.errstate(over="ignore"):
-        x = np.asarray(x, np.uint64)
-        x = ~(x + (x << U64(21)))
-        x = x ^ (x >> U64(24))
-        x = (x + (x << U64(3))) + (x << U64(8))
-        x = x ^ (x >> U64(14))
-        x = (x + (x << U64(2))) + (x << U64(4))
-        x = x ^ (x >> U64(28))
-        return x + (x << U64(31))
-
-
-def is_seed(keys, c):
-    return mm_hash64(keys) < U64((2 ** 64 - 1) // c)
 
 
 def window_seeds(seqs, k, c):
     """seqs: (n, L) uint8 ASCII rows of A/C/G/T.  For every window end i in [20, L) (each window a 21-mer): the seed key
     min(forward k-mer ending at i, reverse complement of the k-mer starting at i - 20) and whether it is a seed at c.
     Returns (keys (n, L - 20) uint32, is_seed (n, L - 20) bool); column j is window end 20 + j."""
-    s = np.atleast_2d(np.asarray(seqs, np.uint8))
-    code = _CODE[s]
-    L = s.shape[1]
-    W = L - (MARKER_K - 1)
-    fs = np.zeros((len(s), W), np.uint64)
-    rs = np.zeros((len(s), W), np.uint64)
-    for j in range(k):
-        fs |= code[:, MARKER_K - 1 - j:L - j] << U64(2 * j)              # base i - j at bits 2j
-        rs |= (U64(3) - code[:, j:j + W]) << U64(2 * j)                  # complement of base i - 20 + j at bits 2j
-    seed = np.where(rs > fs, fs, rs)
+    _, _, fs, rs = seed_ref.windows(seqs, k)
+    seed = np.where(fs < rs, fs, rs)
     return seed.astype(np.uint32), is_seed(seed, c)
 
 
 def contig_records(seq, k, c):
-    """(window end positions, keys) of the records one contig contributes: every window the 4-lane seeder visits (it
-    skips the last (L - 20) mod 4 windows) whose key is a seed"""
-    keys, ok = window_seeds(seq, k, c)
-    n = len(seq)
-    last = MARKER_K - 1 + 4 * ((n - MARKER_K + 1) // 4) if n >= 2 * MARKER_K else MARKER_K - 1
-    ok = ok[0, :last - (MARKER_K - 1)]
-    pos = np.nonzero(ok)[0]
-    return pos + MARKER_K - 1, keys[0, pos]
+    """(window end positions, keys) of the records one contig contributes under the 4-lane seeder"""
+    pos, keys, _, _ = seed_ref.contig_seeds(seq, k, c)
+    return pos.astype(np.int64), keys

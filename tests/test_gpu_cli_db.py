@@ -1,6 +1,6 @@
 """GPU: `skani-b200 sketch` writes a skani v0.3.0 database whose content (decoded by the independent Python decoder) is
-bit-identical to the oracle's sketches, and `skani-b200 search` on it reproduces the oracle's search rows (the oracle's
-search is pinned by the reference's golden G7, tests/test_oracle_goldens.py).  Covers the consolidated database, the
+bit-identical to the oracle's sketches, and `skani-b200 search` on it reproduces the oracle's search rows (no test pins
+the oracle's search to the reference's golden G7; tests/test_oracle_goldens.py covers G2-G4, G8 and G10-G13).  Covers the consolidated database, the
 --separate-sketches layout, FASTA queries and .sketch queries (src/sketch.rs, src/search.rs, src/sketch_db.rs)."""
 import os
 import subprocess
