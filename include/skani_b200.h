@@ -525,6 +525,37 @@ typedef struct {
 int sk_neighbor_joining(sk_ctx* ctx, uint32_t n_genomes, const sk_ani_result* results, uint64_t n_results, sk_nj_join* joins,
                         sk_nj_stats* stats /* may be NULL */);
 
+/* ---- greedy dereplication of an in-memory sketch set (what galah and dRep do on top of skani): sk_cluster's greedy
+ *      representatives without the triangle.  Only genome x representative pairs are screened and chained.
+ * Contract: for any set (with its name ranks), mp, rank permutation and min_ani, rep[] and cluster[] equal those of
+ * sk_cluster (single_linkage = 0, same min_ani and rank) run on the rows of sk_screen_triangle + sk_chain_pairs over the same
+ * set, and for every member g, join[g] is byte for byte the row sk_cluster's edge[g] points to.  For a representative,
+ * join[g] is all zero but ani = NaN and ref_id = query_id = g.  The result does not depend on dp->wave.
+ * Exactness rests on two facts: a pair's chain result depends only on the pair, the set, its name ranks and mp; and the greedy
+ * outcome depends only on the edges that touch a representative.  Every pair is screened with the triangle's rule (the
+ * smaller genome index is screen_refs' query, so only its marker count can rescue the pair) and chained as (min << 32 | max).
+ * Algorithm: genomes are visited in rank order in waves of dp->wave genomes (0 = the library default: 64 genomes, doubling per wave up to 4096).  A wave is
+ * screened and chained against the representatives chosen so far (a wave genome with an edge to one is a member), then the
+ * wave's undecided genomes against each other, decided by sk_cluster's greedy rounds; the new representatives' markers join
+ * the index.  Finally every member is screened against all representatives and the pairs not chained yet are chained; each
+ * member takes its representative neighbour of highest ANI, ties to the smaller rank.
+ * Refusals (SK_ERR_PARAM with a message): NULL arguments, a rank that is not a permutation, a NaN min_ani, more than
+ * 2^22 - 1 representatives (or undecided genomes in one wave) in an index, or 2^31 or more markers in one.  The set must be
+ * one context's in-memory set (sk_sketch_store sets are not taken).
+ * stats (may be NULL): pairs that passed a screen, pairs chained, edges among the chained rows, clusters, waves, greedy rounds,
+ * and the seconds spent screening, chaining, deciding (greedy rounds and assignment) and in all. */
+typedef struct {
+  float min_ani;   /* as a fraction, e.g. 0.95 */
+  uint32_t wave;   /* genomes per wave; 0 = library default */
+} sk_derep_params;
+typedef struct {
+  uint64_t pairs_screened, pairs_chained, n_edges;
+  uint32_t n_clusters, waves, rounds;
+  double t_screen, t_chain, t_decide, t_total;
+} sk_derep_stats;
+int sk_dereplicate(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* rank, const sk_derep_params* dp,
+                   uint32_t* rep, uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats /* may be NULL */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -67,6 +67,16 @@ class NjStats(C.Structure):
     _fields_ = [("n_edges", C.c_uint64), ("joins", C.c_uint32), ("compactions", C.c_uint32), ("t_device", C.c_double)]
 
 
+class DerepParams(C.Structure):
+    _fields_ = [("min_ani", C.c_float), ("wave", C.c_uint32)]
+
+
+class DerepStats(C.Structure):
+    _fields_ = [("pairs_screened", C.c_uint64), ("pairs_chained", C.c_uint64), ("n_edges", C.c_uint64), ("n_clusters", C.c_uint32),
+                ("waves", C.c_uint32), ("rounds", C.c_uint32), ("t_screen", C.c_double), ("t_chain", C.c_double),
+                ("t_decide", C.c_double), ("t_total", C.c_double)]
+
+
 # every symbol include/skani_b200.h declares: (name, restype, argtypes)
 vp, u64, u32, i32 = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int
 PP = C.POINTER
@@ -138,6 +148,7 @@ SYMBOLS = [
     ("sk_cluster", i32, [vp, u32, vp, u64, vp, PP(ClusterParams), vp, vp, vp, PP(ClusterStats)]),
     ("sk_cluster_linkage", i32, [vp, u32, vp, u64, vp, PP(LinkageParams), vp, vp, vp, vp, PP(ClusterStats)]),
     ("sk_neighbor_joining", i32, [vp, u32, vp, u64, vp, PP(NjStats)]),
+    ("sk_dereplicate", i32, [vp, vp, PP(MapParams), vp, PP(DerepParams), vp, vp, vp, PP(DerepStats)]),
 ]
 
 _lib = None

@@ -171,6 +171,7 @@ struct Opts {
   bool single_linkage = false;      // cluster --single-linkage
   std::string linkage;              // cluster --linkage average|complete
   std::string dendrogram;           // cluster --dendrogram FILE
+  std::string representatives;      // dereplicate --representatives FILE
   std::string tree_method = "nj";   // tree --method nj|average|complete
 };
 
@@ -570,41 +571,66 @@ using BlockWriter = std::function<bool(const std::vector<sk_ani_result>& rows, b
 // `stream`, the in-memory path chains and hands over the rows in blocks of INTERMEDIATE_WRITE_COUNT rows instead
 // (src/triangle.rs:113-138), so a long run leaves its finished rows on disk and holds at most one block of results in memory.
 // Returns 0, or the exit code after an ERROR line.
-int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_result>& res, const BlockWriter* stream) {
+// The inputs of a triangle (triangle, cluster, tree, dereplicate) in two halves.  open_triangle_inputs resolves the presets,
+// opens sketch inputs and decides whether the run takes the host sketch store path; load_triangle_inputs then reads FASTA
+// inputs (in memory), creates the context on --device and fills the store or imports the sketch inputs.  Both return 0, or
+// the exit code after an ERROR line.
+struct TriangleInputs {
+  bool sketches = false;              // .sketch files and databases
+  skdb::SketchInputs si;
+  bool use_store = false;
+  double need_gb = 0;                 // the store path's estimate
+  sk_sketch_params sp{};
+  sk_sketch_set* loaded = nullptr;    // sketch inputs imported in memory (FASTA inputs are sketched by the caller)
+  sk_sketch_store* store = nullptr;   // the store path's sketches
+};
+
+int open_triangle_inputs(Opts& op, TriangleInputs& ti) {
   resolve_presets(op);
   if (op.files.empty()) { fprintf(stderr, "ERROR No reference inputs found.\n"); return 1; }
-  const bool refs_are_sketch = sketch_inputs_given(op.files);
-  skdb::SketchInputs si;
-  if (refs_are_sketch) {      // .sketch files and databases (src/triangle.rs:16-24): opened here, decoded in groups below
+  ti.sketches = sketch_inputs_given(op.files);
+  if (ti.sketches) {      // .sketch files and databases (src/triangle.rs:16-24): opened here, decoded in groups below
     fprintf(stderr, "INFO Sketches detected.\n");
-    if (!skdb::open_sketch_inputs(op.files, si)) return 1;   // file_io::sketches_from_sketch (src/file_io.rs:680-717)
-    if (si.entries.empty()) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }
-    warn_sketch_params(op, si);
+    if (!skdb::open_sketch_inputs(op.files, ti.si)) return 1;   // file_io::sketches_from_sketch (src/file_io.rs:680-717)
+    if (ti.si.entries.empty()) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }
+    warn_sketch_params(op, ti.si);
   }
-  double need_gb = 0;
-  const bool use_store = triangle_needs_store(op, refs_are_sketch, si, &need_gb);
-  if (!refs_are_sketch && !use_store) {
+  ti.use_store = triangle_needs_store(op, ti.sketches, ti.si, &ti.need_gb);
+  return 0;
+}
+
+int load_triangle_inputs(Opts& op, Inputs& in, sk_ctx*& ctx, TriangleInputs& ti) {
+  if (!ti.sketches && !ti.use_store) {
     load_inputs(op.files, op.individual, std::max(op.threads, 1), in);
     if (in.genomes.empty()) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }   // src/triangle.rs:46-49
   }
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
-  sk_sketch_params sp = refs_are_sketch ? params_of(si) : sk_sketch_params{op.c, op.k, op.m};
-  sk_sketch_set* loaded = nullptr;
-  sk_sketch_store* store = nullptr;
-  if (use_store) {
-    info_store_path(op, need_gb, false);
-    store = refs_are_sketch ? store_sketch_inputs(ctx, si, std::max(op.threads, 1), sp, in.genomes)
-                            : fill_store(ctx, op, op.files, op.individual, in.genomes, sp);
-    if (!store) {      // sketch inputs: an entry could not be loaded (reported)
-      if (!refs_are_sketch) fprintf(stderr, "ERROR No genomes/sketches found.\n");
+  ti.sp = ti.sketches ? params_of(ti.si) : sk_sketch_params{op.c, op.k, op.m};
+  if (ti.use_store) {
+    info_store_path(op, ti.need_gb, false);
+    ti.store = ti.sketches ? store_sketch_inputs(ctx, ti.si, std::max(op.threads, 1), ti.sp, in.genomes)
+                           : fill_store(ctx, op, op.files, op.individual, in.genomes, ti.sp);
+    if (!ti.store) {      // sketch inputs: an entry could not be loaded (reported)
+      if (!ti.sketches) fprintf(stderr, "ERROR No genomes/sketches found.\n");
       return 1;
     }
-  } else if (refs_are_sketch) {
-    in.genomes.resize(si.entries.size());
+  } else if (ti.sketches) {
+    in.genomes.resize(ti.si.entries.size());
     bool ok = true;
-    loaded = import_sketch_inputs(ctx, si, 0, si.entries.size(), std::max(op.threads, 1), sp, in.genomes.data(), ok);
+    ti.loaded = import_sketch_inputs(ctx, ti.si, 0, ti.si.entries.size(), std::max(op.threads, 1), ti.sp, in.genomes.data(), ok);
     if (!ok) return 1;
   }
+  return 0;
+}
+
+int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_result>& res, const BlockWriter* stream) {
+  TriangleInputs ti;
+  if (const int rc = open_triangle_inputs(op, ti)) return rc;
+  if (const int rc = load_triangle_inputs(op, in, ctx, ti)) return rc;
+  const bool refs_are_sketch = ti.sketches;
+  const sk_sketch_params sp = ti.sp;
+  sk_sketch_set* loaded = ti.loaded;
+  sk_sketch_store* store = ti.store;
   if (op.cmd == "triangle" && in.genomes.size() > 500 && !op.sparse) fprintf(stderr, "WARN > 500 genomes detected. The output matrix will be large. Consider using -E or --sparse for a tsv output instead.\n");
   const sk_map_params mp = map_params(op, !op.no_learned && op.c >= 70 && !op.individual && !op.median);
   const std::vector<uint64_t> ranks = name_ranks(in.genomes)[0];
@@ -742,6 +768,30 @@ std::vector<uint32_t> length_rank(const Inputs& in) {
   return rank;
 }
 
+// The TSV of cluster and dereplicate (-o or stdout): one row per genome in genome-index order with its representative, its
+// cluster and the ANI / aligned fractions of row(g), the result row joining g to rep[g] (nullptr: NA).  false after an ERROR line.
+bool write_clusters(const Opts& op, const Inputs& in, const std::vector<uint32_t>& rep, const std::vector<uint32_t>& cluster,
+                    const std::function<const sk_ani_result*(uint32_t)>& row) {
+  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
+  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return false; }
+  fprintf(o, "Genome_file\tRepresentative_file\tCluster\tANI\tAlign_fraction_genome\tAlign_fraction_representative\tGenome_name\tRepresentative_name\n");
+  for (uint32_t g = 0; g < (uint32_t)rep.size(); g++) {
+    const Genome &gg = in.genomes[g], &rg = in.genomes[rep[g]];
+    fprintf(o, "%s\t%s\t%u\t", gg.file_name.c_str(), rg.file_name.c_str(), cluster[g]);
+    const sk_ani_result* r = rep[g] == g ? nullptr : row(g);
+    if (rep[g] == g) fputs("100.00\t100.00\t100.00", o);
+    else if (!r) fputs("NA\tNA\tNA", o);
+    else {
+      const bool is_ref = r->ref_id == g;
+      fprintf(o, "%.2f\t%.2f\t%.2f", (double)(r->ani * 100.f), (double)((is_ref ? r->af_ref : r->af_query) * 100.f),
+              (double)((is_ref ? r->af_query : r->af_ref) * 100.f));
+    }
+    fprintf(o, "\t%s\t%s\n", short_name(gg.contigs[0], op.short_header).c_str(), short_name(rg.contigs[0], op.short_header).c_str());
+  }
+  if (o != stdout) fclose(o);
+  return true;
+}
+
 // cluster: the triangle's results (the rows `triangle -E` prints) clustered on the GPU by sk_cluster at ANI >= --ani, greedy
 // representatives or --single-linkage, or by sk_cluster_linkage (--linkage average|complete: every printed row is a
 // similarity, --ani the cut; --dendrogram FILE writes the scipy linkage matrix), genomes ranked by total sequence length
@@ -787,29 +837,67 @@ int run_cluster(Opts& op) {
     for (const sk_merge& m : merges) fprintf(z, "%u\t%u\t%.6f\t%llu\n", m.a, m.b, 100.0 * m.height, (unsigned long long)m.size);
     fclose(z);
   }
-  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
-  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
-  fprintf(o, "Genome_file\tRepresentative_file\tCluster\tANI\tAlign_fraction_genome\tAlign_fraction_representative\tGenome_name\tRepresentative_name\n");
-  for (uint32_t g = 0; g < N; g++) {
-    const Genome &gg = in.genomes[g], &rg = in.genomes[rep[g]];
-    fprintf(o, "%s\t%s\t%u\t", gg.file_name.c_str(), rg.file_name.c_str(), cluster[g]);
-    if (rep[g] == g) fputs("100.00\t100.00\t100.00", o);
-    else if (edge[g] == UINT64_MAX) fputs("NA\tNA\tNA", o);
-    else {
-      const sk_ani_result& r = res[edge[g]];
-      const bool is_ref = r.ref_id == g;
-      fprintf(o, "%.2f\t%.2f\t%.2f", (double)(r.ani * 100.f), (double)((is_ref ? r.af_ref : r.af_query) * 100.f),
-              (double)((is_ref ? r.af_query : r.af_ref) * 100.f));
-    }
-    fprintf(o, "\t%s\t%s\n", short_name(gg.contigs[0], op.short_header).c_str(), short_name(rg.contigs[0], op.short_header).c_str());
-  }
-  if (o != stdout) fclose(o);
+  if (!write_clusters(op, in, rep, cluster, [&](uint32_t g) { return edge[g] == UINT64_MAX ? nullptr : &res[edge[g]]; })) return 1;
   if (op.linkage.empty())
     fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (%s), clustering %.1f ms\n", N, st.n_clusters, op.cluster_ani,
             op.single_linkage ? "single linkage" : "greedy", st.t_device * 1e3);
   else
     fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (%s linkage, %u rounds), clustering %.1f ms\n", N, st.n_clusters,
             op.cluster_ani, op.linkage.c_str(), st.rounds, st.t_device * 1e3);
+  sk_ctx_destroy(ctx);
+  return 0;
+}
+
+// dereplicate: cluster's greedy clusters (same inputs, presets, name ranks, length ranking and TSV) from sk_dereplicate, which
+// screens and chains only genome x representative pairs instead of the whole triangle.  In-memory sets on one GPU only:
+// inputs that need the host sketch store, and --gpus N, are left to cluster.  --representatives FILE: one line per
+// representative in cluster-id order, its file name (-i: its first contig name).
+int run_dereplicate(Opts& op) {
+  if (op.single_linkage || !op.linkage.empty() || !op.dendrogram.empty()) {
+    fprintf(stderr, "ERROR --single-linkage, --linkage and --dendrogram are cluster options; dereplicate is greedy clustering only: use cluster.\n");
+    return 2;
+  }
+  if (op.sparse || op.full_matrix || op.diagonal || op.distance || op.ci || op.detailed) {
+    fprintf(stderr, "ERROR -E/--sparse, --full-matrix, --diagonal, --distance, --ci and --detailed are triangle output options; dereplicate does not take them.\n");
+    return 2;
+  }
+  if (op.gpus > 1) { fprintf(stderr, "ERROR --gpus %d: dereplicate runs on one GPU; use cluster --gpus %d.\n", op.gpus, op.gpus); return 2; }
+  TriangleInputs ti;
+  if (const int rc = open_triangle_inputs(op, ti)) return rc;
+  if (ti.use_store) {
+    fprintf(stderr, "ERROR dereplicate keeps the sketches on the GPU, and these inputs (~%.1f GB estimated%s) need the host sketch store: use cluster, "
+            "which takes the store path.\n", ti.need_gb, device_budget() ? ", SK_DEVICE_BUDGET_MB set" : "");
+    return 1;
+  }
+  Inputs in;
+  sk_ctx* ctx = nullptr;
+  if (const int rc = load_triangle_inputs(op, in, ctx, ti)) return rc;
+  const sk_map_params mp = map_params(op, !op.no_learned && op.c >= 70 && !op.individual && !op.median);
+  const std::vector<uint64_t> ranks = name_ranks(in.genomes)[0];
+  sk_sketch_set* set = ti.loaded ? ti.loaded : sketch(ctx, in, ti.sp);
+  sk_sketch_set_set_name_ranks(set, ranks.data());
+  const uint32_t N = (uint32_t)in.genomes.size();
+  const std::vector<uint32_t> rank = length_rank(in);
+  std::vector<uint32_t> rep(N), cluster(N);
+  std::vector<sk_ani_result> join(N);
+  // SK_DEREP_WAVE: genomes per wave (a test hook: many waves on small inputs); it only sizes the waves
+  const char* w = getenv("SK_DEREP_WAVE");
+  const sk_derep_params dp{(float)(op.cluster_ani / 100.0), w ? (uint32_t)std::max(1ll, atoll(w)) : 0u};
+  sk_derep_stats st{};
+  CK(ctx, sk_dereplicate(ctx, set, &mp, rank.data(), &dp, rep.data(), cluster.data(), join.data(), &st));
+  sk_sketch_set_free(set);
+  if (!write_clusters(op, in, rep, cluster, [&](uint32_t g) { return &join[g]; })) return 1;
+  if (!op.representatives.empty()) {
+    FILE* f = fopen(op.representatives.c_str(), "w");
+    if (!f) { fprintf(stderr, "ERROR cannot open %s\n", op.representatives.c_str()); return 1; }
+    std::vector<uint32_t> by_cluster(st.n_clusters);
+    for (uint32_t g = 0; g < N; g++) if (rep[g] == g) by_cluster[cluster[g]] = g;
+    for (uint32_t g : by_cluster) fprintf(f, "%s\n", (op.individual ? in.genomes[g].contigs[0] : in.genomes[g].file_name).c_str());
+    fclose(f);
+  }
+  fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (greedy), %u waves, %llu pairs screened, %llu chained; "
+          "screen %.2f s, chain %.2f s, decide %.2f s, total %.2f s\n", N, st.n_clusters, op.cluster_ani, st.waves,
+          (unsigned long long)st.pairs_screened, (unsigned long long)st.pairs_chained, st.t_screen, st.t_chain, st.t_decide, st.t_total);
   sk_ctx_destroy(ctx);
   return 0;
 }
@@ -1419,6 +1507,10 @@ void usage() {
           "      genomes first, --single-linkage components, or --linkage average / complete (UPGMA / complete linkage of\n"
           "      100 - ANI, 100 for pairs not printed, cut at 100 - T); one TSV row per genome with its representative and\n"
           "      cluster; --dendrogram writes the linkage matrix (a b height size, heights in percent) that scipy takes\n"
+          "  skani-b200 dereplicate [fasta | sketch ... | -l list] [-i] [--ani T] [-o out] [--representatives FILE]\n"
+          "      cluster's greedy clusters (same TSV), screening and chaining only genome x representative pairs instead of\n"
+          "      the whole triangle; --representatives writes one representative per line in cluster order.  One GPU, sketches\n"
+          "      in device memory (larger inputs: cluster)\n"
           "  skani-b200 tree [fasta | sketch ... | -l list] [-i] [--method nj|average|complete] [-o tree.nwk]\n"
           "      the triangle's genomes as a Newick tree of 100 - ANI (100 for pairs not printed), branch lengths in percent:\n"
           "      neighbour joining (default; unrooted, basal trifurcation) or the average / complete linkage dendrogram\n"
@@ -1435,7 +1527,7 @@ int main(int argc, char** argv) {
   Opts op;
   op.cmd = argv[1];
   if (op.cmd != "triangle" && op.cmd != "dist" && op.cmd != "sketch" && op.cmd != "search" && op.cmd != "ingest" && op.cmd != "cluster" &&
-      op.cmd != "tree") { usage(); return 2; }
+      op.cmd != "tree" && op.cmd != "dereplicate") { usage(); return 2; }
   std::vector<std::string> positional;
   enum { NONE, QS, RS } multi = NONE;
   for (int i = 2; i < argc; i++) {
@@ -1483,7 +1575,7 @@ int main(int argc, char** argv) {
     else if (a == "--device") op.device = atoi(val().c_str());
     else if (a == "-d") op.db_dir = val();
     else if (a == "--separate-sketches") op.separate_sketches = true;
-    else if (a == "--ani" && op.cmd == "cluster") {
+    else if (a == "--ani" && (op.cmd == "cluster" || op.cmd == "dereplicate")) {
       const std::string v = val();
       char* end = nullptr;
       op.cluster_ani = strtod(v.c_str(), &end);
@@ -1492,18 +1584,19 @@ int main(int argc, char** argv) {
         return 2;
       }
     }
-    else if (a == "--single-linkage" && op.cmd == "cluster") op.single_linkage = true;
-    else if (a == "--linkage" && op.cmd == "cluster") op.linkage = val();
-    else if (a == "--dendrogram" && op.cmd == "cluster") op.dendrogram = val();
+    else if (a == "--single-linkage" && (op.cmd == "cluster" || op.cmd == "dereplicate")) op.single_linkage = true;
+    else if (a == "--linkage" && (op.cmd == "cluster" || op.cmd == "dereplicate")) op.linkage = val();
+    else if (a == "--dendrogram" && (op.cmd == "cluster" || op.cmd == "dereplicate")) op.dendrogram = val();
+    else if (a == "--representatives" && op.cmd == "dereplicate") op.representatives = val();
     else if (a == "--method" && op.cmd == "tree") op.tree_method = val();
     else if (a == "--keep-refs") {}   // search already loads every passing reference exactly once
     else if (a == "-v" || a == "--debug" || a == "--trace") {}
     else { fprintf(stderr, "ERROR unknown option %s\n", a.c_str()); usage(); return 2; }
   }
-  if (op.cmd == "triangle" || op.cmd == "sketch" || op.cmd == "ingest" || op.cmd == "cluster" || op.cmd == "tree") {
+  if (op.cmd == "triangle" || op.cmd == "sketch" || op.cmd == "ingest" || op.cmd == "cluster" || op.cmd == "tree" || op.cmd == "dereplicate") {
     op.files.insert(op.files.end(), positional.begin(), positional.end());
     return op.cmd == "triangle" ? run_triangle(op) : op.cmd == "sketch" ? run_sketch(op) : op.cmd == "cluster" ? run_cluster(op)
-         : op.cmd == "tree" ? run_tree(op) : run_ingest(op);
+         : op.cmd == "tree" ? run_tree(op) : op.cmd == "dereplicate" ? run_dereplicate(op) : run_ingest(op);
   }
   if (op.cmd == "search") {
     op.queries.insert(op.queries.end(), positional.begin(), positional.end());

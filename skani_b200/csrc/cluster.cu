@@ -369,10 +369,50 @@ int sk::build_graph(sk_ctx* ctx, const char* who, uint32_t n, const sk_ani_resul
   return SK_OK;
 }
 
-namespace {
+int sk::greedy_rounds(sk_ctx* ctx, const char* who, const uint32_t* frontier, uint32_t m, const Graph& g, const uint32_t* d_rank,
+                      uint8_t* state, uint32_t* rounds) {
+  cudaStream_t st = ctx->stream;
+  const auto launched = [&](unsigned k = 1) { count_launch(ctx, k); return cudaGetLastError(); };
+  DTmp<uint32_t> front[2], d_m;
+  SK_TRY(cl_alloc(ctx, front[0], m, "frontier", who));
+  SK_TRY(cl_alloc(ctx, front[1], m, "frontier", who));
+  SK_TRY(cl_alloc(ctx, d_m, 1, "frontier size", who));
+  SK_CUDA(cudaMemcpyAsync(front[0].p, frontier, (size_t)m * 4, cudaMemcpyDeviceToDevice, st));
+  size_t tb = 0;
+  SK_CUDA(cub::DeviceSelect::If(nullptr, tb, front[0].p, front[1].p, d_m.p, (int)m, Undecided{state}, st));
+  DTmp<uint8_t> tmp;
+  SK_TRY(cl_alloc(ctx, tmp, tb, "frontier compaction", who));
+  const uint32_t m0 = m;
+  uint32_t r = 0;
+  int cur = 0;
+  // each round decides at least the undecided vertex of smallest rank, so m rounds always finish
+  while (m) {
+    for (int k = 0; k < GREEDY_ROUNDS; k++) {
+      cl_greedy_kernel<<<blocks_for(m), TPB, 0, st>>>(front[cur].p, m, g.off.p, g.adj, d_rank, state);
+      r++;
+    }
+    SK_CUDA(launched(GREEDY_ROUNDS));
+    SK_CUDA(cub::DeviceSelect::If(tmp.p, tb, front[cur].p, front[cur ^ 1].p, d_m.p, (int)m, Undecided{state}, st));
+    SK_CUDA(launched());
+    SK_CUDA(cudaMemcpyAsync(&m, d_m.p, 4, cudaMemcpyDeviceToHost, st));
+    SK_CUDA(cudaStreamSynchronize(st));
+    cur ^= 1;
+    if (r > m0 + GREEDY_ROUNDS) { ctx->err = std::string(who) + ": greedy rounds did not converge"; return SK_ERR_STATE; }
+  }
+  *rounds += r;
+  return SK_OK;
+}
+
+int sk::greedy_assign(sk_ctx* ctx, uint32_t n, const Graph& g, const uint32_t* d_rank, const uint8_t* state, uint32_t* d_rep,
+                      uint64_t* d_edge, uint32_t* flag) {
+  cl_assign_kernel<<<blocks_for(n), TPB, 0, ctx->stream>>>(n, g.off.p, g.adj, g.adj_e, g.eani.p, g.erow.p, d_rank, state, d_rep, d_edge, flag);
+  count_launch(ctx, 1);
+  SK_CUDA(cudaGetLastError());
+  return SK_OK;
+}
 
 // representatives (flag[rank[v]] = 1) numbered in rank order, then rep / cluster / edge read back
-int number_and_read_back(sk_ctx* ctx, const char* who, uint32_t n, const uint32_t* d_rank, const uint32_t* d_rep, const uint64_t* d_edge,
+int sk::number_and_read_back(sk_ctx* ctx, const char* who, uint32_t n, const uint32_t* d_rank, const uint32_t* d_rep, const uint64_t* d_edge,
                          uint32_t* flag, uint32_t* d_cluster, uint32_t* rep, uint32_t* cluster, uint64_t* edge, uint32_t* n_clusters) {
   cudaStream_t st = ctx->stream;
   *n_clusters = 0;
@@ -393,6 +433,8 @@ int number_and_read_back(sk_ctx* ctx, const char* who, uint32_t n, const uint32_
   SK_CUDA(cudaStreamSynchronize(st));
   return SK_OK;
 }
+
+namespace {
 
 int cluster_impl(sk_ctx* ctx, uint32_t n, const sk_ani_result* results, uint64_t n_results, const uint32_t* rank,
                  const sk_cluster_params* cp, uint32_t* rep, uint32_t* cluster, uint64_t* edge, sk_cluster_stats* stats) {
@@ -418,35 +460,10 @@ int cluster_impl(sk_ctx* ctx, uint32_t n, const sk_ani_result* results, uint64_t
   uint32_t rounds = 0;
   if (!cp->single_linkage) {
     DTmp<uint8_t> state;
-    DTmp<uint32_t> front[2], d_m;
     SK_TRY(cl_alloc(ctx, state, n, "states"));
-    SK_TRY(cl_alloc(ctx, front[0], n, "frontier"));
-    SK_TRY(cl_alloc(ctx, front[1], n, "frontier"));
-    SK_TRY(cl_alloc(ctx, d_m, 1, "frontier size"));
     SK_CUDA(cudaMemsetAsync(state.p, 0, n, st));
-    SK_CUDA(cudaMemcpyAsync(front[0].p, order.p, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-    size_t tb = 0;
-    SK_CUDA(cub::DeviceSelect::If(nullptr, tb, front[0].p, front[1].p, d_m.p, (int)n, Undecided{state.p}, st));
-    DTmp<uint8_t> tmp;
-    SK_TRY(cl_alloc(ctx, tmp, tb, "frontier compaction"));
-    uint32_t m = n;
-    int cur = 0;
-    // each round decides at least the undecided vertex of smallest rank, so n rounds always finish
-    while (m) {
-      for (int k = 0; k < GREEDY_ROUNDS; k++) {
-        cl_greedy_kernel<<<blocks_for(m), TPB, 0, st>>>(front[cur].p, m, g.off.p, adj, d_rank.p, state.p);
-        rounds++;
-      }
-      SK_CUDA(launched(GREEDY_ROUNDS));
-      SK_CUDA(cub::DeviceSelect::If(tmp.p, tb, front[cur].p, front[cur ^ 1].p, d_m.p, (int)m, Undecided{state.p}, st));
-      SK_CUDA(launched());
-      SK_CUDA(cudaMemcpyAsync(&m, d_m.p, 4, cudaMemcpyDeviceToHost, st));
-      SK_CUDA(cudaStreamSynchronize(st));
-      cur ^= 1;
-      if (rounds > n + GREEDY_ROUNDS) { ctx->err = "sk_cluster: greedy rounds did not converge"; return SK_ERR_STATE; }
-    }
-    cl_assign_kernel<<<blocks_for(n), TPB, 0, st>>>(n, g.off.p, adj, adj_e, g.eani.p, g.erow.p, d_rank.p, state.p, d_rep.p, d_edge.p, flag.p);
-    SK_CUDA(launched());
+    SK_TRY(greedy_rounds(ctx, "sk_cluster", order.p, n, g, d_rank.p, state.p, &rounds));
+    SK_TRY(greedy_assign(ctx, n, g, d_rank.p, state.p, d_rep.p, d_edge.p, flag.p));
   } else {
     DTmp<uint32_t> parent, changed;
     SK_TRY(cl_alloc(ctx, parent, n, "parents"));
@@ -475,8 +492,10 @@ int cluster_impl(sk_ctx* ctx, uint32_t n, const sk_ani_result* results, uint64_t
   return SK_OK;
 }
 
+}  // namespace
+
 // rank must be a permutation of 0 .. n - 1: the reason it is not, empty when it is
-std::string rank_error(uint32_t n, const uint32_t* rank) {
+std::string sk::rank_error(uint32_t n, const uint32_t* rank) {
   std::vector<uint8_t> seen(n, 0);
   for (uint32_t g = 0; g < n; g++) {
     if (rank[g] >= n || seen[rank[g]]) return "rank is not a permutation of 0.." + std::to_string(n) + " - 1 (genome " + std::to_string(g) + ")";
@@ -484,6 +503,8 @@ std::string rank_error(uint32_t n, const uint32_t* rank) {
   }
   return "";
 }
+
+namespace {
 
 constexpr int LK_ROUNDS = 8;   // linkage rounds between two read-backs of the pair count
 

@@ -1,0 +1,448 @@
+// derep.cu -- sk_dereplicate: sk_cluster's greedy representatives of an in-memory sketch set without the triangle.
+//
+// Genomes are visited in rank order in waves.  A uint8 state per genome (CL_UNDECIDED / CL_REP / CL_MEMBER) stays on the
+// device for the whole call.  Per wave:
+//   1. the wave's genomes are screened against the representative index (the markers of the representatives chosen so far)
+//      and the passing pairs chained; dr_mark_kernel makes every wave genome with an edge to one of them a member.  Every
+//      earlier representative ranks before the wave, so such an edge decides the genome; the others may still meet a
+//      representative chosen earlier in this wave.
+//   2. U = the wave's genomes still undecided.  A temporary index of U's markers screens the pairs inside U (each unordered
+//      pair once), they are chained, and sk_cluster's greedy rounds run over U as the frontier on a CSR of those edges.  A
+//      genome of U has no edge to an earlier representative, and its edges to members do not matter, so the CSR of U's own
+//      edges decides it exactly as the full triangle's graph would.
+//   3. the new representatives' markers are sorted and merged into the index (cub::DeviceMerge).
+// Then every member is screened against the complete index; the pairs not chained during the waves (a set difference on the
+// sorted pair keys) are chained, and cl_assign over the graph of every chained row gives each member its representative.  The
+// chained rows contain every edge that touches a representative, which is all the greedy rule reads, so the outcome is
+// sk_cluster's on the triangle's rows.
+//
+// The index is one sorted array of dr_key(marker, slot) (derep_core.cuh) with 16-bit prefix buckets, as the pipelined
+// triangle's TriScreen keeps it.  dr_rows_kernel runs one block per row genome and counts shared markers per slot in
+// shared-memory tiles; every slot of a tile is then decided by the oriented predicate (dr_screen_pass), so a slot with no
+// shared marker that the rescue lets through is emitted like any other.
+#include <cub/cub.cuh>
+
+#include <algorithm>
+#include <chrono>
+#include <cmath>
+#include <string>
+#include <vector>
+
+#include "cluster_core.cuh"
+#include "derep_core.cuh"
+#include "sk_internal.h"
+
+using namespace sk;
+
+namespace {
+
+const char* const WHO = "sk_dereplicate";
+constexpr int TPB = 256;
+// default wave sizes: the first wave holds 64 genomes and each next one twice as many, up to 4096.  Early waves meet few
+// representatives, so most of their genomes reach step 2, where every family met twice in one wave chains its pairs
+// among itself; later waves are mostly members decided in step 1, and larger waves need fewer host round trips.
+constexpr uint32_t FIRST_WAVE = 64, MAX_WAVE = 4096;
+constexpr uint32_t TILE = 48 * 1024;   // slots counted per shared-memory tile (192 KiB)
+
+inline unsigned blocks_for(uint64_t n) { return (unsigned)std::max<uint64_t>(1, (n + TPB - 1) / TPB); }
+using clk = std::chrono::steady_clock;
+inline double secs(clk::time_point t0) { return std::chrono::duration<double>(clk::now() - t0).count(); }
+
+// the keys of list[s]'s markers, slot slot0 + s, at kofs[s] (the exclusive prefix of the list's marker counts)
+__global__ void dr_keys_kernel(const uint64_t* __restrict__ markers, const uint64_t* __restrict__ off, const uint32_t* __restrict__ list,
+                               const uint64_t* __restrict__ kofs, uint32_t slot0, uint64_t* __restrict__ keys) {
+  const uint32_t s = blockIdx.x, g = list[s];
+  const uint64_t b = off[g], e = off[g + 1], at = kofs[s];
+  for (uint64_t i = b + threadIdx.x; i < e; i += blockDim.x) keys[at + i - b] = dr_key(markers[i], slot0 + s);
+}
+
+// bucket[p] = first index position whose key prefix is >= p; bucket[2^16] = n
+__global__ void dr_bucket_kernel(const uint64_t* __restrict__ key, uint64_t n, uint32_t* __restrict__ bucket) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p > (1u << DR_PREFIX_BITS)) return;
+  uint64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) >> 1;
+    if ((key[mid] >> DR_PREFIX_SHIFT) < p) lo = mid + 1; else hi = mid;
+  }
+  bucket[p] = (uint32_t)lo;
+}
+
+// One block per row genome rows[k]; columns are the index's slots (upper: only slots > k, for an index whose slot k is row k).
+// For each marker of the row the run of that marker is walked from slot t0 to t1 (keys are sorted by marker, then slot).
+__global__ void __launch_bounds__(256)
+dr_rows_kernel(const uint64_t* __restrict__ markers, const uint64_t* __restrict__ off, const uint32_t* __restrict__ rows,
+               const uint64_t* __restrict__ key, uint64_t n_keys, const uint32_t* __restrict__ bucket,
+               const uint32_t* __restrict__ slot_genome, uint32_t n_slots, int upper, int rescue_small, double cutoff,
+               uint32_t tile, uint64_t* __restrict__ pairs, unsigned long long* __restrict__ n_pairs, unsigned long long cap) {
+  extern __shared__ uint32_t counts[];
+  const uint32_t k = blockIdx.x, g = rows[k];
+  const uint64_t mb = off[g], me = off[g + 1], card_g = me - mb;
+  for (uint32_t t0 = upper ? k + 1 : 0; t0 < n_slots; t0 += tile) {
+    const uint32_t t1 = min(n_slots, t0 + tile);
+    for (uint32_t c = threadIdx.x; c < t1 - t0; c += blockDim.x) counts[c] = 0;
+    __syncthreads();
+    for (uint64_t e = mb + threadIdx.x; e < me; e += blockDim.x) {
+      const uint64_t m = markers[e], k0 = dr_key(m, t0), k1 = dr_key(m, t1);
+      const uint32_t p = (uint32_t)(k0 >> DR_PREFIX_SHIFT);
+      uint64_t lo = bucket[p], hi = bucket[p + 1];
+      while (lo < hi) {
+        const uint64_t mid = (lo + hi) >> 1;
+        if (key[mid] < k0) lo = mid + 1; else hi = mid;
+      }
+      for (uint64_t t = lo; t < n_keys; t++) {
+        const uint64_t kk = key[t];
+        if (kk >= k1) break;
+        atomicAdd(&counts[dr_key_slot(kk) - t0], 1u);
+      }
+    }
+    __syncthreads();
+    for (uint32_t c = threadIdx.x; c < t1 - t0; c += blockDim.x) {
+      const uint32_t r = slot_genome[t0 + c];
+      if (dr_screen_pass(g, card_g, r, off[r + 1] - off[r], counts[c], rescue_small, cutoff)) {
+        const unsigned long long at = atomicAdd(n_pairs, 1ull);
+        if (at < cap) pairs[at] = dr_pair_key(g, r);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// step 1: the wave genome of every chained row that is an edge becomes a member (the row's other genome is a representative)
+__global__ void dr_mark_kernel(const sk_ani_result* __restrict__ rows, uint64_t m, float min_ani, uint8_t* state) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const sk_ani_result& r = rows[i];
+  if (!cl_is_edge(r.ani, min_ani)) return;
+  state[state[r.ref_id] == CL_REP ? r.query_id : r.ref_id] = CL_MEMBER;
+}
+
+struct HasState {
+  const uint8_t* state;
+  uint8_t s;
+  __device__ bool operator()(uint32_t v) const { return state[v] == s; }
+};
+
+// the set difference of the final screen: a pair is kept unless the sorted chained keys hold it
+struct NotChained {
+  const uint64_t* chained;
+  uint64_t n;
+  __device__ bool operator()(uint64_t k) const {
+    uint64_t lo = 0, hi = n;
+    while (lo < hi) {
+      const uint64_t mid = (lo + hi) >> 1;
+      if (chained[mid] < k) lo = mid + 1; else hi = mid;
+    }
+    return lo == n || chained[lo] != k;
+  }
+};
+
+// a marker index over slots 0 .. slots - 1 (slot s = genome slot_genome[s]).  Its slots may all be without markers: the
+// buckets then stay zero and n = 0, so no row walks the (absent) keys.
+struct Index {
+  DTmp<uint64_t> key[2];
+  int cur = 0;
+  uint64_t n = 0;
+  DTmp<uint32_t> bucket, slot_genome;
+  uint32_t slots = 0;
+};
+
+// a cub call run twice: sizing, then on temporaries from the arena
+template <typename F>
+int cub_run(sk_ctx* ctx, const char* what, F&& f) {
+  size_t tb = 0;
+  SK_CUDA(f((void*)nullptr, tb));
+  DTmp<uint8_t> tmp;
+  SK_TRY(cl_alloc(ctx, tmp, tb, what, WHO));
+  SK_CUDA(f((void*)tmp.p, tb));
+  count_launch(ctx, 1);
+  return SK_OK;
+}
+
+struct Run {
+  sk_ctx* ctx;
+  const sk_sketch_set* set;
+  const sk_map_params* mp;
+  float min_ani;
+  double cutoff;
+  uint32_t N;
+  DTmp<uint64_t> d_off;
+  DTmp<uint32_t> d_rank;
+  DTmp<uint8_t> state;
+  std::vector<sk_ani_result> rows;   // every chained row, in chaining order
+  std::vector<uint64_t> chained;     // their pair keys
+  sk_derep_stats st{};
+
+  // genomes list[0 .. m) (host; d_list the same on the device) join ix as slots ix.slots ..
+  int index_add(Index& ix, const uint32_t* list, const uint32_t* d_list, uint32_t m) {
+    if (!m) return SK_OK;
+    cudaStream_t s = ctx->stream;
+    std::vector<uint64_t> kofs(m + 1, 0);
+    for (uint32_t i = 0; i < m; i++) kofs[i + 1] = kofs[i] + set->mk_off[list[i] + 1] - set->mk_off[list[i]];
+    const uint64_t m_new = kofs[m], n_tot = ix.n + m_new;
+    if ((uint64_t)ix.slots + m > DR_MAX_SLOTS) {
+      ctx->err = std::string(WHO) + ": more than 2^22 - 1 genomes (" + std::to_string((uint64_t)ix.slots + m) + ") in one marker index"; return SK_ERR_PARAM;
+    }
+    if (n_tot >= DR_MAX_KEYS) {
+      ctx->err = std::string(WHO) + ": " + std::to_string(n_tot) + " markers in one marker index (at most 2^31 - 1)"; return SK_ERR_PARAM;
+    }
+    SK_CUDA(cudaMemcpyAsync(ix.slot_genome.p + ix.slots, d_list, (size_t)m * 4, cudaMemcpyDeviceToDevice, s));
+    if (m_new) {
+      DTmp<uint64_t> d_kofs, nk, snk;
+      SK_TRY(cl_alloc(ctx, d_kofs, m + 1, "key offsets", WHO));
+      SK_TRY(cl_alloc(ctx, nk, m_new, "index keys", WHO));
+      SK_TRY(cl_alloc(ctx, snk, m_new, "index keys", WHO));
+      SK_CUDA(h2d_small(ctx, d_kofs.p, kofs.data(), (size_t)(m + 1) * 8));
+      dr_keys_kernel<<<m, 256, 0, s>>>(set->markers, d_off.p, d_list, d_kofs.p, ix.slots, nk.p);
+      count_launch(ctx, 1);
+      SK_CUDA(cudaGetLastError());
+      SK_TRY(cub_run(ctx, "index sort", [&](void* t, size_t& tb) {
+        return cub::DeviceRadixSort::SortKeys(t, tb, nk.p, snk.p, (int)m_new, 0, 64, s); }));
+      DTmp<uint64_t>& dst = ix.key[ix.cur ^ 1];
+      SK_TRY(cl_alloc(ctx, dst, n_tot, "marker index", WHO));
+      if (!ix.n) {
+        SK_CUDA(cudaMemcpyAsync(dst.p, snk.p, m_new * 8, cudaMemcpyDeviceToDevice, s));
+      } else {   // keys are distinct (marker, slot) pairs: the merge has one possible output
+        const uint64_t* old = ix.key[ix.cur].p;
+        SK_TRY(cub_run(ctx, "index merge", [&](void* t, size_t& tb) {
+          return cub::DeviceMerge::MergeKeys(t, tb, old, (int)ix.n, snk.p, (int)m_new, dst.p, ::cuda::std::less<uint64_t>{}, s); }));
+      }
+      ix.cur ^= 1;
+      ix.key[ix.cur ^ 1].release();
+      ix.n = n_tot;
+      dr_bucket_kernel<<<((1u << DR_PREFIX_BITS) + 256) / 256, 256, 0, s>>>(ix.key[ix.cur].p, ix.n, ix.bucket.p);
+      count_launch(ctx, 1);
+      SK_CUDA(cudaGetLastError());
+      SK_CUDA(cudaStreamSynchronize(s));   // the temporaries go back to the arena
+    }
+    ix.slots += m;
+    return SK_OK;
+  }
+
+  // the pairs (d_rows[k], slot genome) that pass the triangle's screen, sorted, on the device in out[0 .. *n_out)
+  int screen(const Index& ix, const uint32_t* d_rows, uint32_t n_rows, bool upper, DTmp<uint64_t>& out, uint64_t* n_out) {
+    const auto t0 = clk::now();
+    cudaStream_t s = ctx->stream;
+    *n_out = 0;
+    if (!n_rows || !ix.slots) { st.t_screen += secs(t0); return SK_OK; }
+    const uint32_t tile = std::min(ix.slots, TILE);
+    SK_CUDA(cudaFuncSetAttribute(dr_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TILE * 4));   // constant: see run_screen
+    unsigned long long cap = std::max<unsigned long long>(1ull << 20, 64ull * n_rows), n = 0;
+    DTmp<unsigned long long> d_n;
+    DTmp<uint64_t> d_pairs;
+    SK_TRY(cl_alloc(ctx, d_n, 1, "pair count", WHO));
+    for (int attempt = 0; attempt < 2; attempt++) {
+      SK_TRY(cl_alloc(ctx, d_pairs, cap, "screened pairs", WHO));
+      SK_CUDA(cudaMemsetAsync(d_n.p, 0, 8, s));
+      SK_LAUNCH(ctx, "dr_rows_kernel", (dr_rows_kernel<<<n_rows, 256, (size_t)tile * 4, s>>>(
+          set->markers, d_off.p, d_rows, ix.key[ix.cur].p, ix.n, ix.bucket.p, ix.slot_genome.p, ix.slots, upper, mp->rescue_small, cutoff,
+          tile, d_pairs.p, d_n.p, cap)));
+      SK_CUDA(cudaGetLastError());
+      SK_CUDA(cudaMemcpyAsync(&n, d_n.p, 8, cudaMemcpyDeviceToHost, s));
+      SK_CUDA(cudaStreamSynchronize(s));
+      if (n <= cap) break;
+      cap = n;
+    }
+    SK_TRY(cl_alloc(ctx, out, n, "screened pairs", WHO));
+    if (n) SK_TRY(cub_run(ctx, "pair sort", [&](void* t, size_t& tb) {
+      return cub::DeviceRadixSort::SortKeys(t, tb, d_pairs.p, out.p, (int)n, 0, 64, s); }));
+    SK_CUDA(cudaStreamSynchronize(s));
+    *n_out = n;
+    st.pairs_screened += n;
+    st.t_screen += secs(t0);
+    return SK_OK;
+  }
+
+  // d_pairs[0 .. n) (device) chained as the triangle chains them; the rows are appended to `rows`, the first at *first
+  int chain(const uint64_t* d_pairs, uint64_t n, size_t* first) {
+    *first = rows.size();
+    if (!n) return SK_OK;
+    const auto t0 = clk::now();
+    std::vector<uint64_t> pairs(n);
+    SK_CUDA(cudaMemcpyAsync(pairs.data(), d_pairs, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    SK_CUDA(cudaStreamSynchronize(ctx->stream));
+    rows.resize(*first + n);
+    SK_TRY(sk_chain_pairs(ctx, set, set, pairs.data(), n, mp, rows.data() + *first));
+    chained.insert(chained.end(), pairs.begin(), pairs.end());
+    st.pairs_chained += n;
+    st.t_chain += secs(t0);
+    return SK_OK;
+  }
+
+  // the genomes of list[0 .. m) (device) in state s, order kept, into out; their count
+  int select(const uint32_t* list, uint32_t m, uint8_t s, DTmp<uint32_t>& out, uint32_t* n_out) {
+    DTmp<uint32_t> d_m;
+    SK_TRY(cl_alloc(ctx, out, m, "genome list", WHO));
+    SK_TRY(cl_alloc(ctx, d_m, 1, "genome count", WHO));
+    *n_out = 0;
+    if (!m) return SK_OK;
+    SK_TRY(cub_run(ctx, "genome selection", [&](void* t, size_t& tb) {
+      return cub::DeviceSelect::If(t, tb, list, out.p, d_m.p, (int)m, HasState{state.p, s}, ctx->stream); }));
+    SK_CUDA(cudaMemcpyAsync(n_out, d_m.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    SK_CUDA(cudaStreamSynchronize(ctx->stream));
+    return SK_OK;
+  }
+
+  int to_host(const DTmp<uint32_t>& d, uint32_t m, std::vector<uint32_t>& h) {
+    h.resize(m);
+    if (m) SK_CUDA(cudaMemcpyAsync(h.data(), d.p, (size_t)m * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    SK_CUDA(cudaStreamSynchronize(ctx->stream));
+    return SK_OK;
+  }
+
+  // wave = genomes per wave, 0 for the growing default
+  int run(const uint32_t* rank, uint32_t wave, uint32_t* rep, uint32_t* cluster, sk_ani_result* join) {
+    cudaStream_t s = ctx->stream;
+    const auto t_all = clk::now();
+    std::vector<uint32_t> order(N);
+    for (uint32_t g = 0; g < N; g++) order[rank[g]] = g;
+    DTmp<uint32_t> d_order;
+    Index reps;
+    SK_TRY(cl_alloc(ctx, d_off, (uint64_t)N + 1, "marker offsets", WHO));
+    SK_TRY(cl_alloc(ctx, d_rank, N, "ranks", WHO));
+    SK_TRY(cl_alloc(ctx, d_order, N, "rank order", WHO));
+    SK_TRY(cl_alloc(ctx, state, N, "states", WHO));
+    SK_TRY(cl_alloc(ctx, reps.bucket, (1u << DR_PREFIX_BITS) + 1, "index buckets", WHO));
+    SK_TRY(cl_alloc(ctx, reps.slot_genome, N, "index slots", WHO));
+    SK_CUDA(cudaMemsetAsync(reps.bucket.p, 0, ((1u << DR_PREFIX_BITS) + 1) * 4, s));
+    SK_CUDA(h2d_small(ctx, d_off.p, set->mk_off.data(), ((size_t)N + 1) * 8));
+    SK_CUDA(h2d_small(ctx, d_rank.p, rank, (size_t)N * 4));
+    SK_CUDA(h2d_small(ctx, d_order.p, order.data(), (size_t)N * 4));
+    SK_CUDA(cudaMemsetAsync(state.p, CL_UNDECIDED, N, s));
+    for (uint32_t w0 = 0, size = wave ? wave : FIRST_WAVE; w0 < N; w0 += size, size = wave ? wave : std::min(2 * size, MAX_WAVE)) {
+      const uint32_t w1 = std::min<uint64_t>(N, (uint64_t)w0 + size), nw = w1 - w0;
+      const uint32_t* d_wave = d_order.p + w0;
+      st.waves++;
+      // 1. the wave against the representatives chosen so far
+      DTmp<uint64_t> pairs;
+      uint64_t np = 0;
+      size_t first = 0;
+      SK_TRY(screen(reps, d_wave, nw, false, pairs, &np));
+      SK_TRY(chain(pairs.p, np, &first));
+      const auto t_mark = clk::now();
+      if (np) {
+        DTmp<sk_ani_result> d_res;
+        SK_TRY(cl_alloc(ctx, d_res, np, "chained rows", WHO));
+        SK_TRY(upload_runs(ctx, (uint8_t*)d_res.p, {{(const uint8_t*)(rows.data() + first), np * sizeof(sk_ani_result)}}, false));
+        dr_mark_kernel<<<blocks_for(np), TPB, 0, s>>>(d_res.p, np, min_ani, state.p);
+        count_launch(ctx, 1);
+        SK_CUDA(cudaGetLastError());
+      }
+      DTmp<uint32_t> d_u;
+      uint32_t nu = 0;
+      SK_TRY(select(d_wave, nw, CL_UNDECIDED, d_u, &nu));
+      st.t_decide += secs(t_mark);
+      if (!nu) continue;
+      // 2. inside the wave: U screened against a temporary index of its own markers, each pair once
+      std::vector<uint32_t> u;
+      SK_TRY(to_host(d_u, nu, u));
+      {
+        Index ui;
+        SK_TRY(cl_alloc(ctx, ui.bucket, (1u << DR_PREFIX_BITS) + 1, "index buckets", WHO));
+        SK_TRY(cl_alloc(ctx, ui.slot_genome, nu, "index slots", WHO));
+        SK_CUDA(cudaMemsetAsync(ui.bucket.p, 0, ((1u << DR_PREFIX_BITS) + 1) * 4, s));
+        const auto t0 = clk::now();
+        SK_TRY(index_add(ui, u.data(), d_u.p, nu));
+        st.t_screen += secs(t0);
+        SK_TRY(screen(ui, d_u.p, nu, true, pairs, &np));
+      }
+      SK_TRY(chain(pairs.p, np, &first));
+      pairs.release();
+      const auto t_greedy = clk::now();
+      {
+        Graph g;
+        SK_TRY(build_graph(ctx, WHO, N, rows.data() + first, np, min_ani, g));
+        SK_TRY(greedy_rounds(ctx, WHO, d_u.p, nu, g, d_rank.p, state.p, &st.rounds));
+      }
+      // 3. the new representatives join the index
+      DTmp<uint32_t> d_new;
+      uint32_t nn = 0;
+      SK_TRY(select(d_u.p, nu, CL_REP, d_new, &nn));
+      st.t_decide += secs(t_greedy);
+      std::vector<uint32_t> fresh;
+      SK_TRY(to_host(d_new, nn, fresh));
+      const auto t0 = clk::now();
+      SK_TRY(index_add(reps, fresh.data(), d_new.p, nn));
+      st.t_screen += secs(t0);
+    }
+    // every member against every representative; only the pairs not chained yet are chained
+    DTmp<uint32_t> d_mem;
+    uint32_t nm = 0;
+    SK_TRY(select(d_order.p, N, CL_MEMBER, d_mem, &nm));
+    DTmp<uint64_t> pairs, fresh;
+    uint64_t np = 0, nf = 0;
+    SK_TRY(screen(reps, d_mem.p, nm, false, pairs, &np));
+    if (np) {
+      const auto t0 = clk::now();
+      std::vector<uint64_t> done = chained;
+      std::sort(done.begin(), done.end());
+      DTmp<uint64_t> d_done;
+      DTmp<unsigned long long> d_nf;
+      SK_TRY(cl_alloc(ctx, d_done, done.size(), "chained pairs", WHO));
+      SK_TRY(cl_alloc(ctx, fresh, np, "pairs to chain", WHO));
+      SK_TRY(cl_alloc(ctx, d_nf, 1, "pair count", WHO));
+      if (!done.empty()) SK_CUDA(cudaMemcpyAsync(d_done.p, done.data(), done.size() * 8, cudaMemcpyHostToDevice, s));
+      SK_TRY(cub_run(ctx, "set difference", [&](void* t, size_t& tb) {
+        return cub::DeviceSelect::If(t, tb, pairs.p, fresh.p, d_nf.p, (int)np, NotChained{d_done.p, done.size()}, s); }));
+      unsigned long long h = 0;
+      SK_CUDA(cudaMemcpyAsync(&h, d_nf.p, 8, cudaMemcpyDeviceToHost, s));
+      SK_CUDA(cudaStreamSynchronize(s));
+      nf = h;
+      st.t_screen += secs(t0);
+    }
+    pairs.release();
+    size_t first = 0;
+    SK_TRY(chain(fresh.p, nf, &first));
+    fresh.release();
+    // the assignment over every chained row, representatives numbered in rank order
+    const auto t_assign = clk::now();
+    Graph g;
+    SK_TRY(build_graph(ctx, WHO, N, rows.data(), rows.size(), min_ani, g));
+    DTmp<uint32_t> d_rep, d_cluster, flag;
+    DTmp<uint64_t> d_edge;
+    SK_TRY(cl_alloc(ctx, d_rep, N, "representatives", WHO));
+    SK_TRY(cl_alloc(ctx, d_cluster, N, "clusters", WHO));
+    SK_TRY(cl_alloc(ctx, flag, N, "flags", WHO));
+    SK_TRY(cl_alloc(ctx, d_edge, N, "edges per genome", WHO));
+    SK_TRY(greedy_assign(ctx, N, g, d_rank.p, state.p, d_rep.p, d_edge.p, flag.p));
+    std::vector<uint32_t> h_rep(N), h_cluster(N);   // read back here first: the caller's outputs may alias each other
+    std::vector<uint64_t> edge(N);
+    SK_TRY(number_and_read_back(ctx, WHO, N, d_rank.p, d_rep.p, d_edge.p, flag.p, d_cluster.p, h_rep.data(), h_cluster.data(), edge.data(),
+                                &st.n_clusters));
+    st.t_decide += secs(t_assign);
+    st.n_edges = g.E;
+    for (uint32_t v = 0; v < N; v++) {
+      if (h_rep[v] == v) {
+        join[v] = sk_ani_result{};
+        join[v].ani = NAN;
+        join[v].ref_id = join[v].query_id = v;
+      } else if (edge[v] == UINT64_MAX) {
+        ctx->err = std::string(WHO) + ": member " + std::to_string(v) + " has no chained row to its representative";
+        return SK_ERR_STATE;
+      } else {
+        join[v] = rows[edge[v]];
+      }
+    }
+    std::copy(h_rep.begin(), h_rep.end(), rep);
+    std::copy(h_cluster.begin(), h_cluster.end(), cluster);
+    st.t_total = secs(t_all);
+    return SK_OK;
+  }
+};
+
+}  // namespace
+
+int sk_dereplicate(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* rank, const sk_derep_params* dp,
+                   uint32_t* rep, uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats) {
+  if (!ctx) return SK_ERR_PARAM;
+  if (!set || !mp || !dp || !rep || !cluster || !join || (set->G && !rank)) { ctx->err = std::string(WHO) + ": NULL argument"; return SK_ERR_PARAM; }
+  if (std::isnan(dp->min_ani)) { ctx->err = std::string(WHO) + ": min_ani is NaN"; return SK_ERR_PARAM; }
+  const std::string bad = rank_error(set->G, rank);
+  if (!bad.empty()) { ctx->err = std::string(WHO) + ": " + bad; return SK_ERR_PARAM; }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  Run r{ctx, set, mp, dp->min_ani, screen_cutoff(mp), set->G};
+  const uint32_t wave = std::min(dp->wave, DR_MAX_SLOTS);
+  const int rc = r.run(rank, wave, rep, cluster, join);
+  if (rc == SK_OK && stats) *stats = r.st;
+  return rc;
+}

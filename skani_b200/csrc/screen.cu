@@ -37,6 +37,8 @@ static double powi21(double x) {
   return r;
 }
 
+double screen_cutoff(const sk_map_params* mp) { return powi21(mp->screen_val == 0. ? 0.80 : mp->screen_val); }   // src/triangle.rs:34-42
+
 __global__ void fill_genome_kernel(const uint64_t* __restrict__ off, uint32_t base_entry, uint32_t* __restrict__ eg) {
   uint32_t g = blockIdx.x;
   for (uint64_t i = off[g] + threadIdx.x; i < off[g + 1]; i += blockDim.x) eg[base_entry + i] = g;

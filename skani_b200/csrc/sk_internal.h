@@ -234,6 +234,7 @@ int tri_screen_create(sk_ctx* ctx, size_t marker_hint, TriScreen** out);
 int tri_screen_add(TriScreen* ts, const sk_sketch_set* set, uint32_t g_end, uint32_t row_begin, const sk_map_params* mp, uint64_t** pairs, uint64_t* n);
 void tri_screen_free(TriScreen* ts);
 bool tri_screen_supports(uint32_t n_genomes, uint64_t n_markers);
+double screen_cutoff(const sk_map_params* mp);   // the triangle's screen cutoff: screen_val^21 (0 => 0.80), as the screens compute it
 // sketch-set blobs (sk_sketch_set_pack_subset / unpack, the host sketch store): layout and metadata words are derived from
 // SET_ARRAYS in set_layout.hpp
 
@@ -283,4 +284,18 @@ struct Graph {
   const uint32_t* adj_e = nullptr;
 };
 int build_graph(sk_ctx* ctx, const char* who, uint32_t n, const sk_ani_result* results, uint64_t n_results, float min_ani, Graph& g);
+// greedy representatives over g (cluster_core.cuh): rounds of cl_greedy_decide over the undecided vertices of `frontier`
+// (m vertices in rank order, device), reading and writing state (CL_* per genome id, device) until none of them is left
+// undecided; vertices outside the frontier keep their states.  *rounds grows by the rounds run.
+int greedy_rounds(sk_ctx* ctx, const char* who, const uint32_t* frontier, uint32_t m, const Graph& g, const uint32_t* d_rank,
+                  uint8_t* state, uint32_t* rounds);
+// every genome's representative (cl_assign over g; itself for a representative), the result row joining them (UINT64_MAX
+// for none) and flag[rank[v]] = v is a representative, all on the device
+int greedy_assign(sk_ctx* ctx, uint32_t n, const Graph& g, const uint32_t* d_rank, const uint8_t* state, uint32_t* d_rep,
+                  uint64_t* d_edge, uint32_t* flag);
+// representatives (flag[rank[v]] = 1) numbered in rank order, then rep / cluster / edge read back to the host
+int number_and_read_back(sk_ctx* ctx, const char* who, uint32_t n, const uint32_t* d_rank, const uint32_t* d_rep, const uint64_t* d_edge,
+                         uint32_t* flag, uint32_t* d_cluster, uint32_t* rep, uint32_t* cluster, uint64_t* edge, uint32_t* n_clusters);
+// rank must be a permutation of 0 .. n - 1: the reason it is not, empty when it is
+std::string rank_error(uint32_t n, const uint32_t* rank);
 }  // namespace sk

@@ -4,7 +4,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import AniResult, ChainDebug, ClusterParams, ClusterStats, LinkageParams, MapParams, NjStats, SketchParams, StoreStats, TriangleStats
+from ._lib import AniResult, ChainDebug, ClusterParams, ClusterStats, DerepParams, DerepStats, LinkageParams, MapParams, NjStats, SketchParams, StoreStats, TriangleStats
 
 # numpy view of sk_ani_result (include/skani_b200.h): lets callers take 10^5..10^6 results without per-row Python objects
 RESULT_DTYPE = np.dtype([(n, np.float32) for n in ("ani", "af_query", "af_ref", "ci_lower", "ci_upper", "std", "q90_q", "q90_r", "q50_q",
@@ -723,3 +723,22 @@ def neighbor_joining(ctx, n_genomes, results):
     st = NjStats()
     ctx.check(ctx.L.sk_neighbor_joining(ctx.h, n, res.ctypes.data if len(res) else None, len(res), joins.ctypes.data, C.byref(st)))
     return joins[:max(n - 1, 0)], st
+
+
+def dereplicate(ctx, sset, rank, min_ani=0.95, mp=None, wave=0):
+    """sk_dereplicate: greedy ANI dereplication of a sketch set, equal to cluster() (greedy) on the rows of screen_triangle +
+    chain_pairs over the same set and mp, but screening and chaining only genome x representative pairs.  rank[g] is a
+    permutation, rank 0 the first choice as a representative; wave = genomes per wave (0 = library default), which never
+    changes the result.  Returns (rep, cluster, join, stats): join[g] is the chained row (RESULT_DTYPE) joining member g to
+    rep[g], for a representative a row with ani = NaN and ref_id = query_id = g; stats the sk_derep_stats struct."""
+    mp = mp or map_params()
+    n = len(sset)
+    rk = np.ascontiguousarray(rank, np.uint32)
+    if len(rk) != n:
+        raise ValueError("rank needs one entry per genome")
+    m = max(n, 1)
+    rep = np.zeros(m, np.uint32); cl = np.zeros(m, np.uint32); join = np.zeros(m, RESULT_DTYPE)
+    dp = DerepParams(float(min_ani), int(wave)); st = DerepStats()
+    ctx.check(ctx.L.sk_dereplicate(ctx.h, sset.h, C.byref(mp), rk.ctypes.data if n else None, C.byref(dp), rep.ctypes.data,
+                                   cl.ctypes.data, join.ctypes.data, C.byref(st)))
+    return rep[:n], cl[:n], join[:n], st

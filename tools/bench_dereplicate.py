@@ -1,0 +1,141 @@
+#!/usr/bin/env python3
+"""Dereplication measurements: `cluster` (triangle + greedy clustering) against `dereplicate`, printed as JSON lines with the
+card's name and power limit read in the same call.
+
+1. Library: sk_screen_triangle + sk_chain_pairs + sk_cluster (greedy) against sk_dereplicate on the same in-memory set of
+   synthetic families (bench_support/synth, genome ids shuffled over the indices as bench.py lays them out, so that length
+   ties rank families in scattered order).  Families of 20 and of 200.  One warm-up call of each, then --reps timed calls
+   alternated (host clock around calls that end in a device synchronise).  rep and cluster must be equal and every member's
+   joining row byte-identical.  Pairs chained by each side are printed.
+2. End to end: `cluster` against `dereplicate` on the same sets written as one FASTA file per genome, alternated --reps
+   times (wall time of the process); stdout must be identical.
+
+  python tools/bench_dereplicate.py [--genomes 2000] [--length 1000000] [--reps 3] [--skip-e2e] [--json OUT]
+The FASTA files go to a temporary directory that is removed at the end."""
+import argparse
+import json
+import os
+import shutil
+import subprocess
+import sys
+import tempfile
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+BIN = os.path.join(ROOT, "skani_b200", "skani-b200")
+
+from bench_sketch import card   # noqa: E402
+
+
+def emit(rec, sink):
+    print(json.dumps(rec), flush=True)
+    sink.append(rec)
+
+
+def family_set(n, L, G, seed):
+    from bench_support import synth
+    return synth.generate_ids(synth.shuffled_ids(n, seed), L, G=G)
+
+
+def bench_lib(n, L, G, reps, sink):
+    import skani_b200 as sk
+    ctx = sk.Context(0)
+    bases, off, goc = family_set(n, L, G, 20261018)
+    s = sk.sketch_contigs(ctx, bases, off, goc, n)
+    total = np.bincount(goc, weights=np.diff(off).astype(np.float64), minlength=n)
+    order = np.lexsort((np.arange(n), -total))          # longest first, ties by genome index (cluster's ranking)
+    rank = np.empty(n, np.uint32); rank[order] = np.arange(n)
+    mp = sk.map_params()
+
+    def via_triangle():
+        pairs = sk.screen_triangle(ctx, s, mp)
+        rows = sk.chain_pairs(ctx, s, s, pairs, mp, as_array=True)
+        rep, cl, edge, _ = sk.cluster(ctx, n, rows, rank, min_ani=0.95)
+        return rep, cl, edge, rows
+
+    def via_derep():
+        return sk.dereplicate(ctx, s, rank, min_ani=0.95, mp=mp)
+
+    tri, der = via_triangle(), via_derep()                 # warm-up, and the equality check
+    rep, cl, edge, rows = tri
+    mem = rep != np.arange(n)
+    equal = bool(np.array_equal(rep, der[0]) and np.array_equal(cl, der[1]) and
+                 der[2][mem].tobytes() == rows[edge[mem].astype(np.int64)].tobytes())
+    t_tri, t_der = [], []
+    for _ in range(reps):
+        t = time.perf_counter(); via_triangle(); t_tri.append(time.perf_counter() - t)
+        t = time.perf_counter(); via_derep(); t_der.append(time.perf_counter() - t)
+    st = der[3]
+    emit({"bench": "library", "genomes": n, "length": L, "family": G, "card": card(), "equal": equal, "clusters": int(st.n_clusters),
+          "triangle_pairs_chained": int(len(rows)), "derep_pairs_chained": int(st.pairs_chained), "derep_pairs_screened": int(st.pairs_screened),
+          "waves": int(st.waves), "t_triangle_cluster_s": sorted(t_tri), "t_dereplicate_s": sorted(t_der),
+          "derep_split_s": {"screen": st.t_screen, "chain": st.t_chain, "decide": st.t_decide, "total": st.t_total}}, sink)
+    s.free()
+    ctx.close()
+    return equal
+
+
+def write_fasta(d, n, L, G):
+    bases, off, goc = family_set(n, L, G, 20261018)
+    files = []
+    for g in range(n):
+        p = os.path.join(d, "g%06d.fa" % g)
+        with open(p, "wb") as f:
+            for i in np.nonzero(goc == g)[0]:
+                f.write(b">g%06d_c%d\n" % (g, i) + bases[int(off[i]):int(off[i + 1])].tobytes() + b"\n")
+        files.append(p)
+    return files
+
+
+def bench_e2e(n, L, G, reps, sink):
+    d = tempfile.mkdtemp(prefix="bench_derep_")
+    try:
+        files = write_fasta(d, n, L, G)
+        lst = os.path.join(d, "list.txt")
+        with open(lst, "w") as f:
+            f.write("\n".join(files) + "\n")
+        out = {}
+        times = {"cluster": [], "dereplicate": []}
+        for r in range(reps + 1):
+            for cmd in ("cluster", "dereplicate"):
+                t = time.perf_counter()
+                p = subprocess.run([BIN, cmd, "-l", lst], capture_output=True, text=True, check=True)
+                if r:
+                    times[cmd].append(time.perf_counter() - t)
+                out[cmd] = p.stdout
+                if cmd == "dereplicate":
+                    info = [ln for ln in p.stderr.splitlines() if "pairs screened" in ln]
+        emit({"bench": "end_to_end", "genomes": n, "length": L, "family": G, "card": card(), "equal": out["cluster"] == out["dereplicate"],
+              "t_cluster_s": sorted(times["cluster"]), "t_dereplicate_s": sorted(times["dereplicate"]), "dereplicate_info": info[-1] if info else ""}, sink)
+        return out["cluster"] == out["dereplicate"]
+    finally:
+        shutil.rmtree(d, ignore_errors=True)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--genomes", type=int, default=2000)
+    ap.add_argument("--length", type=int, default=1_000_000)
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--json")
+    a = ap.parse_args()
+    sink, ok = [], True
+    for G in (20, 200):
+        ok &= bench_lib(a.genomes, a.length, G, a.reps, sink)
+    if not a.skip_e2e:
+        for G in (20, 200):
+            ok &= bench_e2e(a.genomes, a.length, G, a.reps, sink)
+    if a.json:
+        with open(a.json, "w") as f:
+            json.dump(sink, f, indent=1)
+    if not ok:
+        sys.exit("outputs differ")
+
+
+if __name__ == "__main__":
+    main()
