@@ -246,6 +246,26 @@ int sk_chain_pairs(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* 
                    uint64_t n_pairs, const sk_map_params* mp, sk_ani_result* out);
 int sk_sketch_set_set_name_ranks(sk_sketch_set* set, const uint64_t* ranks /* n_genomes */);
 
+/* ---- mappings: where each pair aligns.  One record per chain interval that the non-overlap selection kept
+ *      (get_nonoverlapping_chains, src/chain.rs:1008-1099), joined to the identity estimate of the chunk it was chained in. */
+typedef struct {
+  uint32_t query_contig, ref_contig;  /* contig indices in the pair's query / reference genome (caller's orientation) */
+  uint32_t q0, q1, r0, r1;            /* first / last anchor seed position of the chain on each side, as the chain holds them */
+  uint32_t num_anchors, chunk;        /* anchors in the chain; the pair-local chunk it was chained in */
+  double   chunk_est;                 /* that chunk's identity estimate (raw, before the learned-ANI regression); 0 if none */
+  uint32_t chunk_weight;              /* its weight; 0 if none */
+  uint8_t  reverse, switched, chunk_valid, pad;  /* chunk_valid: 0 no estimate, 1 estimate, 3 estimate after the
+                                                    putative-ANI filter.  switched = 1: the chunks are windows of the reference */
+} sk_mapping;                         /* 48 bytes */
+/* sk_chain_pairs plus the mappings of every pair.  out is byte for byte sk_chain_pairs' out for the same arguments.  Pair i
+ * owns (*maps)[map_off[i] .. map_off[i + 1]) (map_off: n_pairs + 1 entries, caller-allocated; *maps malloc'd, sk_free):
+ * every interval the selection kept for it, whatever its ani (NaN and -1 included), sorted by (query_contig, q0, q1,
+ * ref_contig, r0, r1, reverse, chunk).  A seed position is the index of the last base of its k-mer, so a record covers bases
+ * [q0 - k + 1, q1 + 1) of its query contig and [r0 - k + 1, r1 + 1) of its reference contig. */
+int sk_chain_pairs_mappings(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, const uint64_t* pairs,
+                            uint64_t n_pairs, const sk_map_params* mp, sk_ani_result* out, uint64_t* map_off,
+                            sk_mapping** maps);
+
 /* parity taps (test use), per pair: all outputs are malloc'd (sk_chain_debug_free). anchors: 5 x u32 per anchor
  * (query_contig, query_pos, ref_contig, ref_pos, reverse) in sorted order (src/chain.rs:721); chunk_first: n_chunks+1;
  * score/pointer per anchor (chunk-local pointer, src/chain.rs:881-882); intervals: 11 x i64 per interval in the
@@ -367,6 +387,10 @@ int sk_screen_query_ref_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sket
 int sk_chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
                          const sk_sketch_set* const* queries, const uint64_t* pairs, uint64_t n_pairs,
                          const sk_map_params* mp, sk_ani_result* out);
+/* sk_chain_pairs_multi plus mappings as sk_chain_pairs_mappings: each context's records are merged back into pair order. */
+int sk_chain_pairs_multi_mappings(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
+                                  const sk_sketch_set* const* queries, const uint64_t* pairs, uint64_t n_pairs,
+                                  const sk_map_params* mp, sk_ani_result* out, uint64_t* map_off, sk_mapping** maps);
 
 /* ---- triangle beyond one GPU's memory: sketches live in pinned HOST memory and come back to the device in working sets --
  * A store holds sketches with their k-mer tables, genome-indexed, in fixed-size pinned, device-mapped host slabs.

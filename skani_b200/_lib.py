@@ -118,6 +118,7 @@ SYMBOLS = [
     ("sk_screen_query_ref", i32, [vp, vp, vp, PP(MapParams), i32, PP(PP(u64)), PP(u64)]),
     ("sk_free", None, [vp]),
     ("sk_chain_pairs", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp]),
+    ("sk_chain_pairs_mappings", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp, vp, PP(vp)]),
     ("sk_sketch_set_set_name_ranks", i32, [vp, vp]),
     ("sk_chain_pair_debug", i32, [vp, vp, vp, u64, PP(MapParams), PP(ChainDebug)]),
     ("sk_chain_pairs_debug", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp]),
@@ -136,6 +137,7 @@ SYMBOLS = [
     ("sk_sketch_set_copy", i32, [vp, vp, PP(vp)]),
     ("sk_screen_query_ref_multi", i32, [vp, u32, vp, vp, vp, PP(MapParams), i32, PP(PP(u64)), PP(u64)]),
     ("sk_chain_pairs_multi", i32, [vp, u32, vp, vp, vp, vp, u64, PP(MapParams), vp]),
+    ("sk_chain_pairs_multi_mappings", i32, [vp, u32, vp, vp, vp, vp, u64, PP(MapParams), vp, vp, PP(vp)]),
     ("sk_sketch_store_create", i32, [PP(SketchParams), PP(vp)]),
     ("sk_sketch_store_add", i32, [vp, vp]),
     ("sk_sketch_store_n_genomes", u32, [vp]),

@@ -173,6 +173,7 @@ struct Opts {
   std::string dendrogram;           // cluster --dendrogram FILE
   std::string representatives;      // dereplicate --representatives FILE
   std::string tree_method = "nj";   // tree --method nj|average|complete
+  std::string mappings;             // triangle / dist / search --mappings FILE
 };
 
 void write_header(FILE* o, bool ci, bool detailed) {   // src/file_io.rs:15-23
@@ -203,6 +204,44 @@ void write_perfect(FILE* o, const Genome& g, const Opts& op) {   // write_ani_re
   else if (op.ci) fprintf(o, "\t100.00\t100.00");
   fputc('\n', o);
 }
+
+// --mappings FILE: one row per kept chain interval of every printed pair, 0-based half-open base coordinates.  A seed's
+// position is the last base of its k-mer, so seed positions p0..p1 cover [p0 - k + 1, p1 + 1).
+struct MappingFile {
+  FILE* f = nullptr;
+  uint32_t k = 0;
+  bool open(const std::string& path, uint32_t k_) {
+    k = k_;
+    f = fopen(path.c_str(), "w");
+    if (!f) { fprintf(stderr, "ERROR cannot open %s\n", path.c_str()); return false; }
+    fprintf(f, "Ref_file\tQuery_file\tRef_contig\tRef_start\tRef_end\tQuery_contig\tQuery_start\tQuery_end\tStrand\tAnchors\t"
+               "Chunk_genome\tChunk\tChunk_ANI\tChunk_weight\n");
+    return true;
+  }
+  static const std::string& contig(const Genome& g, uint32_t i) { static const std::string none; return i < g.contigs.size() ? g.contigs[i] : none; }
+  void write(const sk_mapping* m, uint64_t n, const Genome& ref, const Genome& qry, const Opts& op) {
+    for (uint64_t i = 0; i < n; i++) {
+      const sk_mapping& x = m[i];
+      char ani[32];
+      if (x.chunk_valid) snprintf(ani, sizeof(ani), "%.2f", x.chunk_est * 100.);
+      else snprintf(ani, sizeof(ani), "NA");
+      fprintf(f, "%s\t%s\t%s\t%u\t%u\t%s\t%u\t%u\t%c\t%u\t%c\t%u\t%s\t%u\n", ref.file_name.c_str(), qry.file_name.c_str(),
+              short_name(contig(ref, x.ref_contig), op.short_header).c_str(), x.r0 + 1 - k, x.r1 + 1,
+              short_name(contig(qry, x.query_contig), op.short_header).c_str(), x.q0 + 1 - k, x.q1 + 1, x.reverse ? '-' : '+',
+              x.num_anchors, x.switched ? 'R' : 'Q', x.chunk, ani, x.chunk_weight);
+    }
+  }
+  void flush() { if (f) fflush(f); }
+  ~MappingFile() { if (f) fclose(f); }
+};
+
+// the mapping records of a block of result rows: row i owns recs[off[i] .. off[i + 1])
+struct RowMaps {
+  std::vector<uint64_t> off{0};
+  std::vector<sk_mapping> recs;
+  void clear() { off.assign(1, 0); recs.clear(); }
+  void add(const sk_mapping* m, uint64_t n) { recs.insert(recs.end(), m, m + n); off.push_back(recs.size()); }
+};
 
 #define CK(ctx, call) do { int rc__ = (call); if (rc__ != 0) { fprintf(stderr, "ERROR %s failed (%d): %s\n", #call, rc__, sk_last_error(ctx)); exit(1); } } while (0)
 
@@ -626,6 +665,15 @@ int load_triangle_inputs(Opts& op, Inputs& in, sk_ctx*& ctx, TriangleInputs& ti)
 int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_result>& res, const BlockWriter* stream) {
   TriangleInputs ti;
   if (const int rc = open_triangle_inputs(op, ti)) return rc;
+  if (!op.mappings.empty() && ti.use_store) {
+    fprintf(stderr, "ERROR --mappings is not supported when the sketches exceed device memory (host sketch store path); "
+                    "split the inputs into runs that fit the device.\n");
+    return 1;
+  }
+  if (!op.mappings.empty() && op.gpus > 1 && !ti.sketches) {
+    fprintf(stderr, "ERROR --mappings is not supported with triangle --gpus N > 1 (the multi-GPU triangle); run it on one GPU.\n");
+    return 1;
+  }
   if (const int rc = load_triangle_inputs(op, in, ctx, ti)) return rc;
   const bool refs_are_sketch = ti.sketches;
   const sk_sketch_params sp = ti.sp;
@@ -674,6 +722,10 @@ int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_resu
     // rows in blocks of FL: with `stream` each block is handed over and replaced by the next, without it the one block of
     // all rows stays in res
     const size_t N = in.genomes.size(), FL = stream ? intermediate_write_count() : N;
+    // --mappings: the records of the rows the sparse output prints (ani > 0.1, in (i, j) order), written block by block
+    MappingFile mf;
+    if (!op.mappings.empty() && !mf.open(op.mappings, sp.k)) return 1;
+    std::vector<uint64_t> off;
     uint64_t p0 = 0;
     bool ok = true;
     for (size_t r0 = 0; r0 < N && ok; r0 += FL) {
@@ -681,7 +733,17 @@ int triangle_results(Opts& op, Inputs& in, sk_ctx*& ctx, std::vector<sk_ani_resu
       while (p1 < np && (uint32_t)(pairs[p1] >> 32) < r0 + FL) p1++;      // pairs are sorted by (i, j)
       res.resize(p1 - p0);
       const auto t1 = clk::now();
-      CK(ctx, sk_chain_pairs(ctx, set, set, pairs + p0, p1 - p0, &mp, res.data()));
+      if (mf.f) {
+        off.resize(p1 - p0 + 1);
+        sk_mapping* maps = nullptr;
+        CK(ctx, sk_chain_pairs_mappings(ctx, set, set, pairs + p0, p1 - p0, &mp, res.data(), off.data(), &maps));
+        for (size_t i = 0; i < res.size(); i++)
+          if (res[i].ani > 0.1f) mf.write(maps + off[i], off[i + 1] - off[i], in.genomes[res[i].ref_id], in.genomes[res[i].query_id], op);
+        mf.flush();
+        sk_free(maps);
+      } else {
+        CK(ctx, sk_chain_pairs(ctx, set, set, pairs + p0, p1 - p0, &mp, res.data()));
+      }
       timed(t1);
       if (stream) ok = (*stream)(res, r0 + FL < N);
       p0 = p1;
@@ -1010,28 +1072,40 @@ int run_tree(Opts& op) {
 }
 
 // write_query_ref_list (src/file_io.rs:608-678) of dist and search: queries in blocks of INTERMEDIATE_WRITE_COUNT
-// (src/dist.rs:151-175, src/search.rs:255-279).  block(q0, q1, res) fills res with the results of the queries [q0, q1), rows
-// of equal ANI in the order they print, or returns false (after an ERROR line) to end the run with exit code 1.  Each block
-// is grouped by the query's first contig name, each group sorted by ANI (descending, stable) and its top n written, then
-// flushed.
+// (src/dist.rs:151-175, src/search.rs:255-279).  block(q0, q1, res, rm) fills res with the results of the queries [q0, q1),
+// rows of equal ANI in the order they print, and with --mappings (rm non-null, k = the sketches' k) rm with their mapping
+// records; or returns false (after an ERROR line) to end the run with exit code 1.  Each block is grouped by the query's
+// first contig name, each group sorted by ANI (descending, stable) and its top n written, with their mappings, then flushed.
 template <class F>
-int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vector<Genome>& queries, F block) {
+int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vector<Genome>& queries, uint32_t k, F block) {
+  MappingFile mf;
+  if (!op.mappings.empty() && !mf.open(op.mappings, k)) return 1;
   FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
   if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
   write_header(o, op.ci, op.detailed);
   const size_t FL = intermediate_write_count(), NQ = queries.size();
   std::vector<sk_ani_result> res;
+  RowMaps rm;
+  RowMaps* rmp = mf.f ? &rm : nullptr;
   int rc = 0;
   for (size_t q0 = 0; q0 < NQ; q0 += FL) {
-    if (!block(q0, std::min(q0 + FL, NQ), res)) { rc = 1; break; }
+    rm.clear();
+    if (!block(q0, std::min(q0 + FL, NQ), res, rmp)) { rc = 1; break; }
     std::map<std::string, std::vector<const sk_ani_result*>> groups;
     for (auto& r : res) if (r.ani > 0.1f) groups[queries[r.query_id].contigs[0]].push_back(&r);
     for (auto& kv : groups) {
       auto v = kv.second;
       std::stable_sort(v.begin(), v.end(), [](const sk_ani_result* a, const sk_ani_result* b) { return a->ani > b->ani; });
-      for (size_t i = 0; i < v.size() && i < op.n; i++) write_row(o, *v[i], refs[v[i]->ref_id], queries[v[i]->query_id], op);
+      for (size_t i = 0; i < v.size() && i < op.n; i++) {
+        write_row(o, *v[i], refs[v[i]->ref_id], queries[v[i]->query_id], op);
+        if (rmp) {
+          const size_t row = v[i] - res.data();
+          mf.write(rm.recs.data() + rm.off[row], rm.off[row + 1] - rm.off[row], refs[v[i]->ref_id], queries[v[i]->query_id], op);
+        }
+      }
     }
     fflush(o);
+    mf.flush();
     if (q0 + FL < NQ) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", FL);
   }
   if (o != stdout) fclose(o);
@@ -1071,6 +1145,11 @@ int run_dist(Opts& op) {
   // store path: both sides go into host sketch stores in groups and are chained in working sets (sk_query_ref_store)
   double need_gb = 0;
   const bool use_store = dist_needs_store(op, refs_are_sketch, queries_are_sketch, rsi, qsi, &need_gb);
+  if (use_store && !op.mappings.empty()) {
+    fprintf(stderr, "ERROR --mappings is not supported when the sketches exceed device memory (host sketch store path); "
+                    "split the inputs into runs that fit the device.\n");
+    return 1;
+  }
   sk_sketch_store *rstore = nullptr, *qstore = nullptr;
   const int threads = std::max(op.threads, 1);
   if (use_store) {
@@ -1103,7 +1182,7 @@ int run_dist(Opts& op) {
     sk_free(r);
     std::sort(all.begin(), all.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.query_id != b.query_id ? a.query_id < b.query_id : a.ref_id < b.ref_id; });
     size_t p0 = 0;
-    const int rc = write_dist(op, rin.genomes, qin.genomes, [&](size_t, size_t q1, std::vector<sk_ani_result>& res) {
+    const int rc = write_dist(op, rin.genomes, qin.genomes, sp.k, [&](size_t, size_t q1, std::vector<sk_ani_result>& res, RowMaps*) {
       size_t p1 = p0;
       while (p1 < all.size() && all[p1].query_id < q1) p1++;
       res.assign(all.begin() + p0, all.begin() + p1);
@@ -1150,11 +1229,20 @@ int run_dist(Opts& op) {
   sk_free(pairs);
   std::sort(byq.begin(), byq.end(), [](uint64_t a, uint64_t b) { return (uint32_t)a != (uint32_t)b ? (uint32_t)a < (uint32_t)b : a < b; });
   size_t p0 = 0;
-  const int rc = write_dist(op, rin.genomes, qin.genomes, [&](size_t, size_t q1, std::vector<sk_ani_result>& res) {
+  const int rc = write_dist(op, rin.genomes, qin.genomes, sp.k, [&](size_t, size_t q1, std::vector<sk_ani_result>& res, RowMaps* rm) {
     size_t p1 = p0;
     while (p1 < byq.size() && (uint32_t)byq[p1] < q1) p1++;
     res.resize(p1 - p0);
-    CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), byq.data() + p0, p1 - p0, &mp, res.data()));
+    if (rm) {
+      std::vector<uint64_t> off(p1 - p0 + 1);
+      sk_mapping* maps = nullptr;
+      CK(ctx, sk_chain_pairs_multi_mappings(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), byq.data() + p0, p1 - p0, &mp,
+                                            res.data(), off.data(), &maps));
+      for (size_t i = 0; i < res.size(); i++) rm->add(maps + off[i], off[i + 1] - off[i]);
+      sk_free(maps);
+    } else {
+      CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), byq.data() + p0, p1 - p0, &mp, res.data()));
+    }
     p0 = p1;
     return true;
   });
@@ -1417,7 +1505,7 @@ int run_search(Opts& op) {
   std::vector<uint64_t> all_pairs(pairs, pairs + np);
   sk_free(pairs);
   const uint64_t group_records = sketch_group_records((1ull << 31) - 1);
-  const int rc = write_dist(op, refs, qmeta, [&](size_t q0, size_t q1, std::vector<sk_ani_result>& res) {
+  const int rc = write_dist(op, refs, qmeta, sp.k, [&](size_t q0, size_t q1, std::vector<sk_ani_result>& res, RowMaps* rm) {
     std::vector<uint64_t> blockp;
     for (uint64_t x : all_pairs) if ((uint32_t)x >= q0 && (uint32_t)x < q1) blockp.push_back(x);   // stays sorted by (ref, query)
     std::vector<uint32_t> hits;
@@ -1435,6 +1523,7 @@ int run_search(Opts& op) {
     for (size_t d = 0; d < W; d++)
       rd.emplace_back(rsi, std::vector<size_t>(hits.begin() + run[d], hits.begin() + run[d + 1]), context_threads(op, d, W), group_records);
     res.clear();
+    std::vector<std::vector<sk_mapping>> rowmaps;   // with --mappings: the records of res[i]
     for (;;) {
       std::vector<size_t> lo(W, 0), hi(W, 0);                   // this round: context d imports hits [lo[d], hi[d])
       std::vector<sk_sketch_set*> rsets(W, nullptr);
@@ -1463,12 +1552,31 @@ int run_search(Opts& op) {
       }
       if (round_hit.empty()) break;
       std::vector<sk_ani_result> round(local.size());
-      CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(), &mp, round.data()));
-      for (auto& r : round) if (r.ani > 0.5f) { r.ref_id = hits[round_hit[r.ref_id]]; res.push_back(r); }   // src/search.rs:174
+      std::vector<uint64_t> off(rm ? local.size() + 1 : 0);
+      sk_mapping* maps = nullptr;
+      if (rm) CK(ctx, sk_chain_pairs_multi_mappings(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(),
+                                                    &mp, round.data(), off.data(), &maps));
+      else CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(), &mp, round.data()));
+      for (size_t i = 0; i < round.size(); i++) {
+        sk_ani_result& r = round[i];
+        if (!(r.ani > 0.5f)) continue;                                                        // src/search.rs:174
+        r.ref_id = hits[round_hit[r.ref_id]];
+        res.push_back(r);
+        if (rm) rowmaps.emplace_back(maps + off[i], maps + off[i + 1]);
+      }
+      sk_free(maps);
       for (auto* s : rsets) sk_sketch_set_free(s);
     }
     // rows of equal ANI print in (ref, query) order, as one context chaining the hits in order produces them
-    std::sort(res.begin(), res.end(), [](const sk_ani_result& a, const sk_ani_result& b) { return a.ref_id != b.ref_id ? a.ref_id < b.ref_id : a.query_id < b.query_id; });
+    std::vector<size_t> ord(res.size());
+    std::iota(ord.begin(), ord.end(), 0);
+    std::sort(ord.begin(), ord.end(), [&](size_t a, size_t b) { return res[a].ref_id != res[b].ref_id ? res[a].ref_id < res[b].ref_id : res[a].query_id < res[b].query_id; });
+    std::vector<sk_ani_result> sorted(res.size());
+    for (size_t i = 0; i < ord.size(); i++) {
+      sorted[i] = res[ord[i]];
+      if (rm) rm->add(rowmaps[ord[i]].data(), rowmaps[ord[i]].size());
+    }
+    res.swap(sorted);
     return true;
   });
   for (auto* s : qsets) sk_sketch_set_free(s);
@@ -1517,7 +1625,12 @@ void usage() {
           "      (rooted, a node at half its merge height)\n"
           "  common: -c C -m M -k K -s SCREEN%% --min-af P --both-min-af P --robust --median --no-learned-ani --faster-small\n"
           "          --small-genomes --fast --medium --slow --ci --detailed --short-header --no-marker-index -t THREADS --device D\n"
-          "          --gpus N (triangle, dist, search, sketch, cluster, tree: one context per GPU, devices D, D+1, ...)\n");
+          "          --gpus N (triangle, dist, search, sketch, cluster, tree: one context per GPU, devices D, D+1, ...)\n"
+          "  --mappings FILE (triangle, dist, search): where each printed pair aligns, one TSV row per chain interval kept by the\n"
+          "          ANI estimate: contigs, 0-based half-open coordinates, strand, anchors, and the identity of the 20 kb chunk it\n"
+          "          was chained in.  Pairs, order and orientation are those of the main output (triangle: those of -E).  A few\n"
+          "          hundred rows per related 5 Mbp pair: on large triangles the file runs to gigabytes.  Not with inputs beyond\n"
+          "          device memory, nor with triangle --gpus N > 1\n");
 }
 
 }  // namespace
@@ -1589,6 +1702,7 @@ int main(int argc, char** argv) {
     else if (a == "--dendrogram" && (op.cmd == "cluster" || op.cmd == "dereplicate")) op.dendrogram = val();
     else if (a == "--representatives" && op.cmd == "dereplicate") op.representatives = val();
     else if (a == "--method" && op.cmd == "tree") op.tree_method = val();
+    else if (a == "--mappings" && (op.cmd == "triangle" || op.cmd == "dist" || op.cmd == "search")) op.mappings = val();
     else if (a == "--keep-refs") {}   // search already loads every passing reference exactly once
     else if (a == "-v" || a == "--debug" || a == "--trace") {}
     else { fprintf(stderr, "ERROR unknown option %s\n", a.c_str()); usage(); return 2; }

@@ -16,6 +16,7 @@
 //   select_kernel  (block/pair)  bitonic sort of intervals (descending derived order), greedy non-overlap filter
 //   chunkstat_kernel (thread/chunk) seeds inside the padded interval union -> per-chunk identity
 //   final_kernel   (block/pair)  sorted (est, weight) -> trimmed weighted mean, AF, std, bootstrap, cutoffs, GBDT
+//   mapping_scan_kernel + mapping_emit_kernel (sk_chain_pairs_mappings only) kept intervals -> sorted sk_mapping records
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -26,6 +27,7 @@
 #include <numeric>
 
 #include "chain_core.cuh"
+#include "mapping_core.cuh"
 #include "sk_internal.h"
 
 namespace sk {
@@ -100,7 +102,7 @@ struct Workspace {
   uint32_t *acc_total, *acc_rq0, *acc_rq1, *acc_tbcq, *acc_nint, *chunk_head;
   double* chunk_est;
   uint32_t* chunk_w;
-  uint8_t* chunk_valid;
+  uint8_t* chunk_valid;    // 0 no estimate, 1 estimate, 3 estimate after the putative-ANI filter
   uint32_t* chunk_nseeds;
   // per interval (capacity floor(A/3) per pair)
   IntervalKey* iv;
@@ -1221,7 +1223,7 @@ chunkstat_kernel(uint64_t n_chunks, const PairDesc* __restrict__ pairs, SetView 
       uint8_t valid = 0;
       bool filtered;
       if (chunk_estimate(acc, prm.c, prm.k, s_nseeds[threadIdx.x], s_numin[threadIdx.x], s_ul[threadIdx.x], &est, &wgt, &filtered)) {
-        ws.chunk_est[c] = est; ws.chunk_w[c] = wgt; valid = 1;
+        ws.chunk_est[c] = est; ws.chunk_w[c] = wgt; valid = filtered ? 3 : 1;   // 3: the putative-ANI filter applied
         if (prm.c >= 200) atomicAdd(&ws.pair_tqb_ns[ws.chunk_pair[c]], acc.rq1 - acc.rq0 + 2 * prm.c + prm.k);  // !sensitive_af (:261-264)
       }
       ws.chunk_valid[c] = valid;
@@ -1417,6 +1419,80 @@ final_kernel(const PairDesc* __restrict__ pairs, const GenomeMeta* __restrict__ 
   if (threadIdx.x == 0) out[p] = r;
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// K8 (sk_chain_pairs_mappings only): the kept intervals of every pair as sorted sk_mapping records
+// ------------------------------------------------------------------------------------------------------------
+constexpr int MAP_SCAN_T = 256;
+constexpr uint32_t MAP_SMEM_MAX = 512;   // records of a pair sorted in shared memory; a pair with more sorts in global memory
+
+// map_base[0..B] = exclusive prefix of pair_nchains (the kept intervals of each pair), one block
+__global__ void __launch_bounds__(MAP_SCAN_T)
+mapping_scan_kernel(uint32_t B, const uint32_t* __restrict__ nchains, uint64_t* __restrict__ map_base) {
+  using Scan = cub::BlockScan<uint64_t, MAP_SCAN_T>;
+  __shared__ typename Scan::TempStorage tmp;
+  __shared__ uint64_t s_carry;
+  if (threadIdx.x == 0) s_carry = 0;
+  __syncthreads();
+  for (uint32_t i0 = 0; i0 < B; i0 += MAP_SCAN_T) {
+    const uint32_t i = i0 + threadIdx.x;
+    uint64_t ex, tot;
+    Scan(tmp).ExclusiveSum(i < B ? (uint64_t)nchains[i] : 0ull, ex, tot);
+    if (i < B) map_base[i] = s_carry + ex;
+    __syncthreads();
+    if (threadIdx.x == 0) s_carry += tot;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) map_base[B] = s_carry;
+}
+
+// Block per pair: the pair's kept intervals (acc_list, in selection order) become records joined to their chunk's estimate
+// (mapping_record), are bitonic-sorted by mapping_before through an index array and written to out[map_base[p] ..).  Up to
+// MAP_SMEM_MAX records the records and indices live in shared memory; beyond, in the pair's slices of stage (one record per
+// kept interval) and gidx (two indices per kept interval >= the padded power of two).
+__global__ void __launch_bounds__(CT)
+mapping_emit_kernel(const PairDesc* __restrict__ pairs, Workspace ws, const uint64_t* __restrict__ map_base,
+                    sk_mapping* __restrict__ stage, uint32_t* __restrict__ gidx, sk_mapping* __restrict__ out) {
+  __shared__ sk_mapping s_rec[MAP_SMEM_MAX];
+  __shared__ uint32_t s_idx[MAP_SMEM_MAX];
+  const uint32_t p = blockIdx.x;
+  const uint64_t base = map_base[p];
+  const uint32_t n = (uint32_t)(map_base[p + 1] - base);
+  if (n == 0) return;
+  uint32_t npow2 = 1;
+  while (npow2 < n) npow2 <<= 1;
+  const bool in_smem = npow2 <= MAP_SMEM_MAX;
+  sk_mapping* rec = in_smem ? s_rec : stage + base;
+  uint32_t* idx = in_smem ? s_idx : gidx + 2 * base;
+  const uint64_t ib = ws.pairIbase[p], cb = ws.pairCbase[p];
+  const bool sw = pairs[p].switched != 0;
+  const uint32_t NONE = 0xFFFFFFFFu;
+  for (uint32_t a = threadIdx.x; a < npow2; a += blockDim.x) {
+    if (a < n) {
+      const IntervalKey x = ws.iv[ib + ws.acc_list[ib + a]];
+      const uint64_t ch = cb + iv_chunk(x);
+      const uint8_t v = ws.chunk_valid[ch];
+      rec[a] = mapping_record(x, sw, v ? ws.chunk_est[ch] : 0., v ? ws.chunk_w[ch] : 0u, v);
+    }
+    idx[a] = a < n ? a : NONE;   // padding sorts last
+  }
+  __syncthreads();
+  for (uint32_t k = 2; k <= npow2; k <<= 1) {
+    for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+      for (uint32_t i = threadIdx.x; i < npow2; i += blockDim.x) {
+        const uint32_t ixj = i ^ j;
+        if (ixj > i) {
+          const uint32_t a = idx[i], b = idx[ixj];
+          const bool b_lt_a = b != NONE && (a == NONE || mapping_before(rec[b], rec[a]));
+          const bool a_lt_b = a != NONE && (b == NONE || mapping_before(rec[a], rec[b]));
+          if ((i & k) == 0 ? b_lt_a : a_lt_b) { idx[i] = b; idx[ixj] = a; }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) out[base + i] = rec[idx[i]];
+}
+
 __global__ void chunk_size_kernel(uint64_t n, Workspace ws) {
   uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -1549,6 +1625,11 @@ struct ChainScratch {
   size_t c_iv = 0, c_iv_keys = 0, c_iv_order = 0, c_iv_kept = 0, c_iv_next = 0, c_acc_list = 0, c_est_sorted = 0, c_w_sorted = 0;
   PairDesc* d_pairs = nullptr; size_t c_pairs = 0;
   sk_ani_result* d_out = nullptr; size_t c_out = 0;
+  // mapping runs only: per-pair record offsets, the sorted records, and the global-memory sort's records and indices
+  uint64_t* map_base = nullptr; size_t c_map_base = 0;
+  sk_mapping *map_out = nullptr, *map_stage = nullptr; size_t c_map_out = 0, c_map_stage = 0;
+  uint32_t* map_idx = nullptr; size_t c_map_idx = 0;
+  sk_mapping* h_map = nullptr; size_t c_h_map = 0;   // pinned staging of a batch's records on their way to the host
   GenomeMeta *d_m0 = nullptr, *d_m1 = nullptr;
   size_t c_m0 = 0, c_m1 = 0;
   void free_all() {
@@ -1556,12 +1637,23 @@ struct ChainScratch {
                     ws.pairA, ws.pairC, ws.pairAbase, ws.pairCbase, ws.pairIbase, ws.pair_nint, ws.pair_sumlen, ws.pair_nchains, ws.pair_tqb_ns, ws.anc,
                     ws.score, ws.ptr, ws.rootkey, ws.depth, ws.chunk_first, ws.chunk_pair, ws.chunk_qctg, ws.chunk_lo, ws.chunk_hi,
                     ws.acc_total, ws.acc_rq0, ws.acc_rq1, ws.acc_tbcq, ws.acc_nint, ws.chunk_head, ws.chunk_est, ws.chunk_w, ws.chunk_valid,
-                    ws.chunk_nseeds, ws.iv, ws.iv_keys, ws.iv_order, ws.iv_kept, ws.iv_next, ws.acc_list, ws.est_sorted, ws.w_sorted, d_pairs, d_out, d_m0, d_m1};
+                    ws.chunk_nseeds, ws.iv, ws.iv_keys, ws.iv_order, ws.iv_kept, ws.iv_next, ws.acc_list, ws.est_sorted, ws.w_sorted, d_pairs, d_out, d_m0, d_m1,
+                    map_base, map_out, map_stage, map_idx};
     for (void* p : ptrs) if (p) cudaFree(p);
+    if (h_map) cudaFreeHost(h_map);
   }
 };
 
 struct HostPair { uint32_t ref, query; };
+
+// the mappings of a call, collected batch by batch in pair order: count[i] records of pair i, all pairs' n records in recs
+// (malloc'd: handed to the caller as is)
+struct MapOut {
+  std::vector<uint64_t> count;
+  sk_mapping* recs = nullptr;
+  size_t n = 0, cap = 0;
+  ~MapOut() { free(recs); }
+};
 
 // dp_group_kernel's instantiation for the band: FULLBAND when the band fills the lanes' register sets exactly, and then the
 // 25-block register cap unless SK_DP_MINB=1.  TAPS only adds the score / pointer stores.
@@ -1720,7 +1812,7 @@ static int copy_out_debug(sk_ctx* ctx, const Workspace& ws, const std::vector<Pa
 // whole list) the intermediate products of the batch's pairs are copied out as well.
 static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, const sk_sketch_set* qs, const std::vector<PairDesc>& descs,
                      size_t b0, size_t b1, uint64_t total_rec, uint64_t total_chunks, const std::vector<uint32_t>& tile_off, const ChainParams& prm, const SetView& v0, const SetView& v1,
-                     sk_ani_result* host_out, sk_chain_debug* dbg) {
+                     sk_ani_result* host_out, sk_chain_debug* dbg, MapOut* mo) {
   cudaStream_t st = ctx->stream;
   const uint32_t B = (uint32_t)(b1 - b0);
   Workspace& ws = S.ws;
@@ -1801,6 +1893,16 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
     SK_TRY(launch_dp_select(ctx, S, B, TC, prm, true, dbg != nullptr));
     SK_LAUNCH(ctx, "chunkstat_kernel", (chunkstat_kernel<<<(uint32_t)((TC + CS_WARPS * CS_PER_WARP - 1) / (CS_WARPS * CS_PER_WARP)), CS_WARPS * 32, 0, st>>>(TC, S.d_pairs, v0, v1, S.d_m0, S.d_m1, prm, ws, dbg_counts)));
   }
+  std::vector<uint64_t> hmap(mo ? B + 1 : 0);
+  if (mo) {
+    // every pair's kept intervals (pair_nchains of them, acc_list) as sorted records, offsets and records copied out below
+    SK_TRY(ensure(ctx, &S.map_base, &S.c_map_base, B + 1));
+    SK_TRY(ensure(ctx, &S.map_out, &S.c_map_out, NI)); SK_TRY(ensure(ctx, &S.map_stage, &S.c_map_stage, NI));
+    SK_TRY(ensure(ctx, &S.map_idx, &S.c_map_idx, 2 * NI));
+    SK_LAUNCH(ctx, "mapping_scan_kernel", (mapping_scan_kernel<<<1, MAP_SCAN_T, 0, st>>>(B, ws.pair_nchains, S.map_base)));
+    SK_LAUNCH(ctx, "mapping_emit_kernel", (mapping_emit_kernel<<<B, CT, 0, st>>>(S.d_pairs, ws, S.map_base, S.map_stage, S.map_idx, S.map_out)));
+    SK_CUDA(cudaMemcpyAsync(hmap.data(), S.map_base, (B + 1) * 8, cudaMemcpyDeviceToHost, st));
+  }
   // test hook: SK_FINAL_FORCE_REDO=1 takes the sequential bootstrap redo for every pair, as if some draw had been rejected
   const char* fr = getenv("SK_FINAL_FORCE_REDO");
   const int force_redo = (fr && atoi(fr) != 0) ? 1 : 0;
@@ -1809,6 +1911,30 @@ static int run_batch(sk_ctx* ctx, ChainScratch& S, const sk_sketch_set* refs, co
   SK_CUDA(cudaStreamSynchronize(st));
   SK_CUDA(cudaGetLastError());
 
+  if (mo) {
+    const uint64_t n = hmap[B];
+    if (n > TI) { ctx->err = "chain mappings: more kept intervals than the batch's interval capacity"; return SK_ERR_STATE; }
+    if (mo->n + n > mo->cap) {
+      const size_t cap = std::max<size_t>(mo->n + n, 2 * mo->cap);
+      sk_mapping* r = (sk_mapping*)realloc(mo->recs, std::max<size_t>(cap, 1) * sizeof(sk_mapping));
+      if (!r) { ctx->err = "chain mappings: out of host memory"; return SK_ERR_NOMEM; }
+      mo->recs = r; mo->cap = cap;
+    }
+    if (n) {
+      if (n > S.c_h_map) {   // grow-only pinned staging: the copy runs at full PCIe rate
+        if (S.h_map) SK_CUDA(cudaFreeHost(S.h_map));
+        S.h_map = nullptr; S.c_h_map = 0;
+        const size_t c = n + n / 4;
+        SK_CUDA(cudaMallocHost((void**)&S.h_map, c * sizeof(sk_mapping)));
+        S.c_h_map = c;
+      }
+      SK_CUDA(cudaMemcpyAsync(S.h_map, S.map_out, n * sizeof(sk_mapping), cudaMemcpyDeviceToHost, st));
+      SK_CUDA(cudaStreamSynchronize(st));
+      memcpy(mo->recs + mo->n, S.h_map, n * sizeof(sk_mapping));
+      mo->n += n;
+    }
+    for (uint32_t i = 0; i < B; i++) mo->count[b0 + i] = hmap[i + 1] - hmap[i];
+  }
   if (dbg) SK_TRY(copy_out_debug(ctx, ws, descs, b0, B, abase, cbase, ibase, dbg_counts, host_out, dbg));
   return SK_OK;
 }
@@ -1898,7 +2024,7 @@ static int debug_dp_select(sk_ctx* ctx, uint32_t c, uint32_t k, const uint32_t* 
 }
 
 static int chain_impl(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* qs, const uint64_t* pairs, uint64_t n_pairs,
-                      const sk_map_params* mp, sk_ani_result* out, sk_chain_debug* dbg) {
+                      const sk_map_params* mp, sk_ani_result* out, sk_chain_debug* dbg, MapOut* mo) {
   SK_CUDA(cudaSetDevice(ctx->device));
   if (refs->sp.c != qs->sp.c || refs->sp.k != qs->sp.k) { ctx->err = "ref/query sketch parameters differ"; return SK_ERR_PARAM; }
   if (n_pairs == 0) return SK_OK;
@@ -1963,7 +2089,7 @@ static int chain_impl(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_se
       tile_off.push_back(tile_off.back() + (uint32_t)((nr + TILE - 1) / TILE));
       b1++;
     }
-    SK_TRY(run_batch(ctx, S, refs, qs, descs, b0, b1, rec, chunks, tile_off, prm, v0, v1, out, dbg));
+    SK_TRY(run_batch(ctx, S, refs, qs, descs, b0, b1, rec, chunks, tile_off, prm, v0, v1, out, dbg, mo));
     b0 = b1;
   }
   return SK_OK;
@@ -1976,7 +2102,23 @@ extern "C" {
 int sk_chain_pairs(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, const uint64_t* pairs, uint64_t n_pairs,
                    const sk_map_params* mp, sk_ani_result* out) {
   if (!ctx || !refs || !queries || !mp || (n_pairs && (!pairs || !out))) return SK_ERR_PARAM;
-  return sk::chain_impl(ctx, refs, queries, pairs, n_pairs, mp, out, nullptr);
+  return sk::chain_impl(ctx, refs, queries, pairs, n_pairs, mp, out, nullptr, nullptr);
+}
+
+int sk_chain_pairs_mappings(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_set* queries, const uint64_t* pairs,
+                            uint64_t n_pairs, const sk_map_params* mp, sk_ani_result* out, uint64_t* map_off, sk_mapping** maps) {
+  if (!ctx || !refs || !queries || !mp || !map_off || !maps || (n_pairs && (!pairs || !out))) return SK_ERR_PARAM;
+  *maps = nullptr;
+  sk::MapOut mo;
+  mo.count.assign(n_pairs, 0);
+  SK_TRY(sk::chain_impl(ctx, refs, queries, pairs, n_pairs, mp, out, nullptr, &mo));
+  map_off[0] = 0;
+  for (uint64_t i = 0; i < n_pairs; i++) map_off[i + 1] = map_off[i] + mo.count[i];
+  if (!mo.recs) mo.recs = (sk_mapping*)malloc(sizeof(sk_mapping));
+  if (!mo.recs) { ctx->err = "chain mappings: out of host memory"; return SK_ERR_NOMEM; }
+  *maps = mo.recs;
+  mo.recs = nullptr;
+  return SK_OK;
 }
 
 void sk_chain_debug_free(sk_chain_debug* d) {
@@ -2101,7 +2243,7 @@ int sk_chain_pairs_debug(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch
   if (n_pairs == 0) return SK_OK;
   memset(out, 0, n_pairs * sizeof(*out));
   std::vector<sk_ani_result> res(n_pairs);
-  const int rc = sk::chain_impl(ctx, refs, queries, pairs, n_pairs, mp, res.data(), out);
+  const int rc = sk::chain_impl(ctx, refs, queries, pairs, n_pairs, mp, res.data(), out, nullptr);
   if (rc != SK_OK)
     for (uint64_t i = 0; i < n_pairs; i++) sk_chain_debug_free(out + i);
   return rc;

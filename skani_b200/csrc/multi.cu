@@ -454,9 +454,10 @@ extern "C" int sk_screen_query_ref_multi(sk_ctx* const* ctxs, uint32_t n_ctx, co
   return SK_OK;
 }
 
-extern "C" int sk_chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
-                                    const sk_sketch_set* const* queries, const uint64_t* pairs, uint64_t n_pairs,
-                                    const sk_map_params* mp, sk_ani_result* out) {
+// sk_chain_pairs_multi, and with map_off / maps non-null sk_chain_pairs_multi_mappings
+static int chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
+                             const sk_sketch_set* const* queries, const uint64_t* pairs, uint64_t n_pairs,
+                             const sk_map_params* mp, sk_ani_result* out, uint64_t* map_off, sk_mapping** maps) {
   QrBlocks qb;
   SK_TRY(check_qr_args(ctxs, n_ctx, refs, ref_first, queries, mp, qb));
   if (n_pairs && (!pairs || !out)) { ctxs[0]->err = "NULL pairs / out"; return SK_ERR_PARAM; }
@@ -472,7 +473,10 @@ extern "C" int sk_chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const s
     local[d].push_back(((uint64_t)(r - ref_first[d]) << 32) | q);
     where[d].push_back(i);
   }
-  return run_per_context(ctxs, n_ctx, [&](uint32_t d) -> int {
+  const bool with_maps = map_off != nullptr;
+  std::vector<std::vector<uint64_t>> loff(n_ctx);       // mappings: each context's offsets and records, in its local order
+  std::vector<sk_mapping*> lmaps(n_ctx, nullptr);
+  const int rc = run_per_context(ctxs, n_ctx, [&](uint32_t d) -> int {
     if (local[d].empty()) return SK_OK;
     // switch_qr's file-name tie-break (src/chain.rs:19-21) as in the one set of all refs: default ranks are global ref ids,
     // and default query ranks follow all n_refs refs.  Applied on non-owning views; the caller's sets are not touched.
@@ -481,9 +485,48 @@ extern "C" int sk_chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const s
     if (!qv.ranks_user_set) for (uint32_t g = 0; g < qv.G; g++) qv.name_rank[g] += qb.n_refs;
     rv.ranks_user_set = qv.ranks_user_set = true;
     std::vector<sk_ani_result> res(local[d].size());
-    const int rc = sk_chain_pairs(ctxs[d], &rv, &qv, local[d].data(), local[d].size(), mp, res.data());
+    int rc;
+    if (with_maps) {
+      loff[d].resize(local[d].size() + 1);
+      rc = sk_chain_pairs_mappings(ctxs[d], &rv, &qv, local[d].data(), local[d].size(), mp, res.data(), loff[d].data(), &lmaps[d]);
+    } else {
+      rc = sk_chain_pairs(ctxs[d], &rv, &qv, local[d].data(), local[d].size(), mp, res.data());
+    }
     if (rc != SK_OK) return rc;
     for (size_t k = 0; k < res.size(); k++) { res[k].ref_id += ref_first[d]; out[where[d][k]] = res[k]; }
     return SK_OK;
   });
+  if (rc == SK_OK && with_maps) {
+    // records merged back into the caller's pair order
+    std::vector<uint32_t> ctx_of(n_pairs);
+    std::vector<uint64_t> k_of(n_pairs);
+    for (uint32_t d = 0; d < n_ctx; d++)
+      for (size_t k = 0; k < where[d].size(); k++) { ctx_of[where[d][k]] = d; k_of[where[d][k]] = k; }
+    map_off[0] = 0;
+    for (uint64_t i = 0; i < n_pairs; i++) map_off[i + 1] = map_off[i] + loff[ctx_of[i]][k_of[i] + 1] - loff[ctx_of[i]][k_of[i]];
+    *maps = (sk_mapping*)malloc(std::max<uint64_t>(map_off[n_pairs], 1) * sizeof(sk_mapping));
+    if (*maps)
+      for (uint64_t i = 0; i < n_pairs; i++) {
+        const uint64_t* lo = loff[ctx_of[i]].data() + k_of[i];
+        if (lo[1] > lo[0]) memcpy(*maps + map_off[i], lmaps[ctx_of[i]] + lo[0], (lo[1] - lo[0]) * sizeof(sk_mapping));
+      }
+  }
+  for (sk_mapping* m : lmaps) sk_free(m);
+  if (rc == SK_OK && with_maps && !*maps) { ctxs[0]->err = "chain mappings: out of host memory"; return SK_ERR_NOMEM; }
+  return rc;
+}
+
+extern "C" int sk_chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
+                                    const sk_sketch_set* const* queries, const uint64_t* pairs, uint64_t n_pairs,
+                                    const sk_map_params* mp, sk_ani_result* out) {
+  return chain_pairs_multi(ctxs, n_ctx, refs, ref_first, queries, pairs, n_pairs, mp, out, nullptr, nullptr);
+}
+
+extern "C" int sk_chain_pairs_multi_mappings(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs,
+                                             const uint32_t* ref_first, const sk_sketch_set* const* queries, const uint64_t* pairs,
+                                             uint64_t n_pairs, const sk_map_params* mp, sk_ani_result* out, uint64_t* map_off,
+                                             sk_mapping** maps) {
+  if (!map_off || !maps) return SK_ERR_PARAM;
+  *maps = nullptr;
+  return chain_pairs_multi(ctxs, n_ctx, refs, ref_first, queries, pairs, n_pairs, mp, out, map_off, maps);
 }

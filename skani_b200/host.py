@@ -12,6 +12,11 @@ RESULT_DTYPE = np.dtype([(n, np.float32) for n in ("ani", "af_query", "af_ref", 
                         [(n, np.uint32) for n in ("num_contigs_q", "num_contigs_r", "avg_chain_int_len", "total_bases_covered",
                                                   "ref_id", "query_id")])
 assert RESULT_DTYPE.itemsize == C.sizeof(AniResult)
+# sk_mapping: one kept chain interval of a pair in the caller's orientation, with its chunk's identity estimate
+MAPPING_DTYPE = np.dtype([(n, np.uint32) for n in ("query_contig", "ref_contig", "q0", "q1", "r0", "r1", "num_anchors", "chunk")] +
+                         [("chunk_est", np.float64), ("chunk_weight", np.uint32)] +
+                         [(n, np.uint8) for n in ("reverse", "switched", "chunk_valid", "pad")])
+assert MAPPING_DTYPE.itemsize == 48
 
 MIN_LENGTH_CONTIG = 500  # reference src/params.rs:42, applied by file_io::fastx_to_sketches (src/file_io.rs:176)
 
@@ -375,6 +380,26 @@ def chain_pairs(ctx, refs, queries, pairs, mp=None, as_array=False):
     return [AniResult.from_buffer_copy(out[i].tobytes()) for i in range(len(pairs))]
 
 
+def _mappings_out(ctx, n, off, pp):
+    m = np.frombuffer((C.c_uint8 * (int(off[n]) * 48)).from_address(pp.value), MAPPING_DTYPE).copy() \
+        if off[n] else np.zeros(0, MAPPING_DTYPE)
+    ctx.L.sk_free(pp)
+    return m
+
+
+def chain_pairs_mappings(ctx, refs, queries, pairs, mp=None):
+    """sk_chain_pairs_mappings: (results, offsets, mappings).  results is chain_pairs(..., as_array=True); pair i's records
+    are mappings[offsets[i]:offsets[i + 1]] (MAPPING_DTYPE), its kept chain intervals in the caller's orientation."""
+    mp = mp or map_params()
+    pairs = np.ascontiguousarray(pairs, np.uint64)
+    out = np.zeros(max(len(pairs), 1), RESULT_DTYPE)
+    off = np.zeros(len(pairs) + 1, np.uint64)
+    pp = C.c_void_p()
+    ctx.check(ctx.L.sk_chain_pairs_mappings(ctx.h, refs.h, queries.h, pairs.ctypes.data, len(pairs), C.byref(mp), out.ctypes.data,
+                                            off.ctypes.data, C.byref(pp)))
+    return out[:len(pairs)], off, _mappings_out(ctx, len(pairs), off, pp)
+
+
 def _multi_args(ctxs, refs, ref_first, queries):
     hs = (C.c_void_p * len(ctxs))(*[c.h for c in ctxs])
     rh = (C.c_void_p * len(ctxs))(*[None if r is None else r.h for r in refs])
@@ -406,6 +431,20 @@ def chain_pairs_multi(ctxs, refs, ref_first, queries, pairs, mp=None, as_array=F
     if as_array:
         return out
     return [AniResult.from_buffer_copy(out[i].tobytes()) for i in range(len(pairs))]
+
+
+def chain_pairs_multi_mappings(ctxs, refs, ref_first, queries, pairs, mp=None):
+    """sk_chain_pairs_multi_mappings: chain_pairs_multi plus mappings, returned as chain_pairs_mappings returns them."""
+    mp = mp or map_params()
+    hs, rh, rf, qh = _multi_args(ctxs, refs, ref_first, queries)
+    pairs = np.ascontiguousarray(pairs, np.uint64)
+    out = np.zeros(max(len(pairs), 1), RESULT_DTYPE)
+    off = np.zeros(len(pairs) + 1, np.uint64)
+    pp = C.c_void_p()
+    c0 = ctxs[0]
+    c0.check(c0.L.sk_chain_pairs_multi_mappings(hs, len(ctxs), rh, rf.ctypes.data, qh, pairs.ctypes.data, len(pairs), C.byref(mp),
+                                                out.ctypes.data, off.ctypes.data, C.byref(pp)))
+    return out[:len(pairs)], off, _mappings_out(c0, len(pairs), off, pp)
 
 
 def _debug_dict(d):
