@@ -565,7 +565,7 @@ int sk_neighbor_joining(sk_ctx* ctx, uint32_t n_genomes, const sk_ani_result* re
  * member takes its representative neighbour of highest ANI, ties to the smaller rank.
  * Refusals (SK_ERR_PARAM with a message): NULL arguments, a rank that is not a permutation, a NaN min_ani, more than
  * 2^22 - 1 representatives (or undecided genomes in one wave) in an index, or 2^31 or more markers in one.  The set must be
- * one context's in-memory set (sk_sketch_store sets are not taken).
+ * one context's in-memory set; a host sketch store goes to sk_dereplicate_store.
  * stats (may be NULL): pairs that passed a screen, pairs chained, edges among the chained rows, clusters, waves, greedy rounds,
  * and the seconds spent screening, chaining, deciding (greedy rounds and assignment) and in all. */
 typedef struct {
@@ -579,6 +579,31 @@ typedef struct {
 } sk_derep_stats;
 int sk_dereplicate(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* rank, const sk_derep_params* dp,
                    uint32_t* rep, uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats /* may be NULL */);
+
+/* sk_dereplicate_store: sk_dereplicate over every genome of a host sketch store, beyond one GPU's memory and on several GPUs.
+ * Contract: for any store (with its name ranks), mp, rank permutation, min_ani, dp->wave, device_budget and context list,
+ * rep, cluster and join are byte for byte what sk_dereplicate returns on one in-memory set holding every genome of the store
+ * with the same name ranks (join holds store genome ids), and so sk_cluster's greedy result on sk_triangle_store's rows; in
+ * stats, pairs_screened, pairs_chained, n_edges, n_clusters, waves and rounds are equal too.
+ * The markers of every genome are gathered on ctxs[0] (SK_PACK_MARKERS_ONLY), where the waves, the representative index, the
+ * screens and the greedy decisions run exactly as in sk_dereplicate.  Each chain step (a wave against the representatives,
+ * the pairs inside a wave, the final members x representatives) is planned into working sets as sk_triangle_store plans
+ * its pairs, and the contexts, on one device or several, gather and chain them; every pair is chained once, as
+ * (min << 32 | max), in a working set of ascending genome ids, and a gathered set chains exactly like the set that was added.
+ * device_budget: bytes per context (0 = derived from the free device memory after the marker gather, ctxs[0]'s device first
+ * keeping room for the representative index with every genome a representative).  A genome over budget / 2 gives SK_ERR_NOMEM
+ * (before any device work when device_budget is given).  The markers of all genomes stay on ctxs[0]'s device for the whole
+ * call (8 bytes per marker).
+ * Refusals (SK_ERR_PARAM with the message on ctxs[0]): sk_dereplicate's, plus n_ctx = 0, a NULL context and a context listed
+ * twice (n_ctx = 0 or a NULL ctxs / ctxs[0] gives SK_ERR_PARAM without a message).  If any context fails the call fails and
+ * sk_last_error(ctxs[0]) carries that context's message.  Stores of 0 and 1 genomes are valid.  SK_TRACE=1 prints one line
+ * per working set.
+ * stats (may be NULL): as sk_dereplicate's, t_chain covering gathers and chaining (wall time) and t_total the marker gather
+ * too.  store_stats (may be NULL): working sets, split components and gathered bytes summed over the chain steps, the largest
+ * working set, t_gather / t_chain summed over contexts, t_screen = the marker gather. */
+int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp, const uint32_t* rank,
+                         const sk_derep_params* dp, uint64_t device_budget, uint32_t* rep, uint32_t* cluster, sk_ani_result* join,
+                         sk_derep_stats* stats /* may be NULL */, sk_store_stats* store_stats /* may be NULL */);
 
 #ifdef __cplusplus
 }

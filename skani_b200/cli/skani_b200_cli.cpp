@@ -172,6 +172,7 @@ struct Opts {
   std::string linkage;              // cluster --linkage average|complete
   std::string dendrogram;           // cluster --dendrogram FILE
   std::string representatives;      // dereplicate --representatives FILE
+  bool host_store = false;          // dereplicate --host-store
   std::string tree_method = "nj";   // tree --method nj|average|complete
   std::string mappings;             // triangle / dist / search --mappings FILE
 };
@@ -513,10 +514,9 @@ uint64_t total_weight(const skdb::SketchInputs& si) {
 }
 
 bool triangle_needs_store(const Opts& op, bool sketches, const skdb::SketchInputs& si, double* need_gb) {
-  *need_gb = 0;
-  if (op.gpus > 1 && !sketches) return false;
   const double need = sketch_bytes_estimate(op, op.files, sketches) * (sketches ? append_peak(total_weight(si)) : 1.0) + 6.0e9;
   *need_gb = need / 1e9;
+  if (op.gpus > 1 && !sketches) return false;
   return (op.gpus > 1 && sketches) || exceeds_device(op, need);
 }
 
@@ -911,9 +911,10 @@ int run_cluster(Opts& op) {
 }
 
 // dereplicate: cluster's greedy clusters (same inputs, presets, name ranks, length ranking and TSV) from sk_dereplicate, which
-// screens and chains only genome x representative pairs instead of the whole triangle.  In-memory sets on one GPU only:
-// inputs that need the host sketch store, and --gpus N, are left to cluster.  --representatives FILE: one line per
-// representative in cluster-id order, its file name (-i: its first contig name).
+// screens and chains only genome x representative pairs instead of the whole triangle.  By default an in-memory set on one
+// GPU: inputs that need the host sketch store, and --gpus N, are refused.  --host-store takes the store path whatever the
+// input size: sketches in a host sketch store, sk_dereplicate_store on two contexts per GPU of --gpus N, the same output.
+// --representatives FILE: one line per representative in cluster-id order, its file name (-i: its first contig name).
 int run_dereplicate(Opts& op) {
   if (op.single_linkage || !op.linkage.empty() || !op.dendrogram.empty()) {
     fprintf(stderr, "ERROR --single-linkage, --linkage and --dendrogram are cluster options; dereplicate is greedy clustering only: use cluster.\n");
@@ -923,21 +924,24 @@ int run_dereplicate(Opts& op) {
     fprintf(stderr, "ERROR -E/--sparse, --full-matrix, --diagonal, --distance, --ci and --detailed are triangle output options; dereplicate does not take them.\n");
     return 2;
   }
-  if (op.gpus > 1) { fprintf(stderr, "ERROR --gpus %d: dereplicate runs on one GPU; use cluster --gpus %d.\n", op.gpus, op.gpus); return 2; }
+  if (op.gpus > 1 && !op.host_store) {
+    fprintf(stderr, "ERROR --gpus %d: dereplicate keeps the sketches on one GPU; use cluster --gpus %d, or dereplicate --host-store --gpus %d.\n", op.gpus,
+            op.gpus, op.gpus);
+    return 2;
+  }
   TriangleInputs ti;
   if (const int rc = open_triangle_inputs(op, ti)) return rc;
-  if (ti.use_store) {
+  if (ti.use_store && !op.host_store) {
     fprintf(stderr, "ERROR dereplicate keeps the sketches on the GPU, and these inputs (~%.1f GB estimated%s) need the host sketch store: use cluster, "
-            "which takes the store path.\n", ti.need_gb, device_budget() ? ", SK_DEVICE_BUDGET_MB set" : "");
+            "which takes the store path, or dereplicate --host-store.\n", ti.need_gb, device_budget() ? ", SK_DEVICE_BUDGET_MB set" : "");
     return 1;
   }
+  if (op.host_store) ti.use_store = true;
   Inputs in;
   sk_ctx* ctx = nullptr;
   if (const int rc = load_triangle_inputs(op, in, ctx, ti)) return rc;
   const sk_map_params mp = map_params(op, !op.no_learned && op.c >= 70 && !op.individual && !op.median);
   const std::vector<uint64_t> ranks = name_ranks(in.genomes)[0];
-  sk_sketch_set* set = ti.loaded ? ti.loaded : sketch(ctx, in, ti.sp);
-  sk_sketch_set_set_name_ranks(set, ranks.data());
   const uint32_t N = (uint32_t)in.genomes.size();
   const std::vector<uint32_t> rank = length_rank(in);
   std::vector<uint32_t> rep(N), cluster(N);
@@ -946,8 +950,24 @@ int run_dereplicate(Opts& op) {
   const char* w = getenv("SK_DEREP_WAVE");
   const sk_derep_params dp{(float)(op.cluster_ani / 100.0), w ? (uint32_t)std::max(1ll, atoll(w)) : 0u};
   sk_derep_stats st{};
-  CK(ctx, sk_dereplicate(ctx, set, &mp, rank.data(), &dp, rep.data(), cluster.data(), join.data(), &st));
-  sk_sketch_set_free(set);
+  sk_store_stats sst{};
+  size_t n_ctx = 1;
+  if (ti.store) {
+    // two contexts on each of the --gpus devices, as the triangle's store path: one gathers its next working set while the
+    // other chains
+    CK(ctx, sk_sketch_store_set_name_ranks(ti.store, ranks.data()));
+    std::vector<sk_ctx*> sctx = make_contexts(ctx, op, op.gpus, 2);
+    n_ctx = sctx.size();
+    CK(ctx, sk_dereplicate_store(sctx.data(), (uint32_t)sctx.size(), ti.store, &mp, rank.data(), &dp, device_budget(), rep.data(), cluster.data(),
+                                 join.data(), &st, &sst));
+    for (size_t d = sctx.size(); d-- > 1;) sk_ctx_destroy(sctx[d]);
+    sk_sketch_store_free(ti.store);
+  } else {
+    sk_sketch_set* set = ti.loaded ? ti.loaded : sketch(ctx, in, ti.sp);
+    sk_sketch_set_set_name_ranks(set, ranks.data());
+    CK(ctx, sk_dereplicate(ctx, set, &mp, rank.data(), &dp, rep.data(), cluster.data(), join.data(), &st));
+    sk_sketch_set_free(set);
+  }
   if (!write_clusters(op, in, rep, cluster, [&](uint32_t g) { return &join[g]; })) return 1;
   if (!op.representatives.empty()) {
     FILE* f = fopen(op.representatives.c_str(), "w");
@@ -960,6 +980,10 @@ int run_dereplicate(Opts& op) {
   fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (greedy), %u waves, %llu pairs screened, %llu chained; "
           "screen %.2f s, chain %.2f s, decide %.2f s, total %.2f s\n", N, st.n_clusters, op.cluster_ani, st.waves,
           (unsigned long long)st.pairs_screened, (unsigned long long)st.pairs_chained, st.t_screen, st.t_chain, st.t_decide, st.t_total);
+  if (op.host_store)
+    fprintf(stderr, "INFO Store path: %u working sets, %.2f GB gathered (largest working set %.2f GB); marker gather %.2f s, gather %.2f s, chain %.2f s "
+            "(summed over %zu contexts)\n", sst.n_working_sets, sst.gathered_bytes / 1e9, sst.max_working_set_bytes / 1e9, sst.t_screen, sst.t_gather,
+            sst.t_chain, n_ctx);
   sk_ctx_destroy(ctx);
   return 0;
 }
@@ -1615,17 +1639,19 @@ void usage() {
           "      genomes first, --single-linkage components, or --linkage average / complete (UPGMA / complete linkage of\n"
           "      100 - ANI, 100 for pairs not printed, cut at 100 - T); one TSV row per genome with its representative and\n"
           "      cluster; --dendrogram writes the linkage matrix (a b height size, heights in percent) that scipy takes\n"
-          "  skani-b200 dereplicate [fasta | sketch ... | -l list] [-i] [--ani T] [-o out] [--representatives FILE]\n"
+          "  skani-b200 dereplicate [fasta | sketch ... | -l list] [-i] [--ani T] [-o out] [--representatives FILE] [--host-store]\n"
           "      cluster's greedy clusters (same TSV), screening and chaining only genome x representative pairs instead of\n"
-          "      the whole triangle; --representatives writes one representative per line in cluster order.  One GPU, sketches\n"
-          "      in device memory (larger inputs: cluster)\n"
+          "      the whole triangle; --representatives writes one representative per line in cluster order.  By default one\n"
+          "      GPU with the sketches in device memory; --host-store keeps them in host memory and chains in working sets\n"
+          "      (inputs beyond device memory, and --gpus N), with the same output\n"
           "  skani-b200 tree [fasta | sketch ... | -l list] [-i] [--method nj|average|complete] [-o tree.nwk]\n"
           "      the triangle's genomes as a Newick tree of 100 - ANI (100 for pairs not printed), branch lengths in percent:\n"
           "      neighbour joining (default; unrooted, basal trifurcation) or the average / complete linkage dendrogram\n"
           "      (rooted, a node at half its merge height)\n"
           "  common: -c C -m M -k K -s SCREEN%% --min-af P --both-min-af P --robust --median --no-learned-ani --faster-small\n"
           "          --small-genomes --fast --medium --slow --ci --detailed --short-header --no-marker-index -t THREADS --device D\n"
-          "          --gpus N (triangle, dist, search, sketch, cluster, tree: one context per GPU, devices D, D+1, ...)\n"
+          "          --gpus N (triangle, dist, search, sketch, cluster, tree, dereplicate --host-store: one context per GPU, devices\n"
+          "          D, D+1, ...)\n"
           "  --mappings FILE (triangle, dist, search): where each printed pair aligns, one TSV row per chain interval kept by the\n"
           "          ANI estimate: contigs, 0-based half-open coordinates, strand, anchors, and the identity of the 20 kb chunk it\n"
           "          was chained in.  Pairs, order and orientation are those of the main output (triangle: those of -E).  A few\n"
@@ -1701,6 +1727,7 @@ int main(int argc, char** argv) {
     else if (a == "--linkage" && (op.cmd == "cluster" || op.cmd == "dereplicate")) op.linkage = val();
     else if (a == "--dendrogram" && (op.cmd == "cluster" || op.cmd == "dereplicate")) op.dendrogram = val();
     else if (a == "--representatives" && op.cmd == "dereplicate") op.representatives = val();
+    else if (a == "--host-store" && op.cmd == "dereplicate") op.host_store = true;
     else if (a == "--method" && op.cmd == "tree") op.tree_method = val();
     else if (a == "--mappings" && (op.cmd == "triangle" || op.cmd == "dist" || op.cmd == "search")) op.mappings = val();
     else if (a == "--keep-refs") {}   // search already loads every passing reference exactly once

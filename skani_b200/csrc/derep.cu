@@ -20,17 +20,26 @@
 // triangle's TriScreen keeps it.  dr_rows_kernel runs one block per row genome and counts shared markers per slot in
 // shared-memory tiles; every slot of a tile is then decided by the oriented predicate (dr_screen_pass), so a slot with no
 // shared marker that the rescue lets through is emitted like any other.
+//
+// sk_dereplicate_store runs the same waves over a host sketch store: the markers of every genome are gathered once on ctxs[0]
+// (the index, the row screens, the greedy rounds and the set difference run there exactly as above, on the global genome
+// indices), and each chain step's pairs are planned into working sets that the contexts gather from the store and chain, as
+// sk_triangle_store does (store_ws.hpp, ws_plan.hpp).
 #include <cub/cub.cuh>
 
 #include <algorithm>
 #include <chrono>
 #include <cmath>
+#include <cstdio>
+#include <cstdlib>
 #include <string>
 #include <vector>
 
 #include "cluster_core.cuh"
 #include "derep_core.cuh"
 #include "sk_internal.h"
+#include "store_ws.hpp"
+#include "ws_plan.hpp"
 
 using namespace sk;
 
@@ -149,16 +158,30 @@ struct Index {
 
 // a cub call run twice: sizing, then on temporaries from the arena
 template <typename F>
-int cub_run(sk_ctx* ctx, const char* what, F&& f) {
+int cub_run(sk_ctx* ctx, const char* who, const char* what, F&& f) {
   size_t tb = 0;
   SK_CUDA(f((void*)nullptr, tb));
   DTmp<uint8_t> tmp;
-  SK_TRY(cl_alloc(ctx, tmp, tb, what, WHO));
+  SK_TRY(cl_alloc(ctx, tmp, tb, what, who));
   SK_CUDA(f((void*)tmp.p, tb));
   count_launch(ctx, 1);
   return SK_OK;
 }
 
+// chain()'s host sketch store back end (sk_dereplicate_store): the sketches of every genome in a store, the contexts that
+// chain, the working-set budget per context and the sk_store_stats summed over the chain steps
+struct StoreChain {
+  sk_ctx* const* ctxs;
+  uint32_t n_ctx;
+  const sk_sketch_store* st;
+  std::vector<uint64_t> gbytes;   // sk_sketch_store_genome_bytes of every genome
+  uint64_t budget;
+  bool trace;
+  sk_store_stats stats{};
+};
+
+// set: the markers (and mk_off) of every genome, which the index, the row screens and the key offsets read; it is also what
+// chain() chains unless `store` is set, in which case set may hold the markers only (a SK_PACK_MARKERS_ONLY gather)
 struct Run {
   sk_ctx* ctx;
   const sk_sketch_set* set;
@@ -166,6 +189,8 @@ struct Run {
   float min_ani;
   double cutoff;
   uint32_t N;
+  const char* who = WHO;
+  StoreChain* store = nullptr;
   DTmp<uint64_t> d_off;
   DTmp<uint32_t> d_rank;
   DTmp<uint8_t> state;
@@ -181,30 +206,30 @@ struct Run {
     for (uint32_t i = 0; i < m; i++) kofs[i + 1] = kofs[i] + set->mk_off[list[i] + 1] - set->mk_off[list[i]];
     const uint64_t m_new = kofs[m], n_tot = ix.n + m_new;
     if ((uint64_t)ix.slots + m > DR_MAX_SLOTS) {
-      ctx->err = std::string(WHO) + ": more than 2^22 - 1 genomes (" + std::to_string((uint64_t)ix.slots + m) + ") in one marker index"; return SK_ERR_PARAM;
+      ctx->err = std::string(who) + ": more than 2^22 - 1 genomes (" + std::to_string((uint64_t)ix.slots + m) + ") in one marker index"; return SK_ERR_PARAM;
     }
     if (n_tot >= DR_MAX_KEYS) {
-      ctx->err = std::string(WHO) + ": " + std::to_string(n_tot) + " markers in one marker index (at most 2^31 - 1)"; return SK_ERR_PARAM;
+      ctx->err = std::string(who) + ": " + std::to_string(n_tot) + " markers in one marker index (at most 2^31 - 1)"; return SK_ERR_PARAM;
     }
     SK_CUDA(cudaMemcpyAsync(ix.slot_genome.p + ix.slots, d_list, (size_t)m * 4, cudaMemcpyDeviceToDevice, s));
     if (m_new) {
       DTmp<uint64_t> d_kofs, nk, snk;
-      SK_TRY(cl_alloc(ctx, d_kofs, m + 1, "key offsets", WHO));
-      SK_TRY(cl_alloc(ctx, nk, m_new, "index keys", WHO));
-      SK_TRY(cl_alloc(ctx, snk, m_new, "index keys", WHO));
+      SK_TRY(cl_alloc(ctx, d_kofs, m + 1, "key offsets", who));
+      SK_TRY(cl_alloc(ctx, nk, m_new, "index keys", who));
+      SK_TRY(cl_alloc(ctx, snk, m_new, "index keys", who));
       SK_CUDA(h2d_small(ctx, d_kofs.p, kofs.data(), (size_t)(m + 1) * 8));
       dr_keys_kernel<<<m, 256, 0, s>>>(set->markers, d_off.p, d_list, d_kofs.p, ix.slots, nk.p);
       count_launch(ctx, 1);
       SK_CUDA(cudaGetLastError());
-      SK_TRY(cub_run(ctx, "index sort", [&](void* t, size_t& tb) {
+      SK_TRY(cub_run(ctx, who, "index sort", [&](void* t, size_t& tb) {
         return cub::DeviceRadixSort::SortKeys(t, tb, nk.p, snk.p, (int)m_new, 0, 64, s); }));
       DTmp<uint64_t>& dst = ix.key[ix.cur ^ 1];
-      SK_TRY(cl_alloc(ctx, dst, n_tot, "marker index", WHO));
+      SK_TRY(cl_alloc(ctx, dst, n_tot, "marker index", who));
       if (!ix.n) {
         SK_CUDA(cudaMemcpyAsync(dst.p, snk.p, m_new * 8, cudaMemcpyDeviceToDevice, s));
       } else {   // keys are distinct (marker, slot) pairs: the merge has one possible output
         const uint64_t* old = ix.key[ix.cur].p;
-        SK_TRY(cub_run(ctx, "index merge", [&](void* t, size_t& tb) {
+        SK_TRY(cub_run(ctx, who, "index merge", [&](void* t, size_t& tb) {
           return cub::DeviceMerge::MergeKeys(t, tb, old, (int)ix.n, snk.p, (int)m_new, dst.p, ::cuda::std::less<uint64_t>{}, s); }));
       }
       ix.cur ^= 1;
@@ -230,9 +255,9 @@ struct Run {
     unsigned long long cap = std::max<unsigned long long>(1ull << 20, 64ull * n_rows), n = 0;
     DTmp<unsigned long long> d_n;
     DTmp<uint64_t> d_pairs;
-    SK_TRY(cl_alloc(ctx, d_n, 1, "pair count", WHO));
+    SK_TRY(cl_alloc(ctx, d_n, 1, "pair count", who));
     for (int attempt = 0; attempt < 2; attempt++) {
-      SK_TRY(cl_alloc(ctx, d_pairs, cap, "screened pairs", WHO));
+      SK_TRY(cl_alloc(ctx, d_pairs, cap, "screened pairs", who));
       SK_CUDA(cudaMemsetAsync(d_n.p, 0, 8, s));
       SK_LAUNCH(ctx, "dr_rows_kernel", (dr_rows_kernel<<<n_rows, 256, (size_t)tile * 4, s>>>(
           set->markers, d_off.p, d_rows, ix.key[ix.cur].p, ix.n, ix.bucket.p, ix.slot_genome.p, ix.slots, upper, mp->rescue_small, cutoff,
@@ -243,8 +268,8 @@ struct Run {
       if (n <= cap) break;
       cap = n;
     }
-    SK_TRY(cl_alloc(ctx, out, n, "screened pairs", WHO));
-    if (n) SK_TRY(cub_run(ctx, "pair sort", [&](void* t, size_t& tb) {
+    SK_TRY(cl_alloc(ctx, out, n, "screened pairs", who));
+    if (n) SK_TRY(cub_run(ctx, who, "pair sort", [&](void* t, size_t& tb) {
       return cub::DeviceRadixSort::SortKeys(t, tb, d_pairs.p, out.p, (int)n, 0, 64, s); }));
     SK_CUDA(cudaStreamSynchronize(s));
     *n_out = n;
@@ -253,7 +278,8 @@ struct Run {
     return SK_OK;
   }
 
-  // d_pairs[0 .. n) (device) chained as the triangle chains them; the rows are appended to `rows`, the first at *first
+  // d_pairs[0 .. n) (device, sorted) chained as the triangle chains them; the rows are appended to `rows`, the first at *first,
+  // row i of the step being pair i's whatever its ani
   int chain(const uint64_t* d_pairs, uint64_t n, size_t* first) {
     *first = rows.size();
     if (!n) return SK_OK;
@@ -262,21 +288,72 @@ struct Run {
     SK_CUDA(cudaMemcpyAsync(pairs.data(), d_pairs, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
     SK_CUDA(cudaStreamSynchronize(ctx->stream));
     rows.resize(*first + n);
-    SK_TRY(sk_chain_pairs(ctx, set, set, pairs.data(), n, mp, rows.data() + *first));
+    if (store) SK_TRY(chain_store(pairs, rows.data() + *first));
+    else SK_TRY(sk_chain_pairs(ctx, set, set, pairs.data(), n, mp, rows.data() + *first));
     chained.insert(chained.end(), pairs.begin(), pairs.end());
     st.pairs_chained += n;
     st.t_chain += secs(t0);
     return SK_OK;
   }
 
+  // The store back end: the step's sorted pairs planned into working sets (ws_plan.hpp) that the contexts gather and chain
+  // (run_working_sets), as sk_triangle_store does.  Each pair is in exactly one working set and its row goes to the pair's
+  // position in out, so the contexts never write the same row and out does not depend on which context chained what.
+  int chain_store(const std::vector<uint64_t>& pairs, sk_ani_result* out) {
+    StoreChain& sc = *store;
+    skws::Plan plan;
+    std::string perr;
+    if (!skws::plan_working_sets(pairs, sc.gbytes, sc.budget, plan, perr)) { ctx->err = std::string(who) + ": " + perr; return SK_ERR_NOMEM; }
+    auto work = [&](sk_ctx* c, uint32_t d, size_t w, std::vector<sk_ani_result>&, WsTimes& t) {
+      const skws::WorkingSet& ws = plan.sets[w];
+      const auto a = clk::now();
+      sk_sketch_set* wset = nullptr;
+      int rc = sk_sketch_store_gather(c, sc.st, ws.genomes.data(), (uint32_t)ws.genomes.size(), 0, &wset);
+      const double tg = secs(a);
+      const auto b = clk::now();
+      if (rc == SK_OK) {
+        std::vector<uint64_t> lp(ws.pairs.size());
+        for (size_t i = 0; i < lp.size(); i++) {
+          const uint64_t x = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)(ws.pairs[i] >> 32)) - ws.genomes.begin();
+          const uint64_t y = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)ws.pairs[i]) - ws.genomes.begin();
+          lp[i] = (x << 32) | y;
+        }
+        std::vector<sk_ani_result> res(lp.size());
+        rc = sk_chain_pairs(c, wset, wset, lp.data(), lp.size(), mp, res.data());
+        if (rc == SK_OK)
+          for (size_t i = 0; i < res.size(); i++) {
+            sk_ani_result r = res[i];
+            r.ref_id = ws.genomes[r.ref_id];
+            r.query_id = ws.genomes[r.query_id];
+            out[std::lower_bound(pairs.begin(), pairs.end(), ws.pairs[i]) - pairs.begin()] = r;
+          }
+      }
+      if (wset) sk_sketch_set_free(wset);
+      const double tc = secs(b);
+      t.gather += tg; t.chain += tc; t.bytes += ws.bytes;
+      if (sc.trace)
+        fprintf(stderr, "[%s] context %u: working set %zu/%zu%s: %zu genomes, %zu pairs, %.1f MB gathered in %.1f ms, chain %.1f ms\n", who, d, w + 1,
+                plan.sets.size(), ws.chunk_pair ? " (chunk pair)" : "", ws.genomes.size(), ws.pairs.size(), ws.bytes / 1e6, tg * 1e3, tc * 1e3);
+      return rc;
+    };
+    std::vector<sk_ani_result> none;   // every row is written in place: the contexts keep nothing
+    WsTimes t;
+    SK_TRY(run_working_sets(sc.ctxs, sc.n_ctx, plan.sets.size(), work, none, t));
+    sc.stats.n_working_sets += (uint32_t)plan.sets.size();
+    sc.stats.n_split_components += plan.n_split_components;
+    for (auto& ws : plan.sets) sc.stats.max_working_set_bytes = std::max(sc.stats.max_working_set_bytes, ws.bytes);
+    sc.stats.gathered_bytes += t.bytes; sc.stats.t_gather += t.gather; sc.stats.t_chain += t.chain;
+    return SK_OK;
+  }
+
   // the genomes of list[0 .. m) (device) in state s, order kept, into out; their count
   int select(const uint32_t* list, uint32_t m, uint8_t s, DTmp<uint32_t>& out, uint32_t* n_out) {
     DTmp<uint32_t> d_m;
-    SK_TRY(cl_alloc(ctx, out, m, "genome list", WHO));
-    SK_TRY(cl_alloc(ctx, d_m, 1, "genome count", WHO));
+    SK_TRY(cl_alloc(ctx, out, m, "genome list", who));
+    SK_TRY(cl_alloc(ctx, d_m, 1, "genome count", who));
     *n_out = 0;
     if (!m) return SK_OK;
-    SK_TRY(cub_run(ctx, "genome selection", [&](void* t, size_t& tb) {
+    SK_TRY(cub_run(ctx, who, "genome selection", [&](void* t, size_t& tb) {
       return cub::DeviceSelect::If(t, tb, list, out.p, d_m.p, (int)m, HasState{state.p, s}, ctx->stream); }));
     SK_CUDA(cudaMemcpyAsync(n_out, d_m.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
     SK_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -298,12 +375,12 @@ struct Run {
     for (uint32_t g = 0; g < N; g++) order[rank[g]] = g;
     DTmp<uint32_t> d_order;
     Index reps;
-    SK_TRY(cl_alloc(ctx, d_off, (uint64_t)N + 1, "marker offsets", WHO));
-    SK_TRY(cl_alloc(ctx, d_rank, N, "ranks", WHO));
-    SK_TRY(cl_alloc(ctx, d_order, N, "rank order", WHO));
-    SK_TRY(cl_alloc(ctx, state, N, "states", WHO));
-    SK_TRY(cl_alloc(ctx, reps.bucket, (1u << DR_PREFIX_BITS) + 1, "index buckets", WHO));
-    SK_TRY(cl_alloc(ctx, reps.slot_genome, N, "index slots", WHO));
+    SK_TRY(cl_alloc(ctx, d_off, (uint64_t)N + 1, "marker offsets", who));
+    SK_TRY(cl_alloc(ctx, d_rank, N, "ranks", who));
+    SK_TRY(cl_alloc(ctx, d_order, N, "rank order", who));
+    SK_TRY(cl_alloc(ctx, state, N, "states", who));
+    SK_TRY(cl_alloc(ctx, reps.bucket, (1u << DR_PREFIX_BITS) + 1, "index buckets", who));
+    SK_TRY(cl_alloc(ctx, reps.slot_genome, N, "index slots", who));
     SK_CUDA(cudaMemsetAsync(reps.bucket.p, 0, ((1u << DR_PREFIX_BITS) + 1) * 4, s));
     SK_CUDA(h2d_small(ctx, d_off.p, set->mk_off.data(), ((size_t)N + 1) * 8));
     SK_CUDA(h2d_small(ctx, d_rank.p, rank, (size_t)N * 4));
@@ -322,7 +399,7 @@ struct Run {
       const auto t_mark = clk::now();
       if (np) {
         DTmp<sk_ani_result> d_res;
-        SK_TRY(cl_alloc(ctx, d_res, np, "chained rows", WHO));
+        SK_TRY(cl_alloc(ctx, d_res, np, "chained rows", who));
         SK_TRY(upload_runs(ctx, (uint8_t*)d_res.p, {{(const uint8_t*)(rows.data() + first), np * sizeof(sk_ani_result)}}, false));
         dr_mark_kernel<<<blocks_for(np), TPB, 0, s>>>(d_res.p, np, min_ani, state.p);
         count_launch(ctx, 1);
@@ -338,8 +415,8 @@ struct Run {
       SK_TRY(to_host(d_u, nu, u));
       {
         Index ui;
-        SK_TRY(cl_alloc(ctx, ui.bucket, (1u << DR_PREFIX_BITS) + 1, "index buckets", WHO));
-        SK_TRY(cl_alloc(ctx, ui.slot_genome, nu, "index slots", WHO));
+        SK_TRY(cl_alloc(ctx, ui.bucket, (1u << DR_PREFIX_BITS) + 1, "index buckets", who));
+        SK_TRY(cl_alloc(ctx, ui.slot_genome, nu, "index slots", who));
         SK_CUDA(cudaMemsetAsync(ui.bucket.p, 0, ((1u << DR_PREFIX_BITS) + 1) * 4, s));
         const auto t0 = clk::now();
         SK_TRY(index_add(ui, u.data(), d_u.p, nu));
@@ -351,8 +428,8 @@ struct Run {
       const auto t_greedy = clk::now();
       {
         Graph g;
-        SK_TRY(build_graph(ctx, WHO, N, rows.data() + first, np, min_ani, g));
-        SK_TRY(greedy_rounds(ctx, WHO, d_u.p, nu, g, d_rank.p, state.p, &st.rounds));
+        SK_TRY(build_graph(ctx, who, N, rows.data() + first, np, min_ani, g));
+        SK_TRY(greedy_rounds(ctx, who, d_u.p, nu, g, d_rank.p, state.p, &st.rounds));
       }
       // 3. the new representatives join the index
       DTmp<uint32_t> d_new;
@@ -378,11 +455,11 @@ struct Run {
       std::sort(done.begin(), done.end());
       DTmp<uint64_t> d_done;
       DTmp<unsigned long long> d_nf;
-      SK_TRY(cl_alloc(ctx, d_done, done.size(), "chained pairs", WHO));
-      SK_TRY(cl_alloc(ctx, fresh, np, "pairs to chain", WHO));
-      SK_TRY(cl_alloc(ctx, d_nf, 1, "pair count", WHO));
+      SK_TRY(cl_alloc(ctx, d_done, done.size(), "chained pairs", who));
+      SK_TRY(cl_alloc(ctx, fresh, np, "pairs to chain", who));
+      SK_TRY(cl_alloc(ctx, d_nf, 1, "pair count", who));
       if (!done.empty()) SK_CUDA(cudaMemcpyAsync(d_done.p, done.data(), done.size() * 8, cudaMemcpyHostToDevice, s));
-      SK_TRY(cub_run(ctx, "set difference", [&](void* t, size_t& tb) {
+      SK_TRY(cub_run(ctx, who, "set difference", [&](void* t, size_t& tb) {
         return cub::DeviceSelect::If(t, tb, pairs.p, fresh.p, d_nf.p, (int)np, NotChained{d_done.p, done.size()}, s); }));
       unsigned long long h = 0;
       SK_CUDA(cudaMemcpyAsync(&h, d_nf.p, 8, cudaMemcpyDeviceToHost, s));
@@ -397,17 +474,17 @@ struct Run {
     // the assignment over every chained row, representatives numbered in rank order
     const auto t_assign = clk::now();
     Graph g;
-    SK_TRY(build_graph(ctx, WHO, N, rows.data(), rows.size(), min_ani, g));
+    SK_TRY(build_graph(ctx, who, N, rows.data(), rows.size(), min_ani, g));
     DTmp<uint32_t> d_rep, d_cluster, flag;
     DTmp<uint64_t> d_edge;
-    SK_TRY(cl_alloc(ctx, d_rep, N, "representatives", WHO));
-    SK_TRY(cl_alloc(ctx, d_cluster, N, "clusters", WHO));
-    SK_TRY(cl_alloc(ctx, flag, N, "flags", WHO));
-    SK_TRY(cl_alloc(ctx, d_edge, N, "edges per genome", WHO));
+    SK_TRY(cl_alloc(ctx, d_rep, N, "representatives", who));
+    SK_TRY(cl_alloc(ctx, d_cluster, N, "clusters", who));
+    SK_TRY(cl_alloc(ctx, flag, N, "flags", who));
+    SK_TRY(cl_alloc(ctx, d_edge, N, "edges per genome", who));
     SK_TRY(greedy_assign(ctx, N, g, d_rank.p, state.p, d_rep.p, d_edge.p, flag.p));
     std::vector<uint32_t> h_rep(N), h_cluster(N);   // read back here first: the caller's outputs may alias each other
     std::vector<uint64_t> edge(N);
-    SK_TRY(number_and_read_back(ctx, WHO, N, d_rank.p, d_rep.p, d_edge.p, flag.p, d_cluster.p, h_rep.data(), h_cluster.data(), edge.data(),
+    SK_TRY(number_and_read_back(ctx, who, N, d_rank.p, d_rep.p, d_edge.p, flag.p, d_cluster.p, h_rep.data(), h_cluster.data(), edge.data(),
                                 &st.n_clusters));
     st.t_decide += secs(t_assign);
     st.n_edges = g.E;
@@ -417,7 +494,7 @@ struct Run {
         join[v].ani = NAN;
         join[v].ref_id = join[v].query_id = v;
       } else if (edge[v] == UINT64_MAX) {
-        ctx->err = std::string(WHO) + ": member " + std::to_string(v) + " has no chained row to its representative";
+        ctx->err = std::string(who) + ": member " + std::to_string(v) + " has no chained row to its representative";
         return SK_ERR_STATE;
       } else {
         join[v] = rows[edge[v]];
@@ -444,5 +521,83 @@ int sk_dereplicate(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* m
   const uint32_t wave = std::min(dp->wave, DR_MAX_SLOTS);
   const int rc = r.run(rank, wave, rep, cluster, join);
   if (rc == SK_OK && stats) *stats = r.st;
+  return rc;
+}
+
+namespace {
+
+const char* const WHO_STORE = "sk_dereplicate_store";
+
+// sk_dereplicate_store's working-set budget per context when device_budget is 0 (after the marker set is on ctxs[0]):
+// working_set_budget's, except that ctxs[0]'s device first keeps room for the representative index at its largest (every
+// genome a representative): two key buffers of 8 bytes per marker, the new keys and their sorted copy, the sort's
+// temporaries, the per-genome arrays, and 64 MiB for the screens' pair buffers and the buckets
+int derep_store_budget(sk_ctx* const* ctxs, uint32_t n_ctx, uint64_t n_markers, uint32_t n_genomes, uint64_t* budget) {
+  sk_ctx* ctx = ctxs[0];
+  SK_TRY(working_set_budget(ctxs, n_ctx, 0, budget));
+  const double reserve = 5.0 * 8.0 * (double)n_markers + 32.0 * n_genomes + (64ull << 20);
+  uint32_t same = 0;
+  for (uint32_t d = 0; d < n_ctx; d++) same += ctxs[d]->device == ctx->device;
+  size_t free_b = 0, total_b = 0;
+  SK_CUDA(cudaSetDevice(ctx->device));
+  SK_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  const double left = std::max(0.0, (double)free_b - reserve);
+  *budget = std::min<uint64_t>(*budget, (uint64_t)(0.8 * left / (3.0 * same)));
+  return SK_OK;
+}
+
+// a genome over budget / 2 cannot be placed in every chunk pair of a working-set plan
+int check_genome_bytes(sk_ctx* ctx, const std::vector<uint64_t>& gbytes, uint64_t budget) {
+  for (size_t g = 0; g < gbytes.size(); g++)
+    if (gbytes[g] > budget / 2) {
+      ctx->err = std::string(WHO_STORE) + ": genome " + std::to_string(g) + " needs " + std::to_string(gbytes[g]) +
+                 " device bytes, more than half the working-set budget of " + std::to_string(budget) + " bytes";
+      return SK_ERR_NOMEM;
+    }
+  return SK_OK;
+}
+
+}  // namespace
+
+int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp, const uint32_t* rank,
+                         const sk_derep_params* dp, uint64_t device_budget, uint32_t* rep, uint32_t* cluster, sk_ani_result* join,
+                         sk_derep_stats* stats, sk_store_stats* store_stats) {
+  if (!ctxs || n_ctx == 0 || !ctxs[0]) return SK_ERR_PARAM;
+  sk_ctx* ctx = ctxs[0];
+  const uint32_t N = sk_sketch_store_n_genomes(st);
+  if (!st || !mp || !dp || !rep || !cluster || !join || (N && !rank)) { ctx->err = std::string(WHO_STORE) + ": NULL argument"; return SK_ERR_PARAM; }
+  SK_TRY(check_contexts(ctxs, n_ctx));
+  if (std::isnan(dp->min_ani)) { ctx->err = std::string(WHO_STORE) + ": min_ani is NaN"; return SK_ERR_PARAM; }
+  const std::string bad = rank_error(N, rank);
+  if (!bad.empty()) { ctx->err = std::string(WHO_STORE) + ": " + bad; return SK_ERR_PARAM; }
+  StoreChain sc{ctxs, n_ctx, st, std::vector<uint64_t>(N), device_budget, getenv("SK_TRACE") != nullptr};
+  for (uint32_t g = 0; g < N; g++) sc.gbytes[g] = sk_sketch_store_genome_bytes(st, g);
+  if (device_budget) SK_TRY(check_genome_bytes(ctx, sc.gbytes, device_budget));   // before any device work
+  if (N == 0) {   // what sk_dereplicate returns for an empty set: no wave, no pair, no cluster
+    if (stats) *stats = sk_derep_stats{};
+    if (store_stats) *store_stats = sk_store_stats{};
+    return SK_OK;
+  }
+  // the markers of every genome on ctxs[0]
+  SK_CUDA(cudaSetDevice(ctx->device));
+  const auto t0 = clk::now();
+  std::vector<uint32_t> all(N);
+  for (uint32_t g = 0; g < N; g++) all[g] = g;
+  sk_sketch_set* mk = nullptr;
+  SK_TRY(sk_sketch_store_gather(ctx, st, all.data(), N, SK_PACK_MARKERS_ONLY, &mk));
+  sc.stats.t_screen = secs(t0);
+  int rc = SK_OK;
+  if (!device_budget) {
+    rc = derep_store_budget(ctxs, n_ctx, mk->mk_off[N], N, &sc.budget);
+    if (rc == SK_OK) rc = check_genome_bytes(ctx, sc.gbytes, sc.budget);
+  }
+  if (rc == SK_OK) {
+    Run r{ctx, mk, mp, dp->min_ani, screen_cutoff(mp), N, WHO_STORE, &sc};
+    rc = r.run(rank, std::min(dp->wave, DR_MAX_SLOTS), rep, cluster, join);
+    r.st.t_total += sc.stats.t_screen;
+    if (rc == SK_OK && stats) *stats = r.st;
+  }
+  sk_sketch_set_free(mk);
+  if (rc == SK_OK && store_stats) *store_stats = sc.stats;
   return rc;
 }

@@ -781,3 +781,25 @@ def dereplicate(ctx, sset, rank, min_ani=0.95, mp=None, wave=0):
     ctx.check(ctx.L.sk_dereplicate(ctx.h, sset.h, C.byref(mp), rk.ctypes.data if n else None, C.byref(dp), rep.ctypes.data,
                                    cl.ctypes.data, join.ctypes.data, C.byref(st)))
     return rep[:n], cl[:n], join[:n], st
+
+
+def dereplicate_store(ctxs, store, rank, min_ani=0.95, mp=None, wave=0, device_budget=0):
+    """sk_dereplicate_store: dereplicate() over every genome of a SketchStore, with rep, cluster and join byte for byte what
+    dereplicate() returns on one in-memory set of the same genomes and name ranks.  The markers are gathered on ctxs[0]; each
+    chain step's pairs are chained in working sets of at most device_budget bytes per context (0 = derived from free device
+    memory).  ctxs: one Context or a list (two on one device overlap gather and chain).  Returns (rep, cluster, join, stats,
+    store_stats): stats the sk_derep_stats struct, store_stats the StoreStats summed over the chain steps."""
+    ctxs = list(ctxs) if isinstance(ctxs, (list, tuple)) else [ctxs]
+    mp = mp or map_params()
+    n = store.n_genomes()
+    rk = np.ascontiguousarray(rank, np.uint32)
+    if len(rk) != n:
+        raise ValueError("rank needs one entry per genome")
+    m = max(n, 1)
+    rep = np.zeros(m, np.uint32); cl = np.zeros(m, np.uint32); join = np.zeros(m, RESULT_DTYPE)
+    dp = DerepParams(float(min_ani), int(wave)); st = DerepStats(); sst = StoreStats()
+    hs = (C.c_void_p * len(ctxs))(*[c.h for c in ctxs])
+    c0 = ctxs[0]
+    c0.check(c0.L.sk_dereplicate_store(hs, len(ctxs), store.h, C.byref(mp), rk.ctypes.data if n else None, C.byref(dp), int(device_budget),
+                                       rep.ctypes.data, cl.ctypes.data, join.ctypes.data, C.byref(st), C.byref(sst)))
+    return rep[:n], cl[:n], join[:n], st, sst

@@ -9,8 +9,14 @@ card's name and power limit read in the same call.
    joining row byte-identical.  Pairs chained by each side are printed.
 2. End to end: `cluster` against `dereplicate` on the same sets written as one FASTA file per genome, alternated --reps
    times (wall time of the process); stdout must be identical.
+3. --host-store (instead of 1 and 2): sk_dereplicate on the in-memory set against sk_dereplicate_store on a host sketch
+   store of the same genomes (sketched in four groups, each added and freed), with one context, two contexts on one device
+   (derived budgets) and two contexts with a budget of about one family's bytes (many working sets).  Families of 20 and of
+   200.  rep, cluster and join must be byte-identical.  Each row prints the pairs chained, the working sets, the bytes
+   gathered, and how the time splits: the marker gather, the screens on ctxs[0] (t_screen), the chain steps (t_chain, wall
+   time of gathers plus chaining) and the gather / chain seconds summed over the contexts.
 
-  python tools/bench_dereplicate.py [--genomes 2000] [--length 1000000] [--reps 3] [--skip-e2e] [--json OUT]
+  python tools/bench_dereplicate.py [--genomes 2000] [--length 1000000] [--reps 3] [--skip-e2e] [--host-store] [--json OUT]
 The FASTA files go to a temporary directory that is removed at the end."""
 import argparse
 import json
@@ -79,6 +85,58 @@ def bench_lib(n, L, G, reps, sink):
     return equal
 
 
+def bench_store(n, L, G, reps, sink):
+    import skani_b200 as sk
+    ctxs = [sk.Context(0), sk.Context(0)]
+    bases, off, goc = family_set(n, L, G, 20261018)
+    s = sk.sketch_contigs(ctxs[0], bases, off, goc, n)
+    s.set_name_ranks(np.arange(n))
+    st = sk.SketchStore()
+    bounds = np.linspace(0, n, 5).astype(int)
+    for a, b in zip(bounds[:-1], bounds[1:]):
+        idx = np.nonzero((goc >= a) & (goc < b))[0]
+        lo, hi = int(off[idx[0]]), int(off[idx[-1] + 1])
+        part = sk.sketch_contigs(ctxs[0], bases[lo:hi], off[idx[0]:idx[-1] + 2] - off[idx[0]], goc[idx] - a, b - a)
+        st.add(part)
+        part.free()
+    st.set_name_ranks(np.arange(n))
+    total = np.bincount(goc, weights=np.diff(off).astype(np.float64), minlength=n)
+    order = np.lexsort((np.arange(n), -total))
+    rank = np.empty(n, np.uint32); rank[order] = np.arange(n)
+    mp = sk.map_params()
+    gb = np.array([st.genome_bytes(g) for g in range(n)])
+    small = int(max(1.05 * G * gb.max(), 2 * gb.max() + 1))
+    runs = {"in_memory": lambda: sk.dereplicate(ctxs[0], s, rank, min_ani=0.95, mp=mp),
+            "store_1ctx": lambda: sk.dereplicate_store(ctxs[:1], st, rank, min_ani=0.95, mp=mp),
+            "store_2ctx": lambda: sk.dereplicate_store(ctxs, st, rank, min_ani=0.95, mp=mp),
+            "store_2ctx_small_budget": lambda: sk.dereplicate_store(ctxs, st, rank, min_ani=0.95, mp=mp, device_budget=small)}
+    last = {k: f() for k, f in runs.items()}              # warm-up, and the equality check
+    ref = last["in_memory"]
+    equal = all(np.array_equal(v[0], ref[0]) and np.array_equal(v[1], ref[1]) and v[2].tobytes() == ref[2].tobytes() for v in last.values())
+    times = {k: [] for k in runs}
+    for _ in range(reps):
+        for k, f in runs.items():
+            t = time.perf_counter(); last[k] = f(); times[k].append(time.perf_counter() - t)
+    for k in runs:
+        dst = last[k][3]
+        rec = {"bench": "host_store", "run": k, "genomes": n, "length": L, "family": G, "card": card(), "equal": equal,
+               "clusters": int(dst.n_clusters), "pairs_chained": int(dst.pairs_chained), "pairs_screened": int(dst.pairs_screened),
+               "waves": int(dst.waves), "t_s": sorted(times[k]),
+               "derep_split_s": {"screen": dst.t_screen, "chain": dst.t_chain, "decide": dst.t_decide, "total": dst.t_total}}
+        if k != "in_memory":
+            sst = last[k][4]
+            rec.update({"device_budget": small if k.endswith("small_budget") else 0, "working_sets": int(sst.n_working_sets),
+                        "split_components": int(sst.n_split_components), "gathered_bytes": int(sst.gathered_bytes),
+                        "max_working_set_bytes": int(sst.max_working_set_bytes), "store_bytes": int(gb.sum()),
+                        "store_split_s": {"marker_gather": sst.t_screen, "gather_summed": sst.t_gather, "chain_summed": sst.t_chain}})
+        emit(rec, sink)
+    st.free()
+    s.free()
+    for c in ctxs:
+        c.close()
+    return equal
+
+
 def write_fasta(d, n, L, G):
     bases, off, goc = family_set(n, L, G, 20261018)
     files = []
@@ -122,12 +180,17 @@ def main():
     ap.add_argument("--length", type=int, default=1_000_000)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--host-store", action="store_true", help="in-memory dereplicate against dereplicate_store only")
     ap.add_argument("--json")
     a = ap.parse_args()
     sink, ok = [], True
-    for G in (20, 200):
-        ok &= bench_lib(a.genomes, a.length, G, a.reps, sink)
-    if not a.skip_e2e:
+    if a.host_store:
+        for G in (20, 200):
+            ok &= bench_store(a.genomes, a.length, G, a.reps, sink)
+    else:
+        for G in (20, 200):
+            ok &= bench_lib(a.genomes, a.length, G, a.reps, sink)
+    if not a.skip_e2e and not a.host_store:
         for G in (20, 200):
             ok &= bench_e2e(a.genomes, a.length, G, a.reps, sink)
     if a.json:
