@@ -31,7 +31,7 @@ uint64_t count_launch(sk_ctx* ctx, uint64_t n) {
 // kernels
 // ------------------------------------------------------------------------------------------------------------
 constexpr int PACK_THREADS = 256;
-constexpr uint32_t UCOARSE_SHIFT = 8;   // host-built index: contig of every 256th unit (4 B per 8 KB of sequence)
+constexpr uint32_t UCOARSE_SHIFT = 8;   // coarse index: contig of every 256th unit (4 B per 8 KB of sequence)
 
 // contig lookup for a unit: narrowed binary search over the unit prefix offsets
 __device__ __forceinline__ uint32_t find_contig(const uint32_t* __restrict__ cuoff, uint32_t u, uint32_t lo_hint, uint32_t hi_hint) {
@@ -47,6 +47,21 @@ __device__ __forceinline__ uint32_t find_contig(const uint32_t* __restrict__ cuo
 __device__ __forceinline__ uint32_t contig_of_unit(const uint32_t* __restrict__ ucoarse, const uint32_t* __restrict__ cuoff, uint32_t u) {
   const uint32_t lo = __ldg(ucoarse + (u >> UCOARSE_SHIFT)), hi = __ldg(ucoarse + (u >> UCOARSE_SHIFT) + 1) + 1;
   return find_contig(cuoff, u, lo, hi);
+}
+
+// the coarse unit -> contig index: entry j = the last contig starting at or before unit j << UCOARSE_SHIFT (n_contigs >= 1).
+// Built on the device from cuoff: on the host, the 4 bytes per 8 KB of sequence cost a fresh, page-faulting buffer and a
+// copy in every sub-batch while the device waits for its first launch.
+__global__ void ucoarse_kernel(const uint32_t* __restrict__ cuoff, uint32_t n_contigs, uint32_t n, uint32_t* __restrict__ ucoarse) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint64_t u = (uint64_t)j << UCOARSE_SHIFT;
+  uint32_t lo = 0, hi = n_contigs;      // invariant: cuoff[lo] <= u, and the answer is below hi
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (cuoff[mid] <= u) lo = mid; else hi = mid;
+  }
+  ucoarse[j] = lo;
 }
 
 // ASCII -> 2-bit units + N mask for the units [u_begin, n_units) of a sub-batch (the units before u_begin arrived packed
@@ -153,36 +168,116 @@ hashpass_kernel(const uint64_t* __restrict__ P, const uint32_t* __restrict__ NM,
   else PM[u] = unit_pass_mask_var<V>(lo, hi, nlo, nhi, n, ul, (uint32_t)seed_mask, threshold, c24, c14, c28);
 }
 
-// one thread per unit with a non-empty pass mask: regenerate the few passing windows and emit their records
-__global__ void __launch_bounds__(256)
-expand_kernel(const uint64_t* __restrict__ P, const uint32_t* __restrict__ ucoarse, const uint32_t* __restrict__ cuoff,
-              const uint32_t* __restrict__ clocal, uint32_t n_units, const uint32_t* __restrict__ PM,
-              const uint32_t* __restrict__ uoff, uint64_t seed_mask, uint64_t threshold_marker,
-              uint32_t* __restrict__ pv_kmer, uint32_t* __restrict__ pv_pos, uint32_t* __restrict__ pv_cc,
-              uint64_t* __restrict__ mkv) {
-  uint32_t u = blockIdx.x * 256 + threadIdx.x;
-  if (u >= n_units) return;
-  uint32_t pass = PM[u];
-  if (pass == 0) return;
-  uint32_t ci = contig_of_unit(ucoarse, cuoff, u);
-  uint32_t ul = u - cuoff[ci];
-  uint64_t hi = P[u];
-  uint64_t lo = ul ? P[u - 1] : 0ull;
-  WindowCtx w = make_window_ctx(lo, hi);
-  uint32_t o = uoff[u];
-  uint32_t cl = clocal[ci];
-  while (pass) {
-    uint32_t j = __ffs(pass) - 1;
-    pass &= pass - 1;
-    bool canon;
-    uint32_t seed = window_seed(w, j, seed_mask, &canon);
-    pv_kmer[o] = seed;
-    pv_pos[o] = 32u * ul + j;                       // index of the window's last base (src/avx2_seeding.rs:184,207)
-    pv_cc[o] = (cl << 1) | (canon ? 1u : 0u);       // SeedPosition::new (src/types.rs:135-143)
-    // marker gated by the SEED's hash (src/avx2_seeding.rs:197)
-    mkv[o] = (mm_hash64(seed) < threshold_marker) ? window_marker(w, j) : ~0ull;
-    o++;
+constexpr int EXPAND_THREADS = 256;
+constexpr uint32_t EXPAND_UPL = 4;                                        // units per lane and step: one 16-byte pass-mask load
+constexpr uint32_t EXPAND_STEP_UNITS = 32 * EXPAND_UPL;
+constexpr uint32_t EXPAND_WARP_UNITS = 8 * EXPAND_STEP_UNITS;             // units per warp
+
+// position of the n-th (0-based) set bit of m; m has more than n set bits
+__device__ __forceinline__ uint32_t nth_set_bit(uint32_t m, uint32_t n) {
+  uint32_t pos = 0;
+#pragma unroll
+  for (uint32_t s = 16; s; s >>= 1) {
+    const uint32_t c = __popc(m & ((1u << s) - 1u));
+    if (n >= c) { n -= c; m >>= s; pos += s; }
   }
+  return pos;
+}
+
+// Records of the passing windows, one warp per EXPAND_WARP_UNITS consecutive units, in (genome, contig, position) order.
+// Per step every lane loads the pass masks of EXPAND_UPL consecutive units; a warp scan of their popcounts numbers the step's
+// records, which are then handed out one per lane, 32 at a time, so the record arrays are written as contiguous runs.
+// A record's lane regenerates its window from the packed unit (records of one unit re-read the same bytes from L1).
+// Markers (the canonical 21-mer of a record whose SEED hashes below the marker threshold, src/avx2_seeding.rs:197) go to
+// their genome's slice of mk_sparse, which starts at the genome's first record (a genome has at most one marker per record);
+// per-genome counters hand out the slots, one atomic per warp, round and genome.
+__global__ void __launch_bounds__(EXPAND_THREADS)
+expand_kernel(const uint64_t* __restrict__ P, const uint32_t* __restrict__ ucoarse, const uint32_t* __restrict__ cuoff,
+              const uint32_t* __restrict__ clocal, const uint32_t* __restrict__ cgenome, uint32_t n_units,
+              const uint32_t* __restrict__ PM, const uint32_t* __restrict__ uoff, uint64_t seed_mask, uint64_t threshold_marker,
+              uint32_t* __restrict__ pv_kmer, uint32_t* __restrict__ pv_pos, uint32_t* __restrict__ pv_cc,
+              const uint64_t* __restrict__ seed_off, unsigned long long* __restrict__ mk_cnt, uint64_t* __restrict__ mk_sparse) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t u_begin = (blockIdx.x * (EXPAND_THREADS / 32) + threadIdx.x / 32) * EXPAND_WARP_UNITS;
+  if (u_begin >= n_units) return;
+  const uint32_t u_end = min(n_units, u_begin + EXPAND_WARP_UNITS);
+  uint32_t rec = uoff[u_begin];
+  for (uint32_t ub = u_begin; ub < u_end; ub += EXPAND_STEP_UNITS) {
+    const uint32_t u0 = ub + EXPAND_UPL * lane;
+    uint32_t pm[EXPAND_UPL];
+    if (u0 + EXPAND_UPL <= n_units) {
+      const uint4 v = *reinterpret_cast<const uint4*>(PM + u0);
+      pm[0] = v.x; pm[1] = v.y; pm[2] = v.z; pm[3] = v.w;
+    } else {
+#pragma unroll
+      for (uint32_t q = 0; q < EXPAND_UPL; q++) pm[q] = (u0 + q < n_units) ? PM[u0 + q] : 0u;
+    }
+    uint32_t cnt = 0;
+#pragma unroll
+    for (uint32_t q = 0; q < EXPAND_UPL; q++) cnt += __popc(pm[q]);
+    uint32_t incl = cnt;
+#pragma unroll
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+      if (lane >= d) incl += t;
+    }
+    const uint32_t excl = incl - cnt;
+    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+    for (uint32_t r0 = 0; r0 < total; r0 += 32) {
+      const uint32_t r = r0 + lane;
+      uint32_t L = 0;                                 // lane whose units hold record r: the number of lanes with incl <= r
+#pragma unroll
+      for (uint32_t s = 16; s; s >>= 1) if (__shfl_sync(0xFFFFFFFFu, incl, L + s - 1) <= r) L += s;
+      uint32_t loc = r - __shfl_sync(0xFFFFFFFFu, excl, L);
+      uint32_t m[EXPAND_UPL];
+#pragma unroll
+      for (uint32_t q = 0; q < EXPAND_UPL; q++) m[q] = __shfl_sync(0xFFFFFFFFu, pm[q], L);
+      bool has_mk = false;
+      uint64_t mkey = 0;
+      uint32_t g = ~0u;
+      if (r < total) {
+        uint32_t q_at = 0, pass = 0;
+        bool found = false;
+#pragma unroll
+        for (uint32_t q = 0; q < EXPAND_UPL; q++) {
+          const uint32_t c = __popc(m[q]);
+          if (!found) { if (loc < c) { found = true; q_at = q; pass = m[q]; } else loc -= c; }
+        }
+        const uint32_t u = ub + EXPAND_UPL * L + q_at;
+        const uint32_t j = nth_set_bit(pass, loc);
+        const uint32_t ci = contig_of_unit(ucoarse, cuoff, u);
+        const uint32_t ul = u - cuoff[ci];
+        const WindowCtx w = make_window_ctx(ul ? P[u - 1] : 0ull, P[u]);
+        bool canon;
+        const uint32_t seed = window_seed(w, j, seed_mask, &canon);
+        pv_kmer[rec + r] = seed;
+        pv_pos[rec + r] = 32u * ul + j;                             // index of the window's last base (src/avx2_seeding.rs:184,207)
+        pv_cc[rec + r] = (clocal[ci] << 1) | (canon ? 1u : 0u);     // SeedPosition::new (src/types.rs:135-143)
+        if (mm_hash64(seed) < threshold_marker) { has_mk = true; mkey = window_marker(w, j); g = cgenome[ci]; }
+      }
+      if (__ballot_sync(0xFFFFFFFFu, has_mk)) {
+        const uint32_t grp = __match_any_sync(0xFFFFFFFFu, g);     // lanes without a marker share g = ~0u (never a genome)
+        const uint32_t leader = __ffs(grp) - 1;
+        unsigned long long slot = 0;
+        if (has_mk && lane == leader) slot = atomicAdd(mk_cnt + g, (unsigned long long)__popc(grp));
+        slot = __shfl_sync(0xFFFFFFFFu, slot, leader);
+        if (has_mk) mk_sparse[seed_off[g] + slot + __popc(grp & ((1u << lane) - 1u))] = mkey;
+      }
+    }
+    rec += total;
+  }
+}
+
+// genome g's raw markers from its slice of mk_sparse (at seed_off[g]) to [mk_off[g], mk_off[g + 1]) of mk_raw; a warp per
+// genome (a genome has about one marker per marker_c bases: a block per genome would leave most threads idle)
+__global__ void marker_gather_kernel(const uint64_t* __restrict__ seed_off, const uint64_t* __restrict__ mk_off, uint32_t n_genomes,
+                                     const uint64_t* __restrict__ mk_sparse, uint64_t* __restrict__ mk_raw) {
+  const uint32_t g = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
+  if (g >= n_genomes) return;
+  const uint64_t* src = mk_sparse + seed_off[g];
+  uint64_t* dst = mk_raw + mk_off[g];
+  const uint64_t n = mk_off[g + 1] - mk_off[g];
+  for (uint64_t i = threadIdx.x & 31; i < n; i += 32) dst[i] = src[i];
 }
 
 __global__ void gather_u32_kernel(const uint32_t* __restrict__ src, const uint32_t* __restrict__ idx, uint32_t n,
@@ -203,16 +298,6 @@ __global__ void gather_u32_tail_kernel(const uint32_t* __restrict__ src, const u
   uint32_t k = idx[i];
   if (k >= src_len) { const uint32_t t = tail[src_len - 1]; dst[i] = src[src_len - 1] + (tail_is_mask ? (uint32_t)__popc(t) : t); }
   else dst[i] = src[k];
-}
-
-__global__ void marker_flag_kernel(const uint64_t* __restrict__ mkv, uint32_t n, uint32_t* __restrict__ flag) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) flag[i] = (mkv[i] != ~0ull) ? 1u : 0u;
-}
-__global__ void marker_scatter_kernel(const uint64_t* __restrict__ mkv, const uint32_t* __restrict__ scan, uint32_t n,
-                                      uint64_t* __restrict__ out) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n && mkv[i] != ~0ull) out[scan[i]] = mkv[i];
 }
 
 // ---- view building (block per genome) ------------------------------------------------------------------
@@ -676,36 +761,29 @@ int sketch_batch_device(sk_ctx* ctx, const SeedSrc& src, const uint64_t* contig_
   const uint32_t NU = (uint32_t)units;
   const uint32_t n_packed = std::min(src.n_packed, n_contigs);
   if (n_packed && (!src.d_P || !src.d_NM)) { ctx->err = "packed contigs without unit arrays"; return SK_ERR_PARAM; }
-  // coarse unit -> contig index: contig of every 256th unit (= the last contig starting at or before it)
-  std::vector<uint32_t> ucoarse(((size_t)NU >> UCOARSE_SHIFT) + 2, n_contigs ? n_contigs - 1 : 0);
-  {
-    uint32_t ci = 0;
-    for (size_t j = 0; ((uint64_t)j << UCOARSE_SHIFT) < NU; j++) {
-      const uint32_t u = (uint32_t)(j << UCOARSE_SHIFT);
-      while (ci + 1 < n_contigs && cuoff[ci + 1] <= u) ci++;
-      ucoarse[j] = ci;
-    }
-  }
+  const uint32_t n_ucoarse = (NU >> UCOARSE_SHIFT) + 2;
 
   SK_CUDA(ctx->arena.alloc((void**)&set->d_ctg_len, std::max<size_t>(n_contigs, 1) * 4));
   SK_CUDA(ctx->arena.alloc((void**)&set->ctg_rec_off, (size_t)(n_contigs + G + 1) * 4));
   set->seed_off.assign(G + 1, 0);
 
   DTmp<uint64_t> d_coff, Pown;
-  DTmp<uint32_t> d_cuoff, d_clen, d_clocal, d_ucoarse, NMown, PM, uoff;
+  DTmp<uint32_t> d_cuoff, d_clen, d_clocal, d_cgenome, d_ucoarse, NMown, PM, uoff;
   mbox_reset(ctx);                           // no readback of an earlier sub-batch is in flight (each one ends synchronised)
   uint64_t* h_raw_mk_off = (uint64_t*)mbox_alloc(ctx, (size_t)(G + 1) * 8);    // raw markers per genome (prefix offsets), pinned
   if (h_raw_mk_off) for (uint32_t g = 0; g <= G; g++) h_raw_mk_off[g] = 0;
-  DTmp<uint64_t> mkv, mraw;
+  DTmp<uint64_t> mraw;
   if (NU > 0) {
     SK_CUDA(d_coff.alloc(n_contigs + 1, ctx)); SK_CUDA(d_cuoff.alloc(n_contigs + 1, ctx));
-    SK_CUDA(d_clen.alloc(n_contigs, ctx)); SK_CUDA(d_clocal.alloc(n_contigs, ctx)); SK_CUDA(d_ucoarse.alloc(ucoarse.size(), ctx));
+    SK_CUDA(d_clen.alloc(n_contigs, ctx)); SK_CUDA(d_clocal.alloc(n_contigs, ctx)); SK_CUDA(d_cgenome.alloc(n_contigs, ctx));
+    SK_CUDA(d_ucoarse.alloc(n_ucoarse, ctx));
     SK_CUDA(h2d_small(ctx, d_coff.p, coff.data(), (n_contigs + 1) * 8));
     SK_CUDA(h2d_small(ctx, d_cuoff.p, cuoff.data(), (n_contigs + 1) * 4));
     SK_CUDA(h2d_small(ctx, d_clen.p, clen.data(), n_contigs * 4));
     SK_CUDA(h2d_small(ctx, d_clocal.p, clocal.data(), n_contigs * 4));
-    SK_CUDA(h2d_small(ctx, d_ucoarse.p, ucoarse.data(), ucoarse.size() * 4));
+    SK_CUDA(h2d_small(ctx, d_cgenome.p, genome_of_contig, n_contigs * 4));
     SK_CUDA(h2d_small(ctx, set->d_ctg_len, clen.data(), n_contigs * 4));
+    ucoarse_kernel<<<div_up(n_ucoarse, 256), 256, 0, st>>>(d_cuoff.p, n_contigs, n_ucoarse, d_ucoarse.p); count_launch(ctx);
     uint64_t* P = src.d_P; uint32_t* NM = src.d_NM;
     if (!P) { SK_CUDA(Pown.alloc(NU, ctx)); SK_CUDA(NMown.alloc(NU, ctx)); P = Pown.p; NM = NMown.p; }
     SK_CUDA(PM.alloc(NU, ctx)); SK_CUDA(uoff.alloc(NU, ctx));
@@ -751,9 +829,6 @@ int sketch_batch_device(sk_ctx* ctx, const SeedSrc& src, const uint64_t* contig_
     SK_CUDA(ctx->arena.alloc((void**)&set->pv_kmer, std::max<size_t>(S, 1) * 4));
     SK_CUDA(ctx->arena.alloc((void**)&set->pv_pos, std::max<size_t>(S, 1) * 4));
     SK_CUDA(ctx->arena.alloc((void**)&set->pv_cc, std::max<size_t>(S, 1) * 4));
-    SK_CUDA(mkv.alloc(S, ctx));
-    SK_LAUNCH(ctx, "expand_kernel", (expand_kernel<<<div_up(NU, 256), 256, 0, st>>>(
-        P, d_ucoarse.p, d_cuoff.p, d_clocal.p, NU, PM.p, uoff.p, seed_mask, thr_m, set->pv_kmer, set->pv_pos, set->pv_cc, mkv.p)));
     // per-genome record offsets + per-contig local record offsets (with one sentinel per genome)
     std::vector<uint32_t> crl(n_contigs + G + 1, 0);
     for (uint32_t g = 0; g < G; g++) {
@@ -766,21 +841,23 @@ int sketch_batch_device(sk_ctx* ctx, const SeedSrc& src, const uint64_t* contig_
     }
     set->seed_off[G] = S;
     SK_CUDA(h2d_small(ctx, set->ctg_rec_off, crl.data(), (size_t)(n_contigs + G) * 4));
-    // raw markers: compact the flagged values (order inside a genome is irrelevant: they are sorted + deduped next).  Their
-    // number is not known to the host yet: the buffer takes the upper bound (one per record), the per-genome offsets travel to
-    // the host asynchronously and are read after build_views' first synchronisation.
+    // records, and the raw markers of every genome in its slice of msparse (order inside a genome is irrelevant: they are
+    // sorted + deduped next).  Their number is not known to the host yet: the per-genome offsets travel to the host
+    // asynchronously and are read after build_views' first synchronisation.
     if (S > 0) {
-      DTmp<uint32_t> mflag, mscan;
-      SK_CUDA(mflag.alloc(S, ctx)); SK_CUDA(mscan.alloc(S, ctx));
-      marker_flag_kernel<<<div_up(S, 256), 256, 0, st>>>(mkv.p, S, mflag.p); count_launch(ctx);
-      SK_TRY(scan_exclusive<uint32_t>(ctx, mflag.p, mscan.p, S));
-      DTmp<uint64_t> d_so, d_mo;
-      SK_CUDA(d_so.alloc(G + 1, ctx)); SK_CUDA(d_mo.alloc(G + 1, ctx));
+      DTmp<uint64_t> d_so, d_mo, msparse;
+      DTmp<unsigned long long> mcnt;
+      SK_CUDA(d_so.alloc(G + 1, ctx)); SK_CUDA(d_mo.alloc(G + 1, ctx)); SK_CUDA(mcnt.alloc(G + 1, ctx));
       SK_CUDA(h2d_small(ctx, d_so.p, set->seed_off.data(), (G + 1) * 8));
-      SK_CUDA(mraw.alloc(S, ctx));
-      marker_scatter_kernel<<<div_up(S, 256), 256, 0, st>>>(mkv.p, mscan.p, S, mraw.p); count_launch(ctx);
-      gather_scan_at_tail_kernel<<<div_up(G + 1, 256), 256, 0, st>>>(mscan.p, d_so.p, G + 1, S, mflag.p, d_mo.p); count_launch(ctx);
+      SK_CUDA(cudaMemsetAsync(mcnt.p, 0, (size_t)(G + 1) * 8, st));
+      SK_CUDA(msparse.alloc(S, ctx));
+      SK_LAUNCH(ctx, "expand_kernel", (expand_kernel<<<div_up(NU, EXPAND_WARP_UNITS * (EXPAND_THREADS / 32)), EXPAND_THREADS, 0, st>>>(
+          P, d_ucoarse.p, d_cuoff.p, d_clocal.p, d_cgenome.p, NU, PM.p, uoff.p, seed_mask, thr_m, set->pv_kmer, set->pv_pos,
+          set->pv_cc, d_so.p, mcnt.p, msparse.p)));
+      SK_TRY(scan_exclusive<uint64_t>(ctx, (const uint64_t*)mcnt.p, d_mo.p, G + 1));
       SK_CUDA(cudaMemcpyAsync(h_raw_mk_off, d_mo.p, (size_t)(G + 1) * 8, cudaMemcpyDeviceToHost, st));
+      SK_CUDA(mraw.alloc(S, ctx));
+      marker_gather_kernel<<<div_up(G, 8), 256, 0, st>>>(d_so.p, d_mo.p, G, msparse.p, mraw.p); count_launch(ctx);
     }
   } else {
     set->S = 0;
@@ -788,7 +865,7 @@ int sketch_batch_device(sk_ctx* ctx, const SeedSrc& src, const uint64_t* contig_
     SK_CUDA(cudaMemsetAsync(set->ctg_rec_off, 0, (size_t)(n_contigs + G + 1) * 4, st));
   }
   // free the big per-base temporaries before the sort temporaries are allocated
-  Pown.release(); NMown.release(); PM.release(); uoff.release(); mkv.release();
+  Pown.release(); NMown.release(); PM.release(); uoff.release();
   if (!h_raw_mk_off) { ctx->err = "out of pinned host memory"; return SK_ERR_NOMEM; }
   SK_TRY(build_views(ctx, set, mraw.p, h_raw_mk_off));
   SK_CUDA(cudaStreamSynchronize(st));
