@@ -23,15 +23,13 @@
 //
 // sk_dereplicate_store runs the same waves over a host sketch store: the markers of every genome are gathered once on ctxs[0]
 // (the index, the row screens, the greedy rounds and the set difference run there exactly as above, on the global genome
-// indices), and each chain step's pairs are planned into working sets that the contexts gather from the store and chain, as
-// sk_triangle_store does (store_ws.hpp, ws_plan.hpp).
+// indices), and each chain step's pairs are planned into working sets (ws_plan.hpp) that the contexts gather from the store
+// and chain through chain_working_sets (store_ws.hpp), as sk_triangle_store does.
 #include <cub/cub.cuh>
 
 #include <algorithm>
 #include <chrono>
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
 #include <string>
 #include <vector>
 
@@ -176,7 +174,6 @@ struct StoreChain {
   const sk_sketch_store* st;
   std::vector<uint64_t> gbytes;   // sk_sketch_store_genome_bytes of every genome
   uint64_t budget;
-  bool trace;
   sk_store_stats stats{};
 };
 
@@ -297,53 +294,16 @@ struct Run {
   }
 
   // The store back end: the step's sorted pairs planned into working sets (ws_plan.hpp) that the contexts gather and chain
-  // (run_working_sets), as sk_triangle_store does.  Each pair is in exactly one working set and its row goes to the pair's
+  // (chain_working_sets), as sk_triangle_store does.  Each pair is in exactly one working set and its row goes to the pair's
   // position in out, so the contexts never write the same row and out does not depend on which context chained what.
   int chain_store(const std::vector<uint64_t>& pairs, sk_ani_result* out) {
     StoreChain& sc = *store;
     skws::Plan plan;
     std::string perr;
     if (!skws::plan_working_sets(pairs, sc.gbytes, sc.budget, plan, perr)) { ctx->err = std::string(who) + ": " + perr; return SK_ERR_NOMEM; }
-    auto work = [&](sk_ctx* c, uint32_t d, size_t w, std::vector<sk_ani_result>&, WsTimes& t) {
-      const skws::WorkingSet& ws = plan.sets[w];
-      const auto a = clk::now();
-      sk_sketch_set* wset = nullptr;
-      int rc = sk_sketch_store_gather(c, sc.st, ws.genomes.data(), (uint32_t)ws.genomes.size(), 0, &wset);
-      const double tg = secs(a);
-      const auto b = clk::now();
-      if (rc == SK_OK) {
-        std::vector<uint64_t> lp(ws.pairs.size());
-        for (size_t i = 0; i < lp.size(); i++) {
-          const uint64_t x = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)(ws.pairs[i] >> 32)) - ws.genomes.begin();
-          const uint64_t y = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)ws.pairs[i]) - ws.genomes.begin();
-          lp[i] = (x << 32) | y;
-        }
-        std::vector<sk_ani_result> res(lp.size());
-        rc = sk_chain_pairs(c, wset, wset, lp.data(), lp.size(), mp, res.data());
-        if (rc == SK_OK)
-          for (size_t i = 0; i < res.size(); i++) {
-            sk_ani_result r = res[i];
-            r.ref_id = ws.genomes[r.ref_id];
-            r.query_id = ws.genomes[r.query_id];
-            out[std::lower_bound(pairs.begin(), pairs.end(), ws.pairs[i]) - pairs.begin()] = r;
-          }
-      }
-      if (wset) sk_sketch_set_free(wset);
-      const double tc = secs(b);
-      t.gather += tg; t.chain += tc; t.bytes += ws.bytes;
-      if (sc.trace)
-        fprintf(stderr, "[%s] context %u: working set %zu/%zu%s: %zu genomes, %zu pairs, %.1f MB gathered in %.1f ms, chain %.1f ms\n", who, d, w + 1,
-                plan.sets.size(), ws.chunk_pair ? " (chunk pair)" : "", ws.genomes.size(), ws.pairs.size(), ws.bytes / 1e6, tg * 1e3, tc * 1e3);
-      return rc;
-    };
-    std::vector<sk_ani_result> none;   // every row is written in place: the contexts keep nothing
-    WsTimes t;
-    SK_TRY(run_working_sets(sc.ctxs, sc.n_ctx, plan.sets.size(), work, none, t));
-    sc.stats.n_working_sets += (uint32_t)plan.sets.size();
-    sc.stats.n_split_components += plan.n_split_components;
-    for (auto& ws : plan.sets) sc.stats.max_working_set_bytes = std::max(sc.stats.max_working_set_bytes, ws.bytes);
-    sc.stats.gathered_bytes += t.bytes; sc.stats.t_gather += t.gather; sc.stats.t_chain += t.chain;
-    return SK_OK;
+    return chain_working_sets(who, sc.ctxs, sc.n_ctx, sc.st, sc.st, plan, mp, [&](uint32_t, const skws::WorkingSet& ws, const std::vector<sk_ani_result>& res) {
+      for (size_t i = 0; i < res.size(); i++) out[std::lower_bound(pairs.begin(), pairs.end(), ws.pairs[i]) - pairs.begin()] = res[i];
+    }, sc.stats);
   }
 
   // the genomes of list[0 .. m) (device) in state s, order kept, into out; their count
@@ -546,17 +506,6 @@ int derep_store_budget(sk_ctx* const* ctxs, uint32_t n_ctx, uint64_t n_markers, 
   return SK_OK;
 }
 
-// a genome over budget / 2 cannot be placed in every chunk pair of a working-set plan
-int check_genome_bytes(sk_ctx* ctx, const std::vector<uint64_t>& gbytes, uint64_t budget) {
-  for (size_t g = 0; g < gbytes.size(); g++)
-    if (gbytes[g] > budget / 2) {
-      ctx->err = std::string(WHO_STORE) + ": genome " + std::to_string(g) + " needs " + std::to_string(gbytes[g]) +
-                 " device bytes, more than half the working-set budget of " + std::to_string(budget) + " bytes";
-      return SK_ERR_NOMEM;
-    }
-  return SK_OK;
-}
-
 }  // namespace
 
 int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp, const uint32_t* rank,
@@ -570,9 +519,13 @@ int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_st
   if (std::isnan(dp->min_ani)) { ctx->err = std::string(WHO_STORE) + ": min_ani is NaN"; return SK_ERR_PARAM; }
   const std::string bad = rank_error(N, rank);
   if (!bad.empty()) { ctx->err = std::string(WHO_STORE) + ": " + bad; return SK_ERR_PARAM; }
-  StoreChain sc{ctxs, n_ctx, st, std::vector<uint64_t>(N), device_budget, getenv("SK_TRACE") != nullptr};
+  StoreChain sc{ctxs, n_ctx, st, std::vector<uint64_t>(N), device_budget};
   for (uint32_t g = 0; g < N; g++) sc.gbytes[g] = sk_sketch_store_genome_bytes(st, g);
-  if (device_budget) SK_TRY(check_genome_bytes(ctx, sc.gbytes, device_budget));   // before any device work
+  std::string perr;   // a genome over budget / 2 cannot be placed in every chunk pair of a working-set plan
+  if (device_budget && !skws::genomes_fit(sc.gbytes, device_budget, perr)) {   // before any device work
+    ctx->err = std::string(WHO_STORE) + ": " + perr;
+    return SK_ERR_NOMEM;
+  }
   if (N == 0) {   // what sk_dereplicate returns for an empty set: no wave, no pair, no cluster
     if (stats) *stats = sk_derep_stats{};
     if (store_stats) *store_stats = sk_store_stats{};
@@ -581,15 +534,13 @@ int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_st
   // the markers of every genome on ctxs[0]
   SK_CUDA(cudaSetDevice(ctx->device));
   const auto t0 = clk::now();
-  std::vector<uint32_t> all(N);
-  for (uint32_t g = 0; g < N; g++) all[g] = g;
   sk_sketch_set* mk = nullptr;
-  SK_TRY(sk_sketch_store_gather(ctx, st, all.data(), N, SK_PACK_MARKERS_ONLY, &mk));
+  SK_TRY(gather_markers(ctx, st, &mk));
   sc.stats.t_screen = secs(t0);
   int rc = SK_OK;
   if (!device_budget) {
     rc = derep_store_budget(ctxs, n_ctx, mk->mk_off[N], N, &sc.budget);
-    if (rc == SK_OK) rc = check_genome_bytes(ctx, sc.gbytes, sc.budget);
+    if (rc == SK_OK && !skws::genomes_fit(sc.gbytes, sc.budget, perr)) { ctx->err = std::string(WHO_STORE) + ": " + perr; rc = SK_ERR_NOMEM; }
   }
   if (rc == SK_OK) {
     Run r{ctx, mk, mp, dp->min_ani, screen_cutoff(mp), N, WHO_STORE, &sc};

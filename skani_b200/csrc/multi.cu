@@ -5,11 +5,13 @@
 //   2. the MARKERS of every block are exchanged device-to-device (peer copies over NVLink when the devices differ, plain
 //      device copies when contexts share a device) and every device screens the whole triangle -> the same sorted pair
 //      list everywhere, from which the pairs that lie inside one block (already chained in step 1) are dropped;
-//   3. the remaining cross-block pairs are cut into equal contiguous slices; a device fetches the sketches its slice
-//      touches as sub-blobs INCLUDING their k-mer hash tables (sk_sketch_set_pack_subset, SK_PACK_TABLES) and chains them.
+//   3. the remaining cross-block pairs are split over the devices by connected component (skws::partition_pairs, ws_plan.hpp);
+//      a device fetches the sketches its share touches as sub-blobs INCLUDING their k-mer hash tables
+//      (sk_sketch_set_pack_subset, SK_PACK_TABLES) and chains them (chain_on_working_set, store_ws.hpp).
 // The same steps run as one process per GPU over torch.distributed/NCCL in skani_b200/multi_gpu.py (bench.py --gpus N).
+// The query x ref calls touch only their own context's memory, so they need neither peer access nor barriers: one host thread
+// per context through run_per_context (store_ws.hpp).
 #include <algorithm>
-#include <chrono>
 #include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
@@ -19,6 +21,9 @@
 #include <vector>
 
 #include "sk_internal.h"
+#include "store_ws.hpp"
+
+using sk::now_s;
 
 extern "C" int sk_triangle_local(sk_ctx* ctx, const uint8_t* bases, const uint64_t* contig_off, uint32_t n_contigs,
                                  const uint32_t* genome_of_contig, uint32_t n_genomes, const sk_sketch_params* sp,
@@ -83,8 +88,6 @@ int unpack_blobs(const char* who, sk_ctx* ctx, const std::vector<const Blob*>& b
   return sk_sketch_set_unpack(ctx, (uint32_t)n, bp.data(), mp.data(), out);
 }
 
-double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
 // peer access between the distinct devices of ctxs[0..n) (ignored when unsupported: copies then stage through the host)
 void enable_peer_access(sk_ctx* const* ctxs, uint32_t n) {
   for (uint32_t a = 0; a < n; a++)
@@ -98,47 +101,6 @@ void enable_peer_access(sk_ctx* const* ctxs, uint32_t n) {
 }
 
 }  // namespace
-
-// Cross-block pairs -> one list per device.  The pairs of one connected component of the pair graph (a cluster of related
-// genomes) stay together, so a device fetches that cluster's sketches once; with a genome order unrelated to relatedness a
-// contiguous slice of the sorted list touches ~5x more genomes (skani_b200/multi_gpu.py partition_pairs is the same rule).
-// Components above half a device's fair share are cut into runs of consecutive pairs; items go to the least loaded device,
-// largest first (ties: first pair).  Deterministic; every list comes out sorted.
-static void partition_pairs(const std::vector<uint64_t>& sorted_pairs, uint32_t W, uint32_t n_genomes, std::vector<std::vector<uint64_t>>& out) {
-  out.assign(W, {});
-  const size_t n = sorted_pairs.size();
-  if (n == 0) return;
-  if (W == 1) { out[0] = sorted_pairs; return; }
-  std::vector<uint32_t> parent(n_genomes);
-  for (uint32_t g = 0; g < n_genomes; g++) parent[g] = g;
-  auto find = [&](uint32_t x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
-  for (uint64_t p : sorted_pairs) {
-    const uint32_t a = find((uint32_t)(p >> 32)), b = find((uint32_t)p);
-    if (a != b) parent[std::max(a, b)] = std::min(a, b);            // root = smallest genome of the component
-  }
-  // pairs grouped by component root (stable: sorted inside a group)
-  std::vector<std::pair<uint32_t, uint64_t>> keyed(n);
-  for (size_t i = 0; i < n; i++) keyed[i] = {find((uint32_t)(sorted_pairs[i] >> 32)), sorted_pairs[i]};
-  std::sort(keyed.begin(), keyed.end());
-  const size_t cap = std::max<size_t>(1, (n + 2 * (size_t)W - 1) / (2 * (size_t)W));
-  struct Item { size_t size, start; };
-  std::vector<Item> items;
-  for (size_t i = 0; i < n;) {
-    size_t j = i;
-    while (j < n && keyed[j].first == keyed[i].first) j++;
-    for (size_t s0 = i; s0 < j; s0 += cap) items.push_back(Item{std::min(cap, j - s0), s0});
-    i = j;
-  }
-  std::sort(items.begin(), items.end(), [&](const Item& a, const Item& b) { return a.size != b.size ? a.size > b.size : keyed[a.start].second < keyed[b.start].second; });
-  std::vector<size_t> load(W, 0);
-  for (const Item& it : items) {
-    uint32_t r = 0;
-    for (uint32_t k = 1; k < W; k++) if (load[k] < load[r]) r = k;
-    for (size_t k = it.start; k < it.start + it.size; k++) out[r].push_back(keyed[k].second);
-    load[r] += it.size;
-  }
-  for (auto& v : out) std::sort(v.begin(), v.end());
-}
 
 extern "C" int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint8_t* bases, const uint64_t* contig_off, uint32_t n_contigs,
                                  const uint32_t* genome_of_contig, uint32_t n_genomes, const sk_sketch_params* sp,
@@ -240,7 +202,7 @@ extern "C" int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint
     const double t2 = now_s();
     // split over the devices by connected component of the pair graph (every thread computes the same split)
     std::vector<std::vector<uint64_t>> share;
-    partition_pairs(cross, W, n_genomes, share);
+    skws::partition_pairs(cross, W, n_genomes, share);
     auto genomes_of_slice = [&](uint32_t r, std::vector<uint32_t>& need) {
       need.clear();
       for (uint64_t pr : share[r]) { need.push_back((uint32_t)(pr >> 32)); need.push_back((uint32_t)pr); }
@@ -271,32 +233,25 @@ extern "C" int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint
     for (uint32_t r = 0; r < W; r++) if (sub[d][r].d) { c->arena.release(sub[d][r].d); sub[d][r].d = nullptr; }
     sk_sketch_set_free(local[d]); local[d] = nullptr;
     const double t3 = now_s();
-    // ---- chain the slice on the working set (ids -> working indices and back)
+    // ---- chain the slice on the working set
     const std::vector<uint64_t>& my_pairs = share[d];
-    const uint64_t lo = 0, hi = my_pairs.size();
-    if (rc == SK_OK && hi > lo) {
+    if (rc == SK_OK && !my_pairs.empty()) {
       if (sk_sketch_set_n_genomes(work) != mine.size()) { c->err = "fetch plan mismatch"; rc = SK_ERR_STATE; }
       std::vector<uint64_t> ranks(mine.size());
       for (size_t i = 0; i < mine.size(); i++) ranks[i] = name_ranks ? name_ranks[mine[i]] : mine[i];
       if (rc == SK_OK) rc = sk_sketch_set_set_name_ranks(work, ranks.data());
-      std::vector<uint64_t> lp(hi - lo);
-      for (uint64_t i = lo; i < hi; i++) {
-        const uint64_t a = std::lower_bound(mine.begin(), mine.end(), (uint32_t)(my_pairs[i] >> 32)) - mine.begin();
-        const uint64_t b = std::lower_bound(mine.begin(), mine.end(), (uint32_t)my_pairs[i]) - mine.begin();
-        lp[i - lo] = (a << 32) | b;
-      }
-      std::vector<sk_ani_result> res(lp.size());
-      if (rc == SK_OK) rc = sk_chain_pairs(c, work, work, lp.data(), lp.size(), mp, res.data());
+      std::vector<sk_ani_result> res;
+      if (rc == SK_OK) rc = sk::chain_on_working_set(c, work, mine, work, mine, my_pairs, mp, res);
       if (rc == SK_OK)
-        for (auto& x : res)
-          if (x.ani > 0.1f) { x.ref_id = mine[x.ref_id]; x.query_id = mine[x.query_id]; results[d].push_back(x); }   // src/triangle.rs:99
-      screened[d] += hi - lo;
+        for (const auto& x : res)
+          if (x.ani > 0.1f) results[d].push_back(x);   // src/triangle.rs:99
+      screened[d] += my_pairs.size();
     }
     if (work) sk_sketch_set_free(work);
     if (trace) fprintf(stderr, "[sk_triangle_multi] device slot %u (gpu %d): block %u..%u local %.1f ms, markers+screen %.1f ms, fetch %.1f ms "
                                "(%zu genomes, %.1f MB remote), chain %.1f ms (%llu cross-block pairs of %zu)\n", d, c->device, gb[d], gb[d + 1],
                        (t1 - t0) * 1e3, (t2 - t1) * 1e3, (t3 - t2) * 1e3, mine.size(), remote_bytes / 1e6, (now_s() - t3) * 1e3,
-                       (unsigned long long)(hi - lo), cross.size());
+                       (unsigned long long)my_pairs.size(), cross.size());
     return rc;
   };
 
@@ -316,18 +271,14 @@ extern "C" int sk_triangle_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const uint
   }
   cudaSetDevice(ctx->device);
   if (rc != SK_OK) return rc;
-  size_t nres = 0;
-  for (auto& v : results) nres += v.size();
-  sk_ani_result* o = (sk_ani_result*)malloc(sizeof(sk_ani_result) * std::max<size_t>(nres, 1));
-  if (!o) return SK_ERR_NOMEM;
-  size_t k = 0;
-  for (auto& v : results) { if (!v.empty()) memcpy(o + k, v.data(), v.size() * sizeof(sk_ani_result)); k += v.size(); }
-  *out = o; *n_out = nres;
+  std::vector<sk_ani_result> all;
+  for (auto& v : results) all.insert(all.end(), v.begin(), v.end());
+  SK_TRY(sk::hand_out(ctx, all, out, n_out));
   if (stats) {
     memset(stats, 0, sizeof(*stats));
     stats->t_total = now_s() - t_begin;
     for (uint64_t s : screened) stats->n_pairs_screened += s;
-    stats->n_pairs_kept = nres;
+    stats->n_pairs_kept = all.size();
   }
   return SK_OK;
 }
@@ -378,12 +329,11 @@ int check_qr_args(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* cons
   auto fail = [&](const std::string& m) { ctx->err = m; return SK_ERR_PARAM; };
   if (!refs || !ref_first || !queries || !mp) return fail("NULL argument");
   if (!queries[0]) return fail("queries[0] is NULL");
+  SK_TRY(sk::check_contexts(ctxs, n_ctx));
   const sk_sketch_set* q0 = queries[0];
   qb.G.assign(n_ctx, 0);
   for (uint32_t d = 0; d < n_ctx; d++) {
     const std::string at = "context " + std::to_string(d) + ": ";
-    if (!ctxs[d]) return fail(at + "NULL context");
-    for (uint32_t e = 0; e < d; e++) if (ctxs[e] == ctxs[d]) return fail(at + "the same context appears twice (one host thread per context)");
     const sk_sketch_set* q = queries[d];
     if (!q || q->ctx != ctxs[d]) return fail(at + "queries[d] must be a set of ctxs[d]");
     if (q->G != q0->G || q->seed_off != q0->seed_off || q->mk_off != q0->mk_off || q->ctg_off != q0->ctg_off)
@@ -402,24 +352,6 @@ int check_qr_args(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* cons
   return SK_OK;
 }
 
-// fn(d) on one host thread per context, device d current.  The calls touch only their own context's memory, so they need
-// neither peer access nor barriers; the call fails if any context failed, with the first failure's message on ctxs[0].
-int run_per_context(sk_ctx* const* ctxs, uint32_t n, const std::function<int(uint32_t)>& fn) {
-  std::vector<int> rcs(n, SK_OK);
-  auto one = [&](uint32_t d) { rcs[d] = cudaSetDevice(ctxs[d]->device) == cudaSuccess ? fn(d) : SK_ERR_CUDA; };
-  if (n == 1) one(0);
-  else {
-    std::vector<std::thread> th;
-    for (uint32_t d = 0; d < n; d++) th.emplace_back(one, d);
-    for (auto& t : th) t.join();
-  }
-  int rc = SK_OK;
-  for (uint32_t d = 0; d < n && rc == SK_OK; d++)
-    if (rcs[d] != SK_OK) { rc = rcs[d]; if (d) ctxs[0]->err = "context " + std::to_string(d) + ": " + ctxs[d]->err; }
-  cudaSetDevice(ctxs[0]->device);
-  return rc;
-}
-
 }  // namespace
 
 extern "C" int sk_screen_query_ref_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_set* const* refs, const uint32_t* ref_first,
@@ -431,7 +363,7 @@ extern "C" int sk_screen_query_ref_multi(sk_ctx* const* ctxs, uint32_t n_ctx, co
   SK_TRY(check_qr_args(ctxs, n_ctx, refs, ref_first, queries, mp, qb));
   if (mode < 0 || mode > 3) { ctxs[0]->err = "mode must be 0..3"; return SK_ERR_PARAM; }
   std::vector<std::vector<uint64_t>> part(n_ctx);
-  SK_TRY(run_per_context(ctxs, n_ctx, [&](uint32_t d) -> int {
+  SK_TRY(sk::run_per_context(ctxs, n_ctx, [&](uint32_t d) -> int {
     if (qb.G[d] == 0) return SK_OK;
     uint64_t* p = nullptr; uint64_t n = 0;
     const int rc = sk_screen_query_ref(ctxs[d], refs[d], queries[d], mp, mode, &p, &n);
@@ -444,14 +376,9 @@ extern "C" int sk_screen_query_ref_multi(sk_ctx* const* ctxs, uint32_t n_ctx, co
     return rc;
   }));
   // every block's list is sorted and the blocks ascend: their concatenation is sorted
-  size_t total = 0;
-  for (auto& v : part) total += v.size();
-  uint64_t* o = (uint64_t*)malloc(std::max<size_t>(total, 1) * 8);
-  if (!o) { ctxs[0]->err = "out of host memory"; return SK_ERR_NOMEM; }
-  size_t k = 0;
-  for (auto& v : part) { if (!v.empty()) memcpy(o + k, v.data(), v.size() * 8); k += v.size(); }
-  *pairs_rq = o; *n_pairs = total;
-  return SK_OK;
+  std::vector<uint64_t> all;
+  for (auto& v : part) all.insert(all.end(), v.begin(), v.end());
+  return sk::hand_out(ctxs[0], all, pairs_rq, n_pairs);
 }
 
 // sk_chain_pairs_multi, and with map_off / maps non-null sk_chain_pairs_multi_mappings
@@ -476,7 +403,7 @@ static int chain_pairs_multi(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketc
   const bool with_maps = map_off != nullptr;
   std::vector<std::vector<uint64_t>> loff(n_ctx);       // mappings: each context's offsets and records, in its local order
   std::vector<sk_mapping*> lmaps(n_ctx, nullptr);
-  const int rc = run_per_context(ctxs, n_ctx, [&](uint32_t d) -> int {
+  const int rc = sk::run_per_context(ctxs, n_ctx, [&](uint32_t d) -> int {
     if (local[d].empty()) return SK_OK;
     // switch_qr's file-name tie-break (src/chain.rs:19-21) as in the one set of all refs: default ranks are global ref ids,
     // and default query ranks follow all n_refs refs.  Applied on non-owning views; the caller's sets are not touched.

@@ -7,14 +7,12 @@
 // pulls them over PCIe straight into a device blob in the layout sk_sketch_set_unpack reads (no host-side copy, no staging
 // buffer), and the existing unpack builds the set without rebuilding the tables.
 // sk_triangle_store screens the markers of every genome, plans working sets (ws_plan.hpp) and lets one host thread per
-// context gather and chain them in plan order.  sk_query_ref_store does the same for every (reference, query) pair of two
-// stores: one marker screen of all references against all queries, working sets that each hold some references and some
-// queries, gathered from their own stores.
+// context gather and chain them in plan order (chain_working_sets, store_ws.hpp).  sk_query_ref_store does the same for every
+// (reference, query) pair of two stores: one marker screen of all references against all queries, working sets that each hold
+// some references and some queries, gathered from their own stores.  Both keep the rows with ani > 0.1.
 #include <algorithm>
-#include <chrono>
-#include <cstdio>
 #include <cstdlib>
-#include <cstring>
+#include <string>
 #include <vector>
 
 #include "sk_internal.h"
@@ -43,14 +41,21 @@ struct sk_sketch_store {
 
 namespace {
 
-double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
-// results as a malloc'd array (sk_free)
-int hand_out(sk_ctx* ctx, const std::vector<sk_ani_result>& res, sk_ani_result** out, uint64_t* n_out) {
-  sk_ani_result* o = (sk_ani_result*)malloc(sizeof(sk_ani_result) * std::max<size_t>(res.size(), 1));
-  if (!o) { ctx->err = "out of host memory"; return SK_ERR_NOMEM; }
-  if (!res.empty()) memcpy(o, res.data(), res.size() * sizeof(sk_ani_result));
-  *out = o; *n_out = res.size();
+// The working sets of plan chained on the contexts (chain_working_sets), keeping ani > 0.1 (src/triangle.rs:99,
+// src/dist.rs:115,139): the kept rows sorted by (ref_id, query_id) as a malloc'd array, and s, holding the screen's time, with
+// the working sets' counts and times in *stats
+template <class Plan>
+int chain_and_keep(const char* who, sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* a, const sk_sketch_store* b, const Plan& plan,
+                   const sk_map_params* mp, sk_store_stats s, sk_ani_result** out, uint64_t* n_out, sk_store_stats* stats) {
+  std::vector<std::vector<sk_ani_result>> kept(n_ctx);
+  SK_TRY(chain_working_sets(who, ctxs, n_ctx, a, b, plan, mp, [&](uint32_t d, const auto&, const std::vector<sk_ani_result>& rows) {
+    for (const sk_ani_result& r : rows) if (r.ani > 0.1f) kept[d].push_back(r);
+  }, s));
+  std::vector<sk_ani_result> res;
+  for (const auto& k : kept) res.insert(res.end(), k.begin(), k.end());
+  std::sort(res.begin(), res.end(), [](const sk_ani_result& x, const sk_ani_result& y) { return x.ref_id != y.ref_id ? x.ref_id < y.ref_id : x.query_id < y.query_id; });
+  SK_TRY(hand_out(ctxs[0], res, out, n_out));
+  if (stats) *stats = s;
   return SK_OK;
 }
 
@@ -207,6 +212,7 @@ int sk_sketch_store_gather(sk_ctx* ctx, const sk_sketch_store* st, const uint32_
 
 int sk_triangle_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp, uint64_t device_budget,
                       sk_ani_result** out, uint64_t* n_out, sk_store_stats* stats) {
+  const char* const who = "sk_triangle_store";
   if (!ctxs || n_ctx == 0 || !ctxs[0]) return SK_ERR_PARAM;
   sk_ctx* ctx = ctxs[0];
   if (!st || !mp || !out || !n_out) { ctx->err = "sk_triangle_store: NULL argument"; return SK_ERR_PARAM; }
@@ -217,21 +223,16 @@ int sk_triangle_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store
   SK_TRY(working_set_budget(ctxs, n_ctx, device_budget, &budget));
   std::vector<uint64_t> gbytes(N);
   for (uint32_t g = 0; g < N; g++) gbytes[g] = sk_sketch_store_genome_bytes(st, g);
-  for (uint32_t g = 0; g < N; g++)
-    if (gbytes[g] > budget / 2) {
-      ctx->err = "sk_triangle_store: genome " + std::to_string(g) + " needs " + std::to_string(gbytes[g]) + " device bytes, more than half the working-set budget of " +
-                 std::to_string(budget) + " bytes";
-      return SK_ERR_NOMEM;
-    }
+  std::string perr;
+  if (!skws::genomes_fit(gbytes, budget, perr)) { ctx->err = std::string(who) + ": " + perr; return SK_ERR_NOMEM; }
   // ---- 1. screen: markers of every genome on context 0
+  sk_store_stats s{};
   const double t0 = now_s();
   std::vector<uint64_t> pairs;
   {
     SK_CUDA(cudaSetDevice(ctx->device));
-    std::vector<uint32_t> all(N);
-    for (uint32_t g = 0; g < N; g++) all[g] = g;
     sk_sketch_set* mk = nullptr;
-    SK_TRY(sk_sketch_store_gather(ctx, st, all.data(), N, SK_PACK_MARKERS_ONLY, &mk));
+    SK_TRY(gather_markers(ctx, st, &mk));
     uint64_t* p = nullptr; uint64_t np = 0;
     const int rc = sk_screen_triangle(ctx, mk, mp, &p, &np);
     sk_sketch_set_free(mk);
@@ -239,57 +240,17 @@ int sk_triangle_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store
     pairs.assign(p, p + np);
     sk_free(p);
   }
-  const double t_screen = now_s() - t0;
+  s.t_screen = now_s() - t0;
   // ---- 2. plan
   skws::Plan plan;
-  std::string perr;
-  if (!skws::plan_working_sets(pairs, gbytes, budget, plan, perr)) { ctx->err = "sk_triangle_store: " + perr; return SK_ERR_NOMEM; }
+  if (!skws::plan_working_sets(pairs, gbytes, budget, plan, perr)) { ctx->err = std::string(who) + ": " + perr; return SK_ERR_NOMEM; }
   // ---- 3. contexts take the working sets in plan order
-  const bool trace = getenv("SK_TRACE") != nullptr;
-  auto work = [&](sk_ctx* c, uint32_t d, size_t w, std::vector<sk_ani_result>& kept, WsTimes& t) {
-    const skws::WorkingSet& ws = plan.sets[w];
-    const double a = now_s();
-    sk_sketch_set* set = nullptr;
-    int rc = sk_sketch_store_gather(c, st, ws.genomes.data(), (uint32_t)ws.genomes.size(), 0, &set);
-    const double bt = now_s();
-    if (rc == SK_OK) {
-      std::vector<uint64_t> lp(ws.pairs.size());
-      for (size_t i = 0; i < lp.size(); i++) {
-        const uint64_t x = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)(ws.pairs[i] >> 32)) - ws.genomes.begin();
-        const uint64_t y = std::lower_bound(ws.genomes.begin(), ws.genomes.end(), (uint32_t)ws.pairs[i]) - ws.genomes.begin();
-        lp[i] = (x << 32) | y;
-      }
-      std::vector<sk_ani_result> res(lp.size());
-      rc = sk_chain_pairs(c, set, set, lp.data(), lp.size(), mp, res.data());
-      if (rc == SK_OK)
-        for (auto& r : res)
-          if (r.ani > 0.1f) { r.ref_id = ws.genomes[r.ref_id]; r.query_id = ws.genomes[r.query_id]; kept.push_back(r); }   // src/triangle.rs:99
-    }
-    if (set) sk_sketch_set_free(set);
-    const double ct = now_s();
-    t.gather += bt - a; t.chain += ct - bt; t.bytes += ws.bytes;
-    if (trace)
-      fprintf(stderr, "[sk_triangle_store] context %u: working set %zu/%zu%s: %zu genomes, %zu pairs, %.1f MB gathered in %.1f ms, chain %.1f ms\n", d, w + 1,
-              plan.sets.size(), ws.chunk_pair ? " (chunk pair)" : "", ws.genomes.size(), ws.pairs.size(), ws.bytes / 1e6, (bt - a) * 1e3, (ct - bt) * 1e3);
-    return rc;
-  };
-  std::vector<sk_ani_result> res;
-  WsTimes t;
-  SK_TRY(run_working_sets(ctxs, n_ctx, plan.sets.size(), work, res, t));
-  SK_TRY(hand_out(ctx, res, out, n_out));
-  if (stats) {
-    memset(stats, 0, sizeof(*stats));
-    stats->n_working_sets = (uint32_t)plan.sets.size();
-    stats->n_split_components = plan.n_split_components;
-    for (auto& ws : plan.sets) stats->max_working_set_bytes = std::max(stats->max_working_set_bytes, ws.bytes);
-    stats->t_screen = t_screen;
-    stats->gathered_bytes = t.bytes; stats->t_gather = t.gather; stats->t_chain = t.chain;
-  }
-  return SK_OK;
+  return chain_and_keep(who, ctxs, n_ctx, st, st, plan, mp, s, out, n_out, stats);
 }
 
 int sk_query_ref_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* refs, const sk_sketch_store* queries, const sk_map_params* mp,
                        int mode, uint64_t device_budget, sk_ani_result** out, uint64_t* n_out, sk_store_stats* stats) {
+  const char* const who = "sk_query_ref_store";
   if (!ctxs || n_ctx == 0 || !ctxs[0]) return SK_ERR_PARAM;
   sk_ctx* ctx = ctxs[0];
   if (!refs || !queries || !mp || !out || !n_out) { ctx->err = "sk_query_ref_store: NULL argument"; return SK_ERR_PARAM; }
@@ -303,25 +264,20 @@ int sk_query_ref_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_stor
   std::vector<uint64_t> rbytes(NR), qbytes(NQ);
   for (uint32_t g = 0; g < NR; g++) rbytes[g] = sk_sketch_store_genome_bytes(refs, g);
   for (uint32_t g = 0; g < NQ; g++) qbytes[g] = sk_sketch_store_genome_bytes(queries, g);
-  for (int side = 0; side < 2; side++) {
-    const std::vector<uint64_t>& b = side ? qbytes : rbytes;
-    for (size_t g = 0; g < b.size(); g++)
-      if (b[g] > budget / 2) {
-        ctx->err = std::string("sk_query_ref_store: ") + (side ? "query " : "reference ") + std::to_string(g) + " needs " + std::to_string(b[g]) +
-                   " device bytes, more than half the working-set budget of " + std::to_string(budget) + " bytes";
-        return SK_ERR_NOMEM;
-      }
+  std::string perr;   // split point NR: every genome of rbytes is a reference, and with split point 0 every one of qbytes a query
+  if (!skws::genomes_fit(rbytes, budget, perr, NR) || !skws::genomes_fit(qbytes, budget, perr, 0)) {
+    ctx->err = std::string(who) + ": " + perr;
+    return SK_ERR_NOMEM;
   }
   // ---- 1. screen: markers of every reference and every query on context 0
+  sk_store_stats s{};
   const double t0 = now_s();
   std::vector<uint64_t> pairs;
   if (NR && NQ) {
     SK_CUDA(cudaSetDevice(ctx->device));
     sk_sketch_set *rm = nullptr, *qm = nullptr;
-    std::vector<uint32_t> all(std::max(NR, NQ));
-    for (uint32_t g = 0; g < all.size(); g++) all[g] = g;
-    int rc = sk_sketch_store_gather(ctx, refs, all.data(), NR, SK_PACK_MARKERS_ONLY, &rm);
-    if (rc == SK_OK) rc = sk_sketch_store_gather(ctx, queries, all.data(), NQ, SK_PACK_MARKERS_ONLY, &qm);
+    int rc = gather_markers(ctx, refs, &rm);
+    if (rc == SK_OK) rc = gather_markers(ctx, queries, &qm);
     uint64_t* p = nullptr; uint64_t np = 0;
     if (rc == SK_OK) rc = sk_screen_query_ref(ctx, rm, qm, mp, mode, &p, &np);
     if (rm) sk_sketch_set_free(rm);
@@ -330,56 +286,12 @@ int sk_query_ref_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_stor
     pairs.assign(p, p + np);    // sorted (r << 32 | q)
     sk_free(p);
   }
-  const double t_screen = now_s() - t0;
+  s.t_screen = now_s() - t0;
   // ---- 2. plan
   skws::QrPlan plan;
-  std::string perr;
-  if (!skws::plan_query_ref_working_sets(pairs, rbytes, qbytes, budget, plan, perr)) { ctx->err = "sk_query_ref_store: " + perr; return SK_ERR_NOMEM; }
-  // ---- 3. contexts take the working sets in plan order: gather the references and the queries, chain, keep ani > 0.1
-  const bool trace = getenv("SK_TRACE") != nullptr;
-  auto work = [&](sk_ctx* c, uint32_t d, size_t w, std::vector<sk_ani_result>& kept, WsTimes& t) {
-    const skws::QrWorkingSet& ws = plan.sets[w];
-    const double a = now_s();
-    sk_sketch_set *R = nullptr, *Q = nullptr;
-    int rc = sk_sketch_store_gather(c, refs, ws.refs.data(), (uint32_t)ws.refs.size(), 0, &R);
-    if (rc == SK_OK) rc = sk_sketch_store_gather(c, queries, ws.queries.data(), (uint32_t)ws.queries.size(), 0, &Q);
-    const double bt = now_s();
-    if (rc == SK_OK) {
-      std::vector<uint64_t> lp(ws.pairs.size());
-      for (size_t i = 0; i < lp.size(); i++) {
-        const uint64_t x = std::lower_bound(ws.refs.begin(), ws.refs.end(), (uint32_t)(ws.pairs[i] >> 32)) - ws.refs.begin();
-        const uint64_t y = std::lower_bound(ws.queries.begin(), ws.queries.end(), (uint32_t)ws.pairs[i]) - ws.queries.begin();
-        lp[i] = (x << 32) | y;
-      }
-      std::vector<sk_ani_result> res(lp.size());
-      rc = sk_chain_pairs(c, R, Q, lp.data(), lp.size(), mp, res.data());
-      if (rc == SK_OK)
-        for (auto& r : res)
-          if (r.ani > 0.1f) { r.ref_id = ws.refs[r.ref_id]; r.query_id = ws.queries[r.query_id]; kept.push_back(r); }   // src/dist.rs:115,139
-    }
-    if (R) sk_sketch_set_free(R);
-    if (Q) sk_sketch_set_free(Q);
-    const double ct = now_s();
-    t.gather += bt - a; t.chain += ct - bt; t.bytes += ws.bytes;
-    if (trace)
-      fprintf(stderr, "[sk_query_ref_store] context %u: working set %zu/%zu%s: %zu references, %zu queries, %zu pairs, %.1f MB gathered in %.1f ms, chain %.1f ms\n",
-              d, w + 1, plan.sets.size(), ws.chunk_pair ? " (chunk pair)" : "", ws.refs.size(), ws.queries.size(), ws.pairs.size(), ws.bytes / 1e6,
-              (bt - a) * 1e3, (ct - bt) * 1e3);
-    return rc;
-  };
-  std::vector<sk_ani_result> res;
-  WsTimes t;
-  SK_TRY(run_working_sets(ctxs, n_ctx, plan.sets.size(), work, res, t));
-  SK_TRY(hand_out(ctx, res, out, n_out));
-  if (stats) {
-    memset(stats, 0, sizeof(*stats));
-    stats->n_working_sets = (uint32_t)plan.sets.size();
-    stats->n_split_components = plan.n_split_components;
-    for (auto& ws : plan.sets) stats->max_working_set_bytes = std::max(stats->max_working_set_bytes, ws.bytes);
-    stats->t_screen = t_screen;
-    stats->gathered_bytes = t.bytes; stats->t_gather = t.gather; stats->t_chain = t.chain;
-  }
-  return SK_OK;
+  if (!skws::plan_query_ref_working_sets(pairs, rbytes, qbytes, budget, plan, perr)) { ctx->err = std::string(who) + ": " + perr; return SK_ERR_NOMEM; }
+  // ---- 3. contexts take the working sets in plan order: gather the references and the queries, chain
+  return chain_and_keep(who, ctxs, n_ctx, refs, queries, plan, mp, s, out, n_out, stats);
 }
 
 }  // extern "C"

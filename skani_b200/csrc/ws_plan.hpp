@@ -1,11 +1,14 @@
-// ws_plan.hpp -- working-set planner of sk_triangle_store and sk_query_ref_store (host only, no CUDA: tests/emu/emu_ws_plan.cpp
-// and tests/emu/emu_qr_plan.cpp run it on the CPU).
+// ws_plan.hpp -- pair components, the multi-context pair split and the working-set planners of the host sketch store paths
+// (host only, no CUDA: tests/emu/emu_partition.cpp, tests/emu/emu_ws_plan.cpp and tests/emu/emu_qr_plan.cpp run them on the CPU).
+//
+// pair_components groups a sorted pair list by connected component of the pair graph (a cluster of related genomes).
+// partition_pairs splits a pair list over the contexts of sk_triangle_multi (multi.cu) by component, so that a context fetches a
+// cluster's sketches once.  genomes_fit is the one refusal of a genome over budget / 2.
 //
 // The triangle's screened pairs are cut into working sets: groups of pairs whose genomes, gathered from the host sketch
 // store, fit a device budget.  A pair's chain result depends only on its two sketches, so every pair is chained in exactly
 // one working set and the union of the working sets' results is the triangle's.
-//   1. Pairs are grouped by connected component of the pair graph (a cluster of related genomes), as partition_pairs in
-//      multi.cu does: a component's genomes are gathered once.
+//   1. Pairs are grouped by connected component (pair_components): a component's genomes are gathered once.
 //   2. A component whose genome bytes fit the budget is one item; items are packed into working sets by first-fit
 //      decreasing (largest first, ties by smallest genome id).
 //   3. A component over budget is cut, in genome-id order, into chunks of at most budget / 2 bytes.  Its working sets are the
@@ -19,6 +22,74 @@
 #include <vector>
 
 namespace skws {
+
+// The pairs of a sorted list of distinct pairs grouped by connected component of the pair graph: groups in order of their
+// root (the component's smallest genome), pairs sorted inside a group.  Group k is pairs[first[k] .. first[k + 1]).
+struct PairComponents {
+  std::vector<uint64_t> pairs;
+  std::vector<size_t> first;
+};
+
+inline PairComponents pair_components(const std::vector<uint64_t>& sorted_pairs, uint32_t n_genomes) {
+  std::vector<uint32_t> parent(n_genomes);
+  for (uint32_t g = 0; g < n_genomes; g++) parent[g] = g;
+  auto find = [&](uint32_t x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
+  for (uint64_t p : sorted_pairs) {
+    const uint32_t a = find((uint32_t)(p >> 32)), b = find((uint32_t)p);
+    if (a != b) parent[std::max(a, b)] = std::min(a, b);            // root = smallest genome of the component
+  }
+  std::vector<std::pair<uint32_t, uint64_t>> keyed(sorted_pairs.size());
+  for (size_t i = 0; i < sorted_pairs.size(); i++) keyed[i] = {find((uint32_t)(sorted_pairs[i] >> 32)), sorted_pairs[i]};
+  std::stable_sort(keyed.begin(), keyed.end(), [](const std::pair<uint32_t, uint64_t>& a, const std::pair<uint32_t, uint64_t>& b) { return a.first < b.first; });
+  PairComponents pc;
+  pc.pairs.resize(keyed.size());
+  for (size_t i = 0; i < keyed.size(); i++) {
+    if (i == 0 || keyed[i].first != keyed[i - 1].first) pc.first.push_back(i);
+    pc.pairs[i] = keyed[i].second;
+  }
+  pc.first.push_back(keyed.size());
+  return pc;
+}
+
+// Pairs -> one list per context.  The pairs of one component stay together, so a context fetches that cluster's sketches once;
+// with a genome order unrelated to relatedness a contiguous slice of the sorted list touches ~5x more genomes.  Components above
+// half a context's fair share are cut into runs of consecutive pairs; items go to the least loaded context, largest first (ties:
+// first pair).  Deterministic; every list comes out sorted.  (skani_b200/multi_gpu.py partition_pairs follows the same rule.)
+inline void partition_pairs(const std::vector<uint64_t>& sorted_pairs, uint32_t W, uint32_t n_genomes, std::vector<std::vector<uint64_t>>& out) {
+  out.assign(W, {});
+  const size_t n = sorted_pairs.size();
+  if (n == 0) return;
+  if (W == 1) { out[0] = sorted_pairs; return; }
+  const PairComponents pc = pair_components(sorted_pairs, n_genomes);
+  const size_t cap = std::max<size_t>(1, (n + 2 * (size_t)W - 1) / (2 * (size_t)W));
+  struct Item { size_t size, start; };
+  std::vector<Item> items;
+  for (size_t k = 0; k + 1 < pc.first.size(); k++)
+    for (size_t s0 = pc.first[k]; s0 < pc.first[k + 1]; s0 += cap) items.push_back(Item{std::min(cap, pc.first[k + 1] - s0), s0});
+  std::sort(items.begin(), items.end(), [&](const Item& a, const Item& b) { return a.size != b.size ? a.size > b.size : pc.pairs[a.start] < pc.pairs[b.start]; });
+  std::vector<size_t> load(W, 0);
+  for (const Item& it : items) {
+    uint32_t r = 0;
+    for (uint32_t k = 1; k < W; k++) if (load[k] < load[r]) r = k;
+    out[r].insert(out[r].end(), pc.pairs.begin() + it.start, pc.pairs.begin() + it.start + it.size);
+    load[r] += it.size;
+  }
+  for (auto& v : out) std::sort(v.begin(), v.end());
+}
+
+// false (and the refusal in err) if a genome is larger than budget / 2: it cannot be placed in every chunk pair.  Genome g is
+// named "genome g"; with a split point n_refs >= 0, genomes [0, n_refs) are "reference g" and genome n_refs + q is "query q".
+inline bool genomes_fit(const std::vector<uint64_t>& genome_bytes, uint64_t budget, std::string& err, int64_t n_refs = -1) {
+  for (uint64_t g = 0; g < genome_bytes.size(); g++)
+    if (genome_bytes[g] > budget / 2) {
+      const std::string name = n_refs < 0 ? "genome " + std::to_string(g)
+                               : g < (uint64_t)n_refs ? "reference " + std::to_string(g) : "query " + std::to_string(g - n_refs);
+      err = name + " needs " + std::to_string(genome_bytes[g]) + " device bytes, more than half the working-set budget of " +
+            std::to_string(budget) + " bytes";
+      return false;
+    }
+  return true;
+}
 
 struct WorkingSet {
   std::vector<uint32_t> genomes;   // ascending global genome ids
@@ -37,38 +108,19 @@ struct Plan {
 inline bool plan_working_sets(const std::vector<uint64_t>& sorted_pairs, const std::vector<uint64_t>& genome_bytes, uint64_t budget,
                               Plan& plan, std::string& err) {
   plan = Plan();
-  const uint32_t n = (uint32_t)genome_bytes.size();
-  for (uint32_t g = 0; g < n; g++)
-    if (genome_bytes[g] > budget / 2) {
-      err = "genome " + std::to_string(g) + " needs " + std::to_string(genome_bytes[g]) + " device bytes, more than half the working-set budget of " +
-            std::to_string(budget) + " bytes";
-      return false;
-    }
+  if (!genomes_fit(genome_bytes, budget, err)) return false;
   if (sorted_pairs.empty()) return true;
-  // connected components, root = smallest genome of the component
-  std::vector<uint32_t> parent(n);
-  for (uint32_t g = 0; g < n; g++) parent[g] = g;
-  auto find = [&](uint32_t x) { while (parent[x] != x) { parent[x] = parent[parent[x]]; x = parent[x]; } return x; };
-  for (uint64_t p : sorted_pairs) {
-    const uint32_t a = find((uint32_t)(p >> 32)), b = find((uint32_t)p);
-    if (a != b) parent[std::max(a, b)] = std::min(a, b);
-  }
-  // pairs grouped by component (stable: sorted inside a group)
-  std::vector<std::pair<uint32_t, uint64_t>> keyed(sorted_pairs.size());
-  for (size_t i = 0; i < sorted_pairs.size(); i++) keyed[i] = {find((uint32_t)(sorted_pairs[i] >> 32)), sorted_pairs[i]};
-  std::stable_sort(keyed.begin(), keyed.end(), [](const std::pair<uint32_t, uint64_t>& a, const std::pair<uint32_t, uint64_t>& b) { return a.first < b.first; });
-  struct Comp { uint32_t root; size_t p0, p1; std::vector<uint32_t> genomes; uint64_t bytes = 0; };
+  const uint32_t n = (uint32_t)genome_bytes.size();
+  const PairComponents pc = pair_components(sorted_pairs, n);
+  struct Comp { size_t p0, p1; std::vector<uint32_t> genomes; uint64_t bytes = 0; };
   std::vector<Comp> comps;
-  for (size_t i = 0; i < keyed.size();) {
-    size_t j = i;
-    while (j < keyed.size() && keyed[j].first == keyed[i].first) j++;
-    Comp c; c.root = keyed[i].first; c.p0 = i; c.p1 = j;
-    for (size_t k = i; k < j; k++) { c.genomes.push_back((uint32_t)(keyed[k].second >> 32)); c.genomes.push_back((uint32_t)keyed[k].second); }
+  for (size_t k = 0; k + 1 < pc.first.size(); k++) {
+    Comp c; c.p0 = pc.first[k]; c.p1 = pc.first[k + 1];
+    for (size_t i = c.p0; i < c.p1; i++) { c.genomes.push_back((uint32_t)(pc.pairs[i] >> 32)); c.genomes.push_back((uint32_t)pc.pairs[i]); }
     std::sort(c.genomes.begin(), c.genomes.end());
     c.genomes.erase(std::unique(c.genomes.begin(), c.genomes.end()), c.genomes.end());
     for (uint32_t g : c.genomes) c.bytes += genome_bytes[g];
     comps.push_back(std::move(c));
-    i = j;
   }
   // components that fit: first-fit decreasing
   std::vector<size_t> fit;
@@ -87,7 +139,7 @@ inline bool plan_working_sets(const std::vector<uint64_t>& sorted_pairs, const s
     WorkingSet ws;
     for (size_t c : bins[b]) {
       ws.genomes.insert(ws.genomes.end(), comps[c].genomes.begin(), comps[c].genomes.end());
-      for (size_t k = comps[c].p0; k < comps[c].p1; k++) ws.pairs.push_back(keyed[k].second);
+      ws.pairs.insert(ws.pairs.end(), pc.pairs.begin() + comps[c].p0, pc.pairs.begin() + comps[c].p1);
     }
     std::sort(ws.genomes.begin(), ws.genomes.end());
     std::sort(ws.pairs.begin(), ws.pairs.end());
@@ -110,7 +162,7 @@ inline bool plan_working_sets(const std::vector<uint64_t>& sorted_pairs, const s
     // pairs by chunk pair (x, y), x <= y because i < j and chunks follow genome order
     std::vector<std::pair<uint64_t, uint64_t>> byc;
     for (size_t k = c.p0; k < c.p1; k++) {
-      const uint64_t p = keyed[k].second;
+      const uint64_t p = pc.pairs[k];
       byc.push_back({((uint64_t)chunk_of[(uint32_t)(p >> 32)] << 32) | chunk_of[(uint32_t)p], p});
     }
     std::sort(byc.begin(), byc.end());
@@ -158,12 +210,7 @@ inline bool plan_query_ref_working_sets(const std::vector<uint64_t>& sorted_pair
   if (NR + query_bytes.size() >= (1ull << 32)) { err = "more than 2^32 references and queries together"; return false; }
   std::vector<uint64_t> bytes(ref_bytes);
   bytes.insert(bytes.end(), query_bytes.begin(), query_bytes.end());
-  for (uint64_t g = 0; g < bytes.size(); g++)
-    if (bytes[g] > budget / 2) {
-      err = (g < NR ? "reference " + std::to_string(g) : "query " + std::to_string(g - NR)) + " needs " + std::to_string(bytes[g]) +
-            " device bytes, more than half the working-set budget of " + std::to_string(budget) + " bytes";
-      return false;
-    }
+  if (!genomes_fit(bytes, budget, err, (int64_t)NR)) return false;
   std::vector<uint64_t> pairs(sorted_pairs_rq.size());
   for (size_t i = 0; i < pairs.size(); i++) pairs[i] = sorted_pairs_rq[i] + NR;   // (r << 32) | (NR + q)
   Plan p;
