@@ -548,6 +548,14 @@ typedef struct {
 } sk_nj_stats;
 int sk_neighbor_joining(sk_ctx* ctx, uint32_t n_genomes, const sk_ani_result* results, uint64_t n_results, sk_nj_join* joins,
                         sk_nj_stats* stats /* may be NULL */);
+/* sk_neighbor_joining with the matrix split over n_ctx contexts (distinct devices, or several contexts on one device):
+ * joins and stats (but t_device) are byte for byte sk_neighbor_joining(ctxs[0], ...)'s for any n_ctx >= 1.  Each context
+ * holds full rows of a band of slots, about 8 n^2 (1 + 9/16) / n_ctx bytes; the contexts exchange the step's minima and two
+ * columns (16 bytes per live node) through peer copies.  The edges are built on ctxs[0], with sk_neighbor_joining's
+ * refusals and messages there.  NULL or repeated contexts give SK_ERR_PARAM, and a failure on context d is reported on
+ * ctxs[0] as "context d: ...".  One host thread drives every context. */
+int sk_neighbor_joining_multi(sk_ctx* const* ctxs, uint32_t n_ctx, uint32_t n_genomes, const sk_ani_result* results, uint64_t n_results,
+                              sk_nj_join* joins, sk_nj_stats* stats /* may be NULL */);
 
 /* ---- greedy dereplication of an in-memory sketch set (what galah and dRep do on top of skani): sk_cluster's greedy
  *      representatives without the triangle.  Only genome x representative pairs are screened and chained.

@@ -150,6 +150,7 @@ SYMBOLS = [
     ("sk_cluster", i32, [vp, u32, vp, u64, vp, PP(ClusterParams), vp, vp, vp, PP(ClusterStats)]),
     ("sk_cluster_linkage", i32, [vp, u32, vp, u64, vp, PP(LinkageParams), vp, vp, vp, vp, PP(ClusterStats)]),
     ("sk_neighbor_joining", i32, [vp, u32, vp, u64, vp, PP(NjStats)]),
+    ("sk_neighbor_joining_multi", i32, [vp, u32, u32, vp, u64, vp, PP(NjStats)]),
     ("sk_dereplicate", i32, [vp, vp, PP(MapParams), vp, PP(DerepParams), vp, vp, vp, PP(DerepStats)]),
     ("sk_dereplicate_store", i32, [vp, u32, vp, PP(MapParams), vp, PP(DerepParams), u64, vp, vp, vp, PP(DerepStats), PP(StoreStats)]),
 ]

@@ -1028,7 +1028,7 @@ std::string newick(uint32_t n_leaves, const std::vector<std::string>& labels,
 }
 
 // tree: the triangle's genomes (every row `triangle -E` prints) as a Newick tree, branch lengths in percent distance.
-// --method nj (default): sk_neighbor_joining, written unrooted with the basal trifurcation (X, Y, K): X and Y the children
+// --method nj (default): sk_neighbor_joining (with --gpus N > 1 sk_neighbor_joining_multi on N contexts, the same tree), written unrooted with the basal trifurcation (X, Y, K): X and Y the children
 // of the last internal node, K the other last node at the full last-edge length.  --method average | complete:
 // sk_cluster_linkage's dendrogram (genomes ranked as cluster ranks them), rooted, a child at (h_parent - h_child) / 2 below
 // its parent, so that patristic distances are the cophenetic ones.  Labels as triangle's matrix names its rows.
@@ -1054,10 +1054,18 @@ int run_tree(Opts& op) {
   std::vector<std::vector<std::pair<uint32_t, double>>> kids(N ? 2 * N : 0);   // node 2N - 1: the NJ trifurcation
   uint32_t root = N ? 2 * N - 2 : 0, steps = 0;
   double t_device = 0;
+  size_t n_ctx = 1;
   if (op.tree_method == "nj") {
     std::vector<sk_nj_join> joins(N > 1 ? N - 1 : 0);
     sk_nj_stats st{};
-    CK(ctx, sk_neighbor_joining(ctx, N, res.data(), res.size(), joins.empty() ? nullptr : joins.data(), &st));
+    if (op.gpus > 1) {   // the distance matrix split over one context per GPU
+      std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, op.gpus);
+      n_ctx = ctxs.size();
+      CK(ctx, sk_neighbor_joining_multi(ctxs.data(), (uint32_t)n_ctx, N, res.data(), res.size(), joins.empty() ? nullptr : joins.data(), &st));
+      for (size_t d = 1; d < ctxs.size(); d++) sk_ctx_destroy(ctxs[d]);
+    } else {
+      CK(ctx, sk_neighbor_joining(ctx, N, res.data(), res.size(), joins.empty() ? nullptr : joins.data(), &st));
+    }
     for (uint32_t t = 0; t < joins.size(); t++) kids[N + t] = {{joins[t].a, joins[t].len_a}, {joins[t].b, joins[t].len_b}};
     if (N >= 3) {   // unroot: the last internal node's children and the other last node, at the whole last edge
       const sk_nj_join& l = joins[N - 2];
@@ -1089,8 +1097,9 @@ int run_tree(Opts& op) {
   if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
   if (N) fputs(newick(N, labels, kids, root).c_str(), o);
   if (o != stdout) fclose(o);
-  fprintf(stderr, "INFO %u genomes, tree by %s (%u %s), %.1f ms on the device\n", N, op.tree_method.c_str(), steps,
-          op.tree_method == "nj" ? "compactions" : "rounds", t_device * 1e3);
+  const std::string on = n_ctx > 1 ? " on " + std::to_string(n_ctx) + " contexts" : "";
+  fprintf(stderr, "INFO %u genomes, tree by %s (%u %s)%s, %.1f ms on the device\n", N, op.tree_method.c_str(), steps,
+          op.tree_method == "nj" ? "compactions" : "rounds", on.c_str(), t_device * 1e3);
   sk_ctx_destroy(ctx);
   return 0;
 }

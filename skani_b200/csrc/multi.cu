@@ -24,6 +24,7 @@
 #include "store_ws.hpp"
 
 using sk::now_s;
+using sk::enable_peer_access;
 
 extern "C" int sk_triangle_local(sk_ctx* ctx, const uint8_t* bases, const uint64_t* contig_off, uint32_t n_contigs,
                                  const uint32_t* genome_of_contig, uint32_t n_genomes, const sk_sketch_params* sp,
@@ -86,18 +87,6 @@ int unpack_blobs(const char* who, sk_ctx* ctx, const std::vector<const Blob*>& b
   if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
   if (e != cudaSuccess) { ctx->err = std::string(who) + ": " + cudaGetErrorString(e); return SK_ERR_CUDA; }
   return sk_sketch_set_unpack(ctx, (uint32_t)n, bp.data(), mp.data(), out);
-}
-
-// peer access between the distinct devices of ctxs[0..n) (ignored when unsupported: copies then stage through the host)
-void enable_peer_access(sk_ctx* const* ctxs, uint32_t n) {
-  for (uint32_t a = 0; a < n; a++)
-    for (uint32_t b = 0; b < n; b++)
-      if (ctxs[a]->device != ctxs[b]->device) {
-        cudaSetDevice(ctxs[a]->device);
-        int can = 0;
-        if (cudaDeviceCanAccessPeer(&can, ctxs[a]->device, ctxs[b]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[b]->device, 0);
-        cudaGetLastError();
-      }
 }
 
 }  // namespace

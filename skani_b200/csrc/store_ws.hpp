@@ -1,6 +1,6 @@
 // store_ws.hpp -- working-set execution shared by the host sketch store paths (store.cu: sk_triangle_store,
 // sk_query_ref_store; derep.cu: sk_dereplicate_store) and the multi-context calls of multi.cu: the context checks, one host
-// thread per context, the per-context device budget, the markers-only gather of a whole store, chaining global pairs on a
+// thread per context, peer access, the per-context device budget, the markers-only gather of a whole store, chaining global pairs on a
 // gathered working set, and chain_working_sets, the one driver that gathers and chains a plan (ws_plan.hpp) on the contexts.
 #pragma once
 #include <algorithm>
@@ -38,6 +38,18 @@ inline int check_contexts(sk_ctx* const* ctxs, uint32_t n_ctx) {
       if (ctxs[e] == ctxs[d]) { ctxs[0]->err = "context " + std::to_string(d) + ": the same context appears twice (one host thread per context)"; return SK_ERR_PARAM; }
   }
   return SK_OK;
+}
+
+// peer access between the distinct devices of ctxs[0..n) (ignored when unsupported: copies then stage through the host)
+inline void enable_peer_access(sk_ctx* const* ctxs, uint32_t n) {
+  for (uint32_t a = 0; a < n; a++)
+    for (uint32_t b = 0; b < n; b++)
+      if (ctxs[a]->device != ctxs[b]->device) {
+        cudaSetDevice(ctxs[a]->device);
+        int can = 0;
+        if (cudaDeviceCanAccessPeer(&can, ctxs[a]->device, ctxs[b]->device) == cudaSuccess && can) cudaDeviceEnablePeerAccess(ctxs[b]->device, 0);
+        cudaGetLastError();
+      }
 }
 
 // fn(d) on one host thread per context (inline for one context), ctxs[d]'s device current.  The call fails if any context

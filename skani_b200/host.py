@@ -764,6 +764,21 @@ def neighbor_joining(ctx, n_genomes, results):
     return joins[:max(n - 1, 0)], st
 
 
+def neighbor_joining_multi(ctxs, n_genomes, results):
+    """sk_neighbor_joining_multi: neighbor_joining with the distance matrix split over the contexts ctxs (one band of rows
+    each).  Returns (joins, stats) equal to neighbor_joining(ctxs[0], ...)'s; errors are reported on ctxs[0]."""
+    res = np.ascontiguousarray(results)
+    if res.dtype != RESULT_DTYPE:
+        raise TypeError("results must be a RESULT_DTYPE array")
+    n = int(n_genomes)
+    joins = np.zeros(max(n - 1, 1), NJ_JOIN_DTYPE)
+    st = NjStats()
+    hs = (C.c_void_p * len(ctxs))(*[None if c is None else c.h for c in ctxs])
+    c0 = ctxs[0]
+    c0.check(c0.L.sk_neighbor_joining_multi(hs, len(ctxs), n, res.ctypes.data if len(res) else None, len(res), joins.ctypes.data, C.byref(st)))
+    return joins[:max(n - 1, 0)], st
+
+
 def dereplicate(ctx, sset, rank, min_ani=0.95, mp=None, wave=0):
     """sk_dereplicate: greedy ANI dereplication of a sketch set, equal to cluster() (greedy) on the rows of screen_triangle +
     chain_pairs over the same set and mp, but screening and chaining only genome x representative pairs.  rank[g] is a

@@ -6,13 +6,16 @@
    call per graph, then --reps timed calls (host clock around the call, which ends in a device synchronise; t_device from
    the stats).  Next to each time: the bytes the scan has to read, the sum over the steps of the pairs of the square it scans
    (the live nodes' square, compacted to at most 4/3 of them) times 8 B, and that over the call's time.  At n <= 1 500 the
-   CPU reference of the tests (tests/nj_ref.py) runs once and its join table must be equal bit for bit.
+   CPU reference of the tests (tests/nj_ref.py) runs once and its join table must be equal bit for bit.  With --gpus N > 1
+   each rep also times sk_neighbor_joining_multi (skani_b200.neighbor_joining_multi) on N contexts, context d on device
+   d % the visible devices (so contexts share a device when fewer are visible), alternating with the one-context call; its
+   join table must equal the one-context table byte for byte.
 2. End to end: `tree` against `triangle --full-matrix --distance` on a seeded synthetic set (bench_support/synth, the set
    tools/bench_cluster.py uses; default 1 000 x 5 Mbp) written as one FASTA file per genome, the two commands alternated
    --reps times (wall time of the process).
 
-  python tools/bench_tree.py [--sizes 1500,5000,10000,20000] [--reps 2] [--genomes 1000] [--length 5000000] [--skip-e2e]
-                             [--skip-lib] [--json OUT]
+  python tools/bench_tree.py [--sizes 1500,5000,10000,20000] [--reps 2] [--gpus 1] [--genomes 1000] [--length 5000000]
+                             [--skip-e2e] [--skip-lib] [--json OUT]
 The FASTA files go to a temporary directory that is removed at the end."""
 import argparse
 import json
@@ -54,25 +57,34 @@ def emit(rec, sink):
     sink.append(rec)
 
 
-def bench_lib(sizes, reps, sink):
+def bench_lib(sizes, reps, gpus, sink):
     import skani_b200 as sk
     import cluster_ref as R
     import nj_ref as N
     ctx = sk.Context(0)
+    ndev = max(ctx.L.sk_device_count(), 1)
+    devs = [d % ndev for d in range(gpus)]
+    ctxs = [ctx] + [sk.Context(dev) for dev in devs[1:]]
     rng = np.random.default_rng(20261017)
     for n in sizes:
         g_n, a, b, ani = R.families(rng, n, 20, 10 * n - (n // 20) * 190, inside=(0.95, 1.0))
         res = R.as_results(a, b, ani)
-        base, _ = sk.neighbor_joining(ctx, g_n, res)     # warm-up
+        calls = {1: lambda: sk.neighbor_joining(ctx, g_n, res)}
+        if gpus > 1:
+            calls[gpus] = lambda: sk.neighbor_joining_multi(ctxs, g_n, res)
+        base, _ = calls[1]()     # warm-up
+        for call in list(calls.values())[1:]:
+            call()
         nbytes = scan_bytes(g_n)
         for rep in range(reps):
-            t = time.perf_counter()
-            joins, st = sk.neighbor_joining(ctx, g_n, res)
-            wall = time.perf_counter() - t
-            assert joins.tobytes() == base.tobytes()
-            emit({"bench": "nj", "genomes": g_n, "rows": len(res), "rep": rep, "wall_s": round(wall, 4),
-                  "t_device_s": round(st.t_device, 4), "compactions": st.compactions, "scan_bytes": nbytes,
-                  "scan_GB_per_s": round(nbytes / wall / 1e9, 1)}, sink)
+            for k, call in calls.items():
+                t = time.perf_counter()
+                joins, st = call()
+                wall = time.perf_counter() - t
+                assert joins.tobytes() == base.tobytes()
+                emit({"bench": "nj", "genomes": g_n, "rows": len(res), "contexts": k, "devices": len(set(devs[:k])),
+                      "rep": rep, "wall_s": round(wall, 4), "t_device_s": round(st.t_device, 4), "compactions": st.compactions,
+                      "scan_bytes": nbytes, "scan_GB_per_s": round(nbytes / wall / 1e9, 1)}, sink)
         if g_n <= 1500:
             t = time.perf_counter()
             want = N.nj_results(g_n, a, b, ani)
@@ -80,7 +92,8 @@ def bench_lib(sizes, reps, sink):
                   "equal": want.tobytes() == base.tobytes()}, sink)
             if want.tobytes() != base.tobytes():
                 raise SystemExit("the GPU join table differs from the CPU reference at n = %d" % g_n)
-    ctx.close()
+    for c in ctxs:
+        c.close()
 
 
 def bench_e2e(n, L, reps, sink):
@@ -112,6 +125,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", default="1500,5000,10000,20000")
     ap.add_argument("--reps", type=int, default=2)
+    ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--genomes", type=int, default=1000)
     ap.add_argument("--length", type=int, default=5_000_000)
     ap.add_argument("--skip-e2e", action="store_true")
@@ -121,7 +135,7 @@ def main():
     sink = []
     emit({"card": card()}, sink)
     if not a.skip_lib:
-        bench_lib([int(x) for x in a.sizes.split(",")], a.reps, sink)
+        bench_lib([int(x) for x in a.sizes.split(",")], a.reps, a.gpus, sink)
     if not a.skip_e2e:
         bench_e2e(a.genomes, a.length, a.reps, sink)
     if a.json:
