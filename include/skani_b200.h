@@ -321,6 +321,20 @@ int sk_debug_chain_anchors(sk_ctx* ctx, uint32_t c, uint32_t k, uint64_t n_pairs
 int sk_debug_select_intervals(sk_ctx* ctx, uint32_t c, uint32_t k, uint64_t n_pairs, const uint64_t* pair_iv_off,
                               const int64_t* intervals, const uint32_t* pair_chunks, const uint32_t* switched,
                               sk_chain_debug* out /* n_pairs */, uint32_t* pair_sums /* 2 x n_pairs */);
+/* (test use) sk_dereplicate's marker index and row screen on given genome lists.  Slot s of the index holds genome
+ * slot_genome[s] of set (markers only are read); the slots join it in n_batches index additions of batch_sizes[b] genomes
+ * each (summing to n_slots), as the waves add representatives, merging each batch into the keys built so far.  Then rows
+ * (genome ids) are screened against the index: upper = 0 screens every slot, which gives the triangle's screen pairs with one
+ * genome in rows and the other in slot_genome when the two lists share no genome; upper != 0 screens row k against the slots
+ * above k, which requires rows == slot_genome and gives the triangle's pairs inside the list.  *pairs (malloc'd, sk_free;
+ * never NULL) receives the *n_pairs passing pairs as min << 32 | max, sorted.  keys / n_keys (may both be NULL): the index's
+ * keys, marker << 22 | slot, ascending (malloc'd, sk_free).  bucket (may be NULL): its 2^16 + 1 prefix buckets.  Refusals
+ * (SK_ERR_PARAM with a message): NULL arguments, a genome id >= the set's genomes, batch sizes not summing to n_slots,
+ * upper with rows other than slot_genome, and sk_dereplicate's index limits (more than 2^22 - 1 slots, 2^31 or more keys). */
+int sk_debug_derep_screen(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* slot_genome,
+                          uint32_t n_slots, const uint32_t* batch_sizes, uint32_t n_batches, const uint32_t* rows, uint32_t n_rows,
+                          int upper, uint64_t** pairs, uint64_t* n_pairs, uint64_t** keys /* may be NULL */,
+                          uint64_t* n_keys /* may be NULL */, uint32_t* bucket /* 2^16 + 1, may be NULL */);
 
 /* ---- whole triangle (src/triangle.rs:13-105: sketch -> screen -> chain -> keep ani > 0.1) from HOST sequence
  *      buffers; results malloc'd (sk_free).  Timing breakdown (seconds, device events) optional. -------------- */

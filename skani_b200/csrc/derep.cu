@@ -195,6 +195,13 @@ struct Run {
   std::vector<uint64_t> chained;     // their pair keys
   sk_derep_stats st{};
 
+  // every genome's marker offsets on the device (d_off), which the index and the row screens read
+  int upload_offsets() {
+    SK_TRY(cl_alloc(ctx, d_off, (uint64_t)N + 1, "marker offsets", who));
+    SK_CUDA(h2d_small(ctx, d_off.p, set->mk_off.data(), ((size_t)N + 1) * 8));
+    return SK_OK;
+  }
+
   // genomes list[0 .. m) (host; d_list the same on the device) join ix as slots ix.slots ..
   int index_add(Index& ix, const uint32_t* list, const uint32_t* d_list, uint32_t m) {
     if (!m) return SK_OK;
@@ -335,14 +342,13 @@ struct Run {
     for (uint32_t g = 0; g < N; g++) order[rank[g]] = g;
     DTmp<uint32_t> d_order;
     Index reps;
-    SK_TRY(cl_alloc(ctx, d_off, (uint64_t)N + 1, "marker offsets", who));
+    SK_TRY(upload_offsets());
     SK_TRY(cl_alloc(ctx, d_rank, N, "ranks", who));
     SK_TRY(cl_alloc(ctx, d_order, N, "rank order", who));
     SK_TRY(cl_alloc(ctx, state, N, "states", who));
     SK_TRY(cl_alloc(ctx, reps.bucket, (1u << DR_PREFIX_BITS) + 1, "index buckets", who));
     SK_TRY(cl_alloc(ctx, reps.slot_genome, N, "index slots", who));
     SK_CUDA(cudaMemsetAsync(reps.bucket.p, 0, ((1u << DR_PREFIX_BITS) + 1) * 4, s));
-    SK_CUDA(h2d_small(ctx, d_off.p, set->mk_off.data(), ((size_t)N + 1) * 8));
     SK_CUDA(h2d_small(ctx, d_rank.p, rank, (size_t)N * 4));
     SK_CUDA(h2d_small(ctx, d_order.p, order.data(), (size_t)N * 4));
     SK_CUDA(cudaMemsetAsync(state.p, CL_UNDECIDED, N, s));
@@ -482,6 +488,57 @@ int sk_dereplicate(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* m
   const int rc = r.run(rank, wave, rep, cluster, join);
   if (rc == SK_OK && stats) *stats = r.st;
   return rc;
+}
+
+int sk_debug_derep_screen(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* slot_genome,
+                          uint32_t n_slots, const uint32_t* batch_sizes, uint32_t n_batches, const uint32_t* rows, uint32_t n_rows,
+                          int upper, uint64_t** pairs, uint64_t* n_pairs, uint64_t** keys, uint64_t* n_keys, uint32_t* bucket) {
+  const char* const who = "sk_debug_derep_screen";
+  if (!ctx) return SK_ERR_PARAM;
+  if (!set || !mp || !pairs || !n_pairs || (n_slots && !slot_genome) || (n_batches && !batch_sizes) || (n_rows && !rows) ||
+      (!keys != !n_keys)) {
+    ctx->err = std::string(who) + ": NULL argument"; return SK_ERR_PARAM;
+  }
+  const uint32_t G = set->G;
+  for (uint32_t i = 0; i < n_slots; i++)
+    if (slot_genome[i] >= G) { ctx->err = std::string(who) + ": slot " + std::to_string(i) + " holds genome " + std::to_string(slot_genome[i]) + " >= " + std::to_string(G); return SK_ERR_PARAM; }
+  for (uint32_t i = 0; i < n_rows; i++)
+    if (rows[i] >= G) { ctx->err = std::string(who) + ": row " + std::to_string(i) + " is genome " + std::to_string(rows[i]) + " >= " + std::to_string(G); return SK_ERR_PARAM; }
+  uint64_t sum = 0;
+  for (uint32_t b = 0; b < n_batches; b++) sum += batch_sizes[b];
+  if (sum != n_slots) { ctx->err = std::string(who) + ": batch sizes sum to " + std::to_string(sum) + ", not n_slots = " + std::to_string(n_slots); return SK_ERR_PARAM; }
+  if (upper && (n_rows != n_slots || !std::equal(rows, rows + n_rows, slot_genome))) {
+    ctx->err = std::string(who) + ": upper needs rows equal to slot_genome"; return SK_ERR_PARAM;
+  }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  Run r{ctx, set, mp, 0.f, screen_cutoff(mp), G, who};
+  SK_TRY(r.upload_offsets());
+  Index ix;
+  DTmp<uint32_t> d_slots, d_rows;
+  SK_TRY(cl_alloc(ctx, ix.bucket, (1u << DR_PREFIX_BITS) + 1, "index buckets", who));
+  SK_TRY(cl_alloc(ctx, ix.slot_genome, n_slots, "index slots", who));
+  SK_TRY(cl_alloc(ctx, d_slots, n_slots, "slot list", who));
+  SK_TRY(cl_alloc(ctx, d_rows, n_rows, "rows", who));
+  SK_CUDA(cudaMemsetAsync(ix.bucket.p, 0, ((1u << DR_PREFIX_BITS) + 1) * 4, ctx->stream));
+  SK_CUDA(h2d_small(ctx, d_slots.p, slot_genome, (size_t)n_slots * 4));
+  SK_CUDA(h2d_small(ctx, d_rows.p, rows, (size_t)n_rows * 4));
+  for (uint32_t b = 0, at = 0; b < n_batches; at += batch_sizes[b++]) SK_TRY(r.index_add(ix, slot_genome + at, d_slots.p + at, batch_sizes[b]));
+  DTmp<uint64_t> d_pairs;
+  uint64_t n = 0;
+  SK_TRY(r.screen(ix, d_rows.p, n_rows, upper != 0, d_pairs, &n));
+  uint64_t* hp = (uint64_t*)malloc(std::max<uint64_t>(n, 1) * 8);
+  uint64_t* hk = keys ? (uint64_t*)malloc(std::max<uint64_t>(ix.n, 1) * 8) : nullptr;
+  if (!hp || (keys && !hk)) { free(hp); free(hk); ctx->err = std::string(who) + ": out of host memory"; return SK_ERR_NOMEM; }
+  cudaError_t e = cudaSuccess;
+  if (n) e = cudaMemcpyAsync(hp, d_pairs.p, n * 8, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess && hk && ix.n) e = cudaMemcpyAsync(hk, ix.key[ix.cur].p, ix.n * 8, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess && bucket) e = cudaMemcpyAsync(bucket, ix.bucket.p, ((1u << DR_PREFIX_BITS) + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e != cudaSuccess) { free(hp); free(hk); ctx->err = std::string(who) + ": " + cudaGetErrorString(e); return SK_ERR_CUDA; }
+  *pairs = hp;
+  *n_pairs = n;
+  if (keys) { *keys = hk; *n_keys = ix.n; }
+  return SK_OK;
 }
 
 namespace {

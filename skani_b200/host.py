@@ -535,6 +535,28 @@ def debug_select_intervals(ctx, c, k, pairs, n_chunks, switched=0):
                         (ctx.h, c, k, len(pairs), off.ctypes.data, x.ctypes.data, nc.ctypes.data), switched)
 
 
+def debug_derep_screen(ctx, sset, slot_genome, rows, upper=False, batches=None, mp=None):
+    """sk_debug_derep_screen: dereplicate's marker index over the slots slot_genome (genome ids), built in index additions of
+    batches[b] slots (default: one), and its row screen of rows (upper: rows == slot_genome, row k against the slots above
+    k).  Returns (pairs, keys, bucket): the sorted min << 32 | max pairs that pass, the index keys marker << 22 | slot and the
+    2^16 + 1 prefix buckets."""
+    mp = mp or map_params()
+    sg = np.ascontiguousarray(slot_genome, np.uint32)
+    rw = np.ascontiguousarray(rows, np.uint32)
+    bs = np.ascontiguousarray([len(sg)] if batches is None else batches, np.uint32)
+    pp, kp = C.POINTER(C.c_uint64)(), C.POINTER(C.c_uint64)()
+    n, nk = C.c_uint64(), C.c_uint64()
+    bucket = np.zeros((1 << 16) + 1, np.uint32)
+    ctx.check(ctx.L.sk_debug_derep_screen(ctx.h, sset.h, C.byref(mp), sg.ctypes.data if len(sg) else None, len(sg),
+                                          bs.ctypes.data if len(bs) else None, len(bs), rw.ctypes.data if len(rw) else None, len(rw),
+                                          int(bool(upper)), C.byref(pp), C.byref(n), C.byref(kp), C.byref(nk), bucket.ctypes.data))
+    take = lambda p, m: np.ctypeslib.as_array(p, shape=(m,)).copy() if m else np.zeros(0, np.uint64)
+    pairs, keys = take(pp, n.value), take(kp, nk.value)
+    ctx.L.sk_free(pp)
+    ctx.L.sk_free(kp)
+    return pairs, keys, bucket
+
+
 def triangle(ctx, bases, contig_off, genome_of_contig, n_genomes, sp=None, mp=None, as_array=False):
     """Whole `skani triangle` hot path from host buffers (reference src/triangle.rs:13-105)."""
     sp = sp or sketch_params(); mp = mp or map_params()
