@@ -627,6 +627,33 @@ int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_st
                          const sk_derep_params* dp, uint64_t device_budget, uint32_t* rep, uint32_t* cluster, sk_ani_result* join,
                          sk_derep_stats* stats /* may be NULL */, sk_store_stats* store_stats /* may be NULL */);
 
+/* sk_dereplicate_fixed / sk_dereplicate_store_fixed: dereplication that adds genomes to an existing set of representatives.
+ * F = { g : rank[g] < n_fixed } are fixed representatives (an earlier run's representatives, a curated catalogue).
+ * Contract: rep, cluster and join are what sk_cluster (greedy, same min_ani and rank) returns on the rows of
+ * sk_screen_triangle + sk_chain_pairs over the same set and name ranks after every row whose two genomes are both in F is
+ * removed; join[g] of a member is byte for byte the row sk_cluster's edge[g] points to, a representative's join is as in
+ * sk_dereplicate.  So every genome of F is a representative, even when two of them are joined by an edge; F takes cluster
+ * ids 0 .. n_fixed - 1 in rank order and the new clusters follow.  When no two genomes of F share an edge (always the case
+ * when F is the representative set of an earlier run at the same threshold and parameters) the result is
+ * sk_dereplicate(set, rank)'s.  n_fixed = 0 is sk_dereplicate (sk_dereplicate_store) exactly: outputs, stats and launches.
+ * Algorithm: before the first wave F's states are set to representative and its markers form the representative index;
+ * the waves cover ranks n_fixed .. N - 1, their wave-size schedule starting at the first genome outside F.  Each wave and the
+ * final members x representatives screen run as in sk_dereplicate, F being part of the index from the start.  No pair inside
+ * F is ever screened or chained: pairs_screened and pairs_chained count only pairs with a genome outside F, and waves only
+ * the waves of genomes outside F (n_fixed = N: no wave, no pair).
+ * The result does not depend on dp->wave, device_budget or the context list; the store call equals the in-memory call on one
+ * set holding every genome of the store with the same name ranks, stats counts included, as sk_dereplicate_store does.
+ * Refusals (SK_ERR_PARAM with a message): n_fixed > n_genomes, plus sk_dereplicate's / sk_dereplicate_store's.  The index
+ * limits include F: at most 2^22 - 1 representatives (fixed plus new) and fewer than 2^31 markers in the index; when F
+ * alone is over a limit the message names the fixed representatives. */
+int sk_dereplicate_fixed(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* rank, uint32_t n_fixed,
+                         const sk_derep_params* dp, uint32_t* rep, uint32_t* cluster, sk_ani_result* join,
+                         sk_derep_stats* stats /* may be NULL */);
+int sk_dereplicate_store_fixed(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp,
+                               const uint32_t* rank, uint32_t n_fixed, const sk_derep_params* dp, uint64_t device_budget,
+                               uint32_t* rep, uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats /* may be NULL */,
+                               sk_store_stats* store_stats /* may be NULL */);
+
 #ifdef __cplusplus
 }
 #endif

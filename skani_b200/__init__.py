@@ -6,4 +6,4 @@ from .host import (Context, SketchSet, sketch_params, map_params, sketch_contigs
                    screen_triangle, screen_triangle_rows, screen_triangle_block, screen_query_ref, chain_pairs, chain_pair_debug, chain_pairs_debug, triangle, import_sketches, import_blobs, BlobError,
                    pack_contigs, sketch_contigs_2bit, triangle_local, triangle_multi, triangle_2bit,
                    screen_query_ref_multi, chain_pairs_multi, SketchStore, triangle_store, query_ref_store, cluster, cluster_linkage, neighbor_joining, neighbor_joining_multi,
-                   dereplicate, dereplicate_store, chain_pairs_mappings, chain_pairs_multi_mappings, MAPPING_DTYPE)  # noqa: F401
+                   dereplicate, dereplicate_store, dereplicate_fixed, dereplicate_store_fixed, chain_pairs_mappings, chain_pairs_multi_mappings, MAPPING_DTYPE)  # noqa: F401

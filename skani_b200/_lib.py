@@ -155,6 +155,8 @@ SYMBOLS = [
     ("sk_neighbor_joining_multi", i32, [vp, u32, u32, vp, u64, vp, PP(NjStats)]),
     ("sk_dereplicate", i32, [vp, vp, PP(MapParams), vp, PP(DerepParams), vp, vp, vp, PP(DerepStats)]),
     ("sk_dereplicate_store", i32, [vp, u32, vp, PP(MapParams), vp, PP(DerepParams), u64, vp, vp, vp, PP(DerepStats), PP(StoreStats)]),
+    ("sk_dereplicate_fixed", i32, [vp, vp, PP(MapParams), vp, u32, PP(DerepParams), vp, vp, vp, PP(DerepStats)]),
+    ("sk_dereplicate_store_fixed", i32, [vp, u32, vp, PP(MapParams), vp, u32, PP(DerepParams), u64, vp, vp, vp, PP(DerepStats), PP(StoreStats)]),
 ]
 
 _lib = None

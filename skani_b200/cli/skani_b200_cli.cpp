@@ -36,6 +36,7 @@
 #include <functional>
 #include <map>
 #include <numeric>
+#include <set>
 #include <string>
 #include <thread>
 #include <vector>
@@ -158,7 +159,7 @@ struct Opts {
   std::string cmd, out;
   std::vector<std::string> files, queries, refs;
   uint32_t c = 125, k = 15, m = 1000;
-  bool c_set = false, m_set = false;
+  bool c_set = false, m_set = false, k_set = false;
   double s = 0.0, min_af = -1e9, both_min_af = -1.0;
   bool individual = false, qi = false, ri = false, sparse = false, full_matrix = false, diagonal = false, ci = false, detailed = false,
        short_header = false, distance = false, robust = false, median = false, no_learned = false, faster_small = false,
@@ -173,6 +174,8 @@ struct Opts {
   std::string dendrogram;           // cluster --dendrogram FILE
   std::string representatives;      // dereplicate --representatives FILE
   bool host_store = false;          // dereplicate --host-store
+  std::vector<std::string> fixed_reps;   // dereplicate --fixed-reps PATH / --fixed-reps-list FILE
+  bool fixed_given = false;              // either flag was given
   std::string tree_method = "nj";   // tree --method nj|average|complete
   std::string mappings;             // triangle / dist / search --mappings FILE
 };
@@ -381,18 +384,21 @@ sk_sketch_set* import_sketch_inputs(sk_ctx* ctx, const skdb::SketchInputs& si, s
   return set;
 }
 
-// sketch inputs -> a new host sketch store: each group's set is added and freed before the next group is read, so host
-// memory holds one group of stored sketches besides the pinned store, and the device one imported group.  nullptr when an entry
-// cannot be loaded.
-sk_sketch_store* store_sketch_inputs(sk_ctx* ctx, const skdb::SketchInputs& si, int threads, const sk_sketch_params& sp, std::vector<Genome>& meta) {
-  sk_sketch_store* st = nullptr;
-  CK(ctx, sk_sketch_store_create(&sp, &st));
-  meta.resize(si.entries.size());
-  const bool ok = for_each_sketch_group(ctx, si, 0, si.entries.size(), threads, sp, meta.data(), [&](sk_sketch_set* s) {
+// sketch inputs -> a host sketch store (a new one, or `into` grown after its genomes): each group's set is added and freed
+// before the next group is read, so host memory holds one group of stored sketches besides the pinned store, and the device
+// one imported group.  meta gets the entries' metadata appended.  nullptr when an entry cannot be loaded (a new store is
+// then freed; `into` stays the caller's).
+sk_sketch_store* store_sketch_inputs(sk_ctx* ctx, const skdb::SketchInputs& si, int threads, const sk_sketch_params& sp, std::vector<Genome>& meta,
+                                     sk_sketch_store* into = nullptr) {
+  sk_sketch_store* st = into;
+  if (!st) CK(ctx, sk_sketch_store_create(&sp, &st));
+  const size_t m0 = meta.size();
+  meta.resize(m0 + si.entries.size());
+  const bool ok = for_each_sketch_group(ctx, si, 0, si.entries.size(), threads, sp, meta.data() + m0, [&](sk_sketch_set* s) {
     CK(ctx, sk_sketch_store_add(st, s));
     sk_sketch_set_free(s);
   });
-  if (!ok) { sk_sketch_store_free(st); return nullptr; }
+  if (!ok) { if (!into) sk_sketch_store_free(st); return nullptr; }
   return st;
 }
 
@@ -541,12 +547,14 @@ void info_store_path(const Opts& op, double need_gb, bool dist) {
 
 // The store path of triangle and dist on FASTA inputs: files are sketched in groups, each group's set is added to a host
 // sketch store and freed, so device memory holds one group at a time and host memory one group of sequence plus the
-// sketches.  genomes gets the metadata of every genome in store order (= the order of the in-memory path).  Sketch inputs
-// fill their store through store_sketch_inputs.
+// sketches.  genomes gets the metadata of every genome appended in store order (= the order of the in-memory path).  The
+// store is a new one, or `into` grown after its genomes.  nullptr when the files hold no genome (a new store is then freed;
+// `into` stays the caller's).  Sketch inputs fill their store through store_sketch_inputs.
 sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, const std::vector<std::string>& input_files, bool individual,
-                            std::vector<Genome>& genomes, sk_sketch_params& sp) {
-  sk_sketch_store* st = nullptr;
-  CK(ctx, sk_sketch_store_create(&sp, &st));
+                            std::vector<Genome>& genomes, sk_sketch_params& sp, sk_sketch_store* into = nullptr) {
+  sk_sketch_store* st = into;
+  if (!st) CK(ctx, sk_sketch_store_create(&sp, &st));
+  const size_t g0 = genomes.size();
   std::vector<std::string> files = input_files;
   std::sort(files.begin(), files.end());
   for (size_t f0 = 0; f0 < files.size();) {
@@ -560,7 +568,7 @@ sk_sketch_store* fill_store(sk_ctx* ctx, const Opts& op, const std::vector<std::
     sk_sketch_set_free(set);
     for (auto& g : in.genomes) genomes.push_back(std::move(g));
   }
-  if (genomes.empty()) { sk_sketch_store_free(st); return nullptr; }
+  if (genomes.size() == g0) { if (!into) sk_sketch_store_free(st); return nullptr; }
   return st;
 }
 
@@ -622,7 +630,63 @@ struct TriangleInputs {
   sk_sketch_params sp{};
   sk_sketch_set* loaded = nullptr;    // sketch inputs imported in memory (FASTA inputs are sketched by the caller)
   sk_sketch_store* store = nullptr;   // the store path's sketches
+  // dereplicate --fixed-reps: the fixed group (op.fixed_reps), whose genomes come first; the fields above then describe the
+  // new group (op.files), and loaded / store hold both groups
+  bool fixed_sketches = false;
+  skdb::SketchInputs fsi;
+  uint32_t n_fixed = 0;
 };
+
+// the names a group of inputs gives its genomes: its paths (FASTA), or its sketches' file names
+std::set<std::string> group_names(const std::vector<std::string>& files, bool sketches, const skdb::SketchInputs& si) {
+  std::set<std::string> names;
+  if (sketches) for (auto& e : si.entries) names.insert(e.file_name);
+  else names.insert(files.begin(), files.end());
+  return names;
+}
+
+// dereplicate --fixed-reps: the fixed group opened beside the new one.  Each group follows the triangle's input rules on its
+// own; a FASTA group is sketched with a sketch group's (c, k, m), so an explicit -c / -k / -m that differs from them is
+// refused, as are two sketch groups whose parameters differ and a genome file name in both groups.  Both groups are held in
+// one set at the end, joined by sk_sketch_set_append (the fixed group's set and the joined one at once): the estimate counts
+// both groups twice.
+int open_fixed_inputs(Opts& op, TriangleInputs& ti) {
+  if (op.fixed_reps.empty()) { fprintf(stderr, "ERROR --fixed-reps / --fixed-reps-list: no fixed representatives given.\n"); return 1; }
+  ti.fixed_sketches = sketch_inputs_given(op.fixed_reps);
+  if (ti.fixed_sketches) {
+    fprintf(stderr, "INFO Sketches detected among the fixed representatives.\n");
+    if (!skdb::open_sketch_inputs(op.fixed_reps, ti.fsi)) return 1;
+    if (ti.fsi.entries.empty()) { fprintf(stderr, "ERROR No genomes/sketches found among the fixed representatives.\n"); return 1; }
+  }
+  if (ti.fixed_sketches && ti.sketches) {
+    const skdb::DiskParams &a = ti.fsi.params, &b = ti.si.params;
+    if (a.c != b.c || a.k != b.k || a.marker_c != b.marker_c) {
+      fprintf(stderr, "ERROR Sketch parameters of %s (c = %llu, k = %llu, m = %llu) differ from those of %s (c = %llu, k = %llu, m = %llu). Exiting.\n",
+              op.files[0].c_str(), (unsigned long long)b.c, (unsigned long long)b.k, (unsigned long long)b.marker_c, op.fixed_reps[0].c_str(),
+              (unsigned long long)a.c, (unsigned long long)a.k, (unsigned long long)a.marker_c);
+      return 1;
+    }
+  } else if (ti.fixed_sketches || ti.sketches) {   // one FASTA group, sketched with the sketch group's parameters
+    const skdb::SketchInputs& si = ti.fixed_sketches ? ti.fsi : ti.si;
+    const char* who = ti.fixed_sketches ? "fixed representatives" : "new genomes";
+    const struct { bool set; uint32_t given; uint64_t used; const char* flag; } ps[] = {
+        {op.c_set, op.c, si.params.c, "-c"}, {op.k_set, op.k, si.params.k, "-k"}, {op.m_set, op.m, si.params.marker_c, "-m"}};
+    for (auto& p : ps)
+      if (p.set && p.given != p.used) {
+        fprintf(stderr, "ERROR %s %u differs from the sketch parameter %s %llu of the %s, with which the FASTA inputs are sketched.\n",
+                p.flag, p.given, p.flag, (unsigned long long)p.used, who);
+        return 1;
+      }
+  }
+  const std::set<std::string> fixed = group_names(op.fixed_reps, ti.fixed_sketches, ti.fsi);
+  for (auto& name : group_names(op.files, ti.sketches, ti.si))
+    if (fixed.count(name)) { fprintf(stderr, "ERROR %s is both a fixed representative and a new genome.\n", name.c_str()); return 1; }
+  if (ti.fixed_sketches || ti.sketches) warn_sketch_params(op, ti.fixed_sketches ? ti.fsi : ti.si);
+  const double need = 2.0 * (sketch_bytes_estimate(op, op.fixed_reps, ti.fixed_sketches) + sketch_bytes_estimate(op, op.files, ti.sketches)) + 6.0e9;
+  ti.need_gb = need / 1e9;
+  ti.use_store = exceeds_device(op, need);
+  return 0;
+}
 
 int open_triangle_inputs(Opts& op, TriangleInputs& ti) {
   resolve_presets(op);
@@ -632,8 +696,9 @@ int open_triangle_inputs(Opts& op, TriangleInputs& ti) {
     fprintf(stderr, "INFO Sketches detected.\n");
     if (!skdb::open_sketch_inputs(op.files, ti.si)) return 1;   // file_io::sketches_from_sketch (src/file_io.rs:680-717)
     if (ti.si.entries.empty()) { fprintf(stderr, "ERROR No genomes/sketches found.\n"); return 1; }
-    warn_sketch_params(op, ti.si);
+    if (!op.fixed_given) warn_sketch_params(op, ti.si);
   }
+  if (op.fixed_given) return open_fixed_inputs(op, ti);
   ti.use_store = triangle_needs_store(op, ti.sketches, ti.si, &ti.need_gb);
   return 0;
 }
@@ -658,6 +723,61 @@ int load_triangle_inputs(Opts& op, Inputs& in, sk_ctx*& ctx, TriangleInputs& ti)
     bool ok = true;
     ti.loaded = import_sketch_inputs(ctx, ti.si, 0, ti.si.entries.size(), std::max(op.threads, 1), ti.sp, in.genomes.data(), ok);
     if (!ok) return 1;
+  }
+  return 0;
+}
+
+// One group of dereplicate --fixed-reps' inputs, its genomes' metadata appended to genomes: in memory, one device set on ctx
+// (FASTA sketched, sketch inputs imported) joined to *set with sk_sketch_set_append; on the store path, added to *store.
+// false after an ERROR line.
+bool load_fixed_group(const Opts& op, sk_ctx* ctx, const std::vector<std::string>& files, bool sketches, const skdb::SketchInputs& si,
+                      sk_sketch_params& sp, bool use_store, const char* what, std::vector<Genome>& genomes, sk_sketch_set** set,
+                      sk_sketch_store** store) {
+  const int threads = std::max(op.threads, 1);
+  const size_t g0 = genomes.size();
+  if (use_store) {
+    sk_sketch_store* st = sketches ? store_sketch_inputs(ctx, si, threads, sp, genomes, *store) : fill_store(ctx, op, files, op.individual, genomes, sp, *store);
+    if (!st) {
+      if (!sketches) fprintf(stderr, "ERROR No genomes/sketches found among the %s.\n", what);
+      return false;
+    }
+    *store = st;
+    return true;
+  }
+  sk_sketch_set* s = nullptr;
+  if (sketches) {
+    genomes.resize(g0 + si.entries.size());
+    bool ok = true;
+    s = import_sketch_inputs(ctx, si, 0, si.entries.size(), threads, sp, genomes.data() + g0, ok);
+    if (!ok) { if (s) sk_sketch_set_free(s); return false; }
+  } else {
+    Inputs in;
+    load_inputs(files, op.individual, threads, in);
+    if (in.genomes.empty()) { fprintf(stderr, "ERROR No genomes/sketches found among the %s.\n", what); return false; }
+    s = sketch(ctx, in, sp);
+    for (auto& g : in.genomes) genomes.push_back(std::move(g));
+  }
+  if (!*set) { *set = s; return true; }
+  CK(ctx, sk_sketch_set_append(*set, s));
+  sk_sketch_set_free(s);
+  return true;
+}
+
+// load_triangle_inputs of dereplicate --fixed-reps: the fixed group, then the new one, into one set (in memory, ti.loaded) or
+// one host sketch store (ti.store); in.genomes gets the metadata of both and ti.n_fixed the fixed group's genome count
+int load_fixed_inputs(Opts& op, Inputs& in, sk_ctx*& ctx, TriangleInputs& ti) {
+  if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
+  ti.sp = ti.fixed_sketches ? params_of(ti.fsi) : ti.sketches ? params_of(ti.si) : sk_sketch_params{op.c, op.k, op.m};
+  if (ti.use_store) info_store_path(op, ti.need_gb, false);
+  const bool ok = load_fixed_group(op, ctx, op.fixed_reps, ti.fixed_sketches, ti.fsi, ti.sp, ti.use_store, "fixed representatives", in.genomes,
+                                   &ti.loaded, &ti.store);
+  ti.n_fixed = (uint32_t)in.genomes.size();
+  if (!ok || !load_fixed_group(op, ctx, op.files, ti.sketches, ti.si, ti.sp, ti.use_store, "new genomes", in.genomes, &ti.loaded, &ti.store)) {
+    if (ti.store) sk_sketch_store_free(ti.store);
+    if (ti.loaded) sk_sketch_set_free(ti.loaded);
+    ti.store = nullptr;
+    ti.loaded = nullptr;
+    return 1;
   }
   return 0;
 }
@@ -820,12 +940,16 @@ int run_triangle(Opts& op) {
   return 0;
 }
 
-// genomes ranked by total sequence length, longest first, ties by genome index (cluster's choice of representatives)
-std::vector<uint32_t> length_rank(const Inputs& in) {
+// genomes ranked by total sequence length, longest first, ties by genome index (cluster's choice of representatives).  With
+// n_first > 0 (dereplicate --fixed-reps) genomes 0 .. n_first - 1 take ranks 0 .. n_first - 1 by that rule, and the others
+// the ranks after them.
+std::vector<uint32_t> length_rank(const Inputs& in, uint32_t n_first = 0) {
   const uint32_t N = (uint32_t)in.genomes.size();
   std::vector<uint32_t> order(N), rank(N);
   for (uint32_t g = 0; g < N; g++) order[g] = g;
-  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return in.genomes[a].total_len > in.genomes[b].total_len; });
+  const auto longer = [&](uint32_t a, uint32_t b) { return in.genomes[a].total_len > in.genomes[b].total_len; };
+  std::stable_sort(order.begin(), order.begin() + n_first, longer);
+  std::stable_sort(order.begin() + n_first, order.end(), longer);
   for (uint32_t i = 0; i < N; i++) rank[order[i]] = i;
   return rank;
 }
@@ -915,6 +1039,8 @@ int run_cluster(Opts& op) {
 // GPU: inputs that need the host sketch store, and --gpus N, are refused.  --host-store takes the store path whatever the
 // input size: sketches in a host sketch store, sk_dereplicate_store on two contexts per GPU of --gpus N, the same output.
 // --representatives FILE: one line per representative in cluster-id order, its file name (-i: its first contig name).
+// --fixed-reps PATH / --fixed-reps-list FILE: genomes that are representatives already (sk_dereplicate_fixed): they come
+// first in genome-index and rank order and keep cluster ids 0 .. n - 1; the positional inputs and -l are the new genomes.
 int run_dereplicate(Opts& op) {
   if (op.single_linkage || !op.linkage.empty() || !op.dendrogram.empty()) {
     fprintf(stderr, "ERROR --single-linkage, --linkage and --dendrogram are cluster options; dereplicate is greedy clustering only: use cluster.\n");
@@ -939,11 +1065,11 @@ int run_dereplicate(Opts& op) {
   if (op.host_store) ti.use_store = true;
   Inputs in;
   sk_ctx* ctx = nullptr;
-  if (const int rc = load_triangle_inputs(op, in, ctx, ti)) return rc;
+  if (const int rc = op.fixed_given ? load_fixed_inputs(op, in, ctx, ti) : load_triangle_inputs(op, in, ctx, ti)) return rc;
   const sk_map_params mp = map_params(op, !op.no_learned && op.c >= 70 && !op.individual && !op.median);
   const std::vector<uint64_t> ranks = name_ranks(in.genomes)[0];
   const uint32_t N = (uint32_t)in.genomes.size();
-  const std::vector<uint32_t> rank = length_rank(in);
+  const std::vector<uint32_t> rank = length_rank(in, ti.n_fixed);
   std::vector<uint32_t> rep(N), cluster(N);
   std::vector<sk_ani_result> join(N);
   // SK_DEREP_WAVE: genomes per wave (a test hook: many waves on small inputs); it only sizes the waves
@@ -958,14 +1084,19 @@ int run_dereplicate(Opts& op) {
     CK(ctx, sk_sketch_store_set_name_ranks(ti.store, ranks.data()));
     std::vector<sk_ctx*> sctx = make_contexts(ctx, op, op.gpus, 2);
     n_ctx = sctx.size();
-    CK(ctx, sk_dereplicate_store(sctx.data(), (uint32_t)sctx.size(), ti.store, &mp, rank.data(), &dp, device_budget(), rep.data(), cluster.data(),
-                                 join.data(), &st, &sst));
+    if (op.fixed_given)
+      CK(ctx, sk_dereplicate_store_fixed(sctx.data(), (uint32_t)sctx.size(), ti.store, &mp, rank.data(), ti.n_fixed, &dp, device_budget(), rep.data(),
+                                         cluster.data(), join.data(), &st, &sst));
+    else
+      CK(ctx, sk_dereplicate_store(sctx.data(), (uint32_t)sctx.size(), ti.store, &mp, rank.data(), &dp, device_budget(), rep.data(), cluster.data(),
+                                   join.data(), &st, &sst));
     for (size_t d = sctx.size(); d-- > 1;) sk_ctx_destroy(sctx[d]);
     sk_sketch_store_free(ti.store);
   } else {
     sk_sketch_set* set = ti.loaded ? ti.loaded : sketch(ctx, in, ti.sp);
     sk_sketch_set_set_name_ranks(set, ranks.data());
-    CK(ctx, sk_dereplicate(ctx, set, &mp, rank.data(), &dp, rep.data(), cluster.data(), join.data(), &st));
+    if (op.fixed_given) CK(ctx, sk_dereplicate_fixed(ctx, set, &mp, rank.data(), ti.n_fixed, &dp, rep.data(), cluster.data(), join.data(), &st));
+    else CK(ctx, sk_dereplicate(ctx, set, &mp, rank.data(), &dp, rep.data(), cluster.data(), join.data(), &st));
     sk_sketch_set_free(set);
   }
   if (!write_clusters(op, in, rep, cluster, [&](uint32_t g) { return &join[g]; })) return 1;
@@ -977,8 +1108,10 @@ int run_dereplicate(Opts& op) {
     for (uint32_t g : by_cluster) fprintf(f, "%s\n", (op.individual ? in.genomes[g].contigs[0] : in.genomes[g].file_name).c_str());
     fclose(f);
   }
-  fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (greedy), %u waves, %llu pairs screened, %llu chained; "
-          "screen %.2f s, chain %.2f s, decide %.2f s, total %.2f s\n", N, st.n_clusters, op.cluster_ani, st.waves,
+  char fixed[64] = "";
+  if (op.fixed_given) snprintf(fixed, sizeof(fixed), ", %u fixed representatives", ti.n_fixed);
+  fprintf(stderr, "INFO %u genomes in %u clusters at ANI >= %g (greedy)%s, %u waves, %llu pairs screened, %llu chained; "
+          "screen %.2f s, chain %.2f s, decide %.2f s, total %.2f s\n", N, st.n_clusters, op.cluster_ani, fixed, st.waves,
           (unsigned long long)st.pairs_screened, (unsigned long long)st.pairs_chained, st.t_screen, st.t_chain, st.t_decide, st.t_total);
   if (op.host_store)
     fprintf(stderr, "INFO Store path: %u working sets, %.2f GB gathered (largest working set %.2f GB); marker gather %.2f s, gather %.2f s, chain %.2f s "
@@ -1653,6 +1786,16 @@ void usage() {
           "      the whole triangle; --representatives writes one representative per line in cluster order.  By default one\n"
           "      GPU with the sketches in device memory; --host-store keeps them in host memory and chains in working sets\n"
           "      (inputs beyond device memory, and --gpus N), with the same output\n"
+          "  skani-b200 dereplicate [fasta | sketch ... | -l list] --fixed-reps PATH [--fixed-reps PATH ...] [--fixed-reps-list FILE]\n"
+          "                        [-i] [--ani T] [-o out] [--representatives FILE] [--host-store] [--gpus N]\n"
+          "      adds new genomes (the positional inputs and -l) to representatives that exist already (--fixed-reps, one\n"
+          "      FASTA or sketch input each, and --fixed-reps-list, one per line): every fixed genome stays a representative\n"
+          "      and keeps cluster ids 0 .. n - 1 (fixed genomes ranked longest first, ties in file-name order), the new\n"
+          "      genomes join them or form new clusters by the greedy rule, and no pair of two fixed genomes is screened or\n"
+          "      chained.  Each group is FASTA files or .sketch files and databases; a FASTA group is sketched with a sketch\n"
+          "      group's parameters (an explicit -c / -k / -m that differs is refused).  An earlier run's --representatives\n"
+          "      file passed back as --fixed-reps-list keeps its clusters' ids; with -i that file lists contig names, so pass\n"
+          "      the catalogue as files (or a sketch database) instead\n"
           "  skani-b200 tree [fasta | sketch ... | -l list] [-i] [--method nj|average|complete] [-o tree.nwk]\n"
           "      the triangle's genomes as a Newick tree of 100 - ANI (100 for pairs not printed), branch lengths in percent:\n"
           "      neighbour joining (default; unrooted, basal trifurcation) or the average / complete linkage dendrogram\n"
@@ -1688,7 +1831,7 @@ int main(int argc, char** argv) {
     multi = NONE;
     if (a == "-c") { op.c = (uint32_t)atoi(val().c_str()); op.c_set = true; }
     else if (a == "-m") { op.m = (uint32_t)atof(val().c_str()); op.m_set = true; }
-    else if (a == "-k") op.k = (uint32_t)atoi(val().c_str());
+    else if (a == "-k") { op.k = (uint32_t)atoi(val().c_str()); op.k_set = true; }
     else if (a == "-s") op.s = atof(val().c_str());
     else if (a == "-t") op.threads = atoi(val().c_str());
     else if (a == "-o") op.out = val();
@@ -1737,6 +1880,12 @@ int main(int argc, char** argv) {
     else if (a == "--dendrogram" && (op.cmd == "cluster" || op.cmd == "dereplicate")) op.dendrogram = val();
     else if (a == "--representatives" && op.cmd == "dereplicate") op.representatives = val();
     else if (a == "--host-store" && op.cmd == "dereplicate") op.host_store = true;
+    else if (a == "--fixed-reps" && op.cmd == "dereplicate") { op.fixed_reps.push_back(val()); op.fixed_given = true; }
+    else if (a == "--fixed-reps-list" && op.cmd == "dereplicate") {
+      auto v = read_list(val());
+      op.fixed_reps.insert(op.fixed_reps.end(), v.begin(), v.end());
+      op.fixed_given = true;
+    }
     else if (a == "--method" && op.cmd == "tree") op.tree_method = val();
     else if (a == "--mappings" && (op.cmd == "triangle" || op.cmd == "dist" || op.cmd == "search")) op.mappings = val();
     else if (a == "--keep-refs") {}   // search already loads every passing reference exactly once

@@ -25,6 +25,12 @@
 // (the index, the row screens, the greedy rounds and the set difference run there exactly as above, on the global genome
 // indices), and each chain step's pairs are planned into working sets (ws_plan.hpp) that the contexts gather from the store
 // and chain through chain_working_sets (store_ws.hpp), as sk_triangle_store does.
+//
+// sk_dereplicate_fixed and sk_dereplicate_store_fixed start from fixed representatives, the genomes of rank < n_fixed: their
+// states are CL_REP and their markers fill the index before the first wave, and the waves cover ranks n_fixed .. N - 1 only.
+// No fixed genome is a row of any screen (step 1 and the final screen read wave genomes and members, step 2 undecided wave
+// genomes), so no pair of two fixed genomes is screened or chained, and the outcome is sk_cluster's on the triangle's rows
+// without those pairs.  sk_dereplicate is n_fixed = 0: the same calls, the same launches.
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -334,12 +340,19 @@ struct Run {
     return SK_OK;
   }
 
-  // wave = genomes per wave, 0 for the growing default
-  int run(const uint32_t* rank, uint32_t wave, uint32_t* rep, uint32_t* cluster, sk_ani_result* join) {
+  // wave = genomes per wave, 0 for the growing default; the genomes of rank < n_fixed are representatives from the start
+  int run(const uint32_t* rank, uint32_t n_fixed, uint32_t wave, uint32_t* rep, uint32_t* cluster, sk_ani_result* join) {
     cudaStream_t s = ctx->stream;
     const auto t_all = clk::now();
     std::vector<uint32_t> order(N);
     for (uint32_t g = 0; g < N; g++) order[rank[g]] = g;
+    uint64_t fixed_markers = 0;
+    for (uint32_t i = 0; i < n_fixed; i++) fixed_markers += set->mk_off[order[i] + 1] - set->mk_off[order[i]];
+    if (fixed_markers >= DR_MAX_KEYS) {
+      ctx->err = std::string(who) + ": the " + std::to_string(n_fixed) + " fixed representatives hold " + std::to_string(fixed_markers) +
+                 " markers, more than one marker index takes (at most 2^31 - 1)";
+      return SK_ERR_PARAM;
+    }
     DTmp<uint32_t> d_order;
     Index reps;
     SK_TRY(upload_offsets());
@@ -352,7 +365,17 @@ struct Run {
     SK_CUDA(h2d_small(ctx, d_rank.p, rank, (size_t)N * 4));
     SK_CUDA(h2d_small(ctx, d_order.p, order.data(), (size_t)N * 4));
     SK_CUDA(cudaMemsetAsync(state.p, CL_UNDECIDED, N, s));
-    for (uint32_t w0 = 0, size = wave ? wave : FIRST_WAVE; w0 < N; w0 += size, size = wave ? wave : std::min(2 * size, MAX_WAVE)) {
+    // the fixed representatives: their states and their markers in the index before the first wave
+    std::vector<uint8_t> fixed_state;
+    if (n_fixed) {
+      fixed_state.assign(N, CL_UNDECIDED);
+      for (uint32_t i = 0; i < n_fixed; i++) fixed_state[order[i]] = CL_REP;
+      SK_CUDA(cudaMemcpyAsync(state.p, fixed_state.data(), N, cudaMemcpyHostToDevice, s));
+      const auto t0 = clk::now();
+      SK_TRY(index_add(reps, order.data(), d_order.p, n_fixed));
+      st.t_screen += secs(t0);
+    }
+    for (uint32_t w0 = n_fixed, size = wave ? wave : FIRST_WAVE; w0 < N; w0 += size, size = wave ? wave : std::min(2 * size, MAX_WAVE)) {
       const uint32_t w1 = std::min<uint64_t>(N, (uint64_t)w0 + size), nw = w1 - w0;
       const uint32_t* d_wave = d_order.p + w0;
       st.waves++;
@@ -473,21 +496,43 @@ struct Run {
   }
 };
 
+// the refusal of a fixed set larger than the representative index, before any device work; empty when it fits
+std::string fixed_error(uint32_t n_fixed, uint32_t n_genomes) {
+  if (n_fixed > n_genomes)
+    return "n_fixed = " + std::to_string(n_fixed) + " fixed representatives, more than the " + std::to_string(n_genomes) + " genomes";
+  if (n_fixed > DR_MAX_SLOTS)
+    return "n_fixed = " + std::to_string(n_fixed) + " fixed representatives, more than one marker index takes (at most 2^22 - 1)";
+  return "";
+}
+
+// sk_dereplicate and sk_dereplicate_fixed (who names the caller in messages): sk_dereplicate is n_fixed = 0
+int dereplicate_impl(const char* who, sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* rank, uint32_t n_fixed,
+                     const sk_derep_params* dp, uint32_t* rep, uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats) {
+  if (!ctx) return SK_ERR_PARAM;
+  if (!set || !mp || !dp || !rep || !cluster || !join || (set->G && !rank)) { ctx->err = std::string(who) + ": NULL argument"; return SK_ERR_PARAM; }
+  if (std::isnan(dp->min_ani)) { ctx->err = std::string(who) + ": min_ani is NaN"; return SK_ERR_PARAM; }
+  const std::string bad = rank_error(set->G, rank);
+  if (!bad.empty()) { ctx->err = std::string(who) + ": " + bad; return SK_ERR_PARAM; }
+  const std::string fbad = fixed_error(n_fixed, set->G);
+  if (!fbad.empty()) { ctx->err = std::string(who) + ": " + fbad; return SK_ERR_PARAM; }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  Run r{ctx, set, mp, dp->min_ani, screen_cutoff(mp), set->G, who};
+  const uint32_t wave = std::min(dp->wave, DR_MAX_SLOTS);
+  const int rc = r.run(rank, n_fixed, wave, rep, cluster, join);
+  if (rc == SK_OK && stats) *stats = r.st;
+  return rc;
+}
+
 }  // namespace
 
 int sk_dereplicate(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* rank, const sk_derep_params* dp,
                    uint32_t* rep, uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats) {
-  if (!ctx) return SK_ERR_PARAM;
-  if (!set || !mp || !dp || !rep || !cluster || !join || (set->G && !rank)) { ctx->err = std::string(WHO) + ": NULL argument"; return SK_ERR_PARAM; }
-  if (std::isnan(dp->min_ani)) { ctx->err = std::string(WHO) + ": min_ani is NaN"; return SK_ERR_PARAM; }
-  const std::string bad = rank_error(set->G, rank);
-  if (!bad.empty()) { ctx->err = std::string(WHO) + ": " + bad; return SK_ERR_PARAM; }
-  SK_CUDA(cudaSetDevice(ctx->device));
-  Run r{ctx, set, mp, dp->min_ani, screen_cutoff(mp), set->G};
-  const uint32_t wave = std::min(dp->wave, DR_MAX_SLOTS);
-  const int rc = r.run(rank, wave, rep, cluster, join);
-  if (rc == SK_OK && stats) *stats = r.st;
-  return rc;
+  return dereplicate_impl(WHO, ctx, set, mp, rank, 0, dp, rep, cluster, join, stats);
+}
+
+int sk_dereplicate_fixed(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* rank, uint32_t n_fixed,
+                         const sk_derep_params* dp, uint32_t* rep, uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats) {
+  return dereplicate_impl("sk_dereplicate_fixed", ctx, set, mp, rank, n_fixed, dp, rep, cluster, join, stats);
 }
 
 int sk_debug_derep_screen(sk_ctx* ctx, const sk_sketch_set* set, const sk_map_params* mp, const uint32_t* slot_genome,
@@ -563,24 +608,25 @@ int derep_store_budget(sk_ctx* const* ctxs, uint32_t n_ctx, uint64_t n_markers, 
   return SK_OK;
 }
 
-}  // namespace
-
-int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp, const uint32_t* rank,
-                         const sk_derep_params* dp, uint64_t device_budget, uint32_t* rep, uint32_t* cluster, sk_ani_result* join,
-                         sk_derep_stats* stats, sk_store_stats* store_stats) {
+// sk_dereplicate_store and sk_dereplicate_store_fixed (who names the caller in messages): sk_dereplicate_store is n_fixed = 0
+int dereplicate_store_impl(const char* who, sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp,
+                           const uint32_t* rank, uint32_t n_fixed, const sk_derep_params* dp, uint64_t device_budget, uint32_t* rep,
+                           uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats, sk_store_stats* store_stats) {
   if (!ctxs || n_ctx == 0 || !ctxs[0]) return SK_ERR_PARAM;
   sk_ctx* ctx = ctxs[0];
   const uint32_t N = sk_sketch_store_n_genomes(st);
-  if (!st || !mp || !dp || !rep || !cluster || !join || (N && !rank)) { ctx->err = std::string(WHO_STORE) + ": NULL argument"; return SK_ERR_PARAM; }
+  if (!st || !mp || !dp || !rep || !cluster || !join || (N && !rank)) { ctx->err = std::string(who) + ": NULL argument"; return SK_ERR_PARAM; }
   SK_TRY(check_contexts(ctxs, n_ctx));
-  if (std::isnan(dp->min_ani)) { ctx->err = std::string(WHO_STORE) + ": min_ani is NaN"; return SK_ERR_PARAM; }
+  if (std::isnan(dp->min_ani)) { ctx->err = std::string(who) + ": min_ani is NaN"; return SK_ERR_PARAM; }
   const std::string bad = rank_error(N, rank);
-  if (!bad.empty()) { ctx->err = std::string(WHO_STORE) + ": " + bad; return SK_ERR_PARAM; }
+  if (!bad.empty()) { ctx->err = std::string(who) + ": " + bad; return SK_ERR_PARAM; }
+  const std::string fbad = fixed_error(n_fixed, N);
+  if (!fbad.empty()) { ctx->err = std::string(who) + ": " + fbad; return SK_ERR_PARAM; }
   StoreChain sc{ctxs, n_ctx, st, std::vector<uint64_t>(N), device_budget};
   for (uint32_t g = 0; g < N; g++) sc.gbytes[g] = sk_sketch_store_genome_bytes(st, g);
   std::string perr;   // a genome over budget / 2 cannot be placed in every chunk pair of a working-set plan
   if (device_budget && !skws::genomes_fit(sc.gbytes, device_budget, perr)) {   // before any device work
-    ctx->err = std::string(WHO_STORE) + ": " + perr;
+    ctx->err = std::string(who) + ": " + perr;
     return SK_ERR_NOMEM;
   }
   if (N == 0) {   // what sk_dereplicate returns for an empty set: no wave, no pair, no cluster
@@ -597,15 +643,30 @@ int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_st
   int rc = SK_OK;
   if (!device_budget) {
     rc = derep_store_budget(ctxs, n_ctx, mk->mk_off[N], N, &sc.budget);
-    if (rc == SK_OK && !skws::genomes_fit(sc.gbytes, sc.budget, perr)) { ctx->err = std::string(WHO_STORE) + ": " + perr; rc = SK_ERR_NOMEM; }
+    if (rc == SK_OK && !skws::genomes_fit(sc.gbytes, sc.budget, perr)) { ctx->err = std::string(who) + ": " + perr; rc = SK_ERR_NOMEM; }
   }
   if (rc == SK_OK) {
-    Run r{ctx, mk, mp, dp->min_ani, screen_cutoff(mp), N, WHO_STORE, &sc};
-    rc = r.run(rank, std::min(dp->wave, DR_MAX_SLOTS), rep, cluster, join);
+    Run r{ctx, mk, mp, dp->min_ani, screen_cutoff(mp), N, who, &sc};
+    rc = r.run(rank, n_fixed, std::min(dp->wave, DR_MAX_SLOTS), rep, cluster, join);
     r.st.t_total += sc.stats.t_screen;
     if (rc == SK_OK && stats) *stats = r.st;
   }
   sk_sketch_set_free(mk);
   if (rc == SK_OK && store_stats) *store_stats = sc.stats;
   return rc;
+}
+
+}  // namespace
+
+int sk_dereplicate_store(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp, const uint32_t* rank,
+                         const sk_derep_params* dp, uint64_t device_budget, uint32_t* rep, uint32_t* cluster, sk_ani_result* join,
+                         sk_derep_stats* stats, sk_store_stats* store_stats) {
+  return dereplicate_store_impl(WHO_STORE, ctxs, n_ctx, st, mp, rank, 0, dp, device_budget, rep, cluster, join, stats, store_stats);
+}
+
+int sk_dereplicate_store_fixed(sk_ctx* const* ctxs, uint32_t n_ctx, const sk_sketch_store* st, const sk_map_params* mp,
+                               const uint32_t* rank, uint32_t n_fixed, const sk_derep_params* dp, uint64_t device_budget,
+                               uint32_t* rep, uint32_t* cluster, sk_ani_result* join, sk_derep_stats* stats, sk_store_stats* store_stats) {
+  return dereplicate_store_impl("sk_dereplicate_store_fixed", ctxs, n_ctx, st, mp, rank, n_fixed, dp, device_budget, rep, cluster, join,
+                                stats, store_stats);
 }

@@ -840,3 +840,40 @@ def dereplicate_store(ctxs, store, rank, min_ani=0.95, mp=None, wave=0, device_b
     c0.check(c0.L.sk_dereplicate_store(hs, len(ctxs), store.h, C.byref(mp), rk.ctypes.data if n else None, C.byref(dp), int(device_budget),
                                        rep.ctypes.data, cl.ctypes.data, join.ctypes.data, C.byref(st), C.byref(sst)))
     return rep[:n], cl[:n], join[:n], st, sst
+
+
+def dereplicate_fixed(ctx, sset, rank, n_fixed, min_ani=0.95, mp=None, wave=0):
+    """sk_dereplicate_fixed: dereplicate() with the genomes of rank < n_fixed fixed as representatives, equal to cluster()
+    (greedy) on the rows of screen_triangle + chain_pairs without the rows between two fixed genomes.  No pair of two fixed
+    genomes is screened or chained; n_fixed = 0 is dereplicate().  Returns (rep, cluster, join, stats) as dereplicate()."""
+    mp = mp or map_params()
+    n = len(sset)
+    rk = np.ascontiguousarray(rank, np.uint32)
+    if len(rk) != n:
+        raise ValueError("rank needs one entry per genome")
+    m = max(n, 1)
+    rep = np.zeros(m, np.uint32); cl = np.zeros(m, np.uint32); join = np.zeros(m, RESULT_DTYPE)
+    dp = DerepParams(float(min_ani), int(wave)); st = DerepStats()
+    ctx.check(ctx.L.sk_dereplicate_fixed(ctx.h, sset.h, C.byref(mp), rk.ctypes.data if n else None, int(n_fixed), C.byref(dp),
+                                         rep.ctypes.data, cl.ctypes.data, join.ctypes.data, C.byref(st)))
+    return rep[:n], cl[:n], join[:n], st
+
+
+def dereplicate_store_fixed(ctxs, store, rank, n_fixed, min_ani=0.95, mp=None, wave=0, device_budget=0):
+    """sk_dereplicate_store_fixed: dereplicate_fixed() over every genome of a SketchStore, equal to dereplicate_fixed() on one
+    in-memory set of the same genomes and name ranks; the contexts and device_budget as in dereplicate_store().  Returns
+    (rep, cluster, join, stats, store_stats) as dereplicate_store()."""
+    ctxs = list(ctxs) if isinstance(ctxs, (list, tuple)) else [ctxs]
+    mp = mp or map_params()
+    n = store.n_genomes()
+    rk = np.ascontiguousarray(rank, np.uint32)
+    if len(rk) != n:
+        raise ValueError("rank needs one entry per genome")
+    m = max(n, 1)
+    rep = np.zeros(m, np.uint32); cl = np.zeros(m, np.uint32); join = np.zeros(m, RESULT_DTYPE)
+    dp = DerepParams(float(min_ani), int(wave)); st = DerepStats(); sst = StoreStats()
+    hs = (C.c_void_p * len(ctxs))(*[c.h for c in ctxs])
+    c0 = ctxs[0]
+    c0.check(c0.L.sk_dereplicate_store_fixed(hs, len(ctxs), store.h, C.byref(mp), rk.ctypes.data if n else None, int(n_fixed), C.byref(dp),
+                                             int(device_budget), rep.ctypes.data, cl.ctypes.data, join.ctypes.data, C.byref(st), C.byref(sst)))
+    return rep[:n], cl[:n], join[:n], st, sst

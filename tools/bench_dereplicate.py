@@ -15,8 +15,15 @@ card's name and power limit read in the same call.
    200.  rep, cluster and join must be byte-identical.  Each row prints the pairs chained, the working sets, the bytes
    gathered, and how the time splits: the marker gather, the screens on ctxs[0] (t_screen), the chain steps (t_chain, wall
    time of gathers plus chaining) and the gather / chain seconds summed over the contexts.
+4. --update F (instead of 1 and 2): a catalogue update.  The first 1 - F of the genome indices (families scattered over
+   them) are dereplicated as the catalogue; then its representatives are fixed (in their catalogue rank order) and the other
+   F of the genomes added (sk_dereplicate_fixed, and sk_dereplicate_store_fixed on two contexts of one device), against
+   dereplicating all genomes again (sk_dereplicate, sk_dereplicate_store).  Families of 20 and of 200.  Each store call must
+   equal its in-memory call byte for byte, and every catalogue representative must stay one.  Each row prints the pairs
+   screened and chained and the times.
 
-  python tools/bench_dereplicate.py [--genomes 2000] [--length 1000000] [--reps 3] [--skip-e2e] [--host-store] [--json OUT]
+  python tools/bench_dereplicate.py [--genomes 2000] [--length 1000000] [--reps 3] [--skip-e2e] [--host-store] [--update F]
+                                    [--json OUT]
 The FASTA files go to a temporary directory that is removed at the end."""
 import argparse
 import json
@@ -137,6 +144,79 @@ def bench_store(n, L, G, reps, sink):
     return equal
 
 
+def sketch_genomes(sk, ctx, bases, off, goc, genomes):
+    """the genomes of the list (in list order) as one device set, name ranks = their order by genome id"""
+    idx = [np.nonzero(goc == g)[0] for g in genomes]
+    parts = [bases[int(off[i[0]]):int(off[i[-1] + 1])] for i in idx]
+    lens = np.concatenate([np.diff(off[i[0]:i[-1] + 2]) for i in idx])
+    s = sk.sketch_contigs(ctx, np.concatenate(parts), np.concatenate([[0], np.cumsum(lens)]).astype(np.uint64),
+                          np.concatenate([np.full(len(i), k, np.uint32) for k, i in enumerate(idx)]), len(genomes))
+    names = np.empty(len(genomes), np.uint64); names[np.argsort(genomes, kind="stable")] = np.arange(len(genomes))
+    s.set_name_ranks(names)
+    return s, names
+
+
+def bench_update(n, L, G, frac, reps, sink):
+    import skani_b200 as sk
+    ctxs = [sk.Context(0), sk.Context(0)]
+    ctx = ctxs[0]
+    bases, off, goc = family_set(n, L, G, 20261018)
+    total = np.bincount(goc, weights=np.diff(off).astype(np.float64), minlength=n)
+
+    def length_rank(genomes, n_first=0):
+        t = total[np.asarray(genomes)]
+        k = np.arange(len(genomes))
+        order = np.concatenate([np.lexsort((k[:n_first], -t[:n_first])), n_first + np.lexsort((k[n_first:], -t[n_first:]))])
+        rank = np.empty(len(genomes), np.uint32); rank[order] = np.arange(len(genomes))
+        return rank
+
+    def store_of(s, names):
+        st = sk.SketchStore()
+        st.add(s)
+        st.set_name_ranks(names)
+        return st
+
+    m = int(round((1 - frac) * n))
+    cat = list(range(m))
+    cs, _ = sketch_genomes(sk, ctx, bases, off, goc, cat)
+    crank = length_rank(cat)
+    crep = sk.dereplicate(ctx, cs, crank, min_ani=0.95)[0]
+    cs.free()
+    fixed = [cat[g] for g in np.argsort(crank, kind="stable") if crep[g] == g]     # catalogue rank order
+    upd = fixed + list(range(m, n))                                                 # fixed first, then the new genomes
+    us, unames = sketch_genomes(sk, ctx, bases, off, goc, upd)
+    ust = store_of(us, unames)
+    urank = length_rank(upd, len(fixed))        # among the fixed genomes this is the catalogue's rank order again
+    alls, anames = sketch_genomes(sk, ctx, bases, off, goc, list(range(n)))
+    ast = store_of(alls, anames)
+    arank = length_rank(list(range(n)))
+    nf = len(fixed)
+    runs = {"update_in_memory": lambda: sk.dereplicate_fixed(ctx, us, urank, nf, min_ani=0.95),
+            "update_host_store": lambda: sk.dereplicate_store_fixed(ctxs, ust, urank, nf, min_ani=0.95),
+            "full_in_memory": lambda: sk.dereplicate(ctx, alls, arank, min_ani=0.95),
+            "full_host_store": lambda: sk.dereplicate_store(ctxs, ast, arank, min_ani=0.95)}
+    last = {k: f() for k, f in runs.items()}              # warm-up, and the equality checks
+    same = lambda a, b: all(x.tobytes() == y.tobytes() for x, y in zip(a[:3], b[:3]))
+    equal = bool(same(last["update_in_memory"], last["update_host_store"]) and same(last["full_in_memory"], last["full_host_store"]) and
+                 (last["update_in_memory"][0][:nf] == np.arange(nf)).all())
+    times = {k: [] for k in runs}
+    for _ in range(reps):
+        for k, f in runs.items():
+            t = time.perf_counter(); last[k] = f(); times[k].append(time.perf_counter() - t)
+    for k in runs:
+        dst = last[k][3]
+        emit({"bench": "update", "run": k, "genomes": n, "length": L, "family": G, "update_fraction": frac, "catalogue_genomes": m,
+              "fixed_representatives": nf, "set_genomes": len(upd) if k.startswith("update") else n, "card": card(), "equal": equal,
+              "clusters": int(dst.n_clusters), "pairs_screened": int(dst.pairs_screened), "pairs_chained": int(dst.pairs_chained),
+              "waves": int(dst.waves), "t_s": sorted(times[k]),
+              "derep_split_s": {"screen": dst.t_screen, "chain": dst.t_chain, "decide": dst.t_decide, "total": dst.t_total}}, sink)
+    for x in (ust, ast, us, alls):
+        x.free()
+    for c in ctxs:
+        c.close()
+    return equal
+
+
 def write_fasta(d, n, L, G):
     bases, off, goc = family_set(n, L, G, 20261018)
     files = []
@@ -181,16 +261,20 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--skip-e2e", action="store_true")
     ap.add_argument("--host-store", action="store_true", help="in-memory dereplicate against dereplicate_store only")
+    ap.add_argument("--update", type=float, metavar="F", help="a catalogue update adding the last F of the genomes")
     ap.add_argument("--json")
     a = ap.parse_args()
     sink, ok = [], True
-    if a.host_store:
+    if a.update is not None:
+        for G in (20, 200):
+            ok &= bench_update(a.genomes, a.length, G, a.update, a.reps, sink)
+    elif a.host_store:
         for G in (20, 200):
             ok &= bench_store(a.genomes, a.length, G, a.reps, sink)
     else:
         for G in (20, 200):
             ok &= bench_lib(a.genomes, a.length, G, a.reps, sink)
-    if not a.skip_e2e and not a.host_store:
+    if not a.skip_e2e and not a.host_store and a.update is None:
         for G in (20, 200):
             ok &= bench_e2e(a.genomes, a.length, G, a.reps, sink)
     if a.json:
