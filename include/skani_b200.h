@@ -235,6 +235,24 @@ int sk_screen_query_ref(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_
                         int mode, uint64_t** pairs_rq, uint64_t* n_pairs);
 void sk_free(void* p);
 
+/* ---- persistent reference marker index (search over query groups): the references' markers sorted once, then any
+ *      number of query sets screened against them without re-sorting the references.
+ * sk_ref_index_screen(ctx, idx, queries, mp, mode) returns exactly sk_screen_query_ref(ctx, refs, queries, mp, mode): the
+ * same sorted (ref << 32 | query) list for modes 0-3, query ids local to `queries`.  The index lives on the context that
+ * created it (the CLI's ctxs[0]); the queries must be on that context too, and refs may be freed once it is created.
+ * Device memory: 12 bytes per reference marker (the sorted marker and its reference), 8 bytes per reference and 256 KiB
+ * of prefix buckets per part; creating a part also takes about 16 bytes per marker of the part in temporaries.  The
+ * references are cut into contiguous parts of < 2^31 markers (SK_REF_INDEX_PART_MARKERS, read at creation, lowers the
+ * bound); a query set is screened against each part in turn, so databases of 2^31 markers and more are screened too.
+ * A screen takes 8 bytes per query marker (the lookup slices) besides its pair buffer. */
+typedef struct sk_ref_index sk_ref_index;
+int sk_ref_index_create(sk_ctx* ctx, const sk_sketch_set* refs, sk_ref_index** idx);
+int sk_ref_index_screen(sk_ctx* ctx, const sk_ref_index* idx, const sk_sketch_set* queries, const sk_map_params* mp, int mode,
+                        uint64_t** pairs_rq, uint64_t* n_pairs);
+/* references indexed, parts, device bytes held (any pointer may be NULL) */
+int sk_ref_index_info(const sk_ref_index* idx, uint32_t* n_refs, uint32_t* n_parts, uint64_t* device_bytes);
+int sk_ref_index_free(sk_ref_index* idx);
+
 /* ---- chaining: replaces chain::map_params_from_sketch + chain::chain_seeds (src/chain.rs:88, 144) and
  *      regression::get_model / predict_from_ani_res (src/regression.rs:12, 30) for every listed pair ---------
  * pairs[i] = (ref_index << 32) | query_index; out[i] is the AniEstResult of chain_seeds(refs[ref], queries[query]).

@@ -117,6 +117,10 @@ SYMBOLS = [
     ("sk_screen_triangle_block", i32, [vp, vp, u32, u32, PP(MapParams), PP(PP(u64)), PP(u64)]),
     ("sk_screen_query_ref", i32, [vp, vp, vp, PP(MapParams), i32, PP(PP(u64)), PP(u64)]),
     ("sk_free", None, [vp]),
+    ("sk_ref_index_create", i32, [vp, vp, PP(vp)]),
+    ("sk_ref_index_screen", i32, [vp, vp, vp, PP(MapParams), i32, PP(PP(u64)), PP(u64)]),
+    ("sk_ref_index_info", i32, [vp, PP(u32), PP(u32), PP(u64)]),
+    ("sk_ref_index_free", i32, [vp]),
     ("sk_chain_pairs", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp]),
     ("sk_chain_pairs_mappings", i32, [vp, vp, vp, vp, u64, PP(MapParams), vp, vp, PP(vp)]),
     ("sk_sketch_set_set_name_ranks", i32, [vp, vp]),

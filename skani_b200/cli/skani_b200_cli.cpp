@@ -10,9 +10,9 @@
 // breaks removed, records < 500 bp dropped, src/file_io.rs:141-362).  On-disk formats: sketch_db.hpp.
 // All heavy work happens on the GPU through libskani_b200.so.  search keeps the reference's structure but not its memory
 // model: instead of deserialising a reference sketch from the mmap'd database for every passing pair
-// (src/search.rs:142-166) it screens ALL queries against ALL marker sketches in one GPU pass, loads each reference sketch
-// that passed for some query exactly once (per block of queries), imports them to the device in groups through the same
-// reader as triangle's and dist's sketch inputs, and chains every pair there.
+// (src/search.rs:142-166) it screens each group of queries against all marker sketches, indexed once on the GPU, loads each
+// reference sketch that passed for some query exactly once (per block of queries), imports them to the device in groups
+// through the same reader as triangle's and dist's sketch inputs, and chains every pair there.
 // --gpus N: dist and search split the references into contiguous blocks, one per GPU, and copy the query set to every GPU
 // (sk_screen_query_ref_multi / sk_chain_pairs_multi); the output is byte-identical to one GPU's.
 // sketch encodes the database entries on the GPU (sk_sketch_set_encode) and, with --gpus N, sketches each group of files
@@ -43,6 +43,7 @@
 
 #include "../../include/skani_b200.h"
 #include "fastx.hpp"
+#include "search_plan.hpp"
 #include "sketch_db.hpp"
 
 namespace {
@@ -464,17 +465,22 @@ std::vector<size_t> split_balanced(const std::vector<uint64_t>& w, size_t W) {
   return b;
 }
 
-// sorted files [f0, end) form the next group that goes through the GPU at once: at most 4096 files and about 8 GiB of
-// sequence (file sizes x 4, as gz inflates ~4x), at least one file.  SK_SKETCH_GROUP_FILES lowers the file bound (a test
-// hook: many groups from a few files).
-size_t file_group_end(const std::vector<std::string>& files, size_t f0) {
+// the file bound of a group: 4096 files; SK_SKETCH_GROUP_FILES lowers it (a test hook: many groups from a few files)
+size_t group_max_files() {
   static const size_t max_files = [] {
     const char* e = getenv("SK_SKETCH_GROUP_FILES");
     return e ? (size_t)std::max(1ll, std::min(4096ll, atoll(e))) : (size_t)4096;
   }();
+  return max_files;
+}
+
+// sorted files [f0, end) form the next group that goes through the GPU at once: at most group_max_files() files and about
+// max_bytes (8 GiB) of sequence (file sizes x 4, as gz inflates ~4x), at least one file.
+size_t file_group_end(const std::vector<std::string>& files, size_t f0, uint64_t max_bytes = 8ull << 30) {
+  const size_t max_files = group_max_files();
   size_t f1 = f0;
   uint64_t bytes = 0;
-  while (f1 < files.size() && (f1 == f0 || (f1 - f0 < max_files && bytes < (8ull << 30)))) {
+  while (f1 < files.size() && (f1 == f0 || (f1 - f0 < max_files && bytes < max_bytes))) {
     struct stat st;
     bytes += stat(files[f1].c_str(), &st) == 0 ? (uint64_t)st.st_size * 4 : 0;
     f1++;
@@ -1237,26 +1243,27 @@ int run_tree(Opts& op) {
   return 0;
 }
 
-// write_query_ref_list (src/file_io.rs:608-678) of dist and search: queries in blocks of INTERMEDIATE_WRITE_COUNT
-// (src/dist.rs:151-175, src/search.rs:255-279).  block(q0, q1, res, rm) fills res with the results of the queries [q0, q1),
-// rows of equal ANI in the order they print, and with --mappings (rm non-null, k = the sketches' k) rm with their mapping
-// records; or returns false (after an ERROR line) to end the run with exit code 1.  Each block is grouped by the query's
-// first contig name, each group sorted by ANI (descending, stable) and its top n written, with their mappings, then flushed.
-template <class F>
-int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vector<Genome>& queries, uint32_t k, F block) {
+// write_query_ref_list (src/file_io.rs:608-678) of dist and search, one block of queries at a time: the block's rows (rows of
+// equal ANI in the order they print) are grouped by the query's first contig name, each group sorted by ANI (descending,
+// stable) and its top n written, with their mapping records under --mappings (rm.recs[rm.off[i] .. rm.off[i + 1]) belong to
+// row i), then flushed.  more() prints the line the reference prints between two blocks.
+struct DistWriter {
+  const Opts& op;
+  const std::vector<Genome>& refs;
+  const std::vector<Genome>& queries;
   MappingFile mf;
-  if (!op.mappings.empty() && !mf.open(op.mappings, k)) return 1;
-  FILE* o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
-  if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return 1; }
-  write_header(o, op.ci, op.detailed);
-  const size_t FL = intermediate_write_count(), NQ = queries.size();
-  std::vector<sk_ani_result> res;
-  RowMaps rm;
-  RowMaps* rmp = mf.f ? &rm : nullptr;
-  int rc = 0;
-  for (size_t q0 = 0; q0 < NQ; q0 += FL) {
-    rm.clear();
-    if (!block(q0, std::min(q0 + FL, NQ), res, rmp)) { rc = 1; break; }
+  FILE* o = nullptr;
+  DistWriter(const Opts& op_, const std::vector<Genome>& refs_, const std::vector<Genome>& queries_) : op(op_), refs(refs_), queries(queries_) {}
+  // false after an ERROR line; k = the sketches' k
+  bool open(uint32_t k) {
+    if (!op.mappings.empty() && !mf.open(op.mappings, k)) return false;
+    o = op.out.empty() ? stdout : fopen(op.out.c_str(), "w");
+    if (!o) { fprintf(stderr, "ERROR cannot open %s\n", op.out.c_str()); return false; }
+    write_header(o, op.ci, op.detailed);
+    return true;
+  }
+  bool mappings() const { return mf.f != nullptr; }
+  void write(const std::vector<sk_ani_result>& res, const RowMaps& rm) {
     std::map<std::string, std::vector<const sk_ani_result*>> groups;
     for (auto& r : res) if (r.ani > 0.1f) groups[queries[r.query_id].contigs[0]].push_back(&r);
     for (auto& kv : groups) {
@@ -1264,7 +1271,7 @@ int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vecto
       std::stable_sort(v.begin(), v.end(), [](const sk_ani_result* a, const sk_ani_result* b) { return a->ani > b->ani; });
       for (size_t i = 0; i < v.size() && i < op.n; i++) {
         write_row(o, *v[i], refs[v[i]->ref_id], queries[v[i]->query_id], op);
-        if (rmp) {
+        if (mf.f) {
           const size_t row = v[i] - res.data();
           mf.write(rm.recs.data() + rm.off[row], rm.off[row + 1] - rm.off[row], refs[v[i]->ref_id], queries[v[i]->query_id], op);
         }
@@ -1272,10 +1279,29 @@ int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vecto
     }
     fflush(o);
     mf.flush();
-    if (q0 + FL < NQ) fprintf(stderr, "INFO Writing results for %zu query sequences.\n", FL);
   }
-  if (o != stdout) fclose(o);
-  return rc;
+  void more() { fprintf(stderr, "INFO Writing results for %zu query sequences.\n", intermediate_write_count()); }
+  ~DistWriter() { if (o && o != stdout) fclose(o); }
+};
+
+// dist's queries in blocks of INTERMEDIATE_WRITE_COUNT (src/dist.rs:151-175).  block(q0, q1, res, rm) fills res with the
+// results of the queries [q0, q1), rows of equal ANI in the order they print, and with --mappings (rm non-null, k = the
+// sketches' k) rm with their mapping records; or returns false (after an ERROR line) to end the run with exit code 1.
+template <class F>
+int write_dist(const Opts& op, const std::vector<Genome>& refs, const std::vector<Genome>& queries, uint32_t k, F block) {
+  DistWriter w(op, refs, queries);
+  if (!w.open(k)) return 1;
+  const size_t FL = intermediate_write_count(), NQ = queries.size();
+  std::vector<sk_ani_result> res;
+  RowMaps rm;
+  RowMaps* rmp = w.mappings() ? &rm : nullptr;
+  for (size_t q0 = 0; q0 < NQ; q0 += FL) {
+    rm.clear();
+    if (!block(q0, std::min(q0 + FL, NQ), res, rmp)) return 1;
+    w.write(res, rm);
+    if (q0 + FL < NQ) w.more();
+  }
+  return 0;
 }
 
 int run_dist(Opts& op) {
@@ -1571,6 +1597,17 @@ int run_sketch(Opts& op) {
   return 0;
 }
 
+// the bases bound of a query group of search: 8 GiB.  SK_SEARCH_GROUP_BASES lowers it (a test hook: one multi-record file
+// cut into several query groups with --qi).
+uint64_t search_group_bases() {
+  if (const char* e = getenv("SK_SEARCH_GROUP_BASES")) return (uint64_t)std::max(1ll, atoll(e));
+  return 8ull << 30;
+}
+
+// search streams its queries: they are read in groups of files, each query group is sketched (or imported), copied to the
+// --gpus contexts, screened against a reference marker index built once on ctx (sk_ref_index_screen) and chained, and the
+// results are written in blocks of INTERMEDIATE_WRITE_COUNT queries as each block's last query is done.  The output is that
+// of one pass over all queries: name ranks come from search_plan::NameRanks, which needs the reference names only.
 int run_search(Opts& op) {
   if (op.db_dir.empty()) { fprintf(stderr, "ERROR search needs -d <sketched database folder>\n"); return 1; }
   if (op.queries.empty()) { fprintf(stderr, "ERROR No query files found.\n"); return 1; }
@@ -1606,33 +1643,32 @@ int run_search(Opts& op) {
   sk_sketch_params sp{(uint32_t)dp.c, (uint32_t)dp.k, (uint32_t)dp.marker_c};
   sk_ctx* ctx = nullptr;
   if (sk_ctx_create(op.device, &ctx) != 0) { fprintf(stderr, "ERROR a CUDA device is required (no CPU fallback)\n"); return 1; }
-  // ---- queries: FASTA/FASTQ sketched with the DATABASE's parameters (src/search.rs:112-123), or .sketch files
+  // ---- queries: FASTA/FASTQ sketched with the DATABASE's parameters (src/search.rs:112-123), or .sketch files.  qfiles holds
+  //      them in query order: paths sorted (genomes then follow in (file_name, contig_order) order, as load_inputs gives
+  //      them), or .sketch files stably sorted by the name stored inside (src/file_io.rs:715).
   bool queries_are_sketch = true;
   for (auto& q : op.queries) if (q.find(".sketch") == std::string::npos && q.find("markers.bin") == std::string::npos) { queries_are_sketch = false; break; }
-  std::vector<Genome> qmeta;
-  sk_sketch_set* qset = nullptr;
+  std::vector<std::string> qfiles;
   if (queries_are_sketch) {
-    std::vector<skdb::HostSketch> qs;
+    // first pass: the stored names (and the warnings, in argument order); the sketches are decoded again group by group below
+    std::vector<std::pair<std::string, std::string>> named;   // (file_name stored inside, path)
     for (auto& q : op.queries) {
       if (q.find("markers.bin") != std::string::npos) continue;
       std::vector<uint8_t> b;
       if (!skdb::read_file(q, b)) { fprintf(stderr, "ERROR Problem reading sketch file %s. Perhaps your file path is wrong? Exiting.\n", q.c_str()); return 1; }
       skdb::DiskParams qp;
-      try { qs.push_back(skdb::read_blob(b.data(), b.size(), &qp)); }
+      skdb::HostSketch h;
+      try { h = skdb::read_blob(b.data(), b.size(), &qp); }
       catch (const std::exception&) { fprintf(stderr, "ERROR %s is not a valid .sketch file or is corrupted.\n", q.c_str()); continue; }
       if (!(qp == dp)) fprintf(stderr, "WARN Query sketch parameters for %s not equal to reference sketch parameters; no ANI calculated\n", q.c_str());
+      named.emplace_back(h.file_name, q);
     }
-    std::stable_sort(qs.begin(), qs.end(), [](const skdb::HostSketch& a, const skdb::HostSketch& b) { return a.file_name < b.file_name; });   // src/file_io.rs:715
-    if (qs.empty()) { fprintf(stderr, "ERROR No query sketches found.\n"); return 1; }
-    Flat f;
-    for (auto& h : qs) { f.add(h, true); qmeta.push_back(genome_of(h)); }
-    qset = f.import(ctx, sp);
+    std::stable_sort(named.begin(), named.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+    if (named.empty()) { fprintf(stderr, "ERROR No query sketches found.\n"); return 1; }
+    for (auto& n : named) qfiles.push_back(n.second);
   } else {
-    Inputs qin;
-    load_inputs(op.queries, op.qi, std::max(op.threads, 1), qin);
-    if (qin.genomes.empty()) { fprintf(stderr, "ERROR No query sequences found.\n"); return 1; }
-    qset = sketch(ctx, qin, sp);
-    qmeta = std::move(qin.genomes);
+    qfiles = op.queries;
+    std::sort(qfiles.begin(), qfiles.end());
   }
   sk_map_params mp{};
   mp.screen_val = op.s == 0.0 ? 0.80 : op.s / 100.0;              // SEARCH_ANI_CUTOFF_DEFAULT (src/search.rs:40-49)
@@ -1645,35 +1681,37 @@ int run_search(Opts& op) {
   mp.learned_ani = dp.c >= 70 && !op.qi && !op.median;
   if (mp.learned_ani) fprintf(stderr, "INFO Learned ANI mode detected. ANI may be adjusted according to a regression model trained on MAGs.\n");
   const bool use_index = (op.queries.size() > 50 || op.qi) && !op.no_marker_index;   // src/parse.rs:436-442
-  // ---- marker sketches of every reference -> device, one screen of all queries against all references
-  sk_sketch_set* rmk = nullptr;
+  const int mode = use_index ? 3 : 1;
+  // ---- marker sketches of every reference -> one index on ctx, sorted once; every query group is screened against it
+  sk_ref_index* idx = nullptr;
   {
     Flat f;
     for (auto& h : ref_mk) f.add(h, false);
-    rmk = f.import(ctx, sp);
+    sk_sketch_set* rmk = f.import(ctx, sp);
+    CK(ctx, sk_ref_index_create(ctx, rmk, &idx));
+    sk_sketch_set_free(rmk);
+    uint32_t n_parts = 0; uint64_t bytes = 0;
+    sk_ref_index_info(idx, nullptr, &n_parts, &bytes);
+    fprintf(stderr, "INFO Reference marker index: %zu references in %u part(s), %.1f MB on GPU %d.\n", refs.size(), n_parts, bytes / 1e6, op.device);
   }
-  uint64_t* pairs = nullptr; uint64_t np = 0;
-  CK(ctx, sk_screen_query_ref(ctx, rmk, qset, &mp, use_index ? 3 : 1, &pairs, &np));
-  sk_sketch_set_free(rmk);
-  const auto ranks = name_ranks(refs, qmeta);
-  sk_sketch_set_set_name_ranks(qset, ranks[1].data());
-  // --gpus N: the query set is copied to every context once; each query block's references are spread over them below
+  const search_plan::NameRanks ranks([&] { std::vector<std::string> v; for (auto& g : refs) v.push_back(g.file_name); return v; }());
+  std::vector<uint64_t> ref_rank(refs.size());
+  for (size_t r = 0; r < refs.size(); r++) ref_rank[r] = ranks.ref(refs[r].file_name);
   const size_t W = op.gpus;
   std::vector<sk_ctx*> ctxs = make_contexts(ctx, op, W);
-  std::vector<sk_sketch_set*> qsets(W, qset);
-  for (size_t d = 1; d < W; d++) CK(ctxs[d], sk_sketch_set_copy(ctxs[d], qset, &qsets[d]));
-  // ---- queries are processed, and their results appended, in blocks of INTERMEDIATE_WRITE_COUNT (src/search.rs:255-279).
-  //      Inside a block: the references that passed for at least one of its queries ("hits") are loaded ONCE each and their
+  const uint64_t group_records = sketch_group_records((1ull << 31) - 1);
+  // ---- chaining: the references that passed for at least one of a run of queries ("hits") are loaded ONCE each and their
   //      pairs chained (the reference deserialises a sketch per passing PAIR, src/search.rs:142-166).  The hits are cut into
   //      W contiguous runs balanced by estimated records (marker counts), one per context, and each context reads its run in
   //      groups of < 2^31 - 1 records.  Every round, each context imports its next group (-t threads split over the contexts
-  //      read it), then one sk_chain_pairs_multi call chains the round's pairs on all contexts.
-  std::vector<uint64_t> all_pairs(pairs, pairs + np);
-  sk_free(pairs);
-  const uint64_t group_records = sketch_group_records((1ull << 31) - 1);
-  const int rc = write_dist(op, refs, qmeta, sp.k, [&](size_t q0, size_t q1, std::vector<sk_ani_result>& res, RowMaps* rm) {
+  //      read it), then one sk_chain_pairs_multi call chains the round's pairs on all contexts.  chain_run chains the group
+  //      queries [q0, q1) (gpairs: the group's screen pairs, qsets: the group on every context) and appends the rows that
+  //      pass, with global query ids (the group's first query is q_first), to rows and, with --mappings, to rowmaps.
+  std::vector<sk_ani_result> rows;
+  std::vector<std::vector<sk_mapping>> rowmaps;
+  auto chain_run = [&](size_t q0, size_t q1, size_t q_first, const std::vector<uint64_t>& gpairs, const std::vector<sk_sketch_set*>& qsets, bool maps_on) {
     std::vector<uint64_t> blockp;
-    for (uint64_t x : all_pairs) if ((uint32_t)x >= q0 && (uint32_t)x < q1) blockp.push_back(x);   // stays sorted by (ref, query)
+    for (uint64_t x : gpairs) if ((uint32_t)x >= q0 && (uint32_t)x < q1) blockp.push_back(x);   // stays sorted by (ref, query)
     std::vector<uint32_t> hits;
     std::vector<size_t> hit_pairs;          // pairs of hits[h]: blockp[hit_pairs[h], hit_pairs[h + 1])
     for (size_t i = 0; i < blockp.size(); i++)
@@ -1688,8 +1726,6 @@ int run_search(Opts& op) {
     rd.reserve(W);
     for (size_t d = 0; d < W; d++)
       rd.emplace_back(rsi, std::vector<size_t>(hits.begin() + run[d], hits.begin() + run[d + 1]), context_threads(op, d, W), group_records);
-    res.clear();
-    std::vector<std::vector<sk_mapping>> rowmaps;   // with --mappings: the records of res[i]
     for (;;) {
       std::vector<size_t> lo(W, 0), hi(W, 0);                   // this round: context d imports hits [lo[d], hi[d])
       std::vector<sk_sketch_set*> rsets(W, nullptr);
@@ -1700,7 +1736,7 @@ int run_search(Opts& op) {
         lo[d] = run[d] + rd[d].first;
         hi[d] = lo[d] + g.size();
         std::vector<uint64_t> rk(g.size());
-        for (size_t i = 0; i < g.size(); i++) rk[i] = ranks[0][hits[lo[d] + i]];
+        for (size_t i = 0; i < g.size(); i++) rk[i] = ref_rank[hits[lo[d] + i]];
         rsets[d] = import_group(ctxs[d], g, sp, [&](size_t i) { return rsi.entries[hits[lo[d] + i]].file_name; });
         if (!rsets[d]) { load_failed = true; return; }
         sk_sketch_set_set_name_ranks(rsets[d], rk.data());
@@ -1718,34 +1754,147 @@ int run_search(Opts& op) {
       }
       if (round_hit.empty()) break;
       std::vector<sk_ani_result> round(local.size());
-      std::vector<uint64_t> off(rm ? local.size() + 1 : 0);
+      std::vector<uint64_t> off(maps_on ? local.size() + 1 : 0);
       sk_mapping* maps = nullptr;
-      if (rm) CK(ctx, sk_chain_pairs_multi_mappings(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(),
-                                                    &mp, round.data(), off.data(), &maps));
+      if (maps_on) CK(ctx, sk_chain_pairs_multi_mappings(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(),
+                                                         &mp, round.data(), off.data(), &maps));
       else CK(ctx, sk_chain_pairs_multi(ctxs.data(), (uint32_t)W, rsets.data(), ref_first.data(), qsets.data(), local.data(), local.size(), &mp, round.data()));
       for (size_t i = 0; i < round.size(); i++) {
         sk_ani_result& r = round[i];
         if (!(r.ani > 0.5f)) continue;                                                        // src/search.rs:174
         r.ref_id = hits[round_hit[r.ref_id]];
-        res.push_back(r);
-        if (rm) rowmaps.emplace_back(maps + off[i], maps + off[i + 1]);
+        r.query_id += (uint32_t)q_first;
+        rows.push_back(r);
+        if (maps_on) rowmaps.emplace_back(maps + off[i], maps + off[i + 1]);
       }
       sk_free(maps);
       for (auto* s : rsets) sk_sketch_set_free(s);
     }
-    // rows of equal ANI print in (ref, query) order, as one context chaining the hits in order produces them
-    std::vector<size_t> ord(res.size());
-    std::iota(ord.begin(), ord.end(), 0);
-    std::sort(ord.begin(), ord.end(), [&](size_t a, size_t b) { return res[a].ref_id != res[b].ref_id ? res[a].ref_id < res[b].ref_id : res[a].query_id < res[b].query_id; });
-    std::vector<sk_ani_result> sorted(res.size());
-    for (size_t i = 0; i < ord.size(); i++) {
-      sorted[i] = res[ord[i]];
-      if (rm) rm->add(rowmaps[ord[i]].data(), rowmaps[ord[i]].size());
-    }
-    res.swap(sorted);
     return true;
-  });
-  for (auto* s : qsets) sk_sketch_set_free(s);
+  };
+  // ---- queries are processed, and their results appended, in blocks of INTERMEDIATE_WRITE_COUNT (src/search.rs:255-279).
+  //      A block that spans two query groups keeps its rows until its last query is chained.
+  std::vector<Genome> qmeta;                // every query so far, in global order
+  DistWriter w(op, refs, qmeta);
+  bool opened = false;
+  const size_t FL = intermediate_write_count();
+  size_t blocks_written = 0;
+  auto write_block = [&] {
+    // rows of equal ANI print in (ref, query) order, as one context chaining the hits in order produces them
+    std::vector<size_t> ord(rows.size());
+    std::iota(ord.begin(), ord.end(), 0);
+    std::sort(ord.begin(), ord.end(), [&](size_t a, size_t b) { return rows[a].ref_id != rows[b].ref_id ? rows[a].ref_id < rows[b].ref_id : rows[a].query_id < rows[b].query_id; });
+    std::vector<sk_ani_result> res(rows.size());
+    RowMaps rm;
+    for (size_t i = 0; i < ord.size(); i++) {
+      res[i] = rows[ord[i]];
+      if (w.mappings()) rm.add(rowmaps[ord[i]].data(), rowmaps[ord[i]].size());
+    }
+    if (blocks_written++) w.more();
+    w.write(res, rm);
+    rows.clear();
+    rowmaps.clear();
+  };
+  // one query group: its genomes' metadata appended to qmeta, the group as a device set on ctx (which process() owns)
+  size_t n_groups = 0;
+  auto process = [&](sk_sketch_set* qset, uint64_t bases) {
+    const size_t q_end = qmeta.size(), q_first = q_end - sk_sketch_set_n_genomes(qset);
+    fprintf(stderr, "INFO Query group %zu: genomes %zu-%zu (%llu bases).\n", ++n_groups, q_first, q_end - 1, (unsigned long long)bases);
+    if (!opened) { if (!w.open(sp.k)) return false; opened = true; }
+    std::vector<uint64_t> qr(q_end - q_first);
+    for (size_t i = 0; i < qr.size(); i++) qr[i] = ranks.query(qmeta[q_first + i].file_name);
+    sk_sketch_set_set_name_ranks(qset, qr.data());
+    uint64_t* pairs = nullptr; uint64_t np = 0;
+    CK(ctx, sk_ref_index_screen(ctx, idx, qset, &mp, mode, &pairs, &np));
+    std::vector<uint64_t> gpairs(pairs, pairs + np);
+    sk_free(pairs);
+    // --gpus N: the group is copied to every context; each run's references are spread over them in chain_run
+    std::vector<sk_sketch_set*> qsets(W, qset);
+    for (size_t d = 1; d < W; d++) CK(ctxs[d], sk_sketch_set_copy(ctxs[d], qset, &qsets[d]));
+    bool ok = true;
+    for (size_t s0 = q_first; s0 < q_end && ok;) {
+      const size_t block_end = (s0 / FL + 1) * FL, s1 = std::min(block_end, q_end);
+      ok = chain_run(s0 - q_first, s1 - q_first, q_first, gpairs, qsets, w.mappings());
+      if (ok && s1 == block_end) write_block();
+      s0 = s1;
+    }
+    for (size_t d = 1; d < W; d++) sk_sketch_set_free(qsets[d]);
+    sk_sketch_set_free(qset);
+    return ok;
+  };
+  // ---- the queries in read groups of files (file_group_end; a group of .sketch files is one query group, a group of FASTA
+  //      files is cut into query groups by search_plan::cut_groups).  The next read group is read and laid out on a host
+  //      thread while the current one is sketched, screened and chained: host memory holds at most two groups of queries.
+  const uint64_t max_bases = search_group_bases();
+  std::vector<size_t> fb{0};
+  while (fb.back() < qfiles.size()) fb.push_back(file_group_end(qfiles, fb.back(), max_bases));
+  const size_t n_reads = fb.size() - 1;
+  struct QueryRead {
+    Inputs in;                        // FASTA: the files' genomes, cut into query groups at bounds
+    std::vector<size_t> bounds{0};
+    Flat flat;                        // .sketch files: one query group
+    std::vector<Genome> meta;
+    bool failed = false;
+  };
+  auto load = [&](size_t k, QueryRead* r) {
+    const std::vector<std::string> files(qfiles.begin() + fb[k], qfiles.begin() + fb[k + 1]);
+    if (!queries_are_sketch) {
+      load_inputs(files, op.qi, std::max(op.threads, 1), r->in);
+      const auto& gs = r->in.genomes;
+      std::vector<uint32_t> gfile(gs.size());
+      std::vector<uint64_t> gbases(gs.size());
+      for (size_t g = 0; g < gs.size(); g++) {
+        gfile[g] = g == 0 ? 0 : gfile[g - 1] + (gs[g].file_name != gs[g - 1].file_name);
+        gbases[g] = gs[g].total_len;
+      }
+      r->bounds = search_plan::cut_groups(gfile, gbases, group_max_files(), max_bases, op.qi);
+      return;
+    }
+    for (auto& q : files) {
+      std::vector<uint8_t> b;
+      skdb::HostSketch h;
+      try {
+        if (!skdb::read_file(q, b)) throw std::runtime_error("read");
+        h = skdb::read_blob(b.data(), b.size());
+      } catch (const std::exception&) {
+        fprintf(stderr, "ERROR Problem reading sketch file %s. Exiting.\n", q.c_str());
+        r->failed = true;
+        return;
+      }
+      r->flat.add(h, true);
+      r->meta.push_back(genome_of(h));
+    }
+    r->bounds = {0, r->meta.size()};
+  };
+  QueryRead cur, next;
+  std::thread reader;
+  int rc = 0;
+  if (n_reads) load(0, &cur);
+  for (size_t k = 0; k < n_reads && rc == 0; k++) {
+    if (k + 1 < n_reads) reader = std::thread(load, k + 1, &next);
+    if (cur.failed) rc = 1;
+    for (size_t j = 0; j + 1 < cur.bounds.size() && rc == 0; j++) {
+      const size_t g0 = cur.bounds[j], g1 = cur.bounds[j + 1];
+      sk_sketch_set* qset = nullptr;
+      uint64_t bases = 0;
+      if (queries_are_sketch) {
+        qset = cur.flat.import(ctx, sp);
+        for (auto& g : cur.meta) { bases += g.total_len; qmeta.push_back(std::move(g)); }
+      } else {
+        qset = sketch(ctx, cur.in, sp, g0, g1);
+        for (size_t g = g0; g < g1; g++) { bases += cur.in.genomes[g].total_len; qmeta.push_back(std::move(cur.in.genomes[g])); }
+      }
+      if (!process(qset, bases)) rc = 1;
+    }
+    cur = QueryRead();                  // the group's sequence is no longer needed
+    if (reader.joinable()) reader.join();
+    cur = std::move(next);
+    next = QueryRead();
+  }
+  if (reader.joinable()) reader.join();
+  if (rc == 0 && qmeta.empty()) { fprintf(stderr, "ERROR No query sequences found.\n"); rc = 1; }
+  if (rc == 0 && qmeta.size() > blocks_written * FL) write_block();   // the last, partial block
+  sk_ref_index_free(idx);
   for (size_t d = W; d-- > 0;) sk_ctx_destroy(ctxs[d]);
   return rc;
 }
@@ -1775,6 +1924,8 @@ void usage() {
           "      index.db and sketches.db), mixed freely; a database stands for all of its sketches\n"
           "  skani-b200 sketch [fasta ... | -l list] -o new_folder [-i] [--separate-sketches]\n"
           "  skani-b200 search -d sketch_folder [query ... | -q ... | --ql list] [--qi] [-n N] [-o out]\n"
+          "      queries are read, sketched, screened and chained in groups of whole files (up to 4096 files, about 8 GiB of\n"
+          "      sequence; with --qi a larger file is cut between records) against the database's markers indexed once\n"
           "  skani-b200 cluster [fasta | sketch ... | -l list] [-i] [--ani T] [--single-linkage | --linkage average|complete]\n"
           "                    [--dendrogram Z.tsv] [-o out]\n"
           "      the triangle's genomes clustered at ANI >= T %% (default 95, 10 < T <= 100): greedy representatives, longest\n"

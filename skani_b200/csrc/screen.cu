@@ -140,6 +140,59 @@ screen_rows_kernel(const uint64_t* __restrict__ row_mk_off, const uint64_t* __re
   }
 }
 
+// The row pass of a screen whose ra / rb / scol are laid out: screen_rows_kernel over the rows (row_mod, row_rem) of
+// [0, n_rows_total) against the columns [0, NC) (col_off[j] .. col_off[j + 1] = column j's markers), with a first pair buffer of
+// max(2^20, 64 * cap_rows) pairs and one retry at the exact count when it overflows; the pairs are sorted and returned in a
+// malloc'd host array.
+static int rows_pass(sk_ctx* ctx, const uint64_t* d_row_off, const uint64_t* d_col_off, uint32_t n_rows_total, uint32_t NC,
+                     const uint32_t* ra, const uint32_t* rb, const uint32_t* scol, int mode, int rescue_small, double cutoff,
+                     uint32_t cap_rows, uint32_t row_mod, uint32_t row_rem, uint64_t** out_pairs, uint64_t* out_n) {
+  cudaStream_t st = ctx->stream;
+  // check_markers_quickly returns true outright for screen_val == 0 (src/screen.rs:91-93); callers substitute the default
+  // first, so this only triggers for an explicit 0 that survived: never through the reference CLI.
+  const int all_pass = 0;
+  const uint32_t tile = std::min<uint32_t>(NC, 48 * 1024);
+  const size_t smem = (size_t)tile * 4;
+  // always the same (maximal) value: the attribute is per device, and several contexts may screen on one device concurrently
+  SK_CUDA(cudaFuncSetAttribute(screen_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024 * 4));
+  unsigned long long cap = std::max<unsigned long long>(1ull << 20, 64ull * cap_rows);
+  DTmp<unsigned long long> d_n;
+  SK_CUDA(d_n.alloc(1, ctx));
+  DTmp<uint64_t> d_pairs;
+  unsigned long long n = 0;
+  for (int attempt = 0; attempt < 2; attempt++) {
+    SK_CUDA(d_pairs.alloc(cap, ctx));
+    SK_CUDA(cudaMemsetAsync(d_n.p, 0, 8, st));
+    const uint32_t n_rows_launch = n_rows_total > row_rem ? (n_rows_total - row_rem + row_mod - 1) / row_mod : 0;
+    if (n_rows_launch) {
+      SK_LAUNCH(ctx, "screen_rows_kernel", (screen_rows_kernel<<<n_rows_launch, 256, smem, st>>>(
+          d_row_off, d_col_off, n_rows_total, NC, ra, rb, scol, mode, rescue_small, cutoff, all_pass, tile, d_pairs.p, d_n.p, cap,
+          row_mod, row_rem)));
+    }
+    SK_CUDA(cudaMemcpyAsync(&n, d_n.p, 8, cudaMemcpyDeviceToHost, st));
+    SK_CUDA(cudaStreamSynchronize(st));
+    SK_CUDA(cudaGetLastError());
+    if (n <= cap) break;
+    cap = n;
+  }
+  uint64_t* host = (uint64_t*)malloc(std::max<size_t>(n, 1) * 8);
+  if (!host) return SK_ERR_NOMEM;
+  if (n > 0) {
+    DTmp<uint64_t> sorted;
+    SK_CUDA(sorted.alloc(n, ctx));
+    size_t tb = 0;
+    SK_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, d_pairs.p, sorted.p, (uint64_t)n, 0, 64, st));
+    DTmp<uint8_t> tmp;
+    SK_CUDA(tmp.alloc(tb, ctx));
+    SK_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, tb, d_pairs.p, sorted.p, (uint64_t)n, 0, 64, st));
+    SK_CUDA(cudaMemcpyAsync(host, sorted.p, n * 8, cudaMemcpyDeviceToHost, st));
+    SK_CUDA(cudaStreamSynchronize(st));
+  }
+  *out_pairs = host;
+  *out_n = n;
+  return SK_OK;
+}
+
 static int run_screen(sk_ctx* ctx, const sk_sketch_set* rows, const sk_sketch_set* cols, int mode, const sk_map_params* mp,
                       uint64_t** out_pairs, uint64_t* out_n, uint32_t row_mod = 1, uint32_t row_rem = 0) {
   cudaStream_t st = ctx->stream;
@@ -152,9 +205,6 @@ static int run_screen(sk_ctx* ctx, const sk_sketch_set* rows, const sk_sketch_se
   if (N >= (1ull << 31)) { ctx->err = "marker table too large for one screen call (>= 2^31 entries)"; return SK_ERR_PARAM; }
   double screen_val = mp->screen_val == 0. ? 0.80 : mp->screen_val;  // src/triangle.rs:34-42, src/dist.rs:68-77
   const double cutoff = powi21(screen_val);
-  // check_markers_quickly returns true outright for screen_val == 0 (src/screen.rs:91-93); callers substitute the default
-  // first, so this only triggers for an explicit 0 that survived: never through the reference CLI.
-  const int all_pass = 0;
 
   DTmp<uint64_t> d_row_off, d_col_off;
   SK_CUDA(d_row_off.alloc(NR + 1, ctx)); SK_CUDA(d_col_off.alloc(NC + 1, ctx));
@@ -204,48 +254,9 @@ static int run_screen(sk_ctx* ctx, const sk_sketch_set* rows, const sk_sketch_se
     }
     SK_CUDA(cudaStreamSynchronize(st));
   }
-  // ---- row pass with retry on capacity overflow
-  const uint32_t tile = std::min<uint32_t>(NC, 48 * 1024);
-  const size_t smem = (size_t)tile * 4;
-  // always the same (maximal) value: the attribute is per device, and several contexts may screen on one device concurrently
-  SK_CUDA(cudaFuncSetAttribute(screen_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024 * 4));
-  unsigned long long cap = std::max<unsigned long long>(1ull << 20, 64ull * NR);
-  DTmp<unsigned long long> d_n;
-  SK_CUDA(d_n.alloc(1, ctx));
-  DTmp<uint64_t> d_pairs;
-  unsigned long long n = 0;
-  for (int attempt = 0; attempt < 2; attempt++) {
-    SK_CUDA(d_pairs.alloc(cap, ctx));
-    SK_CUDA(cudaMemsetAsync(d_n.p, 0, 8, st));
-    const uint32_t n_rows_total = tri ? (NR > 0 ? NR - 1 : 0) : NR;  // src/triangle.rs:71: rows 0..N-2
-    const uint32_t n_rows_launch = n_rows_total > row_rem ? (n_rows_total - row_rem + row_mod - 1) / row_mod : 0;
-    if (n_rows_launch) {
-      SK_LAUNCH(ctx, "screen_rows_kernel", (screen_rows_kernel<<<n_rows_launch, 256, smem, st>>>(
-          d_row_off.p, d_col_off.p, n_rows_total, NC, ra.p, rb.p, scol.p, mode, mp->rescue_small, cutoff, all_pass, tile, d_pairs.p, d_n.p, cap,
-          row_mod, row_rem)));
-    }
-    SK_CUDA(cudaMemcpyAsync(&n, d_n.p, 8, cudaMemcpyDeviceToHost, st));
-    SK_CUDA(cudaStreamSynchronize(st));
-    SK_CUDA(cudaGetLastError());
-    if (n <= cap) break;
-    cap = n;
-  }
-  uint64_t* host = (uint64_t*)malloc(std::max<size_t>(n, 1) * 8);
-  if (!host) return SK_ERR_NOMEM;
-  if (n > 0) {
-    DTmp<uint64_t> sorted;
-    SK_CUDA(sorted.alloc(n, ctx));
-    size_t tb = 0;
-    SK_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb, d_pairs.p, sorted.p, (uint64_t)n, 0, 64, st));
-    DTmp<uint8_t> tmp;
-    SK_CUDA(tmp.alloc(tb, ctx));
-    SK_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, tb, d_pairs.p, sorted.p, (uint64_t)n, 0, 64, st));
-    SK_CUDA(cudaMemcpyAsync(host, sorted.p, n * 8, cudaMemcpyDeviceToHost, st));
-    SK_CUDA(cudaStreamSynchronize(st));
-  }
-  *out_pairs = host;
-  *out_n = n;
-  return SK_OK;
+  // ---- row pass with retry on capacity overflow (src/triangle.rs:71: triangle rows 0..N-2)
+  return rows_pass(ctx, d_row_off.p, d_col_off.p, tri ? (NR > 0 ? NR - 1 : 0) : NR, NC, ra.p, rb.p, scol.p, mode, mp->rescue_small, cutoff, NR,
+                   row_mod, row_rem, out_pairs, out_n);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -264,14 +275,14 @@ __global__ void ts_keys_kernel(const uint64_t* __restrict__ markers, const uint6
   const uint64_t base = off[g_begin];
   for (uint64_t i = off[g] + threadIdx.x; i < off[g + 1]; i += blockDim.x) keys[i - base] = (markers[i] << TS_GBITS) | g;
 }
-// bucket[b] = first table position whose key prefix is >= b; bucket[2^16] = n
-__global__ void ts_bucket_kernel(const uint64_t* __restrict__ key, uint32_t n, uint32_t* __restrict__ bucket) {
+// bucket[b] = first table position whose key prefix (key >> shift, 16 bits) is >= b; bucket[2^16] = n
+__global__ void ts_bucket_kernel(const uint64_t* __restrict__ key, uint32_t n, uint32_t shift, uint32_t* __restrict__ bucket) {
   const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b > (1u << TS_PREFIX_BITS)) return;
   uint32_t lo = 0, hi = n;
   while (lo < hi) {
     const uint32_t mid = (lo + hi) >> 1;
-    if ((key[mid] >> TS_PREFIX_SHIFT) < b) lo = mid + 1; else hi = mid;
+    if ((key[mid] >> shift) < b) lo = mid + 1; else hi = mid;
   }
   bucket[b] = lo;
 }
@@ -406,7 +417,7 @@ int tri_screen_add(TriScreen* ts, const sk_sketch_set* set, uint32_t g_end, uint
   unsigned long long n = 0;
   if (G > row_begin && G > 1) {
     // (a row's walk always ends at its own table entry, so it never runs past the end of the table)
-    ts_bucket_kernel<<<((1u << TS_PREFIX_BITS) + 256) / 256, 256, 0, st>>>(ts->key[ts->cur], (uint32_t)n_tot, ts->bucket); count_launch(ctx);
+    ts_bucket_kernel<<<((1u << TS_PREFIX_BITS) + 256) / 256, 256, 0, st>>>(ts->key[ts->cur], (uint32_t)n_tot, TS_PREFIX_SHIFT, ts->bucket); count_launch(ctx);
     const uint32_t tile = std::min<uint32_t>(std::max<uint32_t>(G, 1), 48 * 1024);
     const size_t smem = (size_t)tile * 4;
     SK_CUDA(cudaFuncSetAttribute(ts_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024 * 4));   // constant: see run_screen
@@ -444,6 +455,174 @@ int tri_screen_add(TriScreen* ts, const sk_sketch_set* set, uint32_t g_end, uint
   }
   *out_pairs = host;
   *out_n = n;
+  return SK_OK;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Persistent reference marker index (search: many query groups against one database).  The query x ref screen of
+// run_screen sorts the reference and query markers together for every call; here the reference markers are sorted ONCE,
+// per contiguous part of the references, into (marker, local reference) entries -- a stable sort of the genome-major
+// markers, so a run's entries stay in reference order exactly as inside run_screen's runs -- with a 16-bit prefix bucket
+// table.  A query group then only looks each of its markers up (ri_lookup_kernel writes the run's slice as ra / rb, as
+// qr_ranges_kernel does) and runs the same screen_rows_kernel and pair sort as run_screen, once per part.
+constexpr uint32_t RI_PREFIX_SHIFT = 2 * MARKER_K - TS_PREFIX_BITS;
+
+// entry i of the part [r0, r0 + gridDim.x) of a genome-major set belongs to local reference blockIdx.x
+__global__ void ri_part_ref_kernel(const uint64_t* __restrict__ off, uint32_t r0, uint32_t* __restrict__ ref) {
+  const uint32_t g = r0 + blockIdx.x;
+  const uint64_t base = off[r0];
+  for (uint64_t i = off[g] + threadIdx.x; i < off[g + 1]; i += blockDim.x) ref[i - base] = blockIdx.x;
+}
+// query marker e -> the slice [ra[e], rb[e]) of the part's sorted keys that holds the same marker (empty when none does)
+__global__ void __launch_bounds__(256)
+ri_lookup_kernel(const uint64_t* __restrict__ markers, uint64_t n_markers, const uint64_t* __restrict__ key,
+                 const uint32_t* __restrict__ bucket, uint32_t* __restrict__ ra, uint32_t* __restrict__ rb) {
+  for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n_markers; e += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t m = markers[e];
+    const uint64_t b = m >> RI_PREFIX_SHIFT;
+    uint32_t lo = 0, hi = 0;
+    if (b < (1u << TS_PREFIX_BITS)) {      // markers are < 2^42 (import refuses larger ones): every prefix has a bucket
+      const uint32_t end = bucket[b + 1];
+      lo = bucket[b];
+      hi = end;
+      while (lo < hi) {                    // first key >= m
+        const uint32_t mid = (lo + hi) >> 1;
+        if (key[mid] < m) lo = mid + 1; else hi = mid;
+      }
+      hi = end;
+      uint32_t l2 = lo;
+      while (l2 < hi) {                    // first key > m (a larger marker of the next prefix starts at bucket[b + 1])
+        const uint32_t mid = (l2 + hi) >> 1;
+        if (key[mid] <= m) l2 = mid + 1; else hi = mid;
+      }
+      hi = l2;
+    }
+    ra[e] = lo;
+    rb[e] = hi;
+  }
+}
+
+struct RefIndexPart {
+  uint32_t r0 = 0, r1 = 0;        // references [r0, r1)
+  size_t n = 0;                   // entries = their markers
+  uint64_t* key = nullptr;        // [n] markers, sorted
+  uint32_t* scol = nullptr;       // [n] local reference (r - r0) of each sorted entry
+  uint32_t* bucket = nullptr;     // [2^16 + 1] first entry of each 16-bit marker prefix
+};
+
+// entries per part: < 2^31 (cub's item count, and the 32-bit ra / rb slices of screen_rows_kernel).  SK_REF_INDEX_PART_MARKERS
+// lowers it (a test hook: many parts from a small database); read when an index is created.
+static size_t ref_index_part_limit() {
+  size_t lim = (1ull << 31) - 1;
+  if (const char* e = getenv("SK_REF_INDEX_PART_MARKERS")) lim = std::min<size_t>(lim, (size_t)std::max(1ll, atoll(e)));
+  return lim;
+}
+
+}  // namespace sk
+
+struct sk_ref_index {
+  sk_ctx* ctx = nullptr;
+  uint32_t G = 0;
+  uint64_t* col_off = nullptr;    // [G + 1] device copy of the references' marker offsets
+  std::vector<sk::RefIndexPart> parts;
+  size_t bytes = 0;               // device bytes held
+};
+
+namespace sk {
+
+static void ref_index_release(sk_ref_index* x) {
+  if (!x) return;
+  for (auto& p : x->parts) {
+    if (p.key) x->ctx->arena.release(p.key);
+    if (p.scol) x->ctx->arena.release(p.scol);
+    if (p.bucket) x->ctx->arena.release(p.bucket);
+  }
+  if (x->col_off) x->ctx->arena.release(x->col_off);
+  delete x;
+}
+
+// the parts of x (ctx, G set) from refs; on failure the caller releases x
+static int ref_index_build(sk_ctx* ctx, const sk_sketch_set* refs, sk_ref_index* x) {
+  cudaStream_t st = ctx->stream;
+  auto fail = [&](const char* msg) { ctx->err = msg; return SK_ERR_NOMEM; };
+  const auto alloc = [&](void** p, size_t bytes) { x->bytes += bytes; return ctx->arena.alloc(p, std::max<size_t>(bytes, 8)); };
+  if (alloc((void**)&x->col_off, ((size_t)x->G + 1) * 8) != cudaSuccess) return fail("ref_index: out of device memory");
+  SK_CUDA(h2d_small(ctx, x->col_off, refs->mk_off.data(), ((size_t)x->G + 1) * 8));
+  const size_t lim = ref_index_part_limit();
+  for (uint32_t r0 = 0; r0 < x->G;) {
+    uint32_t r1 = r0 + 1;     // at least one reference; a genome holds far fewer than 2^31 markers
+    while (r1 < x->G && refs->mk_off[r1 + 1] - refs->mk_off[r0] <= lim) r1++;
+    RefIndexPart p;
+    p.r0 = r0; p.r1 = r1;
+    p.n = refs->mk_off[r1] - refs->mk_off[r0];
+    x->parts.push_back(p);
+    RefIndexPart& q = x->parts.back();
+    if (alloc((void**)&q.key, q.n * 8) != cudaSuccess || alloc((void**)&q.scol, q.n * 4) != cudaSuccess ||
+        alloc((void**)&q.bucket, ((1u << TS_PREFIX_BITS) + 1) * 4) != cudaSuccess)
+      return fail("ref_index: out of device memory");
+    if (q.n > 0) {
+      DTmp<uint32_t> ref;
+      SK_CUDA(ref.alloc(q.n, ctx));
+      ri_part_ref_kernel<<<r1 - r0, 256, 0, st>>>(x->col_off, r0, ref.p); count_launch(ctx);
+      // stable on the marker bits: inside a run the references stay ascending (the set is genome-major), as in run_screen
+      size_t tb = 0;
+      const uint64_t* in = refs->markers + refs->mk_off[r0];
+      SK_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, in, q.key, ref.p, q.scol, (int)q.n, 0, 2 * MARKER_K, st));
+      DTmp<uint8_t> tmp;
+      SK_CUDA(tmp.alloc(tb, ctx));
+      SK_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, in, q.key, ref.p, q.scol, (int)q.n, 0, 2 * MARKER_K, st));
+    }
+    ts_bucket_kernel<<<((1u << TS_PREFIX_BITS) + 256) / 256, 256, 0, st>>>(q.key, (uint32_t)q.n, RI_PREFIX_SHIFT, q.bucket); count_launch(ctx);
+    SK_CUDA(cudaStreamSynchronize(st));   // the temporaries go back to the arena
+    r0 = r1;
+  }
+  SK_CUDA(cudaGetLastError());
+  return SK_OK;
+}
+
+static int ref_index_create(sk_ctx* ctx, const sk_sketch_set* refs, sk_ref_index** out) {
+  sk_ref_index* x = new sk_ref_index();
+  x->ctx = ctx;
+  x->G = refs->G;
+  const int rc = ref_index_build(ctx, refs, x);
+  if (rc != SK_OK) { ref_index_release(x); return rc; }
+  *out = x;
+  return SK_OK;
+}
+
+static int ref_index_screen(sk_ctx* ctx, const sk_ref_index* x, const sk_sketch_set* queries, const sk_map_params* mp, int mode,
+                            uint64_t** out_pairs, uint64_t* out_n) {
+  cudaStream_t st = ctx->stream;
+  const uint32_t NR = queries->G;
+  *out_pairs = nullptr; *out_n = 0;
+  if (NR == 0 || x->G == 0) { *out_pairs = (uint64_t*)malloc(8); return *out_pairs ? SK_OK : SK_ERR_NOMEM; }
+  const double cutoff = powi21(mp->screen_val == 0. ? 0.80 : mp->screen_val);   // src/dist.rs:68-77
+  const size_t Mr = queries->M;
+  DTmp<uint64_t> d_row_off;
+  SK_CUDA(d_row_off.alloc((size_t)NR + 1, ctx));
+  SK_CUDA(h2d_small(ctx, d_row_off.p, queries->mk_off.data(), ((size_t)NR + 1) * 8));
+  DTmp<uint32_t> ra, rb;
+  SK_CUDA(ra.alloc(Mr, ctx)); SK_CUDA(rb.alloc(Mr, ctx));
+  std::vector<uint64_t> all;
+  for (const RefIndexPart& p : x->parts) {
+    if (Mr) {
+      const uint32_t blocks = (uint32_t)std::min<uint64_t>((Mr + 255) / 256, 1u << 20);
+      ri_lookup_kernel<<<blocks, 256, 0, st>>>(queries->markers, Mr, p.key, p.bucket, ra.p, rb.p); count_launch(ctx);
+    }
+    uint64_t* pairs = nullptr; uint64_t n = 0;
+    SK_TRY(rows_pass(ctx, d_row_off.p, x->col_off + p.r0, NR, p.r1 - p.r0, ra.p, rb.p, p.scol, mode, mp->rescue_small, cutoff, NR, 1, 0,
+                     &pairs, &n));
+    // pairs are (local ref << 32 | query), sorted; parts ascend, so the concatenation stays sorted
+    const uint64_t shift = (uint64_t)p.r0 << 32;
+    if (x->parts.size() == 1) { *out_pairs = pairs; *out_n = n; return SK_OK; }
+    for (uint64_t i = 0; i < n; i++) all.push_back(pairs[i] + shift);
+    free(pairs);
+  }
+  uint64_t* host = (uint64_t*)malloc(std::max<size_t>(all.size(), 1) * 8);
+  if (!host) return SK_ERR_NOMEM;
+  if (!all.empty()) memcpy(host, all.data(), all.size() * 8);
+  *out_pairs = host;
+  *out_n = all.size();
   return SK_OK;
 }
 
@@ -488,6 +667,38 @@ int sk_screen_query_ref(sk_ctx* ctx, const sk_sketch_set* refs, const sk_sketch_
   if (!ctx || !refs || !queries || !mp || !pairs || !n || mode < 0 || mode > 3) return SK_ERR_PARAM;
   SK_CUDA(cudaSetDevice(ctx->device));
   return sk::run_screen(ctx, queries, refs, mode, mp, pairs, n);
+}
+
+int sk_ref_index_create(sk_ctx* ctx, const sk_sketch_set* refs, sk_ref_index** idx) {
+  if (!ctx || !refs || !idx) return SK_ERR_PARAM;
+  *idx = nullptr;
+  if (refs->ctx != ctx) { ctx->err = "sk_ref_index_create: the set lives on another context"; return SK_ERR_PARAM; }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  return sk::ref_index_create(ctx, refs, idx);
+}
+
+int sk_ref_index_screen(sk_ctx* ctx, const sk_ref_index* idx, const sk_sketch_set* queries, const sk_map_params* mp, int mode,
+                        uint64_t** pairs, uint64_t* n) {
+  if (!ctx || !idx || !queries || !mp || !pairs || !n || mode < 0 || mode > 3) return SK_ERR_PARAM;
+  if (idx->ctx != ctx || queries->ctx != ctx) { ctx->err = "sk_ref_index_screen: the index and the queries must live on ctx"; return SK_ERR_PARAM; }
+  SK_CUDA(cudaSetDevice(ctx->device));
+  return sk::ref_index_screen(ctx, idx, queries, mp, mode, pairs, n);
+}
+
+int sk_ref_index_info(const sk_ref_index* idx, uint32_t* n_refs, uint32_t* n_parts, uint64_t* device_bytes) {
+  if (!idx) return SK_ERR_PARAM;
+  if (n_refs) *n_refs = idx->G;
+  if (n_parts) *n_parts = (uint32_t)idx->parts.size();
+  if (device_bytes) *device_bytes = idx->bytes;
+  return SK_OK;
+}
+
+int sk_ref_index_free(sk_ref_index* idx) {
+  if (!idx) return SK_OK;
+  sk_ctx* ctx = idx->ctx;
+  SK_CUDA(cudaSetDevice(ctx->device));
+  sk::ref_index_release(idx);
+  return SK_OK;
 }
 
 }  // extern "C"

@@ -368,6 +368,39 @@ def screen_query_ref(ctx, refs, queries, mp=None, mode=0):
     return arr
 
 
+class RefIndex:
+    """sk_ref_index: the markers of a reference set sorted once on ctx, in contiguous parts of < 2^31 markers
+    (SK_REF_INDEX_PART_MARKERS at creation lowers the bound).  screen() of any query set on ctx returns
+    screen_query_ref(ctx, refs, queries, mp, mode); refs may be freed once the index exists."""
+
+    def __init__(self, ctx, refs):
+        self.ctx = ctx
+        h = C.c_void_p()
+        ctx.check(ctx.L.sk_ref_index_create(ctx.h, refs.h, C.byref(h)))
+        self.h = h
+
+    def screen(self, queries, mp=None, mode=0):
+        mp = mp or map_params()
+        return _pairs_out(self.ctx, self.ctx.L.sk_ref_index_screen, self.ctx.h, self.h, queries.h, C.byref(mp), int(mode))
+
+    def info(self):
+        """(references, parts, device bytes held)"""
+        g, p, b = C.c_uint32(), C.c_uint32(), C.c_uint64()
+        self.ctx.check(self.ctx.L.sk_ref_index_info(self.h, C.byref(g), C.byref(p), C.byref(b)))
+        return g.value, p.value, b.value
+
+    def free(self):
+        if self.h:
+            self.ctx.L.sk_ref_index_free(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.free()
+        except Exception:
+            pass
+
+
 def chain_pairs(ctx, refs, queries, pairs, mp=None, as_array=False):
     """sk_chain_pairs.  as_array=True returns a numpy structured array (RESULT_DTYPE) instead of a list of AniResult."""
     mp = mp or map_params()
